@@ -99,6 +99,10 @@ def lib() -> C.CDLL:
     L.fpngb_debug_inline_crc.argtypes = [C.c_int]
     L.fpngb_debug_decode_staged.restype = None
     L.fpngb_debug_decode_staged.argtypes = [C.c_int]
+    L.fpngb_debug_decode_repairs.restype = C.c_ulonglong
+    L.fpngb_debug_decode_repairs.argtypes = [C.c_int]
+    L.fpngb_debug_decode_preroll.restype = C.c_int
+    L.fpngb_debug_decode_preroll.argtypes = [C.c_uint32]
     L.fpngb_debug_rows_per_warp.restype = None
     L.fpngb_debug_rows_per_warp.argtypes = [C.c_uint32]
     L.fpngb_debug_static_table.restype = C.c_int

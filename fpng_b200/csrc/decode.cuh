@@ -7,7 +7,8 @@ namespace fpngb {
 constexpr int kDecThreads = 256;            // subsequences per CTA in the scan / write kernels
 constexpr int kLinkThreads = 1024;          // subsequences linked per step by the per-file chain kernel
 constexpr uint32_t kSubBits = 1024;         // bits per subsequence (>> longest token: 12 + 5 + 1 bits)
-constexpr uint32_t kPreRoll = 256;          // speculative lead-in before a subsequence (self-synchronisation distance)
+constexpr uint32_t kPreRoll = 256;          // speculative lead-in before a subsequence (self-synchronisation distance); the
+                                            // default of DecodeParams::pre_roll and its maximum (the scan kernel's window lead)
 
 // Per-subsequence record.  After decode_scan_kernel: start/exit/eob_end are absolute aligned-stream bit positions,
 // n_out/nlit/lits describe the tokens starting in the subsequence.  decode_link_kernel rewrites it for the write
@@ -42,6 +43,7 @@ struct DecodeParams {
     uint8_t* d_out; size_t out_stride;
     uint32_t* d_status;                     // [n] FPNG_DECODE_* codes
     uint32_t w, h, chans;
+    uint32_t pre_roll;                      // speculative lead-in bits of decode_scan_kernel, 0..kPreRoll (kPreRoll unless a test sets it)
 };
 
 void launch_decode(const DecodeParams& p, uint32_t n, uint32_t desired, cudaStream_t s);
@@ -49,5 +51,6 @@ void decode_profile_enable(bool on);
 int decode_profile_read(float* ms, int n);
 unsigned long long decode_link_repairs(bool reset);
 void decode_set_staged(bool on);            // write pass through the shared-memory staged kernel (default) or decode_write_kernel alone
+bool decode_set_pre_roll(uint32_t bits);    // DecodeParams::pre_roll of later calls; false (unchanged) above kPreRoll
 
 }  // namespace fpngb

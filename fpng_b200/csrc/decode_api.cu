@@ -264,6 +264,9 @@ FPNGB_API int fpngb_decode_profile_read(float* ms, int n) { return decode_profil
 // test hook: number of subsequences the link pass had to decode again since the last reset (synchronises the device)
 FPNGB_API void fpngb_debug_decode_staged(int on) { decode_set_staged(on != 0); }   // tests / A/B: 0 = decode_write_kernel alone
 FPNGB_API unsigned long long fpngb_debug_decode_repairs(int reset) { cudaDeviceSynchronize(); return decode_link_repairs(reset != 0); }
+// test hook: speculative lead-in (bits) of the scan kernel for later decode calls, default 256; 0 makes nearly every guessed subsequence
+// start wrong, so the link pass has to repair it.  Pixels and statuses never depend on it.  FPNGB_ERR_INVALID_ARG (unchanged) above 256.
+FPNGB_API int fpngb_debug_decode_preroll(uint32_t bits) { return decode_set_pre_roll(bits) ? FPNGB_OK : FPNGB_ERR_INVALID_ARG; }
 
 int fpngb_get_info_ex(const void* file, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs, uint32_t* idat_len)
 {

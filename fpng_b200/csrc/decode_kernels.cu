@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(32) decode_prepare_kernel(DecodeParams p)
 // D2: token decode.  The token bit-string of a file is cut into subsequences of kSubBits bits (absolute multiples of
 // kSubBits in the aligned-stream bit coordinate).  Three kernels:
 //   D2a decode_scan_kernel   one thread per subsequence, all files and subsequences in parallel: the thread starts
-//                            kPreRoll bits early (speculatively), lets the self-synchronising prefix code lock on, takes
+//                            p.pre_roll (kPreRoll) bits early (speculatively), lets the self-synchronising prefix code lock on, takes
 //                            the first token boundary inside its subsequence as its start, then decodes to its exit (first
 //                            boundary in the next subsequence) counting output bytes and remembering the last 4 literals.
 //   D2b decode_link_kernel   one CTA per file walks the subsequences in order, 1024 at a time: verifies that every
@@ -745,7 +745,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_scan_kernel(DecodeParams p
         origin = sp.tok0;
         r = scan_window(s_win, (uint32_t)(origin - 32ull * sm.sw_base), s_fast, lutg, 0u, 0u, (uint32_t)((g + 1) * kSubBits - origin));
     } else {
-        origin = lo_abs - kPreRoll < sp.tok0 ? sp.tok0 : lo_abs - kPreRoll;     // never pre-roll across the block header
+        origin = lo_abs < sp.tok0 + p.pre_roll ? sp.tok0 : lo_abs - p.pre_roll;   // never pre-roll across the block header
         r = scan_window(s_win, (uint32_t)(origin - 32ull * sm.sw_base), s_fast, lutg, 0u, (uint32_t)(lo_abs - origin), (uint32_t)(lo_abs - origin) + kSubBits);
     }
     info->start = origin + r.first;
@@ -1380,8 +1380,22 @@ int decode_profile_read(float* ms, int n)
 static bool g_dec_staged = getenv("FPNGB_DEC_STAGED") && atoi(getenv("FPNGB_DEC_STAGED")) != 0;
 void decode_set_staged(bool on) { g_dec_staged = on; }
 
-void launch_decode(const DecodeParams& p, uint32_t n, uint32_t desired, cudaStream_t s)
+// Speculative lead-in of decode_scan_kernel (fpngb_debug_decode_preroll).  The link pass makes the result independent of it; tests set
+// it below the default to force wrong guesses.  At most kPreRoll: the scan kernel's stream window starts kWinLead words before its
+// first subsequence.
+static_assert(kPreRoll <= kWinLead * 32, "the pre-roll stays inside the scan kernel's stream window");
+static uint32_t g_dec_pre_roll = kPreRoll;
+bool decode_set_pre_roll(uint32_t bits)
 {
+    if (bits > kPreRoll) return false;
+    g_dec_pre_roll = bits;
+    return true;
+}
+
+void launch_decode(const DecodeParams& params, uint32_t n, uint32_t desired, cudaStream_t s)
+{
+    DecodeParams p = params;
+    p.pre_roll = g_dec_pre_roll;
     DEC_MARK(0);
     decode_prepare_kernel<<<n, 32, 0, s>>>(p);
     DEC_MARK(1);

@@ -5,6 +5,7 @@ G0 "gradient":        R = floor(255 x/(w-1)), G = floor(255 y/(h-1)), B = (x + y
 G1 "gradient+noise":  G0 + per-channel uniform integer noise in [-3, 3] (MT19937, seed 1234 + i); literal-dominated,
                       out/in ~ 0.55-0.6.
 G2 "random":          uniform bytes (MT19937); always lands on the stored-block fallback.
+U<k> "uniform deltas": Up-filtered bytes uniform over k values; near-fixed-length Huffman codes when encoded 2-pass.
 plus the mutation families of the reference's encoder fuzzers (src/fpng_test.cpp:381-615): colour runs, byte fills.
 """
 from __future__ import annotations
@@ -69,9 +70,19 @@ def mutated(w: int, h: int, chans: int, seed: int) -> np.ndarray:
 KINDS = {"g0": gradient, "g1": gradient_noise, "g2": random_bytes}
 
 
+def uniform_deltas(w: int, h: int, chans: int, k: int, index: int = 0) -> np.ndarray:
+    """Image whose Up-filtered bytes are uniform over 0..k-1 (MT19937, seed 5678 + i): noisy low-bit-depth content.  Its
+    2-pass Huffman table is close to a fixed-length code, which hardly resynchronises after a wrong start: the decoder's
+    speculative subsequence starts (decode_scan_kernel) are mostly wrong and the link pass repairs them in chains."""
+    rs = np.random.RandomState(5678 + index)
+    return from_deltas(rs.randint(0, k, size=(h, w, chans)))
+
+
 def make(kind: str, w: int, h: int, chans: int, index: int = 0) -> np.ndarray:
     if kind in KINDS:
         return KINDS[kind](w, h, chans, index)
+    if kind[:1] == "u" and kind[1:].isdigit():                    # "u128", "u64", "u16", "u2"
+        return uniform_deltas(w, h, chans, int(kind[1:]), index)
     if kind == "runs":
         return colour_runs(w, h, chans, index)
     if kind == "mut":

@@ -23,9 +23,11 @@ import numpy as np
 import pytest
 
 import imagegen
+from common import with_text_chunk as _with_text_chunk
 
 K_SUB_BITS = 1024          # csrc/decode.cuh
 K_PRE_ROLL = 256
+K_LINK_THREADS = 1024      # subsequences per step of decode_link_kernel
 POS_END, POS_ERR = -1, -2  # exit flags (kPosEnd / kPosErr)
 
 LEN_BASE = [3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258]
@@ -241,6 +243,59 @@ class Model:
         ok = (not err) and done and out_pos == total_out and used + 4 == self.idat_len      # fpng.cpp:2559-2584
         return ok, jobs
 
+    # ---- decode_link_kernel as the device runs it: chunks of K_LINK_THREADS subsequences; inside a chunk every iteration repairs
+    # ALL mismatches at once against the exits of the previous iteration, until no start moves; the chunk's last exit is the
+    # carry into the next chunk.  A subsequence whose predecessor is repaired in the same iteration may have to be repaired
+    # again, so the repair count can exceed the number of subsequences (fpngb_debug_decode_repairs counts the same way).
+    def link_parallel(self, subs, max_iters=None):
+        """-> (ok, jobs, repairs, iterations per chunk); `max_iters` cuts the loop short (to show the tests discriminate)"""
+        total_out = (self.w * self.chans + 1) * self.h
+        carry_start, carry_out, ln, lv = self.tok0, 0, 0, 0
+        jobs, done, err, eob_end, repairs, iters = [], False, False, 0, 0, []
+        pos = lambda x: x >= 0                                             # a real position, not POS_END / POS_ERR
+        for base in range(0, len(subs), K_LINK_THREADS):
+            chunk = [dict(s) for s in subs[base:base + K_LINK_THREADS]]
+            pad = K_LINK_THREADS - len(chunk)                              # threads without a subsequence: exit = kPosErr
+            it = 0
+            while max_iters is None or it < max_iters:
+                exits = [s["exit"] for s in chunk]
+                bad = [t for t, s in enumerate(chunk) if pos(carry_start if t == 0 else exits[t - 1])
+                       and (carry_start if t == 0 else exits[t - 1]) != s["start"]]
+                if not bad:
+                    break
+                it += 1
+                for t in bad:
+                    want = carry_start if t == 0 else exits[t - 1]
+                    hi = (self.g0 + base + t + 1) * K_SUB_BITS
+                    chunk[t] = dict(start=want, exit=want, eob_end=0, n_out=0, nlit=0, lits=0) if want >= hi else self.scan(want, want, hi)
+                repairs += len(bad)
+            iters.append(it)
+            first_bad = next((t for t, s in enumerate(chunk) if not pos(s["exit"])), len(chunk) if pad else K_LINK_THREADS)
+            for t, s in enumerate(chunk[:first_bad + 1]):
+                if carry_out + s["n_out"] > total_out:
+                    err = True
+                jobs.append(dict(g=self.g0 + base + t, start=s["start"], out_pos=carry_out, n_out=s["n_out"], tail=lv))
+                carry_out += s["n_out"]
+                ln, lv = self.lit_combine(ln, lv, s["nlit"], s["lits"])
+            if first_bad < len(chunk):
+                if chunk[first_bad]["exit"] == POS_END:
+                    done, eob_end = True, chunk[first_bad]["eob_end"]
+                else:
+                    err = True
+            carry_start = chunk[-1]["exit"] if not pad else POS_ERR
+            if carry_out > total_out:
+                err = True
+            if done or err:
+                break
+        used = (eob_end - self.bits.bit0 + 7) >> 3 if eob_end >= self.bits.bit0 else 0
+        ok = (not err) and done and carry_out == total_out and used + 4 == self.idat_len      # fpng.cpp:2559-2584
+        return ok, jobs, repairs, iters
+
+    def decode_parallel(self, shuffle_seed=0, max_iters=None):
+        """decode() with the link pass of the device (link_parallel) -> (pixels or None, repairs, iterations per chunk)"""
+        ok, jobs, repairs, iters = self.link_parallel(self.scan_all(), max_iters)
+        return (self.write_jobs(jobs, shuffle_seed) if ok else None), repairs, iters
+
     # ---- decode_write_range: one subsequence, no other context
     def write(self, job, stream: bytearray):
         chans, bpl, h = self.chans, self.w * self.chans, self.h
@@ -280,8 +335,9 @@ class Model:
 
     def decode(self, shuffle_seed=0):
         ok, jobs = self.link(self.scan_all())
-        if not ok:
-            return None
+        return self.write_jobs(jobs, shuffle_seed) if ok else None
+
+    def write_jobs(self, jobs, shuffle_seed):
         bpl = self.w * self.chans
         stream = bytearray((bpl + 1) * self.h)
         order = list(range(len(jobs)))
@@ -293,14 +349,6 @@ class Model:
         assert np.array_equal(rows[:, 0], np.array([0] + [2] * (self.h - 1), np.uint8))
         # unfilter_kernel: running byte-wise sum down the columns (fpng.cpp:2439-2466)
         return np.cumsum(rows[:, 1:].astype(np.uint32), axis=0).astype(np.uint8).reshape(-1)
-
-
-def _with_text_chunk(png: bytes, payload_len: int) -> bytes:
-    """inserts a valid ancillary chunk in front of fdEC: moves the zlib stream to another byte alignment (Stream::bit0)"""
-    import zlib
-    body = bytes(range(65, 65 + payload_len))
-    ch = len(body).to_bytes(4, "big") + b"tEXt" + body + (zlib.crc32(b"tEXt" + body) & 0xFFFFFFFF).to_bytes(4, "big")
-    return png[:33] + ch + png[33:]
 
 
 CASES = [("g1", 160, 24, 3, 0), ("g1", 97, 31, 4, 0), ("g0", 256, 40, 4, 0), ("g0", 333, 20, 3, 0), ("runs", 300, 17, 3, 0),
@@ -357,3 +405,69 @@ def test_reference_written_file_and_truncation(oracle, ref):
     assert info[0] == 0 and ref.decode(bad, chans)[0] == 1
     ok, _ = (lambda mm: mm.link(mm.scan_all()))(Model(bad, info))
     assert not ok
+
+
+def model_repairs(file: bytes, pre_roll=K_PRE_ROLL):
+    """subsequences decode_link_kernel decodes again for `file` (fpngb_debug_decode_repairs after one decode of it): 0 when the
+    decoder never reaches the link pass (container or block header rejected, stored blocks)"""
+    import fpng_b200
+    info = fpng_b200.get_info_ex(file)
+    if info[0] != 0:
+        return 0
+    try:
+        m = Model(file, info, pre_roll=pre_roll)
+    except (AssertionError, IndexError, TypeError):                         # prepare() rejected the header / stored blocks
+        return 0
+    return m.link_parallel(m.scan_all())[2]
+
+
+# Slow-synchronising files: Up-filtered bytes uniform over k values (imagegen "u<k>").  Encoded 2-pass, the per-image table is
+# close to a fixed-length code and wrong subsequence starts hardly ever fall back onto the token grid within the pre-roll; the
+# link pass repairs most subsequences, in chains that take several iterations per chunk.  1-pass uses the shipped table (k = 128
+# and 64 then fall back to stored blocks).  Floors: repairs per subsequence, and the most iterations any chunk needed.
+U_CASES = [("u128", 640, 100, 3, 1, 1.2, 6), ("u128", 400, 100, 4, 1, 1.2, 6), ("u64", 520, 120, 3, 1, 0.6, 4),
+           ("u16", 720, 100, 4, 1, 0.1, 2), ("u2", 700, 140, 4, 0, 0.1, 2)]
+
+
+@pytest.mark.parametrize("kind,w,h,chans,flags,min_rate,min_iters", U_CASES)
+def test_link_loop_recovers_slow_synchronising_files(oracle, kind, w, h, chans, flags, min_rate, min_iters):
+    import fpng_b200
+    img = imagegen.make(kind, w, h, chans, 1)
+    png = oracle.encode(img, w, h, chans, flags)
+    for pad in range(4):                                                   # all four alignments of the zlib stream inside its word
+        f = png if pad == 0 else _with_text_chunk(png, pad)
+        m = Model(f, fpng_b200.get_info_ex(f))
+        nsub = m.g1 - m.g0 + 1
+        px, repairs, iters = m.decode_parallel(shuffle_seed=pad)
+        assert px is not None and np.array_equal(px, np.asarray(img).reshape(-1)), (kind, w, h, chans, flags, pad)
+        assert nsub > K_LINK_THREADS and len(iters) >= 2, nsub                # the carry between chunks is exercised
+        assert repairs >= min_rate * nsub and max(iters) >= min_iters, (kind, pad, nsub, repairs, iters)
+        assert m.link(m.scan_all())[0]                                     # the serial restatement agrees
+        if min_iters >= 2:                                                 # a loop cut after one iteration must not recover them
+            assert Model(f, fpng_b200.get_info_ex(f)).decode_parallel(max_iters=1)[0] is None
+
+
+def test_uniform_delta_files_match_reference(oracle, ref):
+    """the u-kind files of the CPU and GPU tests are what the unmodified reference encoder writes"""
+    shapes = [c[:5] for c in U_CASES] + [(k, w, h, c, f) for k in ("u128", "u64", "u16", "u2") for (w, h) in ((1024, 160), (1920, 200))
+                                         for c in (3, 4) for f in (0, 1)]
+    for kind, w, h, chans, flags in shapes:
+        img = imagegen.make(kind, w, h, chans, 1)
+        assert oracle.encode(img, w, h, chans, flags) == ref.encode(img, w, h, chans, flags), (kind, w, h, chans, flags)
+
+
+def test_parallel_link_restates_serial_link_on_ordinary_files(oracle):
+    """on files that lock on within the pre-roll the device loop and the serial chain agree, and pre-roll 0 forces repairs in
+    both; the parallel count is never below the serial one (a repaired subsequence may be repaired again)"""
+    import fpng_b200
+    for kind, w, h, chans, flags in (("g1", 640, 200, 3, 0), ("runs", 300, 17, 3, 0), ("g0", 1100, 6, 3, 1)):
+        img = imagegen.make(kind, w, h, chans, 5)
+        png = oracle.encode(img, w, h, chans, flags)
+        for pre_roll in (K_PRE_ROLL, 0, 13):
+            m = Model(png, fpng_b200.get_info_ex(png), pre_roll=pre_roll)
+            subs = m.scan_all()
+            ok, jobs = m.link(subs)
+            pok, pjobs, repairs, iters = m.link_parallel(subs)
+            assert ok and pok and jobs == pjobs and repairs >= m.repairs, (kind, pre_roll)
+            if pre_roll == 0:
+                assert repairs > (m.g1 - m.g0) // 2
