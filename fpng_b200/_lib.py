@@ -50,6 +50,11 @@ def lib() -> C.CDLL:
     L.fpngb_decode_batch_device.restype = C.c_int
     L.fpngb_decode_batch_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
                                             C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+    L.fpngb_get_info_batch_device.restype = C.c_int
+    L.fpngb_get_info_batch_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+    L.fpngb_decode_packed_device.restype = C.c_int
+    L.fpngb_decode_packed_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32,
+                                             C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.fpngb_compact_batch_device.restype = C.c_int
     L.fpngb_compact_batch_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.fpngb_decode_batch_host.restype = C.c_int

@@ -204,6 +204,67 @@ def decode_batch_device(files_dev, sizes, idat_ofs, idat_len, w: int, h: int, ch
     return out, status
 
 
+FPNGB_DECODE_SHAPE_MISMATCH = 100   # decode_packed_device only: a valid file whose w/h/chans differ from the call's
+
+
+def _packed_args(data, offsets, sizes):
+    import torch
+
+    assert data.is_cuda and data.dtype == torch.uint8 and data.is_contiguous(), "data: flat uint8 CUDA tensor"
+    assert offsets.is_cuda and offsets.dtype == torch.int64 and offsets.is_contiguous(), "offsets: int64 CUDA tensor"
+    assert sizes.is_cuda and sizes.dtype == torch.int32 and sizes.is_contiguous() and sizes.dim() == 1, "sizes: int32 CUDA tensor"
+    n = sizes.shape[0]
+    assert offsets.numel() >= n, "one offset per file (dist.compact's extra total at the end is ignored)"
+    return n
+
+
+def get_info_batch_device(data, offsets, sizes, stream=None):
+    """Container walk on the device of the files packed in `data` (file i: sizes[i] bytes at offsets[i]) -- the layout of
+    dist.compact and of the gather window.  data: flat uint8 CUDA tensor, offsets: int64 CUDA tensor (>= n entries),
+    sizes: int32 CUDA tensor [n] (uint32 values; 0 = no file).  Returns an int32 CUDA tensor [n, 6]: per file
+    (status, w, h, chans, idat_ofs, idat_len) as get_info_ex.  Enqueued on the current torch stream (or `stream`); no
+    host synchronisation."""
+    import torch
+
+    n = _packed_args(data, offsets, sizes)
+    info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
+    if n == 0:
+        return info
+    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    check(lib().fpngb_get_info_batch_device(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, info.data_ptr(), s),
+          "get_info_batch_device")
+    return info
+
+
+def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: int, desired_channels: int, max_file_size=None,
+                         out=None, status=None, stream=None):
+    """Decode the w x h x chans_in_file fpng files packed in device memory (same arguments as get_info_batch_device; every
+    file 4-byte aligned).  The container walk runs on the device: no host synchronisation and no host copy.
+    Returns (pixels uint8 [n, h, w, desired_channels], status int32 [n]).  status[i] is fpng_decode_memory's code for file i,
+    or FPNGB_DECODE_SHAPE_MISMATCH for a valid file of another shape, or FPNG_DECODE_INVALID_ARG for size 0, size >
+    max_file_size or an offset that is not a multiple of 4; pixels of files with a non-zero status are left untouched.
+    max_file_size (bytes) bounds every file and sizes the decoder's workspace; the default, max_encoded_size(w, h,
+    chans_in_file), holds for every file this library or the reference encoder writes.  A smaller bound known to the
+    caller saves workspace and launch overhead."""
+    import torch
+
+    n = _packed_args(data, offsets, sizes)
+    if max_file_size is None:
+        max_file_size = min(max_encoded_size(w, h, chans_in_file), 0xFFFFFFFF)
+    if out is None:
+        out = torch.empty((n, h, w, desired_channels), dtype=torch.uint8, device=data.device)
+    if status is None:
+        status = torch.empty((n,), dtype=torch.int32, device=data.device)
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= n * h * w * desired_channels
+    assert status.is_cuda and status.dtype == torch.int32 and status.is_contiguous() and status.numel() >= n
+    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    rc = lib().fpngb_decode_packed_device(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, max_file_size, w, h,
+                                          chans_in_file, desired_channels, out.data_ptr(), h * w * desired_channels,
+                                          status.data_ptr(), s)
+    check(rc, "decode_packed_device")
+    return out, status
+
+
 def decode_batch_host(file_ptrs, sizes, desired_channels: int, out, out_stride: int):
     """Pipelined host-buffer batch decode (fpngb_decode_batch_host).  file_ptrs: array of host addresses (uint64), sizes:
     uint32 array, out: host buffer (numpy uint8 / pinned torch tensor) with out_stride bytes per image.

@@ -18,8 +18,11 @@ struct SubInfo {
     uint32_t n_out, lits, nlit, pad_;
 };
 
-struct FileDesc {                           // filled by the host container walk (fpng.cpp:2930-3077)
-    uint32_t file_size, idat_ofs, idat_len, pad_;
+struct FileDesc {                           // filled by the container walk (fpng.cpp:2930-3077), on the host or by container_walk_kernel
+    unsigned long long base;                // byte offset of the file from DecodeParams::d_files (a multiple of 4)
+    uint32_t file_size, idat_ofs, idat_len;
+    uint32_t pre_status;                    // != 0: the file failed before decoding (FPNG_DECODE_* / FPNGB_DECODE_SHAPE_MISMATCH);
+                                            // no kernel reads its bytes and decode_status_kernel reports this code
 };
 
 struct DecodeState {
@@ -33,7 +36,7 @@ struct DecodeState {
 constexpr uint32_t kFastWords = 4096 + 64;   // 4096 fast entries, then the 256 literal code sizes (bytes)
 
 struct DecodeParams {
-    const uint8_t* d_files; size_t file_stride;
+    const uint8_t* d_files;                 // file f starts at d_files + files[f].base
     const FileDesc* files;                  // [n] device
     DecodeState* state;                     // [n]
     uint32_t* luts;                         // [n][4096]  fused entries, see decode_kernels.cu
@@ -52,5 +55,17 @@ int decode_profile_read(float* ms, int n);
 unsigned long long decode_link_repairs(bool reset);
 void decode_set_staged(bool on);            // write pass through the shared-memory staged kernel (default) or decode_write_kernel alone
 bool decode_set_pre_roll(uint32_t bits);    // DecodeParams::pre_roll of later calls; false (unchanged) above kPreRoll
+
+// container_walk_kernel (container_kernels.cu): one thread per file of a packed buffer (d_base + offsets[i], sizes[i] bytes).
+// info != nullptr: the six values of fpngb_get_info_ex per file, {status, w, h, chans, idat_ofs, idat_len}.
+// files != nullptr: the FileDesc of the packed decode; pre_status holds the argument checks (size 0, size > max_file_size,
+// offset % 4), the walk's code, or FPNGB_DECODE_SHAPE_MISMATCH when a valid file is not w x h x chans.
+struct WalkParams {
+    const uint8_t* base; const unsigned long long* offsets; const uint32_t* sizes; uint32_t n;
+    uint32_t* info;                         // [n][6] or nullptr
+    FileDesc* files;                        // [n] or nullptr
+    uint32_t max_file_size, w, h, chans;    // checks of the `files` output
+};
+void launch_container_walk(const WalkParams& p, cudaStream_t s);
 
 }  // namespace fpngb

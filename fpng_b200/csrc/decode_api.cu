@@ -2,71 +2,19 @@
 #include "../../include/fpng_b200.h"
 #include "kernels.cuh"
 #include "decode.cuh"
+#include "container.cuh"
 #include "runtime.h"
 #include <string.h>
 #include <vector>
 
 namespace fpngb {
 
-static uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint32_t)p[1] << 16) | ((uint32_t)p[2] << 8) | p[3]; }
-
-// PNG signature / IHDR / chunk walk with the reference's acceptance rules and return codes
-// (fpng.cpp:2930-3077).  Only chunk headers and the CRCs of the small non-IDAT chunks are touched: this is the
-// part of the container that stays on the host (SURVEY.md section 1).
-int container_info(const uint8_t* f, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs, uint32_t* idat_len)
-{
-    static const uint8_t sig[8] = {0x89, 'P', 'N', 'G', 0x0D, 0x0A, 0x1A, 0x0A};
-    *w = *h = *chans = 0; *idat_ofs = *idat_len = 0;
-    if (size < 8 + 25 + 8 + 1 + 4 + 12) return FPNGB_DECODE_FAILED_NOT_PNG;
-    if (memcmp(f, sig, 8) != 0) return FPNGB_DECODE_FAILED_NOT_PNG;
-    if (be32(f + 8) != 13) return FPNGB_DECODE_FAILED_NOT_PNG;
-    if (host_crc32(f + 12, 17, 0) != be32(f + 29)) return FPNGB_DECODE_FAILED_HEADER_CRC32;
-    *w = be32(f + 16); *h = be32(f + 20);
-    if (!*w || !*h || *w > (1u << 24) || *h > (1u << 24)) return FPNGB_DECODE_FAILED_INVALID_DIMENSIONS;
-    if ((uint64_t)*w * *h > (1u << 30)) return FPNGB_DECODE_FAILED_INVALID_DIMENSIONS;
-    if (f[26] || f[27] || f[28] || f[24] != 8) return FPNGB_DECODE_NOT_FPNG;
-    if (f[25] == 2) *chans = 3; else if (f[25] == 6) *chans = 4;
-    if (!*chans) return FPNGB_DECODE_NOT_FPNG;
-    bool have_fdec = false;
-    size_t ofs = 33;
-    for (;;) {
-        if (ofs >= size || size - ofs < 12) return FPNGB_DECODE_FAILED_CHUNK_PARSING;
-        const uint32_t len = be32(f + ofs);
-        if ((uint64_t)ofs + 8 + len + 4 > size) return FPNGB_DECODE_FAILED_CHUNK_PARSING;
-        const uint8_t* ty = f + ofs + 4;
-        for (int i = 0; i < 4; i++) {
-            const bool up = ty[i] >= 65 && ty[i] <= 90, lo = ty[i] >= 97 && ty[i] <= 122;
-            if (!up && !lo) return FPNGB_DECODE_FAILED_CHUNK_PARSING;
-        }
-        const bool is_idat = memcmp(ty, "IDAT", 4) == 0;
-        if (!is_idat && host_crc32(ty, 4 + (size_t)len, 0) != be32(f + ofs + 8 + len)) return FPNGB_DECODE_FAILED_HEADER_CRC32;
-        const uint8_t* d = f + ofs + 8;
-        if (memcmp(ty, "IEND", 4) == 0) break;
-        if (is_idat) {
-            if (*idat_ofs || !have_fdec) return FPNGB_DECODE_NOT_FPNG;
-            *idat_ofs = (uint32_t)ofs; *idat_len = len;
-            if (len < 7) return FPNGB_DECODE_FAILED_INVALID_IDAT;
-        } else if (memcmp(ty, "fdEC", 4) == 0) {
-            if (have_fdec || len != 5) return FPNGB_DECODE_NOT_FPNG;
-            if (d[0] != 82 || d[1] != 36 || d[2] != 147 || d[3] != 227 || d[4] != 0) return FPNGB_DECODE_NOT_FPNG;
-            have_fdec = true;
-        } else if (!(ty[0] & 32)) return FPNGB_DECODE_NOT_FPNG;
-        ofs += 8 + (size_t)len + 4;
-    }
-    if (!have_fdec || !*idat_ofs) return FPNGB_DECODE_NOT_FPNG;
-    return FPNGB_DECODE_SUCCESS;
-}
-
-}  // namespace fpngb
-
-namespace fpngb {
-
 static Buffer g_dec_ws;        // FileDesc[n] | DecodeState[n] | luts | delta scratch
 static Buffer g_dec_pin;       // pinned staging for the FileDesc upload / status download
 
-// Enqueue the decode pipeline for n files already resident on the device.  Caller holds context().mu.
-static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const FileDesc* h_files, uint32_t n, uint32_t w, uint32_t h,
-                               uint32_t chans, uint32_t desired, uint8_t* d_out, size_t out_stride, uint32_t* d_status, cudaStream_t s)
+// Reserves the workspace of a decode call for n files whose IDAT chunks are at most max_idat bytes, orders it after the
+// previous call's kernels, and points p's workspace fields into it (p.files included).  Caller holds context().mu.
+static int decode_workspace_locked(uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t max_idat, cudaStream_t s, DecodeParams& p)
 {
     const uint32_t bpl = w * chans, pitch = (uint32_t)align_up(bpl, 16);
     size_t o = 0;
@@ -74,31 +22,52 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     const size_t o_state = o; o = align_up(o + (size_t)n * sizeof(DecodeState), 256);
     const size_t o_luts = o; o = align_up(o + (size_t)n * 4096 * 4, 256);
     const size_t o_fast = o; o = align_up(o + (size_t)n * kFastWords * 4, 256);
-    uint32_t max_idat = 0;
-    for (uint32_t i = 0; i < n; i++) if (h_files[i].idat_len > max_idat) max_idat = h_files[i].idat_len;
     const uint32_t subs_per_file = (uint32_t)(((uint64_t)max_idat * 8 + 32) / kSubBits + 2);
     const size_t o_subs = o; o = align_up(o + (size_t)n * subs_per_file * sizeof(SubInfo), 256);
     const size_t o_delta = o; o = align_up(o + (size_t)n * pitch * h + 64, 256);
     int rc = g_dec_ws.reserve(o); if (rc) return rc;
     rc = context().ws_acquire(s); if (rc) return rc;
+    uint8_t* b = (uint8_t*)g_dec_ws.p;
+    p.files = (const FileDesc*)(b + o_files); p.state = (DecodeState*)(b + o_state);
+    p.luts = (uint32_t*)(b + o_luts); p.fast = (uint32_t*)(b + o_fast); p.subs = (SubInfo*)(b + o_subs); p.subs_per_file = subs_per_file;
+    p.delta = b + o_delta; p.delta_pitch = pitch;
+    p.w = w; p.h = h; p.chans = chans;
+    return 0;
+}
+
+// Enqueue the decode pipeline for n files already resident on the device, file i at d_files + i * file_stride, described by host
+// FileDescs (their base and pre_status are set here).  Caller holds context().mu.
+static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const FileDesc* h_files, uint32_t n, uint32_t w, uint32_t h,
+                               uint32_t chans, uint32_t desired, uint8_t* d_out, size_t out_stride, uint32_t* d_status, cudaStream_t s)
+{
+    uint32_t max_idat = 0;
+    for (uint32_t i = 0; i < n; i++) if (h_files[i].idat_len > max_idat) max_idat = h_files[i].idat_len;
+    DecodeParams p{};
+    int rc = decode_workspace_locked(n, w, h, chans, max_idat, s, p); if (rc) return rc;
     g_dec_pin.pinned = true;
     rc = g_dec_pin.reserve((size_t)n * sizeof(FileDesc)); if (rc) return rc;
     // the pinned staging buffer may still be in flight from the previous call on another stream: wait for it
     static cudaEvent_t staged = nullptr;
     if (!staged) FPNGB_CUDA_OK(cudaEventCreateWithFlags(&staged, cudaEventDisableTiming));
     else FPNGB_CUDA_OK(cudaEventSynchronize(staged));
-    memcpy(g_dec_pin.p, h_files, (size_t)n * sizeof(FileDesc));
-    uint8_t* b = (uint8_t*)g_dec_ws.p;
-    FPNGB_CUDA_OK(cudaMemcpyAsync(b + o_files, g_dec_pin.p, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
+    FileDesc* staging = (FileDesc*)g_dec_pin.p;
+    for (uint32_t i = 0; i < n; i++) { staging[i] = h_files[i]; staging[i].base = (unsigned long long)i * file_stride; staging[i].pre_status = 0; }
+    FPNGB_CUDA_OK(cudaMemcpyAsync((void*)p.files, g_dec_pin.p, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
     FPNGB_CUDA_OK(cudaEventRecord(staged, s));
-    DecodeParams p{};
-    p.d_files = d_files; p.file_stride = file_stride; p.files = (const FileDesc*)(b + o_files); p.state = (DecodeState*)(b + o_state);
-    p.luts = (uint32_t*)(b + o_luts); p.fast = (uint32_t*)(b + o_fast); p.subs = (SubInfo*)(b + o_subs); p.subs_per_file = subs_per_file; p.delta = b + o_delta; p.delta_pitch = pitch; p.d_out = d_out; p.out_stride = out_stride;
-    p.d_status = d_status; p.w = w; p.h = h; p.chans = chans;
+    p.d_files = d_files; p.d_out = d_out; p.out_stride = out_stride; p.d_status = d_status;
     launch_decode(p, n, desired, s);
     count_launch(8);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
+}
+
+// the host instantiation of the container walk (container.cuh)
+struct HostCrc {
+    uint32_t operator()(const uint8_t* p, size_t n) const { return host_crc32(p, n, 0); }
+};
+int container_info(const uint8_t* f, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs, uint32_t* idat_len)
+{
+    return container_walk(f, size, HostCrc{}, w, h, chans, idat_ofs, idat_len);
 }
 
 }  // namespace fpngb
@@ -122,7 +91,7 @@ int fpngb_decode_batch_device(const void* d_files, size_t file_stride, const uin
     std::vector<FileDesc> fds(n);
     for (uint32_t i = 0; i < n; i++) {
         if ((uint64_t)idat_ofs[i] + 8 + idat_len[i] + 4 > file_sizes[i] || file_sizes[i] > file_stride) return FPNGB_ERR_INVALID_ARG;
-        fds[i] = FileDesc{file_sizes[i], idat_ofs[i], idat_len[i], 0};
+        fds[i] = FileDesc{0, file_sizes[i], idat_ofs[i], idat_len[i], 0};
     }
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
@@ -150,7 +119,7 @@ int fpngb_decode_host(const void* file, uint32_t size, void* out, size_t out_cap
     uint32_t* d_status = (uint32_t*)((uint8_t*)c.dev_out.p + align_up(need, 16));
     cudaStream_t s = c.stream;
     cudaMemcpyAsync(c.dev_in.p, file, size, cudaMemcpyHostToDevice, s);
-    FileDesc fd{size, idat_ofs, idat_len, 0};
+    FileDesc fd{0, size, idat_ofs, idat_len, 0};
     if (decode_batch_locked((const uint8_t*)c.dev_in.p, fstride, &fd, 1, ww, hh, cc, desired, (uint8_t*)c.dev_out.p, align_up(need, 16), d_status, s))
         return FPNGB_DECODE_INVALID_ARG;
     uint32_t* h_status = (uint32_t*)c.pin_small.p;
@@ -185,7 +154,7 @@ int fpngb_decode_batch_host(const void* const* files, const uint32_t* sizes, uin
     for (uint32_t i = 0; i < n; i++) {
         uint32_t ww = 0, hh = 0, cc = 0, io = 0, il = 0;
         status[i] = (!files[i] || !sizes[i]) ? FPNGB_DECODE_INVALID_ARG : container_info((const uint8_t*)files[i], sizes[i], &ww, &hh, &cc, &io, &il);
-        fds[i] = FileDesc{sizes[i], io, il, 0};
+        fds[i] = FileDesc{0, sizes[i], io, il, 0};
         if (status[i]) continue;
         if (!W) { W = ww; H = hh; C = cc; }
         else if (ww != W || hh != H || cc != C) return FPNGB_ERR_INVALID_ARG;
@@ -272,6 +241,49 @@ int fpngb_get_info_ex(const void* file, uint32_t size, uint32_t* w, uint32_t* h,
 {
     if (!file || !w || !h || !chans || !idat_ofs || !idat_len) return FPNGB_DECODE_INVALID_ARG;
     return container_info((const uint8_t*)file, size, w, h, chans, idat_ofs, idat_len);
+}
+
+int fpngb_get_info_batch_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t* d_info, void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_info || n == 0) return FPNGB_ERR_INVALID_ARG;
+    WalkParams p{};
+    p.base = (const uint8_t*)d_base; p.offsets = (const unsigned long long*)d_offsets; p.sizes = d_sizes; p.n = n; p.info = d_info;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    launch_container_walk(p, (cudaStream_t)stream);
+    count_launch(1);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return FPNGB_OK;
+}
+
+int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
+                               uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out, size_t out_stride,
+                               int32_t* d_status, void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_status || n == 0 || n > 65535 || !max_file_size) return FPNGB_ERR_INVALID_ARG;
+    if ((chans_in_file != 3 && chans_in_file != 4) || (desired_chans != 3 && desired_chans != 4) || !w || !h) return FPNGB_ERR_INVALID_ARG;
+    if (w > (1u << 24) || h > (1u << 24) || (uint64_t)w * h > (1ull << 30)) return FPNGB_ERR_INVALID_ARG;
+    if ((uint64_t)w * h * desired_chans > 0xFFFFFFFFull || out_stride < (size_t)w * h * desired_chans) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    if ((uintptr_t)d_base % 4) return FPNGB_ERR_ALIGNMENT;
+    const cudaStream_t s = (cudaStream_t)stream;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    // an IDAT chunk is shorter than its file: max_file_size bounds the stream of every file that reaches the decode kernels
+    DecodeParams p{};
+    int rc = decode_workspace_locked(n, w, h, chans_in_file, max_file_size, s, p); if (rc) return rc;
+    WalkParams wp{};
+    wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n;
+    wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = w; wp.h = h; wp.chans = chans_in_file;
+    launch_container_walk(wp, s);
+    p.d_files = (const uint8_t*)d_base; p.d_out = (uint8_t*)d_out; p.out_stride = out_stride; p.d_status = (uint32_t*)d_status;
+    launch_decode(p, n, desired_chans, s);
+    count_launch(9);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return context().ws_release(s);
 }
 
 }  // extern "C"

@@ -116,15 +116,17 @@ __global__ void __launch_bounds__(32) decode_prepare_kernel(DecodeParams p)
     const uint32_t f = blockIdx.x, lane = threadIdx.x;
     const FileDesc fd = p.files[f];
     DecodeState* st = p.state + f;
-    const uint8_t* z = p.d_files + (size_t)f * p.file_stride + fd.idat_ofs + 8;
+    const uint8_t* z = p.d_files + fd.base + fd.idat_ofs + 8;
     BitSrc src{z, fd.file_size - (fd.idat_ofs + 8)};
     uint32_t* lut = p.luts + (size_t)f * 4096;
 
     if (lane == 0) {
         s_fail = 0;
         st->status = 0; st->stored = 0; st->token_start = 0; st->out_bytes = 0; st->end_byte = 0;
+        // a file that failed before decoding (container walk, argument or shape checks): its bytes are never read
+        if (fd.pre_status) s_fail = 1;
         // zlib header and block type (fpng.cpp:2219-2244)
-        if (fd.idat_len < 7 || z[0] != 0x78 || z[1] != 0x01) s_fail = 1;
+        else if (fd.idat_len < 7 || z[0] != 0x78 || z[1] != 0x01) s_fail = 1;
         else if ((z[2] & 6) == 0) st->stored = 1;
         else if ((z[2] & 7) != 5) s_fail = 1;           // BFINAL = 1, BTYPE = 2
     }
@@ -728,7 +730,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_scan_kernel(DecodeParams p
     const DecodeState st = p.state[f];
     if (st.status || st.stored) return;
     const FileDesc fd = p.files[f];
-    Stream sm = open_stream(p.d_files + (size_t)f * p.file_stride, fd);
+    Stream sm = open_stream(p.d_files + fd.base, fd);
     const FileSpan sp = file_span(st, sm, fd);
     const unsigned long long g = sp.g0 + (unsigned long long)blockIdx.x * kDecThreads + tid;
     if (sp.g0 + (unsigned long long)blockIdx.x * kDecThreads > sp.g1) return;
@@ -780,7 +782,7 @@ __global__ void __launch_bounds__(kLinkThreads) decode_link_kernel(DecodeParams 
     if (stp->status || stp->stored) return;
     const DecodeState st = *stp;
     const FileDesc fd = p.files[f];
-    const Stream sm = open_stream(p.d_files + (size_t)f * p.file_stride, fd);
+    const Stream sm = open_stream(p.d_files + fd.base, fd);
     const FileSpan sp = file_span(st, sm, fd);
     const uint32_t chans = p.chans, bpl = p.w * chans, h = p.h;
     const unsigned long long total_out = (unsigned long long)(bpl + 1) * h;
@@ -919,7 +921,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_write_kernel(DecodeParams 
     DecodeState* stp = p.state + f;
     if (stp->status || stp->stored) return;
     const FileDesc fd = p.files[f];
-    Stream sm = open_stream(p.d_files + (size_t)f * p.file_stride, fd);
+    Stream sm = open_stream(p.d_files + fd.base, fd);
     const FileSpan sp = file_span(*stp, sm, fd);
     if (sp.g0 + (unsigned long long)blockIdx.x * kDecThreads > sp.g1) return;
     const unsigned long long g = sp.g0 + (unsigned long long)blockIdx.x * kDecThreads + tid;
@@ -1113,7 +1115,7 @@ __global__ void __launch_bounds__(kWsThreads) decode_write_staged_kernel(DecodeP
     DecodeState* stp = p.state + f;
     if (stp->status || stp->stored) return;
     const FileDesc fd = p.files[f];
-    Stream sm = open_stream(p.d_files + (size_t)f * p.file_stride, fd);
+    Stream sm = open_stream(p.d_files + fd.base, fd);
     const FileSpan sp = file_span(*stp, sm, fd);
     const unsigned long long first_sub = sp.g0 + (unsigned long long)blockIdx.x * kWsThreads;
     if (first_sub > sp.g1) return;
@@ -1220,7 +1222,7 @@ __global__ void __launch_bounds__(256) decode_stored_kernel(DecodeParams p)
     DecodeState* st = p.state + f;
     if (st->status || !st->stored) return;
     const FileDesc fd = p.files[f];
-    const uint8_t* z = p.d_files + (size_t)f * p.file_stride + fd.idat_ofs + 8;
+    const uint8_t* z = p.d_files + fd.base + fd.idat_ofs + 8;
     const uint32_t avail = fd.file_size - (fd.idat_ofs + 8);
     const uint32_t bpl = p.w * p.chans, h = p.h, pitch = p.delta_pitch;
     const unsigned long long raw = (unsigned long long)(bpl + 1) * h, nblk = (raw + 65534ull) / 65535ull;
@@ -1349,7 +1351,10 @@ __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p)
 __global__ void decode_status_kernel(DecodeParams p, uint32_t n)
 {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f < n) p.d_status[f] = p.state[f].status ? 1u /*FPNG_DECODE_NOT_FPNG*/ : 0u;
+    if (f < n) {
+        const uint32_t pre = p.files[f].pre_status;
+        p.d_status[f] = pre ? pre : (p.state[f].status ? 1u /*FPNG_DECODE_NOT_FPNG*/ : 0u);
+    }
 }
 
 // Optional per-kernel timing of the decode pipeline (bench.py): events recorded between the launches of the most recent

@@ -109,6 +109,37 @@ FPNGB_API int fpngb_decode_batch_host(const void* const* files, const uint32_t* 
 FPNGB_API int fpngb_get_info_ex(const void* file, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans,
                                 uint32_t* idat_ofs, uint32_t* idat_len);
 
+/* ---- files that are already in DEVICE memory, packed back to back (no reference counterpart) -----------------------------
+ * File i is the d_sizes[i] bytes at d_base + d_offsets[i]; d_base, d_offsets (n x uint64) and d_sizes (n x uint32) are all
+ * device memory.  This is the layout of fpngb_compact_batch_device (n+1 offsets: the last is ignored) and of the window
+ * fpngb_gather_encoded_device returns (pass its window, offsets, all_sizes and nranks*nmax; unused slots have size 0).
+ * Both calls are stream-ordered on `stream` (NULL = the CUDA default stream): they do no host synchronisation and no host
+ * copy of file bytes, offsets or sizes, so no pinned staging is needed.  The container walk runs on the device
+ * (container_walk_kernel: one thread per file) and is the same function as the host walk of fpngb_get_info_ex.
+ *
+ * fpngb_get_info_batch_device: d_info[i*6 + 0..5] = {status, w, h, chans, idat_ofs, idat_len}, the six values
+ *   fpngb_get_info_ex returns for file i; a size of 0 gives FPNGB_DECODE_INVALID_ARG.  Any offset alignment.
+ *
+ * fpngb_decode_packed_device: decodes every file of shape w x h x chans_in_file into d_out + i*out_stride
+ *   (w*h*desired_chans bytes).  d_status[i] is what fpng_decode_memory would return for file i (the walk's code, then
+ *   FPNGB_DECODE_NOT_FPNG or FPNGB_DECODE_SUCCESS from the decode kernels), with two additions checked in this order:
+ *   FPNGB_DECODE_INVALID_ARG for size 0, size > max_file_size or offset % 4 != 0, then, for a file the walk accepts,
+ *   FPNGB_DECODE_SHAPE_MISMATCH when its w/h/chans differ from the call's.  The pixels of a file whose status is not 0 are
+ *   not written.  max_file_size bounds every decoded file and sizes the decoder's per-file workspace (it replaces the
+ *   host-known maximum IDAT length of fpngb_decode_batch_device); fpngb_max_encoded_size(w, h, chans_in_file) always
+ *   suffices for files this library or the reference wrote.
+ *   Call-level checks as fpngb_decode_batch_device: n <= 65535, the shape limits, out_stride, d_base % 4 == 0.
+ *   Memory read: the decode kernels read whole aligned 32-bit words and clamp every read to the last word of the file, so for
+ *   a 4-aligned file they stay inside [offset, offset + align_up(size, 4)); the walk reads bytes inside [offset, offset +
+ *   size).  The buffer must therefore be readable up to align_up(offset + size, 16) for every file, which the compact and
+ *   gather layouts (16-byte aligned files) provide. */
+enum { FPNGB_DECODE_SHAPE_MISMATCH = 100 };   /* per-file status of the packed decode only: a valid file of another w/h/chans */
+FPNGB_API int fpngb_get_info_batch_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                          uint32_t* d_info, void* stream);
+FPNGB_API int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                         uint32_t max_file_size, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                                         uint32_t desired_chans, void* d_out, size_t out_stride, int32_t* d_status, void* stream);
+
 /* Replace fpng::fpng_crc32 / fpng::fpng_adler32 (src/fpng.h:26-31).  Host buffers.  Buffers of 4 KiB and more are
  * checksummed by the device kernels.  NOTE (the one host-side arithmetic in this library): shorter buffers, and any
  * call made before fpngb_init(), use the small host CRC/Adler routines the container code needs anyway for the 17-byte
