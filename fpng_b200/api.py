@@ -127,26 +127,72 @@ def fpng_decode_file(filename: str, desired_channels: int):
     return fpng_decode_memory(data, desired_channels)
 
 
+def layout_strides(shape, strides):
+    """Byte strides (image_stride, row_pitch, pixel_stride, chan_stride) of an [n, h, w, chans] uint8 view, in the form the
+    *_strided C calls take (include/fpng_b200.h, "Pixel layouts").  Two layouts are supported: interleaved (pixel_stride ==
+    chans, chan_stride == 1: HWC rows at any pitch) and planar (pixel_stride == 1, chan_stride >= 1: CHW or HCW planes).  The
+    stride of a dimension of size 1 is ignored and replaced by the value of a tightly packed batch (w == 1 is interleaved when
+    chan_stride == 1, planar otherwise).  Raises ValueError for any other layout."""
+    n, h, w, c = (int(v) for v in shape)
+    image, row, pixel, chan = (int(v) for v in strides)
+    if c not in (3, 4):
+        raise ValueError(f"layout_strides: {c} channels (3 or 4 are supported)")
+    if min(image, row, pixel, chan) < 0:
+        raise ValueError("layout_strides: negative strides are not supported")
+    if w == 1:
+        pixel = c if chan == 1 else 1
+    interleaved = pixel == c and chan == 1
+    planar = not interleaved and pixel == 1 and chan >= 1
+    if not (interleaved or planar):
+        raise ValueError(f"layout_strides: strides {tuple(strides)} of an {tuple(shape)} view are neither interleaved "
+                         f"(pixel stride {c}, channel stride 1) nor planar (pixel stride 1, channel stride >= 1)")
+    if h == 1:
+        row = w * c if interleaved else w
+    if n == 1:
+        image = h * row
+    return image, row, pixel, chan
+
+
 def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=None):
     """Encode a batch of equally sized device-resident images.
 
-    images: torch.uint8 CUDA tensor [n, h, w, chans] (contiguous). Returns (out [n, stride] uint8, sizes [n] int32 holding
-    uint32 file sizes) on the same device; kernels are enqueued on the current torch stream (or `stream`), not synchronised.
+    images: torch.uint8 CUDA tensor [n, h, w, chans]: contiguous, or any view in one of the two layouts of layout_strides --
+    e.g. x_nchw.permute(0, 2, 3, 1), a crop canvas[:, y0:y1, x0:x1, :] or img.expand(n, -1, -1, -1) -- which is encoded in
+    place, without a copy.  Returns (out [n, stride] uint8, sizes [n] int32 holding uint32 file sizes) on the same device;
+    kernels are enqueued on the current torch stream (or `stream`), not synchronised.
     """
     import torch
 
-    assert images.is_cuda and images.dtype == torch.uint8 and images.is_contiguous() and images.dim() == 4
+    assert images.is_cuda and images.dtype == torch.uint8 and images.dim() == 4
     n, h, w, c = images.shape
+    strided = not images.is_contiguous()
+    if strided:
+        layout = layout_strides(images.shape, images.stride())
     stride = (max_encoded_size(w, h, c) + 15) // 16 * 16
     if out is None:
         out = torch.empty((n, stride), dtype=torch.uint8, device=images.device)
     if sizes is None:
         sizes = torch.empty((n,), dtype=torch.int32, device=images.device)
     s = stream if stream is not None else torch.cuda.current_stream(images.device).cuda_stream
-    rc = lib().fpngb_encode_batch_device(images.data_ptr(), h * w * c, n, w, h, c, flags, out.data_ptr(), out.stride(0),
-                                         sizes.data_ptr(), s)
+    if strided:
+        rc = lib().fpngb_encode_batch_device_strided(images.data_ptr(), *layout, n, w, h, c, flags, out.data_ptr(), out.stride(0),
+                                                     sizes.data_ptr(), s)
+    else:
+        rc = lib().fpngb_encode_batch_device(images.data_ptr(), h * w * c, n, w, h, c, flags, out.data_ptr(), out.stride(0),
+                                             sizes.data_ptr(), s)
     check(rc, "encode_batch_device")
     return out, sizes
+
+
+def _strided_out(out, n, h, w, desired_channels):
+    """The layout of a caller's non-contiguous `out` view (layout_strides), or None for a contiguous one."""
+    import torch
+
+    assert out.is_cuda and out.dtype == torch.uint8
+    if out.is_contiguous():
+        return None
+    assert tuple(out.shape) == (n, h, w, desired_channels), "a non-contiguous out must be an [n, h, w, desired_channels] view"
+    return layout_strides(out.shape, out.stride())
 
 
 def get_info_ex(data):
@@ -184,22 +230,27 @@ def pack_files_for_device(files, device=None):
 
 def decode_batch_device(files_dev, sizes, idat_ofs, idat_len, w: int, h: int, chans_in_file: int, desired_channels: int,
                         out=None, status=None, stream=None):
-    """Decode n fpng files resident on the device (tensor [n, stride] uint8). Returns (pixels [n, h, w, desired], status [n])."""
+    """Decode n fpng files resident on the device (tensor [n, stride] uint8). Returns (pixels [n, h, w, desired], status [n]).
+    out may be any non-overlapping [n, h, w, desired] view in one of the two layouts of layout_strides, e.g.
+    torch.empty(n, desired, h, w).permute(0, 2, 3, 1) for NCHW pixels; the kernels write it in place."""
     import torch
 
     assert files_dev.is_cuda and files_dev.dtype == torch.uint8 and files_dev.dim() == 2 and files_dev.is_contiguous()
     n = files_dev.shape[0]
     if out is None:
         out = torch.empty((n, h, w, desired_channels), dtype=torch.uint8, device=files_dev.device)
+    layout = _strided_out(out, n, h, w, desired_channels)
     if status is None:
         status = torch.empty((n,), dtype=torch.int32, device=files_dev.device)
     s = stream if stream is not None else torch.cuda.current_stream(files_dev.device).cuda_stream
     sizes = np.ascontiguousarray(sizes, dtype=np.uint32); idat_ofs = np.ascontiguousarray(idat_ofs, dtype=np.uint32)
     idat_len = np.ascontiguousarray(idat_len, dtype=np.uint32)
-    rc = lib().fpngb_decode_batch_device(files_dev.data_ptr(), files_dev.stride(0), sizes.ctypes.data_as(C.c_void_p),
-                                         idat_ofs.ctypes.data_as(C.c_void_p), idat_len.ctypes.data_as(C.c_void_p), n, w, h,
-                                         chans_in_file, desired_channels, out.data_ptr(), h * w * desired_channels,
-                                         status.data_ptr(), s)
+    args = (files_dev.data_ptr(), files_dev.stride(0), sizes.ctypes.data_as(C.c_void_p), idat_ofs.ctypes.data_as(C.c_void_p),
+            idat_len.ctypes.data_as(C.c_void_p), n, w, h, chans_in_file, desired_channels, out.data_ptr())
+    if layout is None:
+        rc = lib().fpngb_decode_batch_device(*args, h * w * desired_channels, status.data_ptr(), s)
+    else:
+        rc = lib().fpngb_decode_batch_device_strided(*args, *layout, status.data_ptr(), s)
     check(rc, "decode_batch_device")
     return out, status
 
@@ -240,7 +291,7 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
                          out=None, status=None, stream=None):
     """Decode the w x h x chans_in_file fpng files packed in device memory (same arguments as get_info_batch_device; every
     file 4-byte aligned).  The container walk runs on the device: no host synchronisation and no host copy.
-    Returns (pixels uint8 [n, h, w, desired_channels], status int32 [n]).  status[i] is fpng_decode_memory's code for file i,
+    Returns (pixels uint8 [n, h, w, desired_channels], status int32 [n]); out may be a strided view as in decode_batch_device.  status[i] is fpng_decode_memory's code for file i,
     or FPNGB_DECODE_SHAPE_MISMATCH for a valid file of another shape, or FPNG_DECODE_INVALID_ARG for size 0, size >
     max_file_size or an offset that is not a multiple of 4; pixels of files with a non-zero status are left untouched.
     max_file_size (bytes) bounds every file and sizes the decoder's workspace; the default, max_encoded_size(w, h,
@@ -255,12 +306,16 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
         out = torch.empty((n, h, w, desired_channels), dtype=torch.uint8, device=data.device)
     if status is None:
         status = torch.empty((n,), dtype=torch.int32, device=data.device)
-    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= n * h * w * desired_channels
+    layout = _strided_out(out, n, h, w, desired_channels)
+    assert layout is not None or out.numel() >= n * h * w * desired_channels
     assert status.is_cuda and status.dtype == torch.int32 and status.is_contiguous() and status.numel() >= n
     s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
-    rc = lib().fpngb_decode_packed_device(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, max_file_size, w, h,
-                                          chans_in_file, desired_channels, out.data_ptr(), h * w * desired_channels,
-                                          status.data_ptr(), s)
+    args = (data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, max_file_size, w, h, chans_in_file, desired_channels,
+            out.data_ptr())
+    if layout is None:
+        rc = lib().fpngb_decode_packed_device(*args, h * w * desired_channels, status.data_ptr(), s)
+    else:
+        rc = lib().fpngb_decode_packed_device_strided(*args, *layout, status.data_ptr(), s)
     check(rc, "decode_packed_device")
     return out, status
 

@@ -43,13 +43,17 @@ struct DecodeParams {
     uint32_t* fast;                         // [n][kFastWords]  multi-token entries + literal code sizes of the scan / write loops
     SubInfo* subs; uint32_t subs_per_file;  // [n][subs_per_file]
     uint8_t* delta; uint32_t delta_pitch;   // [n][h][pitch] filtered rows without the filter byte
-    uint8_t* d_out; size_t out_stride;
+    uint8_t* d_out; size_t out_stride;     // pixel (f, y, x, c) at d_out + f*out_stride + y*OutStrides::row + x*OutStrides::pixel + c*OutStrides::chan
     uint32_t* d_status;                     // [n] FPNG_DECODE_* codes
     uint32_t w, h, chans;
     uint32_t pre_roll;                      // speculative lead-in bits of decode_scan_kernel, 0..kPreRoll (kPreRoll unless a test sets it)
 };
 
-void launch_decode(const DecodeParams& p, uint32_t n, uint32_t desired, cudaStream_t s);
+// the rest of the output layout of the decode (unfilter_kernel's second argument; kept out of DecodeParams, which every decode kernel takes)
+struct OutStrides {
+    size_t row, pixel, chan;                // interleaved (pixel = desired, chan = 1) or planar (pixel = 1)
+};
+void launch_decode(const DecodeParams& p, const OutStrides& out, uint32_t n, uint32_t desired, cudaStream_t s);
 void decode_profile_enable(bool on);
 int decode_profile_read(float* ms, int n);
 unsigned long long decode_link_repairs(bool reset);

@@ -3,6 +3,7 @@
 #include "kernels.cuh"
 #include "decode.cuh"
 #include "container.cuh"
+#include "layout.h"
 #include "runtime.h"
 #include <string.h>
 #include <vector>
@@ -35,10 +36,41 @@ static int decode_workspace_locked(uint32_t n, uint32_t w, uint32_t h, uint32_t 
     return 0;
 }
 
+// Output layout of a decode call (layout.h): pixel (i, y, x, c) at d_out + i*image + y*row + x*pixel + c*chan.
+static OutStrides set_output(DecodeParams& p, uint8_t* d_out, const Layout& L)
+{
+    p.d_out = d_out; p.out_stride = L.image;
+    return OutStrides{L.row, L.pixel, L.chan};
+}
+static Layout tight_output(uint32_t w, uint32_t h, uint32_t desired, size_t out_stride)
+{
+    return Layout{out_stride, (uint64_t)w * desired, desired, 1, false};
+}
+
+// Call-level checks shared by the device decode entry points: counts, channels and the container's shape limits
+// (fpng.cpp:2966-2971: keeps w * chans and the scratch pitch inside 32 bits).
+static int decode_shape_check(uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans)
+{
+    if ((chans_in_file != 3 && chans_in_file != 4) || (desired_chans != 3 && desired_chans != 4) || !w || !h) return FPNGB_ERR_INVALID_ARG;
+    if (w > (1u << 24) || h > (1u << 24) || (uint64_t)w * h > (1ull << 30)) return FPNGB_ERR_INVALID_ARG;
+    if ((uint64_t)w * h * desired_chans > 0xFFFFFFFFull) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    return FPNGB_OK;
+}
+// A strided output must be interleaved or planar, addressable, and no two pixels may share a byte.
+static int decode_output_check(const void* d_out, size_t image, size_t row, size_t pixel, size_t chan, uint32_t n, uint32_t w, uint32_t h,
+                               uint32_t desired, Layout& L)
+{
+    uint64_t last = 0;
+    if (!classify_layout(image, row, pixel, chan, n, h, w, desired, L) || !layout_disjoint(L, n, h, w, desired) ||
+        !layout_span(d_out, L, n, h, w, desired, last))
+        return FPNGB_ERR_INVALID_ARG;
+    return FPNGB_OK;
+}
+
 // Enqueue the decode pipeline for n files already resident on the device, file i at d_files + i * file_stride, described by host
 // FileDescs (their base and pre_status are set here).  Caller holds context().mu.
 static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const FileDesc* h_files, uint32_t n, uint32_t w, uint32_t h,
-                               uint32_t chans, uint32_t desired, uint8_t* d_out, size_t out_stride, uint32_t* d_status, cudaStream_t s)
+                               uint32_t chans, uint32_t desired, uint8_t* d_out, const Layout& out, uint32_t* d_status, cudaStream_t s)
 {
     uint32_t max_idat = 0;
     for (uint32_t i = 0; i < n; i++) if (h_files[i].idat_len > max_idat) max_idat = h_files[i].idat_len;
@@ -54,8 +86,8 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     for (uint32_t i = 0; i < n; i++) { staging[i] = h_files[i]; staging[i].base = (unsigned long long)i * file_stride; staging[i].pre_status = 0; }
     FPNGB_CUDA_OK(cudaMemcpyAsync((void*)p.files, g_dec_pin.p, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
     FPNGB_CUDA_OK(cudaEventRecord(staged, s));
-    p.d_files = d_files; p.d_out = d_out; p.out_stride = out_stride; p.d_status = d_status;
-    launch_decode(p, n, desired, s);
+    p.d_files = d_files; p.d_status = d_status;
+    launch_decode(p, set_output(p, d_out, out), n, desired, s);
     count_launch(8);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
@@ -76,17 +108,17 @@ using namespace fpngb;
 
 extern "C" {
 
-int fpngb_decode_batch_device(const void* d_files, size_t file_stride, const uint32_t* file_sizes, const uint32_t* idat_ofs,
-                              const uint32_t* idat_len, uint32_t n, uint32_t w, uint32_t h, uint32_t chans_in_file,
-                              uint32_t desired_chans, void* d_out, size_t out_stride, uint32_t* d_status, void* stream)
+int fpngb_decode_batch_device_strided(const void* d_files, size_t file_stride, const uint32_t* file_sizes, const uint32_t* idat_ofs,
+                                      const uint32_t* idat_len, uint32_t n, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                                      uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                      size_t out_pixel_stride, size_t out_chan_stride, uint32_t* d_status, void* stream)
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_files || !file_sizes || !idat_ofs || !idat_len || !d_out || !d_status || n == 0 || n > 65535) return FPNGB_ERR_INVALID_ARG;
-    if ((chans_in_file != 3 && chans_in_file != 4) || (desired_chans != 3 && desired_chans != 4) || !w || !h) return FPNGB_ERR_INVALID_ARG;
-    // the container limits of fpng_get_info (fpng.cpp:2966-2971): keeps w * chans and the scratch pitch inside 32 bits
-    if (w > (1u << 24) || h > (1u << 24) || (uint64_t)w * h > (1ull << 30)) return FPNGB_ERR_INVALID_ARG;
-    if ((uint64_t)w * h * desired_chans > 0xFFFFFFFFull || out_stride < (size_t)w * h * desired_chans) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
+    Layout out;
+    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, out); if (rc) return rc;
     if (file_stride % 4 || (uintptr_t)d_files % 4) return FPNGB_ERR_ALIGNMENT;
     std::vector<FileDesc> fds(n);
     for (uint32_t i = 0; i < n; i++) {
@@ -96,7 +128,19 @@ int fpngb_decode_batch_device(const void* d_files, size_t file_stride, const uin
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     return decode_batch_locked((const uint8_t*)d_files, file_stride, fds.data(), n, w, h, chans_in_file, desired_chans, (uint8_t*)d_out,
-                               out_stride, d_status, (cudaStream_t)stream);
+                               out, d_status, (cudaStream_t)stream);
+}
+
+int fpngb_decode_batch_device(const void* d_files, size_t file_stride, const uint32_t* file_sizes, const uint32_t* idat_ofs,
+                              const uint32_t* idat_len, uint32_t n, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                              uint32_t desired_chans, void* d_out, size_t out_stride, uint32_t* d_status, void* stream)
+{
+    if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_files || !file_sizes || !idat_ofs || !idat_len || !d_out || !d_status || n == 0 || n > 65535) return FPNGB_ERR_INVALID_ARG;
+    const int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
+    if (out_stride < (size_t)w * h * desired_chans) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    return fpngb_decode_batch_device_strided(d_files, file_stride, file_sizes, idat_ofs, idat_len, n, w, h, chans_in_file, desired_chans, d_out,
+                                             out_stride, (size_t)w * desired_chans, desired_chans, 1, d_status, stream);
 }
 
 int fpngb_decode_host(const void* file, uint32_t size, void* out, size_t out_cap, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t desired)
@@ -120,7 +164,8 @@ int fpngb_decode_host(const void* file, uint32_t size, void* out, size_t out_cap
     cudaStream_t s = c.stream;
     cudaMemcpyAsync(c.dev_in.p, file, size, cudaMemcpyHostToDevice, s);
     FileDesc fd{0, size, idat_ofs, idat_len, 0};
-    if (decode_batch_locked((const uint8_t*)c.dev_in.p, fstride, &fd, 1, ww, hh, cc, desired, (uint8_t*)c.dev_out.p, align_up(need, 16), d_status, s))
+    if (decode_batch_locked((const uint8_t*)c.dev_in.p, fstride, &fd, 1, ww, hh, cc, desired, (uint8_t*)c.dev_out.p,
+                            tight_output(ww, hh, desired, align_up(need, 16)), d_status, s))
         return FPNGB_DECODE_INVALID_ARG;
     uint32_t* h_status = (uint32_t*)c.pin_small.p;
     cudaMemcpyAsync(h_status, d_status, 4, cudaMemcpyDeviceToHost, s);
@@ -205,7 +250,7 @@ int fpngb_decode_batch_host(const void* const* files, const uint32_t* sizes, uin
         }
         cudaEventRecord(ev_in[sl], c.copy_in);
         cudaStreamWaitEvent(c.stream, ev_in[sl], 0);
-        rc = decode_batch_locked(din, fstride, cf.data(), cnt, W, H, C, desired, dout, pstride, dst, c.stream);
+        rc = decode_batch_locked(din, fstride, cf.data(), cnt, W, H, C, desired, dout, tight_output(W, H, desired, pstride), dst, c.stream);
         if (rc) { result = rc; break; }
         cudaEventRecord(ev_done[sl], c.stream);
         cudaStreamWaitEvent(c.copy_out, ev_done[sl], 0);
@@ -258,32 +303,45 @@ int fpngb_get_info_batch_device(const void* d_base, const uint64_t* d_offsets, c
     return FPNGB_OK;
 }
 
-int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
-                               uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out, size_t out_stride,
-                               int32_t* d_status, void* stream)
+int fpngb_decode_packed_device_strided(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
+                                       uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out,
+                                       size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride, size_t out_chan_stride,
+                                       int32_t* d_status, void* stream)
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_base || !d_offsets || !d_sizes || !d_out || !d_status || n == 0 || n > 65535 || !max_file_size) return FPNGB_ERR_INVALID_ARG;
-    if ((chans_in_file != 3 && chans_in_file != 4) || (desired_chans != 3 && desired_chans != 4) || !w || !h) return FPNGB_ERR_INVALID_ARG;
-    if (w > (1u << 24) || h > (1u << 24) || (uint64_t)w * h > (1ull << 30)) return FPNGB_ERR_INVALID_ARG;
-    if ((uint64_t)w * h * desired_chans > 0xFFFFFFFFull || out_stride < (size_t)w * h * desired_chans) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
+    Layout out;
+    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, out); if (rc) return rc;
     if ((uintptr_t)d_base % 4) return FPNGB_ERR_ALIGNMENT;
     const cudaStream_t s = (cudaStream_t)stream;
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     // an IDAT chunk is shorter than its file: max_file_size bounds the stream of every file that reaches the decode kernels
     DecodeParams p{};
-    int rc = decode_workspace_locked(n, w, h, chans_in_file, max_file_size, s, p); if (rc) return rc;
+    rc = decode_workspace_locked(n, w, h, chans_in_file, max_file_size, s, p); if (rc) return rc;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = w; wp.h = h; wp.chans = chans_in_file;
     launch_container_walk(wp, s);
-    p.d_files = (const uint8_t*)d_base; p.d_out = (uint8_t*)d_out; p.out_stride = out_stride; p.d_status = (uint32_t*)d_status;
-    launch_decode(p, n, desired_chans, s);
+    p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status;
+    launch_decode(p, set_output(p, (uint8_t*)d_out, out), n, desired_chans, s);
     count_launch(9);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
+}
+
+int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
+                               uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out, size_t out_stride,
+                               int32_t* d_status, void* stream)
+{
+    if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_status || n == 0 || n > 65535 || !max_file_size) return FPNGB_ERR_INVALID_ARG;
+    const int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
+    if (out_stride < (size_t)w * h * desired_chans) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    return fpngb_decode_packed_device_strided(d_base, d_offsets, d_sizes, n, max_file_size, w, h, chans_in_file, desired_chans, d_out, out_stride,
+                                              (size_t)w * desired_chans, desired_chans, 1, d_status, stream);
 }
 
 }  // extern "C"

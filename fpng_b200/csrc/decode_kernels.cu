@@ -1263,8 +1263,25 @@ __device__ __forceinline__ uint32_t vadd4(uint32_t a, uint32_t b)
     return s ^ ((a ^ b) & 0x80808080u);
 }
 
-template <int SRC, int DST>
-__global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p)
+// the 4 pixels of o[] (DST interleaved channels) as one 32-bit word per channel plane
+template <int DST>
+__device__ __forceinline__ void planes_of(const uint32_t (&o)[DST], uint32_t (&pl)[DST])
+{
+    if (DST == 4) {
+        const uint32_t t01 = __byte_perm(o[0], o[1], 0x5140), t23 = __byte_perm(o[2], o[DST - 1], 0x5140);   // c0 c1 of pixels 0,1 / 2,3
+        const uint32_t u01 = __byte_perm(o[0], o[1], 0x7362), u23 = __byte_perm(o[2], o[DST - 1], 0x7362);   // c2 c3
+        pl[0] = __byte_perm(t01, t23, 0x5410); pl[1] = __byte_perm(t01, t23, 0x7632);
+        pl[2] = __byte_perm(u01, u23, 0x5410); pl[DST - 1] = __byte_perm(u01, u23, 0x7632);
+    } else {                 // o = r0 g0 b0 r1 | g1 b1 r2 g2 | b2 r3 g3 b3
+        pl[0] = __byte_perm(__byte_perm(o[0], o[1], 0x0630), o[2], 0x5210);
+        pl[1] = __byte_perm(__byte_perm(o[0], o[1], 0x0741), o[2], 0x6210);
+        pl[2] = __byte_perm(__byte_perm(o[0], o[1], 0x0052), o[2], 0x7410);
+    }
+}
+
+// Output layouts (DecodeParams): interleaved rows at any pitch (PLANAR false) or one byte plane per channel (PLANAR true).
+template <int SRC, int DST, bool PLANAR>
+__global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p, OutStrides os)
 {
     const uint32_t f = blockIdx.y;
     const DecodeState st = p.state[f];
@@ -1278,8 +1295,8 @@ __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p)
     const bool next_full = lane < 31u && x0 + 8u <= w;                           // the next lane of this warp owns a whole group
     const uint32_t npx = min(4u, w - x0);
     const uint8_t* delta = p.delta + (size_t)f * pitch * h + (size_t)x0 * SRC;
-    uint8_t* out = p.d_out + (size_t)f * p.out_stride + (size_t)x0 * DST;
-    const size_t out_pitch = (size_t)w * DST;
+    uint8_t* out = p.d_out + (size_t)f * p.out_stride + (size_t)x0 * (PLANAR ? 1u : DST);
+    const size_t out_pitch = os.row, cs = os.chan;
     const bool full = npx == 4;
     const bool out_aligned = (((uintptr_t)out | out_pitch) & 3) == 0;
     uint32_t acc[SRC];
@@ -1323,6 +1340,19 @@ __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p)
                 o[DST - 1] = __byte_perm(acc[2], acc[SRC - 1], 0x6542);
             }
             uint8_t* orow = out + (size_t)y * out_pitch;
+            if (PLANAR) {
+                // one word per plane when every plane row is 4-byte aligned (x0 % 4 == 0), else bytes
+                uint32_t pl[DST];
+                planes_of<DST>(o, pl);
+                if (full && ((((uintptr_t)orow) | cs) & 3u) == 0u) {
+#pragma unroll
+                    for (int c = 0; c < DST; c++) *reinterpret_cast<uint32_t*>(orow + c * cs) = pl[c];
+                } else {
+#pragma unroll
+                    for (int c = 0; c < DST; c++) for (uint32_t b = 0; b < npx; b++) orow[c * cs + b] = (uint8_t)(pl[c] >> (8u * b));
+                }
+                continue;
+            }
             // output scanlines of any width (w * DST need not be a multiple of 4: 687 x 3 = 2061): the misalignment is the same for every
             // group of a scanline (groups are 4 * DST bytes apart), so the aligned words a thread's bytes straddle are assembled with
             // one funnel shift each, the word shared with the previous group from that lane's last word (shuffle); only the two ends
@@ -1397,7 +1427,7 @@ bool decode_set_pre_roll(uint32_t bits)
     return true;
 }
 
-void launch_decode(const DecodeParams& params, uint32_t n, uint32_t desired, cudaStream_t s)
+void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n, uint32_t desired, cudaStream_t s)
 {
     DecodeParams p = params;
     p.pre_roll = g_dec_pre_roll;
@@ -1425,10 +1455,11 @@ void launch_decode(const DecodeParams& params, uint32_t n, uint32_t desired, cud
     DEC_MARK(5);
     const uint32_t groups = (p.w + 3) / 4;
     dim3 gu((groups + 127) / 128, n);
-    if (p.chans == 3 && desired == 3) unfilter_kernel<3, 3><<<gu, 128, 0, s>>>(p);
-    else if (p.chans == 3) unfilter_kernel<3, 4><<<gu, 128, 0, s>>>(p);
-    else if (desired == 3) unfilter_kernel<4, 3><<<gu, 128, 0, s>>>(p);
-    else unfilter_kernel<4, 4><<<gu, 128, 0, s>>>(p);
+    const bool planar = os.pixel == 1;
+    if (p.chans == 3 && desired == 3) { if (planar) unfilter_kernel<3, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 3, false><<<gu, 128, 0, s>>>(p, os); }
+    else if (p.chans == 3) { if (planar) unfilter_kernel<3, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 4, false><<<gu, 128, 0, s>>>(p, os); }
+    else if (desired == 3) { if (planar) unfilter_kernel<4, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<4, 3, false><<<gu, 128, 0, s>>>(p, os); }
+    else { if (planar) unfilter_kernel<4, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<4, 4, false><<<gu, 128, 0, s>>>(p, os); }
     decode_status_kernel<<<(n + 127) / 128, 128, 0, s>>>(p, n);
     DEC_MARK(6);
     if (g_dec_profile && g_dec_ev_ready) g_dec_ev_valid = true;

@@ -39,9 +39,14 @@ template <int CHANS> __host__ __device__ constexpr int stage16_words() { return 
 __device__ __forceinline__ uint32_t byte1(uint32_t v) { return __byte_perm(v, 0u, 0x4441); }   // (v >> 8) & 0xFF in one PRMT
 __device__ __forceinline__ uint32_t byte2(uint32_t v) { return __byte_perm(v, 0u, 0x4442); }
 
-// scanline loader: staged tiles (TMA / cp.async) for 16-byte aligned scanlines, direct realigning 128-bit loads for any other shape
-template <int CHANS, bool DIRECT> struct Loader16 { using type = Walk16<CHANS>; };
-template <int CHANS> struct Loader16<CHANS, true> { using type = Walk16Direct<CHANS>; };
+// scanline loader: staged tiles (TMA / cp.async) for 16-byte aligned interleaved scanlines, direct realigning 128-bit loads for
+// any other interleaved shape, per-plane loads for planar images (ScanParams::chan_stride != 0)
+enum { kLoad16Staged = 0, kLoad16Direct = 1, kLoad16Planar = 2 };
+template <int CHANS, int LOAD> struct Loader16 { using type = Walk16<CHANS>; };
+template <int CHANS> struct Loader16<CHANS, kLoad16Direct> { using type = Walk16Direct<CHANS>; };
+template <int CHANS> struct Loader16<CHANS, kLoad16Planar> { using type = Walk16Planar<CHANS>; };
+template <class WK> __device__ __forceinline__ void set_planes(WK&, size_t) {}
+template <int CHANS> __device__ __forceinline__ void set_planes(Walk16Planar<CHANS>& wk, size_t chan_stride) { wk.planes(chan_stride); }
 
 template <int CHANS>
 __device__ __forceinline__ uint32_t literal_bits16(const uint8_t* s_lit, uint32_t px)
@@ -62,10 +67,10 @@ __device__ __forceinline__ uint32_t literal_bits16(const uint8_t* s_lit, uint32_
 #else
 #define FPNGB_SCAN_BOUNDS __launch_bounds__(32 * kScan16Rows)
 #endif
-template <int CHANS, bool DIRECT>
+template <int CHANS, int LOAD>
 __global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(ScanParams p)
 {
-    using WK = typename Loader16<CHANS, DIRECT>::type;
+    using WK = typename Loader16<CHANS, LOAD>::type;
     constexpr uint32_t M = max_match_pixels(CHANS);
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     uint8_t* s_lit = dyn_smem + kScan16Rows * WK::kWarpBytes;
@@ -84,14 +89,14 @@ __global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(ScanParams p)
     if (y >= p.h) return;
 
     const uint32_t w = p.w, bpl = w * CHANS;
-    const uint8_t* cur = p.pixels + (size_t)img * p.image_stride + (size_t)y * bpl;
-    const uint8_t* prev = y ? cur - bpl : nullptr;
+    const uint8_t* cur = p.pixels + (size_t)img * p.image_stride + (size_t)y * p.row_pitch;
+    const uint8_t* prev = y ? cur - p.row_pitch : nullptr;
     const uint32_t filt = y ? 2u : 0u;
     const uint32_t nsteps = (w + kStep16 - 1) / kStep16;
     uint8_t* tiles = dyn_smem + warp * WK::kWarpBytes;
     uint2* lane_ofs = p.lane_ofs + ((size_t)img * p.h + y) * p.lane_ofs_pitch;
 
-    WK wk; wk.init(lane, tiles); wk.bind(cur, prev);
+    WK wk; wk.init(lane, tiles); wk.bind(cur, prev); set_planes(wk, p.chan_stride);
     RowCarry carry = {0u, 0u};
     uint32_t row_run = s_lit[filt];              // bits of the row emitted before the current step (filter literal first)
     uint32_t sumA = 0, last_unit = 0;
@@ -179,10 +184,10 @@ __global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(ScanParams p)
 // K1-hist (v2): 288-bin literal/length histogram of 2-pass mode (fpng.cpp:1021-1084, 1299-1363) on the 16-pixel walker.
 // Warp-private shared-memory histograms (no inter-warp contention), merged per CTA, then added to the image's bins.
 // ------------------------------------------------------------------------------------------------
-template <int CHANS, bool DIRECT>
+template <int CHANS, int LOAD>
 __global__ void __launch_bounds__(32 * kScan16Rows) row_hist16_kernel(ScanParams p)
 {
-    using WK = typename Loader16<CHANS, DIRECT>::type;
+    using WK = typename Loader16<CHANS, LOAD>::type;
     constexpr uint32_t M = max_match_pixels(CHANS);
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     uint32_t* s_hist_all = reinterpret_cast<uint32_t*>(dyn_smem + kScan16Rows * WK::kWarpBytes);   // [warps][288]
@@ -198,11 +203,11 @@ __global__ void __launch_bounds__(32 * kScan16Rows) row_hist16_kernel(ScanParams
 
     if (y < p.h) {
         const uint32_t w = p.w, bpl = w * CHANS;
-        const uint8_t* cur = p.pixels + (size_t)img * p.image_stride + (size_t)y * bpl;
-        const uint8_t* prev = y ? cur - bpl : nullptr;
+        const uint8_t* cur = p.pixels + (size_t)img * p.image_stride + (size_t)y * p.row_pitch;
+        const uint8_t* prev = y ? cur - p.row_pitch : nullptr;
         const uint32_t nsteps = (w + kStep16 - 1) / kStep16;
         uint8_t* tiles = dyn_smem + warp * WK::kWarpBytes;
-        WK wk; wk.init(lane, tiles); wk.bind(cur, prev);
+        WK wk; wk.init(lane, tiles); wk.bind(cur, prev); set_planes(wk, p.chan_stride);
         RowCarry carry = {0u, 0u};
         uint32_t dummyA = 0; unsigned long long dummyB = 0;
         if (lane == 0) atomicAdd(&hist[y ? 2 : 0], 1u);               // the filter literal
@@ -441,10 +446,10 @@ __device__ __forceinline__ uint32_t crc_step16(uint32_t crc_s, uint32_t cx, uint
     return v ^ lds_u32(crc_s + b0 * 4u) ^ lds_u32(crc_s + 1024u + b1 * 4u) ^ lds_u32(crc_s + 2048u + b2 * 4u) ^ lds_u32(crc_s + 3072u + b3 * 4u);
 }
 
-template <int CHANS, bool DIRECT>
+template <int CHANS, int LOAD>
 __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParams p, uint32_t rows_per_warp)
 {
-    using WK = typename Loader16<CHANS, DIRECT>::type;
+    using WK = typename Loader16<CHANS, LOAD>::type;
     if (p.stored_only && !p.st[blockIdx.y].stored) return;     // after the fused encoder only stored-block images are left to write
     constexpr uint32_t M = max_match_pixels(CHANS);
     constexpr int kHalfWords = 2 * CHANS;        // filtered words of 8 pixels
@@ -467,9 +472,12 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParam
     const ImageState st = p.st[img];
     if (st.stored) {                             // stored-block fallback (fpng.cpp:818-866): strided copy of the rows
         const uint32_t bpl_s = p.w * CHANS;
-        for (uint32_t y = row0; y < min(row0 + rows_per_warp, p.h); y++)
-            store_row_raw(p.pixels + (size_t)img * p.image_stride + (size_t)y * bpl_s, p.out + (size_t)img * p.out_stride + kPngHeaderSize,
-                          y, bpl_s, lane, &p.row_adler[(size_t)img * p.h + y]);
+        for (uint32_t y = row0; y < min(row0 + rows_per_warp, p.h); y++) {
+            const uint8_t* row = p.pixels + (size_t)img * p.image_stride + (size_t)y * p.row_pitch;
+            uint8_t* zl = p.out + (size_t)img * p.out_stride + kPngHeaderSize;
+            if (LOAD == kLoad16Planar) store_row_raw(PlaneBytes<CHANS>{row, p.chan_stride}, zl, y, bpl_s, lane, &p.row_adler[(size_t)img * p.h + y]);
+            else store_row_raw(row, zl, y, bpl_s, lane, &p.row_adler[(size_t)img * p.h + y]);
+        }
         return;
     }
     for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) {
@@ -512,12 +520,13 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParam
     uint32_t flushed_bits = 0;                   // row bits (incl. the G & 31 lead-in) already flushed to global, multiple of 32
     uint32_t leftover = 0;                       // bits of the partially filled word carried from the previous step (lane 0 seeds with it)
 
-    WK wk; wk.init(lane, tiles);
+    WK wk; wk.init(lane, tiles); set_planes(wk, p.chan_stride);
     uint32_t dummyA = 0; unsigned long long dummyB = 0;
-    {
-        const uint8_t* c0 = img_px + (size_t)row0 * bpl;
-        wk.prefetch(c0, row0 ? c0 - bpl : nullptr, 0, bpl, lane, tiles);
-    }
+    const uint32_t pitch = p.row_pitch;
+    // the current item's scanline, advanced by the pitch at each row end (recomputing img_px + y * pitch per item costs the RGBA
+    // direct-loader kernel 9 registers)
+    const uint8_t* row_px = img_px + (size_t)row0 * pitch;
+    wk.prefetch(row_px, row0 ? row_px - pitch : nullptr, 0, bpl, lane, tiles);
     uint2 mine = lane_ofs[0];
     uint32_t r_i = 0, step = 0;                  // row (relative to row0) and step of the current item
     for (uint32_t item = 0; item < nitems; item++) {
@@ -530,15 +539,15 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParam
             first_pending = true; flushed_bits = 0; leftover = 0;
         }
         uint32_t dw[WK::kWords];
-        { const uint8_t* cc = img_px + (size_t)y * bpl; wk.bind(cc, y ? cc - bpl : nullptr); }
+        wk.bind(row_px, y ? row_px - pitch : nullptr);
         wk.template consume<false>(y != 0, item, step, bpl, lane, tiles, dw, dummyA, dummyB);
         // the next item (possibly the first step of the next scanline) is fetched while this one is emitted
         const bool more = step + 1 < nsteps;     // more steps in this row
         const uint32_t my_ofs = mine.x, info = mine.y;
         if (item + 1 < nitems) {
             const uint32_t ny = more ? y : y + 1, nstep = more ? step + 1 : 0;
-            const uint8_t* nc = img_px + (size_t)ny * bpl;
-            wk.prefetch(nc, ny ? nc - bpl : nullptr, nstep, bpl, lane, tiles);
+            const uint8_t* nc = img_px + (size_t)ny * pitch;
+            wk.prefetch(nc, ny ? nc - pitch : nullptr, nstep, bpl, lane, tiles);
             mine = lane_ofs[(size_t)(ny - row0) * p.lane_ofs_pitch + nstep * 32u];
         }
         // classification of this lane's 16 pixels, as computed by the scan kernel
@@ -681,7 +690,7 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParam
                 if (lane == 0) p.row_crc[ridx0 + r_i] = r;
                 cx = 0;
             }
-            step = 0; r_i++;
+            step = 0; r_i++; row_px += pitch;
         }
     }
 }
@@ -689,48 +698,84 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParam
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
-bool walk16_eligible(const void* base, size_t image_stride, uint32_t w, uint32_t chans)
+bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans)
 {
     const size_t bpl = (size_t)w * chans;
-    return ((uintptr_t)base % 16 == 0) && (image_stride % 16 == 0) && (bpl % 16 == 0);
+    return ((uintptr_t)base % 16 == 0) && (image_stride % 16 == 0) && (row_pitch % 16 == 0) && (bpl % 16 == 0);
 }
-
-template <int CHANS, bool DIRECT> constexpr size_t scan16_smem() { return kScan16Rows * Loader16<CHANS, DIRECT>::type::kWarpBytes + 256 + 96; }
-template <int CHANS, bool DIRECT> constexpr size_t pack16_smem()
+template <class P> static int load16_mode(const P& p, uint32_t chans)
 {
-    return kPack16Rows * Loader16<CHANS, DIRECT>::type::kWarpBytes + ((FPNGB_PACK_LIT64 ? 1024 : 0) + 512 + 88 + kPack16Rows * stage16_words<CHANS>() + 1024) * 4;
+    if (p.chan_stride) return kLoad16Planar;
+    return walk16_eligible(p.pixels, p.image_stride, p.row_pitch, p.w, chans) ? kLoad16Staged : kLoad16Direct;
 }
-template <int CHANS, bool DIRECT> constexpr size_t hist16_smem() { return kScan16Rows * Loader16<CHANS, DIRECT>::type::kWarpBytes + kScan16Rows * 288 * 4; }
 
-// The 16-pixel kernels take any scanline alignment: `direct` selects the realigning-load variant (walk16_eligible() false).
+template <int CHANS, int LOAD> constexpr size_t scan16_smem() { return kScan16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + 256 + 96; }
+template <int CHANS, int LOAD> constexpr size_t pack16_smem()
+{
+    return kPack16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + ((FPNGB_PACK_LIT64 ? 1024 : 0) + 512 + 88 + kPack16Rows * stage16_words<CHANS>() + 1024) * 4;
+}
+template <int CHANS, int LOAD> constexpr size_t hist16_smem() { return kScan16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + kScan16Rows * 288 * 4; }
+
+// The 16-pixel kernels take any scanline alignment and either layout: `load` (load16_mode()) selects the loader.
+#define FPNGB_LAUNCH16_ONE(C, L, kernel, smemfn, grid, threads, ...) do { \
+        FPNGB_SET_SMEM((kernel<C, L>), (smemfn<C, L>())); kernel<C, L><<<grid, threads, smemfn<C, L>(), s>>>(__VA_ARGS__); } while (0)
 #define FPNGB_LAUNCH16(kernel, smemfn, grid, threads, ...) do { \
-        if (chans == 4) { if (direct) { FPNGB_SET_SMEM((kernel<4, true>), (smemfn<4, true>())); kernel<4, true><<<grid, threads, smemfn<4, true>(), s>>>(__VA_ARGS__); } \
-                          else { FPNGB_SET_SMEM((kernel<4, false>), (smemfn<4, false>())); kernel<4, false><<<grid, threads, smemfn<4, false>(), s>>>(__VA_ARGS__); } } \
-        else { if (direct) { FPNGB_SET_SMEM((kernel<3, true>), (smemfn<3, true>())); kernel<3, true><<<grid, threads, smemfn<3, true>(), s>>>(__VA_ARGS__); } \
-               else { FPNGB_SET_SMEM((kernel<3, false>), (smemfn<3, false>())); kernel<3, false><<<grid, threads, smemfn<3, false>(), s>>>(__VA_ARGS__); } } \
+        if (chans == 4) { \
+            if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(4, kLoad16Planar, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(4, kLoad16Direct, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else FPNGB_LAUNCH16_ONE(4, kLoad16Staged, kernel, smemfn, grid, threads, __VA_ARGS__); \
+        } else { \
+            if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(3, kLoad16Planar, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(3, kLoad16Direct, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else FPNGB_LAUNCH16_ONE(3, kLoad16Staged, kernel, smemfn, grid, threads, __VA_ARGS__); \
+        } \
     } while (0)
 
 void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
 {
     // one scanline per warp: the multi-scanline sequence that pays off in the pack kernel measured neutral (RGB) to 4 % slower (RGBA) here
-    const bool direct = !walk16_eligible(p.pixels, p.image_stride, p.w, chans);
+    const int load = load16_mode(p, chans);
     dim3 grid((p.h + kScan16Rows - 1) / kScan16Rows, n);
     FPNGB_LAUNCH16(row_scan16_kernel, scan16_smem, grid, 32 * kScan16Rows, p);
 }
 
 void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
 {
-    const bool direct = !walk16_eligible(p.pixels, p.image_stride, p.w, chans);
+    const int load = load16_mode(p, chans);
     dim3 grid((p.h + kScan16Rows - 1) / kScan16Rows, n);
     FPNGB_LAUNCH16(row_hist16_kernel, hist16_smem, grid, 32 * kScan16Rows, p);
 }
 
 void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
 {
-    const bool direct = !walk16_eligible(p.pixels, p.image_stride, p.w, chans);
+    const int load = load16_mode(p, chans);
     const uint32_t rpw = rows_per_warp16(n, p.h), rows_per_cta = kPack16Rows * rpw;
     dim3 grid((p.h + rows_per_cta - 1) / rows_per_cta, n);
     FPNGB_LAUNCH16(pack_rows16_kernel, pack16_smem, grid, 32 * kPack16Rows, p, rpw);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Strided input for the encoders that read tight interleaved rows only (the generic 4-pixel kernels, the single-pass
+// encoder): one copy into a contiguous [n][h][w * chans] buffer, then the unchanged path.  One CTA per scanline (grid-stride).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) gather_pixels_kernel(GatherParams p)
+{
+    const uint32_t bpl = p.w * p.chans;
+    for (unsigned long long r = blockIdx.x; r < (unsigned long long)p.n * p.h; r += gridDim.x) {
+        const unsigned long long img = r / p.h, y = r - img * p.h;
+        const uint8_t* src = p.src + img * p.image_stride + y * p.row_pitch;
+        uint8_t* dst = p.dst + r * bpl;
+        for (uint32_t i = threadIdx.x; i < bpl; i += blockDim.x) {
+            const uint32_t x = i / p.chans, c = i - x * p.chans;
+            dst[i] = __ldg(src + (size_t)x * p.pixel_stride + (size_t)c * p.chan_stride);
+        }
+    }
+}
+
+void launch_gather_pixels(const GatherParams& p, cudaStream_t s)
+{
+    const unsigned long long rows = (unsigned long long)p.n * p.h;
+    gather_pixels_kernel<<<(uint32_t)min(rows, 65536ull), 256, 0, s>>>(p);
 }
 
 }  // namespace fpngb

@@ -803,7 +803,7 @@ int launch_encode_fused(const uint8_t* pixels, size_t image_stride, uint32_t n, 
     p.merge_first_unit = merge_first_unit; p.inline_crc = inline_crc ? 1u : 0u;
     const uint32_t threads = 32u * R * S;
     const unsigned long long groups = (unsigned long long)n * G;
-    const bool direct = !walk16_eligible(pixels, image_stride, w, chans);
+    const bool direct = !walk16_eligible(pixels, image_stride, w * chans, w, chans);
 #define FPNGB_LAUNCH_FUSED(C, D) do { FPNGB_SET_SMEM((encode_fused_kernel<C, D>), (fused_smem<C, D>())); \
         encode_fused_kernel<C, D><<<(uint32_t)groups, threads, fused_smem<C, D>(), s>>>(p); } while (0)
     if (chans == 4) { if (direct) FPNGB_LAUNCH_FUSED(4, true); else FPNGB_LAUNCH_FUSED(4, false); }

@@ -7,6 +7,7 @@
 // device every entry point fails with FPNGB_ERR_NO_DEVICE.
 #include "../../include/fpng_b200.h"
 #include "kernels.cuh"
+#include "layout.h"
 #include "row_walk.cuh"
 #include "static_tables.h"
 #include "runtime.h"
@@ -186,10 +187,12 @@ struct Workspace {
     uint2* lane_ofs; uint32_t lane_ofs_pitch;
     void* fused_desc;
     uint32_t* row_crc;
+    uint8_t* gather;                            // contiguous copy of a strided batch (encoders without layout support)
 };
 
 
-static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, bool two_pass, Workspace& w, bool fused = false)
+static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, bool two_pass, Workspace& w, bool fused = false,
+                           size_t gather_bytes = 0)
 {
     const size_t rows = (size_t)n * h;
     const uint32_t lane_pitch = ((width + 511u) / 512u) * 32u;       // one uint2 per 16-pixel group, whole warp steps
@@ -203,6 +206,7 @@ static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, b
     const size_t o_lane = o; o = align_up(o + (fused ? 0 : rows * lane_pitch * 8), 256);
     const size_t o_desc = o; o = align_up(o + (fused ? fused_desc_bytes(n, width, h) : 0), 256);
     const size_t o_rcrc = o; o = align_up(o + (fused ? 0 : rows * 4), 256);
+    const size_t o_gather = o; o = align_up(o + gather_bytes, 256);
     int rc = c.ws.reserve(o);
     if (rc) return rc;
     uint8_t* b = (uint8_t*)c.ws.p;
@@ -211,6 +215,7 @@ static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, b
     w.st = (ImageState*)(b + o_st); w.hist = (uint32_t*)(b + o_hist); w.books = (CodeBook*)(b + o_books);
     w.lane_ofs = (uint2*)(b + o_lane); w.lane_ofs_pitch = lane_pitch;
     w.fused_desc = b + o_desc;
+    w.gather = b + o_gather;
     return 0;
 }
 
@@ -263,8 +268,13 @@ static void make_png_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t chans
 //  * the single-pass encoder (encode_fused.cu), selected with FPNGB_FUSED=1 / fpngb_debug_use_fused(1): reads the pixels once
 //    and writes the file once, byte-identical output, measured slower than the two-kernel path because it is bound by
 //    instruction issue, not by HBM.
-static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image_stride, uint32_t n, uint32_t w, uint32_t h,
-                               uint32_t chans, uint32_t flags, uint8_t* d_out, size_t out_stride, uint32_t* d_sizes, cudaStream_t s)
+//
+// The input layout (layout.h) is image_stride / row_pitch and, for planar images, chan_stride (0: interleaved rows).  The 16-pixel
+// scan and pack kernels read every layout in place; the generic kernels and the single-pass encoder read tight interleaved rows
+// only, so a strided batch bound for them is first copied into the workspace by gather_pixels_kernel.
+static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image_stride, uint32_t row_pitch, size_t chan_stride,
+                               uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, uint8_t* d_out, size_t out_stride,
+                               uint32_t* d_sizes, cudaStream_t s)
 {
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
     // second-generation kernels (16 pixels per lane, coalesced 128-bit loads) whenever every scanline is 16-byte aligned;
@@ -280,11 +290,19 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
     const bool want_fused = g_fused_mode == 1 || (g_fused_mode < 0 && env_fused);
     const bool fused = want_fused && !force_generic && !lit1_rule && !(flags & FPNGB_FORCE_UNCOMPRESSED) &&
                        fused_eligible(d_pixels, image_stride, w, h, chans, n);
+    const bool gather = (!v2 || fused) && (chan_stride != 0 || row_pitch != w * chans);
+    const size_t bytes_per_image = (size_t)w * h * chans;
     Workspace ws;
-    int rc = carve_workspace(c, n, h, w, two_pass, ws, fused);
+    int rc = carve_workspace(c, n, h, w, two_pass, ws, fused, gather ? n * bytes_per_image : 0);
     if (rc) return rc;
     rc = c.ws_acquire(s);
     if (rc) return rc;
+    if (gather) {
+        GatherParams gp{d_pixels, image_stride, row_pitch, chan_stride ? 1u : chans, chan_stride ? chan_stride : 1u, ws.gather, n, w, h, chans};
+        launch_gather_pixels(gp, s);
+        count_launch(1);
+        d_pixels = ws.gather; image_stride = bytes_per_image; row_pitch = w * chans; chan_stride = 0;
+    }
     const int mode = pick_load_mode(d_pixels, image_stride, w, chans);
     const CodeBook* books0 = two_pass ? ws.books : c.d_static_books + (chans == 4 ? 1 : 0);
     const uint32_t book_stride = two_pass ? 1u : 0u;
@@ -308,7 +326,7 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
         const size_t r0 = (size_t)i0 * h;
 
         ScanParams sp{};
-        sp.pixels = px; sp.image_stride = image_stride; sp.w = w; sp.h = h;
+        sp.pixels = px; sp.image_stride = image_stride; sp.row_pitch = row_pitch; sp.chan_stride = chan_stride; sp.w = w; sp.h = h;
         sp.books = books; sp.book_stride = book_stride;
         sp.row_bits = ws.row_bits + r0; sp.row_adler = ws.row_adler + r0; sp.st = ws.st + i0; sp.hist = ws.hist + (size_t)i0 * 288;
         sp.merge_first_unit = merge_first_unit;
@@ -326,7 +344,7 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
             count_launch(2);
         }
         PackParams pp{};
-        pp.pixels = px; pp.image_stride = image_stride; pp.w = w; pp.h = h; pp.books = books; pp.book_stride = book_stride;
+        pp.pixels = px; pp.image_stride = image_stride; pp.row_pitch = row_pitch; pp.chan_stride = chan_stride; pp.w = w; pp.h = h; pp.books = books; pp.book_stride = book_stride;
         pp.row_ofs = ws.row_ofs + r0; pp.row_bits = sp.row_bits; pp.lane_ofs = sp.lane_ofs; pp.lane_ofs_pitch = ws.lane_ofs_pitch;
         pp.row_adler = sp.row_adler; pp.st = sp.st; pp.out = out; pp.out_stride = out_stride;
         pp.lit1_rule = lit1_rule;
@@ -467,12 +485,18 @@ FPNGB_API int fpngb_debug_static_table(uint32_t chans, uint8_t* sizes, uint16_t*
     return FPNGB_OK;
 }
 
-int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans,
-                              uint32_t flags, void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream)
+int fpngb_encode_batch_device_strided(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride,
+                                      uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* d_out, size_t out_stride,
+                                      uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_pixels || !d_out || !d_sizes || n == 0 || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
-    if (image_stride < (size_t)w * h * chans) return FPNGB_ERR_INVALID_ARG;
+    // any interleaved or planar layout, overlapping ones included (the pixels are only read); the kernels take a 32-bit row pitch
+    Layout L;
+    uint64_t last = 0;
+    if (!classify_layout(image_stride, row_pitch, pixel_stride, chan_stride, n, h, w, chans, L) || L.row > 0xFFFFFFFFull ||
+        !layout_span(d_pixels, L, n, h, w, chans, last))
+        return FPNGB_ERR_INVALID_ARG;
     if (out_stride < max_encoded_size(w, h, chans)) return FPNGB_ERR_BUFFER_TOO_SMALL;
     if (out_stride % 16 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
     if (n > 65535) return FPNGB_ERR_INVALID_ARG;
@@ -480,7 +504,18 @@ int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     cudaStream_t s = (cudaStream_t)stream;      // NULL = the CUDA default stream, exactly as the caller passed it
-    return encode_batch_locked(c, (const uint8_t*)d_pixels, image_stride, n, w, h, chans, flags, (uint8_t*)d_out, out_stride, d_sizes, s);
+    return encode_batch_locked(c, (const uint8_t*)d_pixels, L.image, (uint32_t)L.row, L.planar ? L.chan : 0, n, w, h, chans, flags,
+                               (uint8_t*)d_out, out_stride, d_sizes, s);
+}
+
+int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans,
+                              uint32_t flags, void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_pixels || !d_out || !d_sizes || n == 0 || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
+    if (image_stride < (size_t)w * h * chans) return FPNGB_ERR_INVALID_ARG;
+    return fpngb_encode_batch_device_strided(d_pixels, image_stride, (size_t)w * chans, chans, 1, n, w, h, chans, flags, d_out, out_stride,
+                                             d_sizes, stream);
 }
 
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)
@@ -499,7 +534,7 @@ int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans
     uint32_t* d_size = (uint32_t*)((uint8_t*)c.dev_out.p + stride);
     cudaStream_t s = c.stream;
     FPNGB_CUDA_OK(cudaMemcpyAsync(c.dev_in.p, pixels, in_bytes, cudaMemcpyHostToDevice, s));
-    rc = encode_batch_locked(c, (const uint8_t*)c.dev_in.p, in_bytes, 1, w, h, chans, flags, (uint8_t*)c.dev_out.p, stride, d_size, s);
+    rc = encode_batch_locked(c, (const uint8_t*)c.dev_in.p, in_bytes, w * chans, 0, 1, w, h, chans, flags, (uint8_t*)c.dev_out.p, stride, d_size, s);
     if (rc) return rc;
     uint32_t* h_size = (uint32_t*)c.pin_small.p;
     FPNGB_CUDA_OK(cudaMemcpyAsync(h_size, d_size, 4, cudaMemcpyDeviceToHost, s));
@@ -571,7 +606,7 @@ int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
         if (e != cudaSuccess) { result = 1000 + (int)e; break; }
         cudaEventRecord(ev_in[sl], c.copy_in);
         cudaStreamWaitEvent(c.stream, ev_in[sl], 0);
-        rc = encode_batch_locked(c, din, in_bytes, cnt, w, h, chans, flags, dout, dstride, dsz, c.stream);
+        rc = encode_batch_locked(c, din, in_bytes, w * chans, 0, cnt, w, h, chans, flags, dout, dstride, dsz, c.stream);
         if (rc) { result = rc; break; }
         cudaEventRecord(ev_done[sl], c.stream);
         cudaStreamWaitEvent(c.copy_out, ev_done[sl], 0);
@@ -734,7 +769,7 @@ int fpngb_train_accumulate_device(const void* d_pixels, size_t image_stride, uin
     int rc = carve_workspace(c, n, h, w, true, ws); if (rc) return rc;
     rc = c.ws_acquire(s); if (rc) return rc;
     ScanParams sp{};
-    sp.pixels = (const uint8_t*)d_pixels; sp.image_stride = image_stride; sp.w = w; sp.h = h; sp.books = c.d_static_books; sp.book_stride = 0;
+    sp.pixels = (const uint8_t*)d_pixels; sp.image_stride = image_stride; sp.row_pitch = w * chans; sp.w = w; sp.h = h; sp.books = c.d_static_books; sp.book_stride = 0;
     sp.row_bits = ws.row_bits; sp.row_adler = ws.row_adler; sp.st = ws.st; sp.hist = ws.hist; sp.lane_ofs = ws.lane_ofs; sp.lane_ofs_pitch = ws.lane_ofs_pitch;
     FPNGB_CUDA_OK(cudaMemsetAsync(ws.hist, 0, (size_t)n * 288 * 4, s));
     static const bool force_generic_t = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;

@@ -11,7 +11,9 @@ constexpr int kOffsetsThreads = 256;
 constexpr int kStageWords = 272;                  // >= (31 + 12 + 128 * 66) / 32 + 1 words per 128-pixel step
 
 struct ScanParams {
-    const uint8_t* pixels; size_t image_stride;   // n images, tightly packed rows (pitch = w * chans)
+    const uint8_t* pixels; size_t image_stride;   // n images
+    uint32_t row_pitch;                           // bytes between scanlines (the generic 4-pixel kernels assume w * chans)
+    size_t chan_stride;                           // 0: interleaved pixels; else planar, channel c of pixel x at row + x + c * chan_stride
     uint32_t w, h;
     const CodeBook* books; uint32_t book_stride;  // 0: one shared (1-pass) book, 1: per-image books (2-pass)
     uint32_t* row_bits;                           // [n*h] token bits per row (incl. the filter literal)
@@ -34,6 +36,7 @@ struct OffsetsParams {
 
 struct PackParams {
     const uint8_t* pixels; size_t image_stride;
+    uint32_t row_pitch; size_t chan_stride;       // see ScanParams
     uint32_t w, h;
     const CodeBook* books; uint32_t book_stride;
     const unsigned long long* row_ofs;
@@ -101,8 +104,16 @@ void launch_crc_stream(const CrcParams& p, uint32_t n, size_t max_file_bytes, cu
 void launch_row_crc_combine(const RowCrcParams& p, uint32_t n, cudaStream_t s);
 int crc_stream_table_ptrs(const uint32_t** f128b, const uint32_t** lane_mul);
 
+// strided input -> contiguous [n][h][w * chans] (encode16_kernels.cu)
+struct GatherParams {
+    const uint8_t* src; size_t image_stride, row_pitch, pixel_stride, chan_stride;
+    uint8_t* dst;
+    uint32_t n, w, h, chans;
+};
+void launch_gather_pixels(const GatherParams& p, cudaStream_t s);
+
 void launch_scan(const ScanParams& p, uint32_t n, uint32_t chans, int mode, bool hist, cudaStream_t s);
-bool walk16_eligible(const void* base, size_t image_stride, uint32_t w, uint32_t chans);
+bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans);
 void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);
 void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);
 void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t s);

@@ -194,11 +194,27 @@ __device__ __forceinline__ uint32_t warp_excl_scan_u32(uint32_t v, uint32_t lane
     return s - v;
 }
 
+// Source bytes of a stored row, in PNG byte order: byte i of an interleaved scanline, or of a planar one (channel i % CHANS
+// of pixel i / CHANS, planes chan_stride bytes apart)
+struct RowBytes {
+    const uint8_t* p;
+    __device__ __forceinline__ uint32_t operator()(unsigned long long i) const { return ld_u8(p + i); }
+};
+template <int CHANS>
+struct PlaneBytes {
+    const uint8_t* p; size_t chan_stride;
+    __device__ __forceinline__ uint32_t operator()(unsigned long long i) const
+    {
+        const unsigned long long x = i / CHANS;
+        return ld_u8(p + x + (i - x * CHANS) * chan_stride);
+    }
+};
+
 // Stored-block fallback for one row (fpng.cpp:818-866): stream byte s (row y, column t; t == 0 is the filter byte 0)
 // lands at zlib offset 2 + 5 * (s / 65535 + 1) + s.  The row is copied block segment by block segment with 32-bit stores
 // (source words rebuilt from byte loads that hit L1); also produces the row's Adler partials over the raw bytes.
-__device__ __forceinline__ void store_row_raw(const uint8_t* __restrict__ cur, uint8_t* __restrict__ zl, uint32_t y, uint32_t bpl,
-                                              uint32_t lane, uint2* adler_out)
+template <class Src>
+__device__ __forceinline__ void store_row_raw(const Src& at, uint8_t* __restrict__ zl, uint32_t y, uint32_t bpl, uint32_t lane, uint2* adler_out)
 {
     const unsigned long long n = (unsigned long long)bpl + 1ull;
     const unsigned long long s0 = (unsigned long long)y * n;
@@ -208,30 +224,35 @@ __device__ __forceinline__ void store_row_raw(const uint8_t* __restrict__ cur, u
         const unsigned long long s = s0 + t, blk = s / 65535ull;
         const unsigned long long seg = min(n - t, (blk + 1ull) * 65535ull - s);      // bytes until the row or the block ends
         uint8_t* dst = zl + 2ull + 5ull * (blk + 1ull) + s;
-        // source of stream index t is 0 (filter) for t == 0, cur[t-1] otherwise
+        // source of stream index t is 0 (filter) for t == 0, row byte t-1 otherwise
         unsigned long long done = 0;
         if (t == 0) { if (lane == 0) dst[0] = 0; done = 1; }
-        const uint8_t* src = cur + (t + done - 1ull);
+        const unsigned long long src = t + done - 1ull;
         uint8_t* d = dst + done;
         const unsigned long long len = seg - done;
         const uint32_t head = (uint32_t)min((unsigned long long)((4u - ((uintptr_t)d & 3u)) & 3u), len);
-        if (lane < head) { const uint32_t v = ld_u8(src + lane); d[lane] = (uint8_t)v; A += v; B += (t + done + lane) * v; }
+        if (lane < head) { const uint32_t v = at(src + lane); d[lane] = (uint8_t)v; A += v; B += (t + done + lane) * v; }
         const unsigned long long body = (len - head) >> 2;
-        const uint8_t* sb = src + head; uint8_t* db = d + head;
+        const unsigned long long sb = src + head; uint8_t* db = d + head;
         const unsigned long long tb = t + done + head;
         for (unsigned long long j = lane; j < body; j += 32) {
-            const uint8_t* q = sb + 4ull * j;
-            const uint32_t v = ld_u8(q) | (ld_u8(q + 1) << 8) | (ld_u8(q + 2) << 16) | (ld_u8(q + 3) << 24);
+            const unsigned long long q = sb + 4ull * j;
+            const uint32_t v = at(q) | (at(q + 1) << 8) | (at(q + 2) << 16) | (at(q + 3) << 24);
             *reinterpret_cast<uint32_t*>(db + 4ull * j) = v;
             const uint32_t t1 = __dp4a(v, 0x01010101u, 0u), t2 = __dp4a(v, 0x03020100u, 0u);
             A += t1; B += (tb + 4ull * j) * t1 + t2;
         }
         const uint32_t tail = (uint32_t)((len - head) & 3ull);
-        if (lane < tail) { const unsigned long long o = head + 4ull * body + lane; const uint32_t v = ld_u8(src + o); d[o] = (uint8_t)v; A += v; B += (t + done + o) * v; }
+        if (lane < tail) { const unsigned long long o = head + 4ull * body + lane; const uint32_t v = at(src + o); d[o] = (uint8_t)v; A += v; B += (t + done + o) * v; }
         t += seg;
     }
     A = warp_sum_u64(A); B = warp_sum_u64(B);
     if (lane == 0) *adler_out = make_uint2((uint32_t)(A % kAdlerMod), (uint32_t)((n * A - B) % kAdlerMod));
+}
+__device__ __forceinline__ void store_row_raw(const uint8_t* __restrict__ cur, uint8_t* __restrict__ zl, uint32_t y, uint32_t bpl,
+                                              uint32_t lane, uint2* adler_out)
+{
+    store_row_raw(RowBytes{cur}, zl, y, bpl, lane, adler_out);
 }
 
 }  // namespace fpngb

@@ -330,6 +330,66 @@ struct Walk16Direct {
     const uint8_t* cur_ = nullptr; const uint8_t* prev_ = nullptr;
 };
 
+// ---- planar (CHW-style) scanlines: one byte plane per channel -------------------------------------------------------
+// Byte (x, c) of a scanline is at cur + x + c * chan_stride.  Each lane loads its 16 bytes of every plane (cur and prev row)
+// with Walk16Direct's realigning 128-bit loads (the lane stride is 16 bytes, so each plane's misalignment is warp-uniform),
+// applies the Up filter per plane (vsub4 is byte-wise: filtering before interleaving is exact) and interleaves the planes
+// with byte permutes into exactly the words the interleaved loaders deliver.  Pixels beyond the scanline read as zero.
+template <int CHANS>
+struct Walk16Planar {
+    static constexpr int kWords = 4 * CHANS;
+    static constexpr int kWarpBytes = 0;                      // no staging buffer
+    __device__ __forceinline__ void init(uint32_t, uint8_t*) {}
+    __device__ __forceinline__ void prefetch(const uint8_t*, const uint8_t*, uint32_t, uint32_t, uint32_t, uint8_t*) const {}
+
+    template <bool kAdler>
+    __device__ __forceinline__ void consume(bool have_prev, uint32_t, uint32_t step, uint32_t bpl, uint32_t lane, uint8_t*,
+                                            uint32_t (&dw)[kWords], uint32_t& sumA, unsigned long long& sumB) const
+    {
+        const uint32_t w = bpl / CHANS;
+        const uint32_t p0 = step * (uint32_t)kStep16 + lane * (uint32_t)kPix16;
+        const uint32_t np = p0 < w ? min(16u, w - p0) : 0u;
+        uint32_t pl[CHANS][4];                               // 16 filtered bytes of each plane
+        if (np) {
+#pragma unroll
+            for (int c = 0; c < CHANS; c++) {
+                Walk16Direct<1>::load_lane(cur_ + p0 + c * cs_, np, pl[c]);
+                if (have_prev) {
+                    uint32_t q[4];
+                    Walk16Direct<1>::load_lane(prev_ + p0 + c * cs_, np, q);
+#pragma unroll
+                    for (int i = 0; i < 4; i++) pl[c][i] = vsub4(pl[c][i], q[i]);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int c = 0; c < CHANS; c++)
+#pragma unroll
+                for (int i = 0; i < 4; i++) pl[c][i] = 0u;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) {                        // pixels 4j .. 4j+3
+            const uint32_t r = pl[0][j], g = pl[1][j], b = pl[2][j];
+            const uint32_t rg_lo = __byte_perm(r, g, 0x5140), rg_hi = __byte_perm(r, g, 0x7362);   // r0 g0 r1 g1 / r2 g2 r3 g3
+            if (CHANS == 4) {
+                const uint32_t a = pl[CHANS - 1][j];
+                const uint32_t ba_lo = __byte_perm(b, a, 0x5140), ba_hi = __byte_perm(b, a, 0x7362);
+                dw[4 * j] = __byte_perm(rg_lo, ba_lo, 0x5410);     dw[4 * j + 1] = __byte_perm(rg_lo, ba_lo, 0x7632);
+                dw[4 * j + 2] = __byte_perm(rg_hi, ba_hi, 0x5410); dw[4 * j + 3] = __byte_perm(rg_hi, ba_hi, 0x7632);
+            } else {
+                dw[3 * j] = __byte_perm(rg_lo, b, 0x2410);                                    // r0 g0 b0 r1
+                dw[3 * j + 1] = __byte_perm(__byte_perm(rg_lo, b, 0x0053), rg_hi, 0x5410);    // g1 b1 r2 g2
+                dw[3 * j + 2] = __byte_perm(rg_hi, b, 0x7326);                                // b2 r3 g3 b3
+            }
+        }
+        if (kAdler) adler_lane16<CHANS>(dw, p0 * CHANS, sumA, sumB);
+    }
+    __device__ __forceinline__ static void pixels(const uint32_t (&dw)[kWords], uint32_t (&px)[16]) { Walk16Tma<CHANS>::pixels(dw, px); }
+    __device__ __forceinline__ void bind(const uint8_t* cur, const uint8_t* prev) { cur_ = cur; prev_ = prev; }
+    __device__ __forceinline__ void planes(size_t chan_stride) { cs_ = chan_stride; }
+    const uint8_t* cur_ = nullptr; const uint8_t* prev_ = nullptr; size_t cs_ = 0;
+};
+
 // RGB: linear TMA tile (48-byte lane stride is bank-conflict free for 128-bit reads); RGBA: padded cp.async tile.
 template <int CHANS> struct Walk16Select { using type = Walk16Tma<CHANS>; };
 template <> struct Walk16Select<4> { using type = Walk16Padded<4>; };

@@ -71,6 +71,29 @@ FPNGB_API int fpngb_encode_batch_device(const void* d_pixels, size_t image_strid
                                         uint32_t w, uint32_t h, uint32_t chans, uint32_t flags,
                                         void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream);
 
+/* ---- Pixel layouts of the *_strided device calls ------------------------------------------------------------------------
+ * A batch is an [n, h, w, chans] array of bytes given by a base pointer and four BYTE strides, as a torch tensor reports them:
+ * byte (i, y, x, c) is at base + i*image_stride + y*row_pitch + x*pixel_stride + c*chan_stride.  Two layouts are supported:
+ *   interleaved: pixel_stride == chans, chan_stride == 1 (HWC rows at any pitch: crops, tiles, padded rows);
+ *   planar:      pixel_stride == 1, chan_stride >= 1 (CHW: chan_stride = h*w, row_pitch = w; HCW fits too).
+ * The stride of a dimension of size 1 is ignored (w == 1 is interleaved when chan_stride == 1, planar otherwise).  Anything else,
+ * such as an RGB view of RGBA pixels (pixel_stride 4, chans 3), and a layout whose last byte overflows the address space, give
+ * FPNGB_ERR_INVALID_ARG.  Strides are unsigned: no negative strides.
+ *   Encode inputs are only read, so they may overlap (stride 0 for a broadcast batch, tiles whose rows interleave); the row
+ *   pitch must be below 2^32.
+ *   Decode outputs must not overlap: with the dimensions of size > 1 ordered by stride, each stride is at least the span of
+ *   the dimensions below it plus one (stride_k >= sum_{j<k} stride_j * (size_j - 1) + 1).
+ * A rejected call enqueues nothing and writes nothing. */
+
+/* fpngb_encode_batch_device with the input in any layout of "Pixel layouts" above: d_pixels and the four strides describe
+ * the [n, h, w, chans] batch; everything else as fpngb_encode_batch_device, with the same output bytes as for a tightly packed
+ * copy.  The scan and pack kernels read interleaved rows at any pitch and planar images in place; where the batch would
+ * go to the generic kernels (a trained RGBA table whose one-pixel-match rule can fire, FPNGB_FORCE_GENERIC) or to the opt-in
+ * single-pass encoder, it is first copied into the library's workspace by one extra kernel. */
+FPNGB_API int fpngb_encode_batch_device_strided(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride,
+                                                size_t chan_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags,
+                                                void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream);
+
 /* Batch of n equally sized images in HOST memory (ideally pinned: see fpngb_host_alloc) -> n files in host memory,
  * out + i*out_stride, sizes[i].  Internally pipelines H2D copy / kernels / D2H copy over chunks of the batch. */
 FPNGB_API int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
@@ -97,6 +120,14 @@ FPNGB_API int fpngb_decode_batch_device(const void* d_files, size_t file_stride,
                                         const uint32_t* idat_ofs, const uint32_t* idat_len, uint32_t n,
                                         uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans,
                                         void* d_out, size_t out_stride, uint32_t* d_status, void* stream);
+/* fpngb_decode_batch_device writing the pixels in any non-overlapping layout of "Pixel layouts" above (chans = desired_chans):
+ * pixel (i, y, x, c) of file i at d_out + i*out_image_stride + y*out_row_pitch + x*out_pixel_stride + c*out_chan_stride.
+ * Failed files leave their pixels untouched, as in fpngb_decode_batch_device. */
+FPNGB_API int fpngb_decode_batch_device_strided(const void* d_files, size_t file_stride, const uint32_t* file_sizes,
+                                                const uint32_t* idat_ofs, const uint32_t* idat_len, uint32_t n,
+                                                uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans,
+                                                void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                                size_t out_pixel_stride, size_t out_chan_stride, uint32_t* d_status, void* stream);
 
 /* Batch of n fpng files in HOST memory (files[i], sizes[i]; ideally pinned) -> pixels in host memory at out + i*out_stride.
  * Container walk per file on the host (src/fpng.cpp:2930-3077), then H2D / decode kernels / D2H pipelined over chunks.
@@ -139,6 +170,12 @@ FPNGB_API int fpngb_get_info_batch_device(const void* d_base, const uint64_t* d_
 FPNGB_API int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                          uint32_t max_file_size, uint32_t w, uint32_t h, uint32_t chans_in_file,
                                          uint32_t desired_chans, void* d_out, size_t out_stride, int32_t* d_status, void* stream);
+/* fpngb_decode_packed_device writing the pixels in any non-overlapping layout of "Pixel layouts" above, as
+ * fpngb_decode_batch_device_strided. */
+FPNGB_API int fpngb_decode_packed_device_strided(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                                 uint32_t max_file_size, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                                                 uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                                 size_t out_pixel_stride, size_t out_chan_stride, int32_t* d_status, void* stream);
 
 /* Replace fpng::fpng_crc32 / fpng::fpng_adler32 (src/fpng.h:26-31).  Host buffers.  Buffers of 4 KiB and more are
  * checksummed by the device kernels.  NOTE (the one host-side arithmetic in this library): shorter buffers, and any
