@@ -64,6 +64,9 @@ def lib() -> C.CDLL:
     L.fpngb_decode_packed_device_strided.restype = C.c_int
     L.fpngb_decode_packed_device_strided.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p] + [C.c_uint32] * 6 + [C.c_void_p] + \
         [C.c_size_t] * 4 + [C.c_void_p, C.c_void_p]
+    L.fpngb_decode_packed_ragged_device.restype = C.c_int
+    L.fpngb_decode_packed_ragged_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p] + [C.c_uint32] * 5 + \
+        [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.fpngb_compact_batch_device.restype = C.c_int
     L.fpngb_compact_batch_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.fpngb_decode_batch_host.restype = C.c_int

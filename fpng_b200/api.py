@@ -320,6 +320,88 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
     return out, status
 
 
+FPNGB_DECODE_OUT_OF_SPACE = 101    # decode_packed_ragged_device only: the file's pixels do not fit in `out`
+
+
+def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h, stream):
+    """The bounds of decode_packed_ragged_device the caller left out, and the exact output size they give: one device walk
+    (get_info_batch_device) and one read-back of (info, sizes, offsets), which synchronises with the stream."""
+    import torch
+
+    info = get_info_batch_device(data, offsets, sizes, stream)
+    if stream is not None:
+        torch.cuda.ExternalStream(stream, device=data.device).synchronize()
+    t = torch.cat([info.long(), (sizes.long() & 0xFFFFFFFF)[:, None], offsets[:n, None]], 1).cpu().numpy()
+    st, w, h, size, ofs = t[:, 0], t[:, 1], t[:, 2], t[:, 6], t[:, 7]
+    walked = st == 0
+    if max_file_size is None:
+        max_file_size = int(size[walked].max()) if walked.any() else 1
+    if max_w is None:
+        max_w = int(w[walked].max()) if walked.any() else 1
+    if max_h is None:
+        max_h = int(h[walked].max()) if walked.any() else 1
+    px = w * h * desired_channels
+    placed = (walked & (size <= max_file_size) & (ofs % 4 == 0) & (ofs + size <= data.numel()) & (w <= max_w) & (h <= max_h)
+              & (px <= 0xFFFFFFFF))
+    total = int(((px[placed] + 15) // 16 * 16).sum())
+    return max_file_size, max_w, max_h, total
+
+
+def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out=None, max_file_size=None, max_w=None, max_h=None,
+                                stream=None):
+    """Decode fpng files of ANY shapes and channel counts packed in device memory (the layout of get_info_batch_device; base_bytes
+    is data.numel()) in one call, pixels placed back to back.  Returns (out uint8 [out_cap], out_offsets int64 [n + 1],
+    info int32 [n, 6], status int32 [n]):
+      * file i's pixels are the h*w*desired_channels bytes at out[out_offsets[i]:], tight HWC rows (ragged_views cuts them out);
+        every decodable file takes its size rounded up to 16 bytes, in index order; out_offsets[n] is the total, with bit 63 set
+        (a negative value) when it exceeds out.numel(), and a file that does not fit gets FPNGB_DECODE_OUT_OF_SPACE;
+      * info[i] is get_info_batch_device's row for file i ({FPNG_DECODE_INVALID_ARG, 0, ...} when its arguments fail);
+      * status[i] is fpng_decode_memory's code, FPNG_DECODE_INVALID_ARG for size 0, size > max_file_size, offset % 4 != 0 or a
+        file that runs past the end of data, FPNGB_DECODE_SHAPE_MISMATCH for a valid file wider than max_w or taller than
+        max_h, or FPNGB_DECODE_OUT_OF_SPACE.  Bytes of out outside the decoded files are left untouched.
+    With `out` (a flat, 16-byte aligned uint8 CUDA tensor) and all three bounds given, the call is stream-ordered: no host
+    synchronisation.  Any of them that is None is computed from one get_info_batch_device and one read-back to the host, which
+    waits for the stream: max_file_size, max_w and max_h become the largest size, width and height of the files the container
+    walk accepts, and out is allocated at the exact total.  Tight bounds save workspace and launch overhead."""
+    import torch
+
+    n = _packed_args(data, offsets, sizes)
+    assert desired_channels in (3, 4), "desired_channels: 3 or 4"
+    if out is None or max_file_size is None or max_w is None or max_h is None:
+        max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
+                                                             stream)
+        if out is None:
+            out = torch.empty((max(total, 16),), dtype=torch.uint8, device=data.device)[:total]
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous(), "out: flat uint8 CUDA tensor"
+    out_offsets = torch.empty((n + 1,), dtype=torch.int64, device=data.device)
+    info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
+    status = torch.empty((n,), dtype=torch.int32, device=data.device)
+    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    rc = lib().fpngb_decode_packed_ragged_device(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n,
+                                                 min(int(max_file_size), 0xFFFFFFFF), int(max_w), int(max_h), desired_channels,
+                                                 out.data_ptr(), out.numel(), out_offsets.data_ptr(), info.data_ptr(),
+                                                 status.data_ptr(), s)
+    check(rc, "decode_packed_ragged_device")
+    return out, out_offsets, info, status
+
+
+def ragged_views(out, out_offsets, info, status, desired_channels: int):
+    """Per file of a decode_packed_ragged_device result, an [h, w, desired_channels] view into `out`, or None when the file's
+    status is not 0.  Reads out_offsets, info and status back to the host, so it waits for the device."""
+    offs = out_offsets.cpu().numpy()
+    inf = info.cpu().numpy()
+    st = status.cpu().numpy()
+    views = []
+    for i in range(st.shape[0]):
+        if st[i] != 0:
+            views.append(None)
+            continue
+        w, h = int(inf[i, 1]), int(inf[i, 2])
+        o = int(offs[i])
+        views.append(out[o:o + h * w * desired_channels].view(h, w, desired_channels))
+    return views
+
+
 def decode_batch_host(file_ptrs, sizes, desired_channels: int, out, out_stride: int):
     """Pipelined host-buffer batch decode (fpngb_decode_batch_host).  file_ptrs: array of host addresses (uint64), sizes:
     uint32 array, out: host buffer (numpy uint8 / pinned torch tensor) with out_stride bytes per image.

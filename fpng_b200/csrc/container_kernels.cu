@@ -37,8 +37,12 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
     if (i >= p.n) return;
     const unsigned long long ofs = p.offsets[i];
     const uint32_t size = p.sizes[i];
+    const bool ragged = p.files && !p.chans;
+    // argument checks: size 0 (fpng.cpp:3092-3096), and for the packed decodes the workspace bound and the alignment of the
+    // decode kernels' word reads; the ragged call also keeps every file inside the buffer and walks only files that pass
+    const bool bad_arg = !size || (p.files && (size > p.max_file_size || (ofs & 3ull) || (ragged && (ofs > p.base_bytes || size > p.base_bytes - ofs))));
     uint32_t st, w = 0, h = 0, c = 0, io = 0, il = 0;
-    if (!size) st = FPNGB_DECODE_INVALID_ARG;                                            // fpng.cpp:3092-3096
+    if (!size || (ragged && bad_arg)) st = FPNGB_DECODE_INVALID_ARG;
     else st = container_walk(p.base + ofs, size, DeviceCrc{}, &w, &h, &c, &io, &il);
     if (p.info) {
         uint32_t* o = p.info + (size_t)i * 6;
@@ -46,11 +50,21 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
     }
     if (p.files) {
         // argument checks first, then the walk's code, then the call's shape
-        uint32_t pre = st;
-        if (!size || size > p.max_file_size || (ofs & 3ull)) pre = FPNGB_DECODE_INVALID_ARG;
-        else if (!pre && (w != p.w || h != p.h || c != p.chans)) pre = FPNGB_DECODE_SHAPE_MISMATCH;
+        uint32_t pre = bad_arg ? (uint32_t)FPNGB_DECODE_INVALID_ARG : st;
+        if (!pre && ragged) {
+            if (w > p.w || h > p.h) pre = FPNGB_DECODE_SHAPE_MISMATCH;
+            else if ((unsigned long long)w * h * p.desired > 0xFFFFFFFFull) pre = FPNGB_DECODE_FAILED_DIMENSIONS_TOO_LARGE;   // fpng.cpp:3103-3105
+        } else if (!pre && (w != p.w || h != p.h || c != p.chans)) pre = FPNGB_DECODE_SHAPE_MISMATCH;
         FileDesc fd;
         fd.base = ofs; fd.file_size = size; fd.idat_ofs = pre ? 0u : io; fd.idat_len = pre ? 0u : il; fd.pre_status = pre;
+        if (ragged) {
+            fd.w = w; fd.h = h; fd.chans = c; fd.pitch = delta_pitch(w, c);
+            fd.delta_base = 0; fd.out_base = 0; fd.sub_base = 0;                 // decode_place_kernel
+        } else {
+            fd.w = p.w; fd.h = p.h; fd.chans = p.chans; fd.pitch = delta_pitch(p.w, p.chans);
+            fd.delta_base = (unsigned long long)i * fd.pitch * p.h; fd.out_base = i * p.out_stride;
+            fd.sub_base = (unsigned long long)i * subs_for(p.max_file_size);
+        }
         p.files[i] = fd;
     }
 }
@@ -58,6 +72,66 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
 void launch_container_walk(const WalkParams& p, cudaStream_t s)
 {
     container_walk_kernel<<<(p.n + 127) / 128, 128, 0, s>>>(p);
+}
+
+// One CTA: exclusive scans of the output bytes, delta bytes and records of the accepted files, kPlaceThreads files per round.
+constexpr uint32_t kPlaceThreads = 1024;
+__global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams p)
+{
+    __shared__ unsigned long long s_warp[3][kPlaceThreads / 32];
+    __shared__ unsigned long long s_carry[3];
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    if (tid < 3) s_carry[tid] = 0;
+    for (uint32_t first = 0; first < p.n; first += kPlaceThreads) {
+        const uint32_t i = first + tid;
+        FileDesc fd{};
+        bool placed = false;
+        if (i < p.n) { fd = p.files[i]; placed = fd.pre_status == 0; }
+        unsigned long long v[3] = {0ull, 0ull, 0ull};
+        if (placed) {
+            v[0] = ((unsigned long long)fd.w * fd.h * p.desired + 15ull) & ~15ull;
+            v[1] = (unsigned long long)fd.h * fd.pitch;
+            v[2] = subs_for(fd.file_size);
+        }
+        unsigned long long x[3];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {                      // inclusive warp scan, then the warp totals
+            x[k] = v[k];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, x[k], o); if (lane >= (uint32_t)o) x[k] += u; }
+            if (lane == 31) s_warp[k][warp] = x[k];
+        }
+        __syncthreads();
+        if (warp == 0) {                                   // exclusive scan of the warp totals, carry of the earlier rounds in front
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                unsigned long long t = s_warp[k][lane];
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, t, o); if (lane >= (uint32_t)o) t += u; }
+                s_warp[k][lane] = s_carry[k] + t - s_warp[k][lane];
+            }
+        }
+        __syncthreads();
+        unsigned long long at[3];
+#pragma unroll
+        for (int k = 0; k < 3; k++) at[k] = s_warp[k][warp] + x[k] - v[k];
+        if (i < p.n) {
+            p.out_offsets[i] = at[0];
+            if (placed) {
+                FileDesc* d = p.files + i;
+                if (at[0] + v[0] > p.out_cap || at[1] + v[1] > p.delta_cap || at[2] + v[2] > p.sub_cap) d->pre_status = FPNGB_DECODE_OUT_OF_SPACE;
+                else { d->out_base = at[0]; d->delta_base = at[1]; d->sub_base = at[2]; }
+            }
+        }
+        if (tid == kPlaceThreads - 1) for (int k = 0; k < 3; k++) s_carry[k] = at[k] + v[k];
+        __syncthreads();
+    }
+    if (tid == 0) p.out_offsets[p.n] = s_carry[0] | (s_carry[0] > p.out_cap ? 1ull << 63 : 0ull);
+}
+
+void launch_decode_place(const PlaceParams& p, cudaStream_t s)
+{
+    decode_place_kernel<<<1, kPlaceThreads, 0, s>>>(p);
 }
 
 }  // namespace fpngb

@@ -21,9 +21,19 @@ struct SubInfo {
 struct FileDesc {                           // filled by the container walk (fpng.cpp:2930-3077), on the host or by container_walk_kernel
     unsigned long long base;                // byte offset of the file from DecodeParams::d_files (a multiple of 4)
     uint32_t file_size, idat_ofs, idat_len;
-    uint32_t pre_status;                    // != 0: the file failed before decoding (FPNG_DECODE_* / FPNGB_DECODE_SHAPE_MISMATCH);
-                                            // no kernel reads its bytes and decode_status_kernel reports this code
+    uint32_t pre_status;                    // != 0: the file failed before decoding (FPNG_DECODE_* / FPNGB_DECODE_SHAPE_MISMATCH /
+                                            // FPNGB_DECODE_OUT_OF_SPACE); no kernel reads its bytes and decode_status_kernel reports this code
+    uint32_t w, h, chans;                   // the file's shape: the call's for the uniform calls, the walk's for the ragged call
+    uint32_t pitch;                         // bytes per delta row, delta_pitch(w, chans)
+    unsigned long long delta_base;          // byte offset of the file's delta rows from DecodeParams::delta (a multiple of 16)
+    unsigned long long out_base;            // byte offset of the file's pixel (0, 0, 0) from DecodeParams::d_out
+    unsigned long long sub_base;            // index of the file's first record in DecodeParams::subs
 };
+static_assert(sizeof(FileDesc) == 64, "FileDesc: one 64-byte record per file");
+
+// delta row pitch of a w x chans file, and the number of SubInfo records a file whose IDAT chunk is at most `bytes` long may use
+__host__ __device__ __forceinline__ uint32_t delta_pitch(uint32_t w, uint32_t chans) { return (w * chans + 15u) & ~15u; }
+__host__ __device__ __forceinline__ uint32_t subs_for(uint32_t bytes) { return (uint32_t)(((uint64_t)bytes * 8 + 32) / kSubBits + 2); }
 
 struct DecodeState {
     uint32_t status;                        // 0 ok, 1 -> FPNG_DECODE_NOT_FPNG
@@ -37,21 +47,23 @@ constexpr uint32_t kFastWords = 4096 + 64;   // 4096 fast entries, then the 256 
 
 struct DecodeParams {
     const uint8_t* d_files;                 // file f starts at d_files + files[f].base
-    const FileDesc* files;                  // [n] device
+    const FileDesc* files;                  // [n] device; shape and workspace bases of every file
     DecodeState* state;                     // [n]
     uint32_t* luts;                         // [n][4096]  fused entries, see decode_kernels.cu
     uint32_t* fast;                         // [n][kFastWords]  multi-token entries + literal code sizes of the scan / write loops
-    SubInfo* subs; uint32_t subs_per_file;  // [n][subs_per_file]
-    uint8_t* delta; uint32_t delta_pitch;   // [n][h][pitch] filtered rows without the filter byte
-    uint8_t* d_out; size_t out_stride;     // pixel (f, y, x, c) at d_out + f*out_stride + y*OutStrides::row + x*OutStrides::pixel + c*OutStrides::chan
+    SubInfo* subs;                          // file f: subs + files[f].sub_base, subs_for(idat_len) records at most
+    uint8_t* delta;                         // file f: h rows of files[f].pitch bytes at delta + files[f].delta_base (filter byte dropped)
+    uint8_t* d_out;                         // pixel (f, y, x, c) at d_out + files[f].out_base + y*row + x*OutStrides::pixel + c*OutStrides::chan
     uint32_t* d_status;                     // [n] FPNG_DECODE_* codes
-    uint32_t w, h, chans;
+    uint32_t max_w, max_h, max_subs;        // launch grids: bounds of every file's w, h and subs_for(idat_len)
+    uint32_t chans;                         // channels of every file (3 or 4), or 0 when the call mixes both
     uint32_t pre_roll;                      // speculative lead-in bits of decode_scan_kernel, 0..kPreRoll (kPreRoll unless a test sets it)
 };
 
 // the rest of the output layout of the decode (unfilter_kernel's second argument; kept out of DecodeParams, which every decode kernel takes)
 struct OutStrides {
-    size_t row, pixel, chan;                // interleaved (pixel = desired, chan = 1) or planar (pixel = 1)
+    size_t row, pixel, chan;                // interleaved (pixel = desired, chan = 1) or planar (pixel = 1); row 0: tight rows of each
+                                            // file's own width (w * desired, the ragged call)
 };
 void launch_decode(const DecodeParams& p, const OutStrides& out, uint32_t n, uint32_t desired, cudaStream_t s);
 void decode_profile_enable(bool on);
@@ -63,13 +75,32 @@ bool decode_set_pre_roll(uint32_t bits);    // DecodeParams::pre_roll of later c
 // container_walk_kernel (container_kernels.cu): one thread per file of a packed buffer (d_base + offsets[i], sizes[i] bytes).
 // info != nullptr: the six values of fpngb_get_info_ex per file, {status, w, h, chans, idat_ofs, idat_len}.
 // files != nullptr: the FileDesc of the packed decode; pre_status holds the argument checks (size 0, size > max_file_size,
-// offset % 4), the walk's code, or FPNGB_DECODE_SHAPE_MISMATCH when a valid file is not w x h x chans.
+// offset % 4, and for the ragged call offset + size > base_bytes), the walk's code, then the shape check:
+//   uniform call (chans != 0): FPNGB_DECODE_SHAPE_MISMATCH when a valid file is not w x h x chans; the workspace bases are
+//     i * (h * delta_pitch(w, chans)), i * out_stride and i * subs_for(max_file_size);
+//   ragged call (chans == 0): the walk runs only when the argument checks pass; FPNGB_DECODE_SHAPE_MISMATCH when the file is
+//     wider than w or taller than h, FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE when w * h * desired > 0xFFFFFFFF; the bases are
+//     set by decode_place_kernel.
 struct WalkParams {
     const uint8_t* base; const unsigned long long* offsets; const uint32_t* sizes; uint32_t n;
     uint32_t* info;                         // [n][6] or nullptr
     FileDesc* files;                        // [n] or nullptr
     uint32_t max_file_size, w, h, chans;    // checks of the `files` output
+    uint32_t desired;                       // ragged call: output channels
+    unsigned long long base_bytes;          // ragged call: length of the buffer behind base
+    unsigned long long out_stride;          // uniform call: output bytes per file
 };
 void launch_container_walk(const WalkParams& p, cudaStream_t s);
+
+// decode_place_kernel (container_kernels.cu), ragged call: one CTA places the files the walk accepted, in index order.  File i
+// takes align_up(w*h*desired, 16) output bytes, h * pitch delta bytes and subs_for(file_size) records; out_offsets[i] is the
+// running output offset (a rejected file takes nothing), out_offsets[n] the total, with bit 63 set when it exceeds out_cap.
+// A file whose output, delta rows or records end past out_cap / delta_cap / sub_cap gets FPNGB_DECODE_OUT_OF_SPACE.
+struct PlaceParams {
+    FileDesc* files; uint32_t n, desired;
+    unsigned long long out_cap, delta_cap, sub_cap;
+    unsigned long long* out_offsets;        // [n + 1]
+};
+void launch_decode_place(const PlaceParams& p, cudaStream_t s);
 
 }  // namespace fpngb

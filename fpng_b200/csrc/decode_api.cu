@@ -13,33 +13,40 @@ namespace fpngb {
 static Buffer g_dec_ws;        // FileDesc[n] | DecodeState[n] | luts | delta scratch
 static Buffer g_dec_pin;       // pinned staging for the FileDesc upload / status download
 
-// Reserves the workspace of a decode call for n files whose IDAT chunks are at most max_idat bytes, orders it after the
-// previous call's kernels, and points p's workspace fields into it (p.files included).  Caller holds context().mu.
-static int decode_workspace_locked(uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t max_idat, cudaStream_t s, DecodeParams& p)
+// Reserves the workspace of a decode call for n files, n_subs SubInfo records and delta_bytes of delta rows in all, orders it
+// after the previous call's kernels, and points p's workspace fields into it (p.files included).  Caller holds context().mu.
+static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes, cudaStream_t s, DecodeParams& p)
 {
-    const uint32_t bpl = w * chans, pitch = (uint32_t)align_up(bpl, 16);
     size_t o = 0;
     const size_t o_files = o; o = align_up(o + (size_t)n * sizeof(FileDesc), 256);
     const size_t o_state = o; o = align_up(o + (size_t)n * sizeof(DecodeState), 256);
     const size_t o_luts = o; o = align_up(o + (size_t)n * 4096 * 4, 256);
     const size_t o_fast = o; o = align_up(o + (size_t)n * kFastWords * 4, 256);
-    const uint32_t subs_per_file = (uint32_t)(((uint64_t)max_idat * 8 + 32) / kSubBits + 2);
-    const size_t o_subs = o; o = align_up(o + (size_t)n * subs_per_file * sizeof(SubInfo), 256);
-    const size_t o_delta = o; o = align_up(o + (size_t)n * pitch * h + 64, 256);
+    const size_t o_subs = o; o = align_up(o + n_subs * sizeof(SubInfo), 256);
+    const size_t o_delta = o; o = align_up(o + delta_bytes + 64, 256);
     int rc = g_dec_ws.reserve(o); if (rc) return rc;
     rc = context().ws_acquire(s); if (rc) return rc;
     uint8_t* b = (uint8_t*)g_dec_ws.p;
     p.files = (const FileDesc*)(b + o_files); p.state = (DecodeState*)(b + o_state);
-    p.luts = (uint32_t*)(b + o_luts); p.fast = (uint32_t*)(b + o_fast); p.subs = (SubInfo*)(b + o_subs); p.subs_per_file = subs_per_file;
-    p.delta = b + o_delta; p.delta_pitch = pitch;
-    p.w = w; p.h = h; p.chans = chans;
+    p.luts = (uint32_t*)(b + o_luts); p.fast = (uint32_t*)(b + o_fast); p.subs = (SubInfo*)(b + o_subs);
+    p.delta = b + o_delta;
+    return 0;
+}
+// The same for n files of one shape whose IDAT chunks are at most max_idat bytes: file i's records and delta rows at i times the
+// per-file share (the bases the uniform calls put in FileDesc), and the launch grids of that shape.
+static int decode_workspace_uniform_locked(uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t max_idat, cudaStream_t s,
+                                           DecodeParams& p)
+{
+    const int rc = decode_workspace_locked(n, (size_t)n * subs_for(max_idat), (size_t)n * delta_pitch(w, chans) * h, s, p);
+    if (rc) return rc;
+    p.max_w = w; p.max_h = h; p.max_subs = subs_for(max_idat); p.chans = chans;
     return 0;
 }
 
 // Output layout of a decode call (layout.h): pixel (i, y, x, c) at d_out + i*image + y*row + x*pixel + c*chan.
 static OutStrides set_output(DecodeParams& p, uint8_t* d_out, const Layout& L)
 {
-    p.d_out = d_out; p.out_stride = L.image;
+    p.d_out = d_out;
     return OutStrides{L.row, L.pixel, L.chan};
 }
 static Layout tight_output(uint32_t w, uint32_t h, uint32_t desired, size_t out_stride)
@@ -75,7 +82,7 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     uint32_t max_idat = 0;
     for (uint32_t i = 0; i < n; i++) if (h_files[i].idat_len > max_idat) max_idat = h_files[i].idat_len;
     DecodeParams p{};
-    int rc = decode_workspace_locked(n, w, h, chans, max_idat, s, p); if (rc) return rc;
+    int rc = decode_workspace_uniform_locked(n, w, h, chans, max_idat, s, p); if (rc) return rc;
     g_dec_pin.pinned = true;
     rc = g_dec_pin.reserve((size_t)n * sizeof(FileDesc)); if (rc) return rc;
     // the pinned staging buffer may still be in flight from the previous call on another stream: wait for it
@@ -83,7 +90,12 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     if (!staged) FPNGB_CUDA_OK(cudaEventCreateWithFlags(&staged, cudaEventDisableTiming));
     else FPNGB_CUDA_OK(cudaEventSynchronize(staged));
     FileDesc* staging = (FileDesc*)g_dec_pin.p;
-    for (uint32_t i = 0; i < n; i++) { staging[i] = h_files[i]; staging[i].base = (unsigned long long)i * file_stride; staging[i].pre_status = 0; }
+    for (uint32_t i = 0; i < n; i++) {
+        FileDesc& fd = staging[i];
+        fd = h_files[i]; fd.base = (unsigned long long)i * file_stride; fd.pre_status = 0;
+        fd.w = w; fd.h = h; fd.chans = chans; fd.pitch = delta_pitch(w, chans);
+        fd.delta_base = (unsigned long long)i * fd.pitch * h; fd.out_base = (unsigned long long)i * out.image; fd.sub_base = (unsigned long long)i * p.max_subs;
+    }
     FPNGB_CUDA_OK(cudaMemcpyAsync((void*)p.files, g_dec_pin.p, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
     FPNGB_CUDA_OK(cudaEventRecord(staged, s));
     p.d_files = d_files; p.d_status = d_status;
@@ -123,7 +135,7 @@ int fpngb_decode_batch_device_strided(const void* d_files, size_t file_stride, c
     std::vector<FileDesc> fds(n);
     for (uint32_t i = 0; i < n; i++) {
         if ((uint64_t)idat_ofs[i] + 8 + idat_len[i] + 4 > file_sizes[i] || file_sizes[i] > file_stride) return FPNGB_ERR_INVALID_ARG;
-        fds[i] = FileDesc{0, file_sizes[i], idat_ofs[i], idat_len[i], 0};
+        fds[i] = FileDesc{}; fds[i].file_size = file_sizes[i]; fds[i].idat_ofs = idat_ofs[i]; fds[i].idat_len = idat_len[i];
     }
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
@@ -163,7 +175,7 @@ int fpngb_decode_host(const void* file, uint32_t size, void* out, size_t out_cap
     uint32_t* d_status = (uint32_t*)((uint8_t*)c.dev_out.p + align_up(need, 16));
     cudaStream_t s = c.stream;
     cudaMemcpyAsync(c.dev_in.p, file, size, cudaMemcpyHostToDevice, s);
-    FileDesc fd{0, size, idat_ofs, idat_len, 0};
+    FileDesc fd{}; fd.file_size = size; fd.idat_ofs = idat_ofs; fd.idat_len = idat_len;
     if (decode_batch_locked((const uint8_t*)c.dev_in.p, fstride, &fd, 1, ww, hh, cc, desired, (uint8_t*)c.dev_out.p,
                             tight_output(ww, hh, desired, align_up(need, 16)), d_status, s))
         return FPNGB_DECODE_INVALID_ARG;
@@ -199,7 +211,7 @@ int fpngb_decode_batch_host(const void* const* files, const uint32_t* sizes, uin
     for (uint32_t i = 0; i < n; i++) {
         uint32_t ww = 0, hh = 0, cc = 0, io = 0, il = 0;
         status[i] = (!files[i] || !sizes[i]) ? FPNGB_DECODE_INVALID_ARG : container_info((const uint8_t*)files[i], sizes[i], &ww, &hh, &cc, &io, &il);
-        fds[i] = FileDesc{0, sizes[i], io, il, 0};
+        fds[i] = FileDesc{}; fds[i].file_size = sizes[i]; fds[i].idat_ofs = io; fds[i].idat_len = il;
         if (status[i]) continue;
         if (!W) { W = ww; H = hh; C = cc; }
         else if (ww != W || hh != H || cc != C) return FPNGB_ERR_INVALID_ARG;
@@ -320,10 +332,11 @@ int fpngb_decode_packed_device_strided(const void* d_base, const uint64_t* d_off
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     // an IDAT chunk is shorter than its file: max_file_size bounds the stream of every file that reaches the decode kernels
     DecodeParams p{};
-    rc = decode_workspace_locked(n, w, h, chans_in_file, max_file_size, s, p); if (rc) return rc;
+    rc = decode_workspace_uniform_locked(n, w, h, chans_in_file, max_file_size, s, p); if (rc) return rc;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = w; wp.h = h; wp.chans = chans_in_file;
+    wp.out_stride = out.image;
     launch_container_walk(wp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status;
     launch_decode(p, set_output(p, (uint8_t*)d_out, out), n, desired_chans, s);
@@ -342,6 +355,62 @@ int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, co
     if (out_stride < (size_t)w * h * desired_chans) return FPNGB_ERR_BUFFER_TOO_SMALL;
     return fpngb_decode_packed_device_strided(d_base, d_offsets, d_sizes, n, max_file_size, w, h, chans_in_file, desired_chans, d_out, out_stride,
                                               (size_t)w * desired_chans, desired_chans, 1, d_status, stream);
+}
+
+// Workspace of the ragged call, from call arguments only (no host synchronisation).  Only files decode_place_kernel places and
+// that fit in out_cap are decoded; they are a prefix of the placed files, so for every one of them the sums below run over
+// decoded files alone.
+//   records:   subs_for(s) <= s/128 + 3 per file of s bytes; files that lie inside the buffer and do not overlap have sizes that
+//              sum to at most base_bytes, so base_bytes/128 + 3n records hold them all.  Every file also has s <= max_file_size.
+//   delta:     a file needs h * align_up(w*c, 16) <= (4/desired) * (w*h*desired) + 15h bytes, h <= max_h and h <= w*h, and the
+//              w*h*desired of the decoded files sum to at most out_cap.  Every file also needs at most max_h * pitch(max_w, 4).
+// A file whose range still ends past a bound (overlapping files) gets FPNGB_DECODE_OUT_OF_SPACE from decode_place_kernel.
+static unsigned long long sat_u64(unsigned __int128 v) { return v > ~0ull ? ~0ull : (unsigned long long)v; }
+static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired,
+                             size_t out_cap, unsigned long long& sub_cap, unsigned long long& delta_cap)
+{
+    typedef unsigned __int128 u128;
+    const u128 by_bytes = (u128)base_bytes / 128 + 3 * (u128)n, by_max = (u128)n * subs_for(max_file_size);
+    sub_cap = sat_u64(by_bytes < by_max ? by_bytes : by_max);
+    const u128 rows = (u128)n * max_h, rows_px = ((u128)out_cap + desired - 1) / desired;
+    const u128 by_out = ((u128)out_cap * 4 + desired - 1) / desired + 16 * (rows < rows_px ? rows : rows_px);
+    const u128 by_shape = rows * delta_pitch(max_w, 4);
+    delta_cap = sat_u64(by_out < by_shape ? by_out : by_shape);
+}
+
+int fpngb_decode_packed_ragged_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
+                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, int32_t* d_status, void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_out_offsets || !d_status || n == 0 || n > 65535 || !max_file_size ||
+        (desired_chans != 3 && desired_chans != 4) || !max_w || !max_h || max_w > (1u << 24) || max_h > (1u << 24))
+        return FPNGB_ERR_INVALID_ARG;
+    if ((uintptr_t)d_base % 4 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    unsigned long long sub_cap = 0, delta_cap = 0;
+    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap, sub_cap, delta_cap);
+    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    const cudaStream_t s = (cudaStream_t)stream;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    DecodeParams p{};
+    int rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p); if (rc) return rc;
+    p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
+    WalkParams wp{};
+    wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
+    wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
+    wp.base_bytes = base_bytes;
+    launch_container_walk(wp, s);
+    PlaceParams pp{};
+    pp.files = (FileDesc*)p.files; pp.n = n; pp.desired = desired_chans;
+    pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
+    launch_decode_place(pp, s);
+    p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
+    launch_decode(p, OutStrides{0, desired_chans, 1}, n, desired_chans, s);
+    count_launch(11);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return context().ws_release(s);
 }
 
 }  // extern "C"

@@ -170,8 +170,8 @@ __global__ void __launch_bounds__(32) decode_prepare_kernel(DecodeParams p)
         for (uint32_t i = 0; i < ndist && !fail; i++) ones += s_sizes[nlit + i] == 1;
         if (!fail) {
             if (ones < 1 || ones > 2) fail = 1;
-            else if (s_sizes[nlit + p.chans - 1] != 1) fail = 1;
-            else if (ones == 2 && s_sizes[nlit + p.chans] != 1) fail = 1;
+            else if (s_sizes[nlit + fd.chans - 1] != 1) fail = 1;
+            else if (ones == 2 && s_sizes[nlit + fd.chans] != 1) fail = 1;
         }
         for (uint32_t i = nlit; i < 288; i++) s_sizes[i] = 0;
         s_fail = fail;
@@ -739,7 +739,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_scan_kernel(DecodeParams p
     stage_wait();
     if (g > sp.g1) return;
     const uint32_t* lutg = p.luts + (size_t)f * 4096;
-    SubInfo* info = p.subs + (size_t)f * p.subs_per_file + (g - sp.g0);
+    SubInfo* info = p.subs + fd.sub_base + (g - sp.g0);
     const unsigned long long lo_abs = g * kSubBits;
     SubScan r;
     unsigned long long origin;
@@ -784,9 +784,9 @@ __global__ void __launch_bounds__(kLinkThreads) decode_link_kernel(DecodeParams 
     const FileDesc fd = p.files[f];
     const Stream sm = open_stream(p.d_files + fd.base, fd);
     const FileSpan sp = file_span(st, sm, fd);
-    const uint32_t chans = p.chans, bpl = p.w * chans, h = p.h;
+    const uint32_t chans = fd.chans, bpl = fd.w * chans, h = fd.h;
     const unsigned long long total_out = (unsigned long long)(bpl + 1) * h;
-    SubInfo* subs = p.subs + (size_t)f * p.subs_per_file;
+    SubInfo* subs = p.subs + fd.sub_base;
     const unsigned long long nsub = sp.g1 - sp.g0 + 1ull;
 
     if (tid == 0) { s_carry_start = sp.tok0; s_carry_out = 0; s_carry_litn = 0; s_carry_litv = 0; s_done = 0; s_err = 0; s_eob_end = 0; s_lut_loaded = 0; }
@@ -926,7 +926,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_write_kernel(DecodeParams 
     if (sp.g0 + (unsigned long long)blockIdx.x * kDecThreads > sp.g1) return;
     const unsigned long long g = sp.g0 + (unsigned long long)blockIdx.x * kDecThreads + tid;
     SubInfo in; in.nlit = 0; in.n_out = 0;
-    if (g <= sp.g1) in = p.subs[(size_t)f * p.subs_per_file + (g - sp.g0)];
+    if (g <= sp.g1) in = p.subs[fd.sub_base + (g - sp.g0)];
     // decode_write_staged_kernel ran first and cleared the live flag of everything it wrote (all of it, for literal-dominated files)
     if (!__syncthreads_or(in.nlit && in.n_out)) return;
     stage_fast_table(s_fast, p.fast + (size_t)f * kFastWords);
@@ -935,11 +935,11 @@ __global__ void __launch_bounds__(kDecThreads) decode_write_kernel(DecodeParams 
     const uint32_t* lutg = p.luts + (size_t)f * 4096;
     if (g > sp.g1) return;
     if (!in.nlit || !in.n_out) return;                                           // dead, empty or already written
-    const uint32_t chans = p.chans, bpl = p.w * chans, h = p.h, pitch = p.delta_pitch;
+    const uint32_t chans = fd.chans, bpl = fd.w * chans, h = fd.h, pitch = fd.pitch;
     uint32_t err = 0;
     const unsigned long long hi_abs = (g + 1) * kSubBits;
     if (in.start < hi_abs) {
-        uint8_t* dl = p.delta + (size_t)f * pitch * h;
+        uint8_t* dl = p.delta + fd.delta_base;
         if (chans == 4) decode_write_range<4>(sm, s_fast, lutg, in.start, (uint32_t)(hi_abs - in.start), dl, pitch, bpl, h, in.exit /*out_pos*/, in.lits /*tail*/, &err);
         else decode_write_range<3>(sm, s_fast, lutg, in.start, (uint32_t)(hi_abs - in.start), dl, pitch, bpl, h, in.exit /*out_pos*/, in.lits /*tail*/, &err);
     }
@@ -1120,7 +1120,7 @@ __global__ void __launch_bounds__(kWsThreads) decode_write_staged_kernel(DecodeP
     const unsigned long long first_sub = sp.g0 + (unsigned long long)blockIdx.x * kWsThreads;
     if (first_sub > sp.g1) return;
     const unsigned long long g = first_sub + tid;
-    SubInfo* sub = p.subs + (size_t)f * p.subs_per_file + (g - sp.g0);
+    SubInfo* sub = p.subs + fd.sub_base + (g - sp.g0);
     SubInfo in; in.nlit = 0; in.n_out = 0; in.start = 0; in.exit = 0; in.lits = 0;
     if (g <= sp.g1) in = *sub;
     const unsigned long long hi_abs = (g + 1) * kSubBits;
@@ -1153,7 +1153,7 @@ __global__ void __launch_bounds__(kWsThreads) decode_write_staged_kernel(DecodeP
     if (tid < 8u) s_stage[(uint32_t)((hi - bw) >> 2) + tid] = 0u;
     stage_wait();
 
-    const uint32_t chans = p.chans, bpl = p.w * chans, h = p.h, pitch = p.delta_pitch, rb = bpl + 1u;
+    const uint32_t chans = fd.chans, bpl = fd.w * chans, pitch = fd.pitch, rb = bpl + 1u;
     StageSink sk; sk.lo = 0u; sk.saddr = 0u; sk.send = 0u;
     const uint32_t live_mask = __ballot_sync(kFullMask, live);                   // the lanes that decode (they vote together inside)
     if (live) {
@@ -1173,7 +1173,7 @@ __global__ void __launch_bounds__(kWsThreads) decode_write_staged_kernel(DecodeP
 
     // ---- staged stream bytes [lo, hi) -> delta rows
     const uint8_t* sb = reinterpret_cast<const uint8_t*>(s_stage);
-    uint8_t* dl = p.delta + (size_t)f * pitch * h;
+    uint8_t* dl = p.delta + fd.delta_base;
     const unsigned long long y0 = lo / rb, y1 = (hi - 1ull) / rb;                // scanlines the range touches (link pass: hi <= rb * h)
     uint32_t bad = 0;
     for (unsigned long long y = y0 + tid; y <= y1; y += kWsThreads) {            // filter bytes: 0 on the first scanline, 2 (Up) below (fpng.cpp:2253-2262)
@@ -1224,9 +1224,9 @@ __global__ void __launch_bounds__(256) decode_stored_kernel(DecodeParams p)
     const FileDesc fd = p.files[f];
     const uint8_t* z = p.d_files + fd.base + fd.idat_ofs + 8;
     const uint32_t avail = fd.file_size - (fd.idat_ofs + 8);
-    const uint32_t bpl = p.w * p.chans, h = p.h, pitch = p.delta_pitch;
+    const uint32_t bpl = fd.w * fd.chans, h = fd.h, pitch = fd.pitch;
     const unsigned long long raw = (unsigned long long)(bpl + 1) * h, nblk = (raw + 65534ull) / 65535ull;
-    uint8_t* delta = p.delta + (size_t)f * pitch * h;
+    uint8_t* delta = p.delta + fd.delta_base;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t y = blockIdx.x * 8 + warp;
     bool bad = false;
@@ -1279,14 +1279,17 @@ __device__ __forceinline__ void planes_of(const uint32_t (&o)[DST], uint32_t (&p
     }
 }
 
-// Output layouts (DecodeParams): interleaved rows at any pitch (PLANAR false) or one byte plane per channel (PLANAR true).
+// Output layouts (OutStrides): interleaved rows at any pitch (PLANAR false) or one byte plane per channel (PLANAR true).  Files
+// with another channel count than SRC are left to the other instantiation (the ragged call launches both).
 template <int SRC, int DST, bool PLANAR>
 __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p, OutStrides os)
 {
     const uint32_t f = blockIdx.y;
     const DecodeState st = p.state[f];
     if (st.status) return;
-    const uint32_t w = p.w, h = p.h, pitch = p.delta_pitch;
+    const FileDesc& fd = p.files[f];
+    if (fd.chans != SRC) return;                                                // the same for the whole CTA
+    const uint32_t w = fd.w, h = fd.h, pitch = fd.pitch;
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;                   // pixel group index
     const uint32_t x0 = g * 4;
     const uint32_t amask = __ballot_sync(kFullMask, x0 < w);                     // lanes of this warp that own a group (they stay converged)
@@ -1294,9 +1297,9 @@ __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p, OutStride
     const uint32_t lane = threadIdx.x & 31u;
     const bool next_full = lane < 31u && x0 + 8u <= w;                           // the next lane of this warp owns a whole group
     const uint32_t npx = min(4u, w - x0);
-    const uint8_t* delta = p.delta + (size_t)f * pitch * h + (size_t)x0 * SRC;
-    uint8_t* out = p.d_out + (size_t)f * p.out_stride + (size_t)x0 * (PLANAR ? 1u : DST);
-    const size_t out_pitch = os.row, cs = os.chan;
+    const uint8_t* delta = p.delta + fd.delta_base + (size_t)x0 * SRC;
+    uint8_t* out = p.d_out + fd.out_base + (size_t)x0 * (PLANAR ? 1u : DST);
+    const size_t out_pitch = os.row ? os.row : (size_t)w * DST, cs = os.chan;
     const bool full = npx == 4;
     const bool out_aligned = (((uintptr_t)out | out_pitch) & 3) == 0;
     uint32_t acc[SRC];
@@ -1434,7 +1437,7 @@ void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n,
     DEC_MARK(0);
     decode_prepare_kernel<<<n, 32, 0, s>>>(p);
     DEC_MARK(1);
-    const uint32_t sub_blocks = (p.subs_per_file + kDecThreads - 1) / kDecThreads;
+    const uint32_t sub_blocks = (p.max_subs + kDecThreads - 1) / kDecThreads;
     dim3 gsub(sub_blocks, n);
     constexpr size_t kDecSmem = (kFastWords + kWinSmemWords) * 4;
     FPNGB_SET_SMEM(decode_scan_kernel, kDecSmem);
@@ -1445,21 +1448,25 @@ void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n,
     DEC_MARK(3);
     if (g_dec_staged) {
         FPNGB_SET_SMEM(decode_write_staged_kernel, kWsSmem);
-        dim3 gws((p.subs_per_file + kWsThreads - 1) / kWsThreads, n);
+        dim3 gws((p.max_subs + kWsThreads - 1) / kWsThreads, n);
         decode_write_staged_kernel<<<gws, kWsThreads, kWsSmem, s>>>(p);
     }
     decode_write_kernel<<<gsub, kDecThreads, kDecSmem, s>>>(p);
     DEC_MARK(4);
-    dim3 gs((p.h + 7) / 8, n);
+    dim3 gs((p.max_h + 7) / 8, n);
     decode_stored_kernel<<<gs, 256, 0, s>>>(p);
     DEC_MARK(5);
-    const uint32_t groups = (p.w + 3) / 4;
+    const uint32_t groups = (p.max_w + 3) / 4;
     dim3 gu((groups + 127) / 128, n);
     const bool planar = os.pixel == 1;
-    if (p.chans == 3 && desired == 3) { if (planar) unfilter_kernel<3, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 3, false><<<gu, 128, 0, s>>>(p, os); }
-    else if (p.chans == 3) { if (planar) unfilter_kernel<3, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 4, false><<<gu, 128, 0, s>>>(p, os); }
-    else if (desired == 3) { if (planar) unfilter_kernel<4, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<4, 3, false><<<gu, 128, 0, s>>>(p, os); }
-    else { if (planar) unfilter_kernel<4, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<4, 4, false><<<gu, 128, 0, s>>>(p, os); }
+    // one instantiation per channel count in the call (a mixed call launches both; each skips the other's files)
+    for (uint32_t src = 3; src <= 4; src++) {
+        if (p.chans && p.chans != src) continue;
+        if (src == 3 && desired == 3) { if (planar) unfilter_kernel<3, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 3, false><<<gu, 128, 0, s>>>(p, os); }
+        else if (src == 3) { if (planar) unfilter_kernel<3, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 4, false><<<gu, 128, 0, s>>>(p, os); }
+        else if (desired == 3) { if (planar) unfilter_kernel<4, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<4, 3, false><<<gu, 128, 0, s>>>(p, os); }
+        else { if (planar) unfilter_kernel<4, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<4, 4, false><<<gu, 128, 0, s>>>(p, os); }
+    }
     decode_status_kernel<<<(n + 127) / 128, 128, 0, s>>>(p, n);
     DEC_MARK(6);
     if (g_dec_profile && g_dec_ev_ready) g_dec_ev_valid = true;

@@ -177,6 +177,34 @@ FPNGB_API int fpngb_decode_packed_device_strided(const void* d_base, const uint6
                                                  uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
                                                  size_t out_pixel_stride, size_t out_chan_stride, int32_t* d_status, void* stream);
 
+/* fpngb_decode_packed_ragged_device: decodes packed files of ANY shapes and either channel count in one call (an image dataset's
+ *   mixed sizes), with the pixels placed back to back in d_out.  Input layout as above; base_bytes is the length of the buffer
+ *   behind d_base.  Per file, in this order, each step only when the earlier ones passed:
+ *     1. FPNGB_DECODE_INVALID_ARG for size 0, size > max_file_size, offset % 4 != 0 or offset + size > base_bytes;
+ *     2. the container walk (the six values of fpngb_get_info_batch_device go to d_info[i*6 + 0..5] when d_info is not NULL;
+ *        a file that failed step 1 is not walked and gets {FPNGB_DECODE_INVALID_ARG, 0, 0, 0, 0, 0});
+ *     3. FPNGB_DECODE_SHAPE_MISMATCH when w > max_w or h > max_h, then FPNGB_DECODE_FAILED_DIMENSIONS_TOO_LARGE when
+ *        w*h*desired_chans > 0xFFFFFFFF (fpng.cpp:3103-3105);
+ *     4. placement: the files that passed take align_up(w*h*desired_chans, 16) bytes each, in index order from offset 0.
+ *        d_out_offsets[i] is the running offset (a file that failed earlier gets it too and takes no bytes); d_out_offsets[n] is
+ *        the total, with bit 63 set when it exceeds out_cap (retry with that size).  A placed file whose bytes end past out_cap
+ *        gets FPNGB_DECODE_OUT_OF_SPACE and is not decoded; the files that fit are a prefix of the placed ones;
+ *     5. decode: tight HWC rows (pitch w*desired_chans) at d_out + d_out_offsets[i]; status 0 or FPNGB_DECODE_NOT_FPNG as in
+ *        fpngb_decode_packed_device.
+ *   The pixels of a file whose status is not 0 are not written, nor is any byte of d_out outside the decoded files.
+ *   Call-level checks: FPNGB_ERR_INVALID_ARG unless n <= 65535, desired_chans is 3 or 4, 1 <= max_w, max_h <= 2^24 and
+ *   max_file_size > 0; FPNGB_ERR_ALIGNMENT unless d_base % 4 == 0 and d_out % 16 == 0.  A rejected call enqueues nothing and
+ *   writes nothing.  The call is stream-ordered: no host synchronisation, no host copy of file bytes, offsets, sizes or shapes.
+ *   The workspace is sized from the arguments alone: records from min(base_bytes, n * max_file_size), delta rows from out_cap and
+ *   n * max_h (see DESIGN.md section 3); launch grids from max_file_size, max_h and max_w, so tight bounds save launch overhead.
+ *   Files that do not overlap always fit the workspace; overlapping ones may get FPNGB_DECODE_OUT_OF_SPACE.
+ *   Memory read: as fpngb_decode_packed_device, and no file is read past base_bytes. */
+enum { FPNGB_DECODE_OUT_OF_SPACE = 101 };     /* ragged packed decode only: the file's pixels do not fit in out_cap */
+FPNGB_API int fpngb_decode_packed_ragged_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
+                                                uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans,
+                                                void* d_out, size_t out_cap, uint64_t* d_out_offsets /* n+1 */, uint32_t* d_info /* n*6 or NULL */,
+                                                int32_t* d_status, void* stream);
+
 /* Replace fpng::fpng_crc32 / fpng::fpng_adler32 (src/fpng.h:26-31).  Host buffers.  Buffers of 4 KiB and more are
  * checksummed by the device kernels.  NOTE (the one host-side arithmetic in this library): shorter buffers, and any
  * call made before fpngb_init(), use the small host CRC/Adler routines the container code needs anyway for the 17-byte
