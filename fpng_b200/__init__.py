@@ -14,4 +14,5 @@ from .api import (  # noqa: F401
     max_encoded_size, encode_batch_device, decode_batch_device, decode_batch_host, decode_files, pack_files_for_device, get_info_ex, launch_count,
     FPNGB_DECODE_SHAPE_MISMATCH, get_info_batch_device, decode_packed_device, layout_strides,
     FPNGB_DECODE_OUT_OF_SPACE, decode_packed_ragged_device, ragged_views,
+    encode_ragged_device, ragged_slot_offsets, compact_packed_device,
 )

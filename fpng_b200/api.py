@@ -184,6 +184,77 @@ def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=Non
     return out, sizes
 
 
+def ragged_slot_offsets(shapes):
+    """The slot offsets of encode_ragged_device for images of the given (h, w, chans) shapes: the exclusive prefix of
+    max_encoded_size rounded up to 16 bytes, in index order, with the total as the last of the n + 1 entries."""
+    ofs = np.zeros(len(shapes) + 1, dtype=np.int64)
+    for i, (h, w, c) in enumerate(shapes):
+        ofs[i + 1] = ofs[i] + (max_encoded_size(int(w), int(h), int(c)) + 15) // 16 * 16
+    return ofs
+
+
+def encode_ragged_device(images, flags: int = 0, out=None, stream=None):
+    """Encode device images of ANY shapes, channel counts and layouts in one call (fpngb_encode_ragged_device).
+
+    images: list of torch.uint8 CUDA tensors [h, w, chans] (chans 3 or 4), each contiguous or any view in one of the two layouts of
+    layout_strides (HWC rows at any pitch, e.g. a crop, or CHW planes, e.g. x_chw.permute(1, 2, 0)); the same tensor may appear
+    more than once.  Any other layout raises FpngB200Error (invalid argument).  Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]): file i is the sizes[i] bytes at
+    out[offsets[i]:], offsets being ragged_slot_offsets of the shapes and offsets[n] the total -- the (data, offsets, sizes)
+    decode_packed_ragged_device takes.  out, if given, is a flat 16-byte aligned uint8 CUDA tensor of at least the total; no byte
+    of it past the total is written.  Kernels are enqueued on the current torch stream (or `stream`), with no host
+    synchronisation."""
+    import torch
+
+    # the per-image work here is the host cost of the call: attribute reads only; the layout rules are checked by the C call
+    # (an unsupported layout raises FpngB200Error "invalid argument")
+    n = len(images)
+    u8 = torch.uint8
+    ptrs, dims, strides = [], [], []
+    for t in images:
+        assert t.is_cuda and t.dtype == u8 and t.dim() == 3, "images: [h, w, chans] uint8 CUDA tensors"
+        h, w, c = t.shape
+        ptrs.append(t.data_ptr()); dims.append((w, h, c)); strides.append(t.stride())
+    ptrs = np.array(ptrs, dtype=np.uint64)
+    dims = np.array(dims, dtype=np.uint32).reshape(n, 3)
+    strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
+    device = images[0].device if n else torch.device("cuda")
+    if out is None:
+        slot = {}
+        for key in map(tuple, dims.tolist()):
+            if key not in slot:
+                slot[key] = (max_encoded_size(*key) + 15) // 16 * 16
+        total = sum(slot[key] for key in map(tuple, dims.tolist()))
+        out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous(), "out: flat uint8 CUDA tensor"
+    offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
+    sizes = torch.empty((n,), dtype=torch.int32, device=device)
+    s = stream if stream is not None else torch.cuda.current_stream(device).cuda_stream
+    rc = lib().fpngb_encode_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
+                                          strides.ctypes.data_as(C.c_void_p), flags, out.data_ptr(), out.numel(),
+                                          offsets.data_ptr(), sizes.data_ptr(), s)
+    check(rc, "encode_ragged_device")
+    return out, offsets, sizes
+
+
+def compact_packed_device(data, offsets, sizes, out=None, stream=None):
+    """Pack the files of a packed device buffer (file i: sizes[i] bytes at data[offsets[i]:], every offset a multiple of 16, e.g.
+    an encode_ragged_device result) back to back, each starting 16-byte aligned (fpngb_compact_packed_device).  Returns
+    (out uint8, dst_offsets int64 [n + 1]): file i at out[dst_offsets[i]:], dst_offsets[n] the total, with bit 63 set (a negative
+    value) when out was too small -- the files that did not fit are not copied.  out defaults to data.numel() bytes, which holds
+    every compaction of files that do not overlap.  Stream-ordered, no host synchronisation."""
+    import torch
+
+    n = _packed_args(data, offsets, sizes)
+    if out is None:
+        out = torch.empty((max(data.numel(), 16),), dtype=torch.uint8, device=data.device)
+    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous(), "out: flat uint8 CUDA tensor"
+    dst_offsets = torch.empty((n + 1,), dtype=torch.int64, device=data.device)
+    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    check(lib().fpngb_compact_packed_device(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, out.data_ptr(), out.numel(),
+                                            dst_offsets.data_ptr(), s), "compact_packed_device")
+    return out, dst_offsets
+
+
 def _strided_out(out, n, h, w, desired_channels):
     """The layout of a caller's non-contiguous `out` view (layout_strides), or None for a contiguous one."""
     import torch

@@ -272,28 +272,32 @@ __global__ void __launch_bounds__(1024) compact_offsets_kernel(const uint32_t* _
     if (tid == 0) offsets[n] = s_base;
 }
 
+// file f at files + src_offsets[f], or at files + f * stride when src_offsets is null
 __global__ void __launch_bounds__(256) compact_copy_kernel(const uint8_t* __restrict__ files, size_t stride, const uint32_t* __restrict__ sizes,
-                                                            unsigned long long* __restrict__ offsets, uint32_t n, uint8_t* __restrict__ dst, size_t dst_cap)
+                                                            unsigned long long* __restrict__ offsets, uint32_t n, uint8_t* __restrict__ dst, size_t dst_cap,
+                                                            const unsigned long long* __restrict__ src_offsets)
 {
     const uint32_t f = blockIdx.y;
     const uint32_t nvec = (sizes[f] + 15u) / 16u;
     const unsigned long long o = offsets[f];
-    if (o + (unsigned long long)nvec * 16ull > dst_cap) {
-        // the file does not fit: it is NOT copied, and bit 63 of offsets[n] (the total) tells the caller so
+    const unsigned long long so = src_offsets ? src_offsets[f] : (unsigned long long)f * stride;
+    if (o + (unsigned long long)nvec * 16ull > dst_cap || (so & 15ull)) {
+        // the file does not fit (or its source is not 16-byte aligned): it is NOT copied, and bit 63 of offsets[n] (the total)
+        // tells the caller so
         if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(&offsets[n], 1ull << 63);
         return;
     }
-    const uint4* src = reinterpret_cast<const uint4*>(files + (size_t)f * stride);
+    const uint4* src = reinterpret_cast<const uint4*>(files + so);
     uint4* d = reinterpret_cast<uint4*>(dst + o);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += gridDim.x * blockDim.x) d[i] = src[i];
 }
 
 void launch_compact(const uint8_t* files, size_t stride, const uint32_t* sizes, uint32_t n, uint8_t* dst, size_t dst_cap,
-                    unsigned long long* offsets, cudaStream_t s)
+                    unsigned long long* offsets, cudaStream_t s, const unsigned long long* src_offsets)
 {
     compact_offsets_kernel<<<1, 1024, 0, s>>>(sizes, n, offsets);
     dim3 grid(64, n);
-    compact_copy_kernel<<<grid, 256, 0, s>>>(files, stride, sizes, offsets, n, dst, dst_cap);
+    compact_copy_kernel<<<grid, 256, 0, s>>>(files, stride, sizes, offsets, n, dst, dst_cap, src_offsets);
 }
 
 }  // namespace fpngb

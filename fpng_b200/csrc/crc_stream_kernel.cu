@@ -74,27 +74,36 @@ __device__ __forceinline__ uint32_t mul_nib(const uint32_t (*t)[16], uint32_t a)
     return r;
 }
 
-// grid (max CTAs per image, n images); only images with st.stored == want_stored (or all when want_stored < 0) are processed
-__global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcParams p)
+// grid (max CTAs per image, n images); only images with st.stored == want_stored (or all when want_stored < 0) are processed.
+// RAGGED: a 1-D grid over p.ragged, each image with the CTAs of its own max_encoded_size (crc_stream_ctas_for); its slot in p.out
+// is ImageDesc::out_ofs.
+template <bool RAGGED = false>
+__global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(std::conditional_t<RAGGED, RaggedParams<CrcParams>, CrcParams> p)
 {
     // one copy of the four slice tables (4 KiB).  Eight bank-disjoint copies (32 KiB, lanes l / 4 sharing a copy) were measured:
     // C2 0.380 -> 0.372 ms, but small files (one CTA per file) paid the 8x table fill (C2 G0 0.043 -> 0.064 ms): not kept.
     __shared__ uint32_t s_f[4][256];
     __shared__ uint32_t s_part[kCs2Warps];
-    const uint32_t img = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint32_t img = blockIdx.y, bx = blockIdx.x;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if constexpr (RAGGED) {
+        const uint32_t i = ragged_locate(p.ragged, blockIdx.x, bx);
+        p.st += i; p.out += p.ragged.desc[i].out_ofs;
+        img = 0;
+    }
     ImageState* st = p.st + img;
     if (p.stored_only && !st->stored) return;
     const uint32_t L = kPngHeaderSize + st->zsize;                           // end of the message (file offset); message starts at byte 54
     const uint32_t wend = L >> 2;                                            // whole words [kCs2FirstWord, wend)
     const uint32_t nwords = wend - kCs2FirstWord;
     const uint32_t nctas = (nwords + kCs2CtaWords - 1) / kCs2CtaWords;
-    if (blockIdx.x >= nctas) return;
+    if (bx >= nctas) return;
     for (uint32_t i = tid; i < 1024; i += blockDim.x) (&s_f[0][0])[i] = (&g2_f128b[0][0])[i];
     __syncthreads();
 
     const uint32_t* fw = reinterpret_cast<const uint32_t*>(p.out + (size_t)img * p.out_stride);
     // CTA b (counted from the END) covers words [wend - (b+1) * kCs2CtaWords, wend - b * kCs2CtaWords); warp m of it (from the end) 8 KiB
-    const long long cta_end = (long long)wend - (long long)blockIdx.x * kCs2CtaWords;
+    const long long cta_end = (long long)wend - (long long)bx * kCs2CtaWords;
     const uint32_t m = kCs2Warps - 1u - warp;                                // warps in file order: warp 7 is the last chunk (m = 0)
     const long long chunk_end = cta_end - (long long)m * kCs2WarpWords, chunk_begin = chunk_end - kCs2WarpWords;
     uint32_t c = 0;
@@ -133,8 +142,8 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcPara
     if (tid == 0) {
         uint32_t acc = 0;
         for (uint32_t u = 0; u < kCs2Warps; u++) acc ^= s_part[u];
-        // blockIdx.x CTAs (64 KiB each) follow this one before the last whole word
-        acc = gf2_mulmod(acc, gf2_pow(c2_xpow2, 32ull * kCs2CtaWords * blockIdx.x));
+        // bx CTAs (64 KiB each) follow this one before the last whole word
+        acc = gf2_mulmod(acc, gf2_pow(c2_xpow2, 32ull * kCs2CtaWords * bx));
         atomicXor(&st->crc_acc, acc);
         __threadfence();
         const uint32_t done = atomicAdd(&st->tiles_done, 1u);
@@ -181,21 +190,32 @@ __device__ __forceinline__ uint32_t xpow_tab(unsigned long long e)
     return r;
 }
 
+// RAGGED: image blockIdx.y of p.desc, with its own CTA count (row_crc_split_for(h)); the grid is sized for the tallest image
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(kRowCrcThreads) row_crc_combine_kernel(RowCrcParams p)
 {
     __shared__ uint32_t s_part[kRowCrcThreads / 32];
-    const uint32_t img = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint32_t img = blockIdx.y, nsplit = gridDim.x;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if constexpr (RAGGED) {
+        const ImageDesc& d = p.desc[img];
+        p.row_crc += d.row_base; p.row_ofs += d.row_base; p.row_bits += d.row_base; p.books = d.book; p.book_stride = 0;
+        p.st += img; p.out += d.out_ofs; p.h = d.h;
+        nsplit = min(kRowCrcSplit, (d.h + kRowCrcThreads - 1) / kRowCrcThreads);
+        if (blockIdx.x >= nsplit) return;
+        img = 0;
+    }
     ImageState* st = p.st + img;
     if (st->stored) return;                                                  // stored-block images: idat_crc_stream_kernel reads the file
     const CodeBook* book = p.books + (size_t)img * p.book_stride;
     const unsigned long long E = (unsigned long long)(kPngHeaderSize + st->zsize) * 8ull;
     const size_t r0 = (size_t)img * p.h;
     uint32_t acc = 0;
-    for (uint32_t y = blockIdx.x * kRowCrcThreads + tid; y < p.h; y += kRowCrcThreads * gridDim.x) {
+    for (uint32_t y = blockIdx.x * kRowCrcThreads + tid; y < p.h; y += kRowCrcThreads * nsplit) {
         const unsigned long long B = ((p.row_ofs[r0 + y] + p.row_bits[r0 + y]) >> 5) + 1ull;
         acc ^= gf2_mulmod(p.row_crc[r0 + y], xpow_tab(E - 32ull * B));
     }
-    if (blockIdx.x == gridDim.x - 1) {
+    if (blockIdx.x == nsplit - 1) {
         // the fixed parts, one 32-bit piece per thread: block header words, "IDAT", end-of-block code, Adler-32, initial value
         const uint32_t hb = book->hdr_bits, nhw = (hb + 31u) >> 5;
         if (tid < nhw) {
@@ -225,7 +245,7 @@ __global__ void __launch_bounds__(kRowCrcThreads) row_crc_combine_kernel(RowCrcP
         atomicXor(&st->crc_acc, acc);
         __threadfence();
         const uint32_t done = atomicAdd(&st->tiles_done, 1u);
-        if (done == gridDim.x - 1) {
+        if (done == nsplit - 1) {
             __threadfence();
             const uint32_t crc = atomicXor(&st->crc_acc, 0u);
             uint8_t* q = p.out + (size_t)img * p.out_stride + kPngHeaderSize + st->zsize;
@@ -234,17 +254,30 @@ __global__ void __launch_bounds__(kRowCrcThreads) row_crc_combine_kernel(RowCrcP
     }
 }
 
+uint32_t row_crc_split_for(uint32_t h) { return std::min(kRowCrcSplit, (h + kRowCrcThreads - 1) / kRowCrcThreads); }
+
 void launch_row_crc_combine(const RowCrcParams& p, uint32_t n, cudaStream_t s)
 {
-    const uint32_t split = std::min(kRowCrcSplit, (p.h + kRowCrcThreads - 1) / kRowCrcThreads);
-    row_crc_combine_kernel<<<dim3(split, n), kRowCrcThreads, 0, s>>>(p);
+    const uint32_t split = row_crc_split_for(p.h);
+    row_crc_combine_kernel<false><<<dim3(split, n), kRowCrcThreads, 0, s>>>(p);
 }
+
+void launch_row_crc_combine_ragged(const RowCrcParams& p, uint32_t n, uint32_t max_split, cudaStream_t s)
+{
+    row_crc_combine_kernel<true><<<dim3(max_split, n), kRowCrcThreads, 0, s>>>(p);
+}
+
+uint32_t crc_stream_ctas_for(size_t max_file_bytes) { return (uint32_t)((max_file_bytes / 4 + kCs2CtaWords - 1) / kCs2CtaWords) + 1u; }
 
 void launch_crc_stream(const CrcParams& p, uint32_t n, size_t max_file_bytes, cudaStream_t s)
 {
-    const uint32_t max_ctas = (uint32_t)((max_file_bytes / 4 + kCs2CtaWords - 1) / kCs2CtaWords) + 1u;
-    dim3 grid(max_ctas, n);
-    idat_crc_stream_kernel<<<grid, 32 * kCs2Warps, 0, s>>>(p);
+    dim3 grid(crc_stream_ctas_for(max_file_bytes), n);
+    idat_crc_stream_kernel<false><<<grid, 32 * kCs2Warps, 0, s>>>(p);
+}
+
+void launch_crc_stream_ragged(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s)
+{
+    idat_crc_stream_kernel<true><<<total_ctas, 32 * kCs2Warps, 0, s>>>(p);
 }
 
 }  // namespace fpngb

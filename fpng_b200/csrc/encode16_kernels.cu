@@ -40,8 +40,7 @@ __device__ __forceinline__ uint32_t byte1(uint32_t v) { return __byte_perm(v, 0u
 __device__ __forceinline__ uint32_t byte2(uint32_t v) { return __byte_perm(v, 0u, 0x4442); }
 
 // scanline loader: staged tiles (TMA / cp.async) for 16-byte aligned interleaved scanlines, direct realigning 128-bit loads for
-// any other interleaved shape, per-plane loads for planar images (ScanParams::chan_stride != 0)
-enum { kLoad16Staged = 0, kLoad16Direct = 1, kLoad16Planar = 2 };
+// any other interleaved shape, per-plane loads for planar images (ScanParams::chan_stride != 0); kLoad16* in kernels.cuh
 template <int CHANS, int LOAD> struct Loader16 { using type = Walk16<CHANS>; };
 template <int CHANS> struct Loader16<CHANS, kLoad16Direct> { using type = Walk16Direct<CHANS>; };
 template <int CHANS> struct Loader16<CHANS, kLoad16Planar> { using type = Walk16Planar<CHANS>; };
@@ -57,6 +56,22 @@ __device__ __forceinline__ uint32_t literal_bits16(const uint8_t* s_lit, uint32_
     return b;
 }
 
+// Ragged launches (RAGGED = true): CTA blockIdx.x is CTA `cta` of one image (ragged_locate); the image's descriptor replaces the
+// call-wide pixels, strides, shape and books, and the row / lane tables, image state and output are rebased to it, so that the
+// kernel bodies run as for image 0 of a uniform batch.  The uniform instantiations compile without any of this.  Returns the
+// image's index in the descriptor table.
+template <class P>
+__device__ __forceinline__ uint32_t ragged_image16(P& p, uint32_t& cta)
+{
+    const uint32_t i = ragged_locate(p.ragged, blockIdx.x, cta);
+    const ImageDesc& d = p.ragged.desc[i];
+    p.pixels = d.pixels; p.image_stride = 0; p.row_pitch = d.row_pitch; p.chan_stride = d.chan_stride; p.w = d.w; p.h = d.h;
+    p.books = d.book; p.book_stride = 0;
+    p.row_bits += d.row_base; p.row_adler += d.row_base; p.st += i;
+    p.lane_ofs += d.lane_base; p.lane_ofs_pitch = d.lane_pitch;
+    return i;
+}
+
 // ------------------------------------------------------------------------------------------------
 // K1 (v2): per-row bit count + Adler partials (+ per-lane bit offsets inside the row for the pack kernel)
 // ------------------------------------------------------------------------------------------------
@@ -67,8 +82,8 @@ __device__ __forceinline__ uint32_t literal_bits16(const uint8_t* s_lit, uint32_
 #else
 #define FPNGB_SCAN_BOUNDS __launch_bounds__(32 * kScan16Rows)
 #endif
-template <int CHANS, int LOAD>
-__global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(ScanParams p)
+template <int CHANS, int LOAD, bool RAGGED = false>
+__global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(std::conditional_t<RAGGED, RaggedParams<ScanParams>, ScanParams> p)
 {
     using WK = typename Loader16<CHANS, LOAD>::type;
     constexpr uint32_t M = max_match_pixels(CHANS);
@@ -79,8 +94,9 @@ __global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(ScanParams p)
     // the warp index as a shuffle result: the compiler then treats everything derived from it (scanline pointers, tile address) as
     // warp-uniform and issues the TMA copies from uniform registers without a per-lane "waterfall" loop
     const uint32_t lane = threadIdx.x & 31, warp = __shfl_sync(kFullMask, threadIdx.x >> 5, 0);
-    const uint32_t img = blockIdx.y;
-    const uint32_t y = blockIdx.x * kScan16Rows + warp;
+    uint32_t img = blockIdx.y, cta = blockIdx.x;
+    if constexpr (RAGGED) { ragged_image16(p, cta); img = 0; }
+    const uint32_t y = cta * kScan16Rows + warp;
     const CodeBook* book = p.books + (size_t)img * p.book_stride;
     static_assert(32 * kScan16Rows == 256, "one table byte per thread");
     s_lit[threadIdx.x] = book->lit_size[threadIdx.x];
@@ -184,8 +200,8 @@ __global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(ScanParams p)
 // K1-hist (v2): 288-bin literal/length histogram of 2-pass mode (fpng.cpp:1021-1084, 1299-1363) on the 16-pixel walker.
 // Warp-private shared-memory histograms (no inter-warp contention), merged per CTA, then added to the image's bins.
 // ------------------------------------------------------------------------------------------------
-template <int CHANS, int LOAD>
-__global__ void __launch_bounds__(32 * kScan16Rows) row_hist16_kernel(ScanParams p)
+template <int CHANS, int LOAD, bool RAGGED = false>
+__global__ void __launch_bounds__(32 * kScan16Rows) row_hist16_kernel(std::conditional_t<RAGGED, RaggedParams<ScanParams>, ScanParams> p)
 {
     using WK = typename Loader16<CHANS, LOAD>::type;
     constexpr uint32_t M = max_match_pixels(CHANS);
@@ -194,8 +210,9 @@ __global__ void __launch_bounds__(32 * kScan16Rows) row_hist16_kernel(ScanParams
     __shared__ uint16_t s_lensym[88];
 
     const uint32_t lane = threadIdx.x & 31, warp = __shfl_sync(kFullMask, threadIdx.x >> 5, 0);   // warp-uniform for the compiler (see the scan kernel)
-    const uint32_t img = blockIdx.y;
-    const uint32_t y = blockIdx.x * kScan16Rows + warp;
+    uint32_t img = blockIdx.y, cta = blockIdx.x;
+    if constexpr (RAGGED) { p.hist += (size_t)ragged_image16(p, cta) * 288; img = 0; }
+    const uint32_t y = cta * kScan16Rows + warp;
     for (uint32_t i = threadIdx.x; i < kScan16Rows * 288; i += blockDim.x) s_hist_all[i] = 0u;
     if (threadIdx.x >= 1 && threadIdx.x <= M) { uint32_t sy, xb, xv; deflate_len_code(threadIdx.x * CHANS, sy, xb, xv); s_lensym[threadIdx.x] = (uint16_t)sy; }
     __syncthreads();
@@ -446,11 +463,18 @@ __device__ __forceinline__ uint32_t crc_step16(uint32_t crc_s, uint32_t cx, uint
     return v ^ lds_u32(crc_s + b0 * 4u) ^ lds_u32(crc_s + 1024u + b1 * 4u) ^ lds_u32(crc_s + 2048u + b2 * 4u) ^ lds_u32(crc_s + 3072u + b3 * 4u);
 }
 
-template <int CHANS, int LOAD>
-__global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParams p, uint32_t rows_per_warp)
+template <int CHANS, int LOAD, bool RAGGED = false>
+__global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(std::conditional_t<RAGGED, RaggedParams<PackParams>, PackParams> p,
+                                                                       uint32_t rows_per_warp)
 {
     using WK = typename Loader16<CHANS, LOAD>::type;
-    if (p.stored_only && !p.st[blockIdx.y].stored) return;     // after the fused encoder only stored-block images are left to write
+    uint32_t img = blockIdx.y, cta = blockIdx.x;
+    if constexpr (RAGGED) {
+        const ImageDesc& d = p.ragged.desc[ragged_image16(p, cta)];
+        p.row_ofs += d.row_base; p.row_crc += d.row_base; p.out += d.out_ofs; p.out_stride = 0;
+        img = 0;
+    }
+    if (p.stored_only && !p.st[img].stored) return;     // after the fused encoder only stored-block images are left to write
     constexpr uint32_t M = max_match_pixels(CHANS);
     constexpr int kHalfWords = 2 * CHANS;        // filtered words of 8 pixels
     extern __shared__ __align__(16) uint8_t dyn_smem[];
@@ -465,8 +489,7 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(PackParam
     uint32_t* s_crc = s_stage_all + kPack16Rows * stage16_words<CHANS>();              // [4][256] CRC slice tables (row_crc only)
 
     const uint32_t lane = threadIdx.x & 31, warp = __shfl_sync(kFullMask, threadIdx.x >> 5, 0);   // warp-uniform for the compiler (see the scan kernel)
-    const uint32_t img = blockIdx.y;
-    const uint32_t row0 = (blockIdx.x * kPack16Rows + warp) * rows_per_warp;           // this warp's first scanline
+    const uint32_t row0 = (cta * kPack16Rows + warp) * rows_per_warp;                  // this warp's first scanline
     const bool do_crc = p.row_crc != nullptr;
     const CodeBook* book = p.books + (size_t)img * p.book_stride;
     const ImageState st = p.st[img];
@@ -717,17 +740,18 @@ template <int CHANS, int LOAD> constexpr size_t pack16_smem()
 template <int CHANS, int LOAD> constexpr size_t hist16_smem() { return kScan16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + kScan16Rows * 288 * 4; }
 
 // The 16-pixel kernels take any scanline alignment and either layout: `load` (load16_mode()) selects the loader.
-#define FPNGB_LAUNCH16_ONE(C, L, kernel, smemfn, grid, threads, ...) do { \
-        FPNGB_SET_SMEM((kernel<C, L>), (smemfn<C, L>())); kernel<C, L><<<grid, threads, smemfn<C, L>(), s>>>(__VA_ARGS__); } while (0)
-#define FPNGB_LAUNCH16(kernel, smemfn, grid, threads, ...) do { \
+// R: the ragged instantiation (the uniform launches pass false)
+#define FPNGB_LAUNCH16_ONE(C, L, R, kernel, smemfn, grid, threads, ...) do { \
+        FPNGB_SET_SMEM((kernel<C, L, R>), (smemfn<C, L>())); kernel<C, L, R><<<grid, threads, smemfn<C, L>(), s>>>(__VA_ARGS__); } while (0)
+#define FPNGB_LAUNCH16(kernel, R, smemfn, grid, threads, ...) do { \
         if (chans == 4) { \
-            if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(4, kLoad16Planar, kernel, smemfn, grid, threads, __VA_ARGS__); \
-            else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(4, kLoad16Direct, kernel, smemfn, grid, threads, __VA_ARGS__); \
-            else FPNGB_LAUNCH16_ONE(4, kLoad16Staged, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(4, kLoad16Planar, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(4, kLoad16Direct, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else FPNGB_LAUNCH16_ONE(4, kLoad16Staged, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
         } else { \
-            if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(3, kLoad16Planar, kernel, smemfn, grid, threads, __VA_ARGS__); \
-            else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(3, kLoad16Direct, kernel, smemfn, grid, threads, __VA_ARGS__); \
-            else FPNGB_LAUNCH16_ONE(3, kLoad16Staged, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(3, kLoad16Planar, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(3, kLoad16Direct, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
+            else FPNGB_LAUNCH16_ONE(3, kLoad16Staged, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
         } \
     } while (0)
 
@@ -736,14 +760,14 @@ void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t
     // one scanline per warp: the multi-scanline sequence that pays off in the pack kernel measured neutral (RGB) to 4 % slower (RGBA) here
     const int load = load16_mode(p, chans);
     dim3 grid((p.h + kScan16Rows - 1) / kScan16Rows, n);
-    FPNGB_LAUNCH16(row_scan16_kernel, scan16_smem, grid, 32 * kScan16Rows, p);
+    FPNGB_LAUNCH16(row_scan16_kernel, false, scan16_smem, grid, 32 * kScan16Rows, p);
 }
 
 void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
 {
     const int load = load16_mode(p, chans);
     dim3 grid((p.h + kScan16Rows - 1) / kScan16Rows, n);
-    FPNGB_LAUNCH16(row_hist16_kernel, hist16_smem, grid, 32 * kScan16Rows, p);
+    FPNGB_LAUNCH16(row_hist16_kernel, false, hist16_smem, grid, 32 * kScan16Rows, p);
 }
 
 void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
@@ -751,7 +775,31 @@ void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t
     const int load = load16_mode(p, chans);
     const uint32_t rpw = rows_per_warp16(n, p.h), rows_per_cta = kPack16Rows * rpw;
     dim3 grid((p.h + rows_per_cta - 1) / rows_per_cta, n);
-    FPNGB_LAUNCH16(pack_rows16_kernel, pack16_smem, grid, 32 * kPack16Rows, p, rpw);
+    FPNGB_LAUNCH16(pack_rows16_kernel, false, pack16_smem, grid, 32 * kPack16Rows, p, rpw);
+}
+
+// Ragged launches: one per (chans, loader) class, over the class's CTAs (the host sums them per image: ceil(h / rows per CTA)).
+uint32_t scan16_rows_per_cta() { return kScan16Rows; }
+uint32_t pack16_rows_per_warp(size_t total_rows)
+{
+    if (g_rows_per_warp_override) return g_rows_per_warp_override;
+    return total_rows >= (size_t)sm_count() * 64u * kRowsPerWarp16 ? kRowsPerWarp16 : 1u;
+}
+uint32_t pack16_rows_per_cta(uint32_t rows_per_warp) { return kPack16Rows * rows_per_warp; }
+
+void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s)
+{
+    FPNGB_LAUNCH16(row_scan16_kernel, true, scan16_smem, ctas, 32 * kScan16Rows, p);
+}
+
+void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s)
+{
+    FPNGB_LAUNCH16(row_hist16_kernel, true, hist16_smem, ctas, 32 * kScan16Rows, p);
+}
+
+void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s)
+{
+    FPNGB_LAUNCH16(pack_rows16_kernel, true, pack16_smem, ctas, 32 * kPack16Rows, p, rows_per_warp);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -164,10 +164,22 @@ __device__ __forceinline__ void store_be32(uint8_t* p, uint32_t v)
     p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v;
 }
 
+// RAGGED: image blockIdx.x of p.desc; its descriptor replaces the call-wide shape, book and header, and the row tables, image
+// state, size and output are rebased to it (the body then runs as for image 0)
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(kOffsetsThreads) row_offsets_kernel(OffsetsParams p)
 {
     __shared__ unsigned long long s_warp[kOffsetsThreads / 32];
-    const uint32_t img = blockIdx.x, tid = threadIdx.x;
+    uint32_t img = blockIdx.x;
+    const uint32_t tid = threadIdx.x;
+    const uint8_t* ragged_header = nullptr;
+    if constexpr (RAGGED) {
+        const ImageDesc& d = p.desc[img];
+        p.row_bits += d.row_base; p.row_ofs += d.row_base; p.books = d.book; p.book_stride = 0; p.st += img;
+        p.out += d.out_ofs; p.sizes += d.index; p.w = d.w; p.h = d.h; p.chans = d.chans;
+        ragged_header = d.png_header;
+        img = 0;
+    }
     const CodeBook* book = p.books + (size_t)img * p.book_stride;
     const uint32_t h = p.h;
     const uint32_t hdr_bits = book->hdr_bits;
@@ -216,7 +228,7 @@ __global__ void __launch_bounds__(kOffsetsThreads) row_offsets_kernel(OffsetsPar
     const uint32_t hend = compressed ? 4u * ((uint32_t)(base >> 5) + 1u) : kPngHeaderSize + 2u;
     for (uint32_t i = tid; i < hend; i += blockDim.x) {
         uint8_t v = 0;
-        if (i < kPngHeaderSize) v = p.png_header[i];
+        if (i < kPngHeaderSize) v = RAGGED ? ragged_header[i] : p.png_header[i];
         else if (i - kPngHeaderSize < hbytes) v = compressed ? book->hdr[i - kPngHeaderSize] : (i == kPngHeaderSize ? 0x78 : 0x01);
         if (i >= 50 && i < 54) v = (uint8_t)(zsize >> (8 * (53 - i)));
         file[i] = v;
@@ -402,10 +414,17 @@ __global__ void __launch_bounds__(kPackThreads) pack_rows_kernel(PackParams p)
 // ------------------------------------------------------------------------------------------------
 // K3b: Adler-32 combine.  State after row r: a' = a + S1_r, b' = b + n*a + S2_r  (mod 65521), start (1, 0).
 // ------------------------------------------------------------------------------------------------
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(kOffsetsThreads) adler_finalize_kernel(AdlerParams p)
 {
     __shared__ unsigned long long s_red[3][kOffsetsThreads / 32];
-    const uint32_t img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint32_t img = blockIdx.x;
+    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if constexpr (RAGGED) {                      // image blockIdx.x of p.desc (see row_offsets_kernel)
+        const ImageDesc& d = p.desc[img];
+        p.row_adler += d.row_base; p.st += img; p.out += d.out_ofs; p.w = d.w; p.h = d.h; p.chans = d.chans;
+        img = 0;
+    }
     const uint32_t h = p.h;
     unsigned long long s1 = 0, s2 = 0, wsum = 0;
     for (uint32_t y = tid; y < h; y += blockDim.x) {
@@ -456,7 +475,17 @@ void launch_scan(const ScanParams& p, uint32_t n, uint32_t chans, int mode, bool
 
 void launch_offsets(const OffsetsParams& p, uint32_t n, cudaStream_t s)
 {
-    row_offsets_kernel<<<n, kOffsetsThreads, 0, s>>>(p);
+    row_offsets_kernel<false><<<n, kOffsetsThreads, 0, s>>>(p);
+}
+
+void launch_offsets_ragged(const OffsetsParams& p, uint32_t n, cudaStream_t s)
+{
+    row_offsets_kernel<true><<<n, kOffsetsThreads, 0, s>>>(p);
+}
+
+void launch_adler_finalize_ragged(const AdlerParams& p, uint32_t n, cudaStream_t s)
+{
+    adler_finalize_kernel<true><<<n, kOffsetsThreads, 0, s>>>(p);
 }
 
 void launch_pack(const PackParams& p, uint32_t n, uint32_t chans, int mode, cudaStream_t s)
@@ -474,7 +503,7 @@ void launch_pack(const PackParams& p, uint32_t n, uint32_t chans, int mode, cuda
 
 void launch_adler_finalize(const AdlerParams& p, uint32_t n, cudaStream_t s)
 {
-    adler_finalize_kernel<<<n, kOffsetsThreads, 0, s>>>(p);
+    adler_finalize_kernel<false><<<n, kOffsetsThreads, 0, s>>>(p);
 }
 
 }  // namespace fpngb

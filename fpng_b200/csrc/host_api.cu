@@ -12,6 +12,7 @@
 #include "static_tables.h"
 #include "runtime.h"
 
+#include <algorithm>
 #include <atomic>
 #include <mutex>
 #include <new>
@@ -412,6 +413,181 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
     return c.ws_release(s);
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Ragged encode: images of any shape and layout in one call (fpngb_encode_ragged_device).
+// ---------------------------------------------------------------------------------------------------------
+// One image as the host sees it after the call-level checks.
+struct RaggedImage {
+    const uint8_t* pixels; uint64_t row, chan;          // chan: 0 for interleaved rows
+    uint32_t w, h, chans;
+    uint64_t slot;                                      // offset of its slot in d_out
+};
+
+// Pinned staging of the descriptor table: a ring of buffers, each reused only once the copy that last read it has completed
+// (cudaEventQuery), so that a call never waits on the stream.
+struct StageSlot { Buffer buf; cudaEvent_t ev = nullptr; };
+static std::vector<StageSlot*> g_ragged_stage;
+
+static int ragged_stage_slot(size_t bytes, StageSlot** out)
+{
+    StageSlot* sl = nullptr;
+    for (StageSlot* x : g_ragged_stage) if (x->buf.cap >= bytes && cudaEventQuery(x->ev) == cudaSuccess) { sl = x; break; }
+    if (!sl) {
+        sl = new (std::nothrow) StageSlot();
+        if (!sl) return FPNGB_ERR_INTERNAL;
+        sl->buf.pinned = true;
+        FPNGB_CUDA_OK(cudaEventCreateWithFlags(&sl->ev, cudaEventDisableTiming));
+        g_ragged_stage.push_back(sl);
+    }
+    const int rc = sl->buf.reserve(bytes);
+    if (rc) return rc;
+    *out = sl;
+    return 0;
+}
+
+static bool force_generic_env()
+{
+    static const bool v = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;
+    return v;
+}
+
+// Enqueues the ragged pipeline for images im[k] (k in `ids`), all bound for the 16-pixel kernels.  Caller holds ctx.mu.
+//
+// Launches: per non-empty (chans, loader) class a scan and a pack kernel (and a hist kernel in 2-pass mode), then one launch each of
+// the per-image kernels -- offsets, Adler-32, scanline-CRC combine, stored-only stream CRC (and the Huffman build in 2-pass mode).
+static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, const std::vector<uint32_t>& ids, uint32_t flags,
+                                uint8_t* d_out, uint32_t* d_sizes, cudaStream_t s, uint8_t* stage)
+{
+    const uint32_t m = (uint32_t)ids.size();
+    const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
+    size_t rows = 0, lanes = 0;
+    for (uint32_t k : ids) { rows += im[k].h; lanes += (size_t)im[k].h * (((im[k].w + 511u) / 512u) * 32u); }
+    const uint32_t rpw = pack16_rows_per_warp(rows), pack_rows = pack16_rows_per_cta(rpw), scan_rows = scan16_rows_per_cta();
+    // class of an image: (chans == 4) * 3 + loader, the loader by the uniform launch's rule for one image
+    constexpr int kClasses = 6;
+    std::vector<uint32_t> cls(m);
+    uint32_t cls_count[kClasses] = {0};
+    for (uint32_t j = 0; j < m; j++) {
+        const RaggedImage& r = im[ids[j]];
+        const int load = r.chan ? kLoad16Planar : walk16_eligible(r.pixels, 0, (uint32_t)r.row, r.w, r.chans) ? kLoad16Staged : kLoad16Direct;
+        cls[j] = (r.chans == 4 ? 3u : 0u) + (uint32_t)load;
+        cls_count[cls[j]]++;
+    }
+
+    // workspace: exact, sum(h) scanlines and sum(h * lane pitch) lane records, then the descriptor table and the work lists
+    const size_t table = align_up((size_t)m * sizeof(ImageDesc), 16) + (size_t)m * 5 * 4;
+    size_t o = 0;
+    const size_t o_bits = o; o = align_up(o + rows * 4, 256);
+    const size_t o_adl = o; o = align_up(o + rows * 8, 256);
+    const size_t o_ofs = o; o = align_up(o + rows * 8, 256);
+    const size_t o_rcrc = o; o = align_up(o + rows * 4, 256);
+    const size_t o_st = o; o = align_up(o + (size_t)m * sizeof(ImageState), 256);
+    const size_t o_hist = o; o = align_up(o + (two_pass ? (size_t)m * 288 * 4 : 0), 256);
+    const size_t o_books = o; o = align_up(o + (two_pass ? (size_t)m * sizeof(CodeBook) : 0), 256);
+    const size_t o_lane = o; o = align_up(o + lanes * 8, 256);
+    const size_t o_table = o; o = align_up(o + table, 256);
+    int rc = c.ws.reserve(o);
+    if (rc) return rc;
+    rc = c.ws_acquire(s);
+    if (rc) return rc;
+    uint8_t* b = (uint8_t*)c.ws.p;
+    uint32_t* row_bits = (uint32_t*)(b + o_bits); uint2* row_adler = (uint2*)(b + o_adl);
+    unsigned long long* row_ofs = (unsigned long long*)(b + o_ofs); uint32_t* row_crc = (uint32_t*)(b + o_rcrc);
+    ImageState* st = (ImageState*)(b + o_st); uint32_t* hist = (uint32_t*)(b + o_hist); CodeBook* books = (CodeBook*)(b + o_books);
+    uint2* lane_ofs = (uint2*)(b + o_lane);
+    const ImageDesc* d_desc = (const ImageDesc*)(b + o_table);
+
+    // the table in staging: ImageDesc[m] | per class, in class order: img[], scan CTA prefix[], pack CTA prefix[] | crc img[], crc prefix[]
+    ImageDesc* desc = (ImageDesc*)stage;
+    uint32_t* lists = (uint32_t*)(stage + align_up((size_t)m * sizeof(ImageDesc), 16));
+    uint32_t* l_img = lists; uint32_t* l_scan = lists + m; uint32_t* l_pack = lists + 2 * m; uint32_t* l_crc_img = lists + 3 * m; uint32_t* l_crc = lists + 4 * m;
+    uint32_t cls_first[kClasses], fill[kClasses];
+    for (int k = 0, acc = 0; k < kClasses; k++) { cls_first[k] = fill[k] = acc; acc += cls_count[k]; }
+    uint64_t cls_scan_ctas[kClasses] = {0}, cls_pack_ctas[kClasses] = {0}, crc_ctas = 0;
+    size_t row_base = 0, lane_base = 0;
+    uint32_t max_split = 1;
+    for (uint32_t j = 0; j < m; j++) {
+        const RaggedImage& r = im[ids[j]];
+        ImageDesc& d = desc[j];
+        memset(&d, 0, sizeof d);
+        d.pixels = r.pixels; d.chan_stride = r.chan; d.row_base = row_base; d.lane_base = lane_base; d.out_ofs = r.slot;
+        d.book = two_pass ? books + j : c.d_static_books + (r.chans == 4 ? 1 : 0);
+        d.row_pitch = (uint32_t)r.row; d.w = r.w; d.h = r.h; d.chans = r.chans; d.lane_pitch = ((r.w + 511u) / 512u) * 32u; d.index = ids[j];
+        make_png_header(d.png_header, r.w, r.h, r.chans);
+        row_base += r.h; lane_base += (size_t)r.h * d.lane_pitch;
+        const uint32_t k = cls[j], q = fill[k]++;
+        l_img[q] = j;
+        l_scan[q] = (uint32_t)cls_scan_ctas[k]; cls_scan_ctas[k] += (r.h + scan_rows - 1) / scan_rows;
+        l_pack[q] = (uint32_t)cls_pack_ctas[k]; cls_pack_ctas[k] += (r.h + pack_rows - 1) / pack_rows;
+        l_crc_img[j] = j; l_crc[j] = (uint32_t)crc_ctas; crc_ctas += crc_stream_ctas_for(max_encoded_size(r.w, r.h, r.chans));
+        max_split = std::max(max_split, row_crc_split_for(r.h));
+    }
+    for (int k = 0; k < kClasses; k++) if (cls_scan_ctas[k] > 0x7FFFFFFFull || cls_pack_ctas[k] > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
+    if (crc_ctas > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
+    FPNGB_CUDA_OK(cudaMemcpyAsync((void*)d_desc, stage, table, cudaMemcpyHostToDevice, s));
+    const uint32_t* d_lists = (const uint32_t*)((const uint8_t*)d_desc + align_up((size_t)m * sizeof(ImageDesc), 16));
+    auto work = [&](int k, int list) {                 // list 1: scan prefix, 2: pack prefix
+        return RaggedWork{d_desc, d_lists + cls_first[k], d_lists + (size_t)list * m + cls_first[k], cls_count[k]};
+    };
+    if (g_profile) g_prof_call++;
+    ProfSet* ps = prof_begin(s);
+
+    RaggedParams<ScanParams> sp{};
+    sp.row_bits = row_bits; sp.row_adler = row_adler; sp.st = st; sp.hist = hist; sp.lane_ofs = lane_ofs;
+    sp.merge_first_unit = 0u;
+    if (two_pass) {
+        FPNGB_CUDA_OK(cudaMemsetAsync(hist, 0, (size_t)m * 288 * 4, s));
+        for (int k = 0; k < kClasses; k++) {
+            if (!cls_count[k]) continue;
+            sp.ragged = work(k, 1);
+            launch_hist16_ragged(sp, (uint32_t)cls_scan_ctas[k], k >= 3 ? 4u : 3u, k % 3, s);
+            count_launch(1);
+        }
+        prof_mark(ps, kProfHist, s);
+        HuffParams hp{hist, books, 0u, 0u, d_desc};
+        launch_huffman_build_ragged(hp, m, s);
+        count_launch(1);
+        prof_mark(ps, kProfHuff, s);
+    }
+    for (int k = 0; k < kClasses; k++) {
+        if (!cls_count[k]) continue;
+        sp.ragged = work(k, 1);
+        sp.merge_first_unit = (!two_pass && k < 3) ? 1u : 0u;           // RGB 1-pass
+        launch_scan16_ragged(sp, (uint32_t)cls_scan_ctas[k], k >= 3 ? 4u : 3u, k % 3, s);
+        count_launch(1);
+    }
+    prof_mark(ps, kProfScan, s);
+    OffsetsParams op{};
+    op.row_bits = row_bits; op.row_ofs = row_ofs; op.st = st; op.out = d_out; op.sizes = d_sizes; op.flags = flags; op.desc = d_desc;
+    launch_offsets_ragged(op, m, s);
+    count_launch(1);
+    prof_mark(ps, kProfOffsets, s);
+    RaggedParams<PackParams> pp{};
+    pp.row_ofs = row_ofs; pp.row_bits = row_bits; pp.lane_ofs = lane_ofs; pp.row_adler = row_adler; pp.st = st; pp.out = d_out;
+    pp.row_crc = row_crc; pp.crc_f128b = c.crc_f128b; pp.crc_lane_mul = c.crc_lane_mul;
+    for (int k = 0; k < kClasses; k++) {
+        if (!cls_count[k]) continue;
+        pp.ragged = work(k, 2);
+        launch_pack16_ragged(pp, (uint32_t)cls_pack_ctas[k], k >= 3 ? 4u : 3u, k % 3, rpw, s);
+        count_launch(1);
+    }
+    prof_mark(ps, kProfPack, s);
+    AdlerParams ap{row_adler, st, d_out, 0, 0, 0, 0, d_desc};
+    launch_adler_finalize_ragged(ap, m, s);
+    count_launch(1);
+    prof_mark(ps, kProfAdler, s);
+    RowCrcParams rp{row_crc, row_ofs, row_bits, nullptr, 0, st, d_out, 0, 0, d_desc};
+    launch_row_crc_combine_ragged(rp, m, max_split, s);
+    RaggedParams<CrcParams> cp{};
+    cp.out = d_out; cp.st = st; cp.msg_start = kPngHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu; cp.stored_only = 1u;
+    cp.ragged = RaggedWork{d_desc, d_lists + 3 * (size_t)m, d_lists + 4 * (size_t)m, m};
+    launch_crc_stream_ragged(cp, (uint32_t)crc_ctas, s);
+    count_launch(2);
+    prof_mark(ps, kProfCrc, s);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return c.ws_release(s);
+}
+
 }  // namespace fpngb
 
 using namespace fpngb;
@@ -516,6 +692,69 @@ int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_
     if (image_stride < (size_t)w * h * chans) return FPNGB_ERR_INVALID_ARG;
     return fpngb_encode_batch_device_strided(d_pixels, image_stride, (size_t)w * chans, chans, 1, n, w, h, chans, flags, d_out, out_stride,
                                              d_sizes, stream);
+}
+
+int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
+                               void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
+    // every image on its own: the layout rules of the strided batch call for a batch of one
+    std::vector<RaggedImage> im(n);
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t w = dims[3 * i], h = dims[3 * i + 1], chans = dims[3 * i + 2];
+        if (!pixels[i] || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
+        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans, pixel = strides ? strides[3 * i + 1] : chans;
+        const uint64_t chan = strides ? strides[3 * i + 2] : 1;
+        Layout L;
+        uint64_t last = 0;
+        if (!classify_layout(0, row, pixel, chan, 1, h, w, chans, L) || L.row > 0xFFFFFFFFull ||
+            !layout_span((const void*)(uintptr_t)pixels[i], L, 1, h, w, chans, last))
+            return FPNGB_ERR_INVALID_ARG;
+        im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
+        total += align_up(max_encoded_size(w, h, chans), 16);
+    }
+    if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    Context& c = g_ctx;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    uint8_t* out = (uint8_t*)d_out;
+
+    // images the 16-pixel kernels do not take (RGBA 1-pass under a table whose one-pixel-match rule is live, or FPNGB_FORCE_GENERIC)
+    // go through the uniform pipeline one at a time, into their slots
+    const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
+    const bool lit1_rgba = !two_pass && c.h_static_books[1].lit1_rule;
+    std::vector<uint32_t> ids;
+    ids.reserve(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const RaggedImage& r = im[i];
+        if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
+            const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
+            const int rc = encode_batch_locked(c, r.pixels, (size_t)r.h * r.row, (uint32_t)r.row, r.chan, 1, r.w, r.h, r.chans, flags,
+                                               out + r.slot, slot, d_sizes + i, s);
+            if (rc) return rc;
+        } else ids.push_back(i);
+    }
+
+    // staging: d_out_offsets (n + 1), then the descriptor table and work lists
+    const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
+    StageSlot* sl = nullptr;
+    int rc = ragged_stage_slot(ofs_bytes + align_up((size_t)n * sizeof(ImageDesc), 16) + (size_t)n * 5 * 4, &sl);
+    if (rc) return rc;
+    uint8_t* stage = (uint8_t*)sl->buf.p;
+    uint64_t* h_ofs = (uint64_t*)stage;
+    for (uint32_t i = 0; i < n; i++) h_ofs[i] = im[i].slot;
+    h_ofs[n] = total;
+    FPNGB_CUDA_OK(cudaMemcpyAsync(d_out_offsets, h_ofs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+    if (!ids.empty()) {
+        rc = encode_ragged_locked(c, im, ids, flags, out, d_sizes, s, stage + ofs_bytes);
+        if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+    }
+    FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
+    return FPNGB_OK;
 }
 
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)
@@ -745,6 +984,20 @@ int fpngb_compact_batch_device(const void* d_files, size_t stride, const uint32_
     if (stride % 16 || (uintptr_t)d_files % 16 || (uintptr_t)d_dst % 16) return FPNGB_ERR_ALIGNMENT;
     FPNGB_CUDA_OK(cudaSetDevice(g_ctx.device));
     launch_compact((const uint8_t*)d_files, stride, d_sizes, n, (uint8_t*)d_dst, dst_cap, (unsigned long long*)d_offsets, (cudaStream_t)stream);
+    count_launch(2);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return FPNGB_OK;
+}
+
+int fpngb_compact_packed_device(const void* d_base, const uint64_t* d_src_offsets, const uint32_t* d_sizes, uint32_t n, void* d_dst,
+                                size_t dst_cap, uint64_t* d_offsets, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_src_offsets || !d_sizes || !d_dst || !d_offsets || n == 0 || n > 65535) return FPNGB_ERR_INVALID_ARG;
+    if ((uintptr_t)d_base % 16 || (uintptr_t)d_dst % 16) return FPNGB_ERR_ALIGNMENT;
+    FPNGB_CUDA_OK(cudaSetDevice(g_ctx.device));
+    launch_compact((const uint8_t*)d_base, 0, d_sizes, n, (uint8_t*)d_dst, dst_cap, (unsigned long long*)d_offsets, (cudaStream_t)stream,
+                   (const unsigned long long*)d_src_offsets);
     count_launch(2);
     FPNGB_CUDA_OK(cudaGetLastError());
     return FPNGB_OK;

@@ -111,6 +111,8 @@ struct DevBitWriter {
     }
 };
 
+// RAGGED: the channel count is image blockIdx.x's (p.desc) instead of the call's
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
 {
     __shared__ HuffScratch s;
@@ -119,7 +121,7 @@ __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
     const uint32_t img = blockIdx.x, lane = threadIdx.x;
     const uint32_t* hist = p.hist + (size_t)img * 288;
     CodeBook* cb = p.books + img;
-    const uint32_t chans = p.chans;
+    const uint32_t chans = RAGGED ? p.desc[img].chans : p.chans;
 
     // --- 16-bit scaled counts (fpng.cpp:1092-1094 then 868-893, then 757)
     uint32_t part = 0;
@@ -234,7 +236,12 @@ __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
 
 void launch_huffman_build(const HuffParams& p, uint32_t n, cudaStream_t s)
 {
-    huffman_build_kernel<<<n, 32, 0, s>>>(p);
+    huffman_build_kernel<false><<<n, 32, 0, s>>>(p);
+}
+
+void launch_huffman_build_ragged(const HuffParams& p, uint32_t n, cudaStream_t s)
+{
+    huffman_build_kernel<true><<<n, 32, 0, s>>>(p);
 }
 
 }  // namespace fpngb

@@ -1,6 +1,7 @@
 // fpng_b200/csrc/kernels.cuh -- kernel parameter blocks and launcher prototypes (host_api.cu <-> *_kernels.cu).
 #pragma once
 #include "common.cuh"
+#include <type_traits>
 
 namespace fpngb {
 
@@ -9,6 +10,42 @@ constexpr int kScanThreads = 32 * kRowsPerBlock;
 constexpr int kPackThreads = 32 * kRowsPerBlock;
 constexpr int kOffsetsThreads = 256;
 constexpr int kStageWords = 272;                  // >= (31 + 12 + 128 * 66) / 32 + 1 words per 128-pixel step
+
+// One image of a ragged encode call (fpngb_encode_ragged_device): its pixels and shape, where its scanlines sit in the row tables
+// and lane records, its code book, its output slot and its container header (the IHDR differs per image).
+struct ImageDesc {
+    const uint8_t* pixels;
+    unsigned long long chan_stride;               // 0: interleaved rows; else planar (see ScanParams)
+    unsigned long long row_base;                  // first entry of the image in row_bits / row_adler / row_ofs / row_crc
+    unsigned long long lane_base;                 // first lane record (uint2) of the image
+    unsigned long long out_ofs;                   // byte offset of the image's slot in the output buffer
+    const CodeBook* book;
+    uint32_t row_pitch, w, h, chans;
+    uint32_t lane_pitch;                          // lane records per scanline: 32 * ceil(w / 512)
+    uint32_t index;                               // the image's index in the call (its d_sizes entry)
+    uint8_t png_header[kPngHeaderSize];
+    uint8_t pad_[6];
+};
+
+// The images one ragged launch covers: CTA b works on image img[j] for the j with cta_start[j] <= b < cta_start[j + 1] (every
+// image has at least one CTA), as that image's CTA b - cta_start[j].
+struct RaggedWork {
+    const ImageDesc* desc;
+    const uint32_t* img;                          // [count] indices into desc
+    const uint32_t* cta_start;                    // [count] exclusive prefix of the images' CTA counts
+    uint32_t count;
+};
+
+__device__ __forceinline__ uint32_t ragged_locate(const RaggedWork& rw, uint32_t b, uint32_t& local_cta)
+{
+    uint32_t lo = 0, hi = rw.count - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (rw.cta_start[mid] <= b) lo = mid; else hi = mid - 1;
+    }
+    local_cta = b - rw.cta_start[lo];
+    return rw.img[lo];
+}
 
 struct ScanParams {
     const uint8_t* pixels; size_t image_stride;   // n images
@@ -32,6 +69,7 @@ struct OffsetsParams {
     uint8_t* out; size_t out_stride; uint32_t* sizes;
     uint32_t w, h, chans, flags;
     uint8_t png_header[kPngHeaderSize];           // IDAT length patched per image on device
+    const ImageDesc* desc;                        // ragged kernel: image blockIdx.x's shape, rows, book, slot and header
 };
 
 struct PackParams {
@@ -60,12 +98,14 @@ struct RowCrcParams {
     const CodeBook* books; uint32_t book_stride;
     ImageState* st; uint8_t* out; size_t out_stride;
     uint32_t h;
+    const ImageDesc* desc;                        // ragged kernel: image blockIdx.y's rows, book, slot and height
 };
 
 struct AdlerParams {
     const uint2* row_adler; ImageState* st;
     uint8_t* out; size_t out_stride;
     uint32_t w, h, chans;
+    const ImageDesc* desc;                        // ragged kernel: image blockIdx.x's rows, slot and shape
 };
 
 struct CrcParams {
@@ -77,11 +117,17 @@ struct CrcParams {
     uint32_t stored_only;                         // only images that fell back to stored blocks (the single-pass encoder computed the others' CRC inline)
 };
 
+// Parameter block of a ragged scan / hist / pack / stream-CRC launch: the uniform block, whose table pointers are the bases an
+// image's row_base / lane_base / index count from, plus the images and CTA map of the launch.  (A separate type, so that the
+// uniform kernels' parameter blocks stay as they are.)
+template <class P> struct RaggedParams : P { RaggedWork ragged; };
+
 struct HuffParams {
     const uint32_t* hist;                         // [n*288]
     CodeBook* books;                              // [n]
     uint32_t chans;
     uint32_t training;                            // 1: table training (fpng.cpp:909-988): symbol 256 keeps its own count in the scaling
+    const ImageDesc* desc;                        // ragged kernel: the channel count of image blockIdx.x
 };
 
 // opt in to > 48 KiB of dynamic shared memory (per kernel instantiation, once per process)
@@ -103,6 +149,22 @@ int crc_stream_tables_init();
 void launch_crc_stream(const CrcParams& p, uint32_t n, size_t max_file_bytes, cudaStream_t s);
 void launch_row_crc_combine(const RowCrcParams& p, uint32_t n, cudaStream_t s);
 int crc_stream_table_ptrs(const uint32_t** f128b, const uint32_t** lane_mul);
+uint32_t crc_stream_ctas_for(size_t max_file_bytes);     // CTAs of the stream CRC kernel for a file of at most that many bytes
+uint32_t row_crc_split_for(uint32_t h);                   // CTAs of the scanline-CRC combine for an image of h scanlines
+void launch_crc_stream_ragged(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s);
+void launch_row_crc_combine_ragged(const RowCrcParams& p, uint32_t n, uint32_t max_split, cudaStream_t s);
+void launch_offsets_ragged(const OffsetsParams& p, uint32_t n, cudaStream_t s);
+void launch_adler_finalize_ragged(const AdlerParams& p, uint32_t n, cudaStream_t s);
+void launch_huffman_build_ragged(const HuffParams& p, uint32_t n, cudaStream_t s);
+
+// ragged 16-pixel kernels (encode16_kernels.cu): one launch per (chans, loader) class over `ctas` CTAs (ScanParams::ragged)
+enum { kLoad16Staged = 0, kLoad16Direct = 1, kLoad16Planar = 2 };
+uint32_t scan16_rows_per_cta();
+uint32_t pack16_rows_per_warp(size_t total_rows);        // the uniform launch's rule for a batch of that many scanlines
+uint32_t pack16_rows_per_cta(uint32_t rows_per_warp);
+void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s);
+void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s);
+void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s);
 
 // strided input -> contiguous [n][h][w * chans] (encode16_kernels.cu)
 struct GatherParams {
@@ -126,8 +188,9 @@ void launch_huffman_build(const HuffParams& p, uint32_t n, cudaStream_t s);
 uint32_t crc_ctas_for(size_t max_file_bytes);
 uint32_t adler_chunk_bytes();
 void launch_adler_buffer(const uint8_t* d_buf, size_t n, uint2* d_partials, cudaStream_t s);
+// src_offsets: file f at files + src_offsets[f] (multiples of 16), or nullptr: at files + f * stride
 void launch_compact(const uint8_t* files, size_t stride, const uint32_t* sizes, uint32_t n, uint8_t* dst, size_t dst_cap,
-                    unsigned long long* offsets, cudaStream_t s);
+                    unsigned long long* offsets, cudaStream_t s, const unsigned long long* src_offsets = nullptr);
 int  checksum_tables_init();                      // uploads CRC slice tables / x^(2^k) powers (idempotent)
 
 // host helpers shared by host_api.cu and the tests

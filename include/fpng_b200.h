@@ -94,6 +94,33 @@ FPNGB_API int fpngb_encode_batch_device_strided(const void* d_pixels, size_t ima
                                                 size_t chan_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags,
                                                 void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream);
 
+/* fpngb_encode_ragged_device: encodes n device images of ANY shapes, channel counts and layouts in one call (a dataset's crops,
+ *   thumbnails, scans and frames, one tensor each), into one output buffer.  The shapes are host arguments:
+ *     pixels   HOST array of n device addresses; image i's byte (y, x, c) is at pixels[i] + y*row_pitch + x*pixel_stride + c*chan_stride
+ *     dims     HOST array of n x {w, h, chans}
+ *     strides  HOST array of n x {row_pitch, pixel_stride, chan_stride}, or NULL for tight HWC rows (w*chans, chans, 1)
+ *   Each image is one image of "Pixel layouts" above: interleaved rows at any pitch or planar (CHW / HCW); inputs may overlap and
+ *   the same pointer may appear more than once.
+ *   Output slots: file i goes to d_out + d_out_offsets[i], where the offsets are the exclusive prefix of
+ *   align_up(fpngb_max_encoded_size(w_i, h_i, chans_i), 16) in index order and d_out_offsets[n] (device, n+1 entries) is the
+ *   total; d_sizes[i] (device) receives the file size.  This is the packed layout fpngb_get_info_batch_device and
+ *   fpngb_decode_packed_ragged_device read (base_bytes = d_out_offsets[n]); fpngb_compact_packed_device packs it to exact size.
+ *   No byte of d_out past the total is written.  The files are byte-identical to fpngb_encode_batch_device's for each image.
+ *   Call-level checks, before anything is enqueued: FPNGB_ERR_INVALID_ARG for n == 0 or n > 65535, a NULL pointer (pixels[i]
+ *   included), an image with invalid dimensions or channels, or an unsupported layout; FPNGB_ERR_BUFFER_TOO_SMALL when out_cap
+ *   is below the total; FPNGB_ERR_ALIGNMENT unless d_out % 16 == 0.  A rejected call enqueues nothing and writes nothing.
+ *   The call is stream-ordered, with no host synchronisation: the per-image descriptors and d_out_offsets go up by
+ *   cudaMemcpyAsync from library-owned pinned staging, a ring of buffers each reused only once its last copy has completed.
+ *   Launches: per non-empty (chans, loader) class -- 3 or 4 channels times staged / direct / planar loader -- one scan and one
+ *   pack kernel, plus one hist kernel with FPNG_ENCODE_SLOWER; then four per-image kernels (offsets, Adler-32, scanline-CRC
+ *   combine, stored-block CRC), plus the Huffman build with FPNG_ENCODE_SLOWER.  fpngb_profile_read reports the call in its
+ *   usual slots.
+ *   Fallbacks: RGBA images in 1-pass mode under an installed table whose one-pixel-match rule can fire (never the shipped
+ *   table), and every image under FPNGB_FORCE_GENERIC, are encoded by the uniform pipeline one image at a time into their
+ *   slots: correct, but one uniform call's launches per image.  The opt-in single-pass encoder is not used by this call. */
+FPNGB_API int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
+                                         void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
+
 /* Batch of n equally sized images in HOST memory (ideally pinned: see fpngb_host_alloc) -> n files in host memory,
  * out + i*out_stride, sizes[i].  Internally pipelines H2D copy / kernels / D2H copy over chunks of the batch. */
 FPNGB_API int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
@@ -222,6 +249,13 @@ FPNGB_API int fpngb_adler32_ex(const void* data, size_t size, uint32_t adler, ui
  * the staging step before the single NCCL gather of a rank's encoded shard (BASELINE.json north_star). */
 FPNGB_API int fpngb_compact_batch_device(const void* d_files, size_t stride, const uint32_t* d_sizes, uint32_t n,
                                          void* d_dst, size_t dst_cap, uint64_t* d_offsets, void* stream);
+/* fpngb_compact_batch_device for files at arbitrary offsets: file i is the d_sizes[i] bytes at d_base + d_src_offsets[i]
+ *   (device, n x uint64, each a multiple of 16 -- e.g. the slots of fpngb_encode_ragged_device).  Destination offsets, alignment
+ *   and the bit-63 rule are those of fpngb_compact_batch_device; a file whose source offset is not a multiple of 16 is not
+ *   copied either, and sets bit 63.  FPNGB_ERR_INVALID_ARG for n == 0, n > 65535 or a NULL pointer; FPNGB_ERR_ALIGNMENT
+ *   unless d_base % 16 == 0 and d_dst % 16 == 0.  Stream-ordered, two launches. */
+FPNGB_API int fpngb_compact_packed_device(const void* d_base, const uint64_t* d_src_offsets, const uint32_t* d_sizes, uint32_t n,
+                                          void* d_dst, size_t dst_cap, uint64_t* d_offsets, void* stream);
 
 /* ---- multi-GPU (SURVEY.md 8b/8e; no reference counterpart: fpng is single-threaded, single-device) ----------------------
  * One process per GPU.  Images shard across ranks with no collective on the data path; afterwards ONE gather brings the
