@@ -15,4 +15,5 @@ from .api import (  # noqa: F401
     FPNGB_DECODE_SHAPE_MISMATCH, get_info_batch_device, decode_packed_device, layout_strides,
     FPNGB_DECODE_OUT_OF_SPACE, decode_packed_ragged_device, ragged_views,
     encode_ragged_device, ragged_slot_offsets, compact_packed_device,
+    FPNGB_DECODE_ADLER_MISMATCH, set_decode_verify, decode_verify,
 )

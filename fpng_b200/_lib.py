@@ -109,6 +109,10 @@ def lib() -> C.CDLL:
     L.fpngb_gather_encoded_device.restype = C.c_int
     L.fpngb_gather_encoded_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_int, C.POINTER(C.c_void_p),
                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]
+    L.fpngb_set_decode_verify.restype = C.c_int
+    L.fpngb_set_decode_verify.argtypes = [C.c_int]
+    L.fpngb_get_decode_verify.restype = C.c_int
+    L.fpngb_get_decode_verify.argtypes = []
     L.fpngb_bind_host_thread_to_device_numa.restype = C.c_int
     L.fpngb_launch_count.restype = C.c_uint64
     L.fpngb_debug_use_fused.restype = None

@@ -22,6 +22,22 @@ FPNG_FORCE_UNCOMPRESSED = 2     # src/fpng.h:41
  FPNG_DECODE_FILE_TOO_LARGE, FPNG_DECODE_FILE_READ_FAILED, FPNG_DECODE_FILE_SEEK_FAILED) = range(13)   # src/fpng.h:57-77
 
 
+FPNGB_DECODE_ADLER_MISMATCH = 102   # include/fpng_b200.h: verified decode, the zlib Adler-32 does not match the inflated stream
+
+
+def set_decode_verify(on: bool) -> None:
+    """Turns the decoder's integrity check on or off for every later decode call of the process (include/fpng_b200.h,
+    fpngb_set_decode_verify): the IDAT CRC-32 (a mismatch gives FPNG_DECODE_FAILED_HEADER_CRC32) and the zlib Adler-32
+    (FPNGB_DECODE_ADLER_MISMATCH), both on the GPU.  Off at load: statuses and pixels are then the reference's.  Works before
+    fpng_init()."""
+    check(lib().fpngb_set_decode_verify(1 if on else 0), "set_decode_verify")
+
+
+def decode_verify() -> bool:
+    """Whether decode calls verify the IDAT CRC-32 and the zlib Adler-32 (set_decode_verify)."""
+    return bool(lib().fpngb_get_decode_verify())
+
+
 def _u8(buf) -> np.ndarray:
     if isinstance(buf, np.ndarray):
         return np.ascontiguousarray(buf).view(np.uint8).reshape(-1)

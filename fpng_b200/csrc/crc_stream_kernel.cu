@@ -11,17 +11,20 @@
 //     chunk and a warp's chunk sits m * 8 KiB before the end of its CTA's 64 KiB: both multipliers are constants (nibble
 //     tables); one modular power per CTA positions the CTA's value in the message; XOR into the image's accumulator; the last
 //     CTA of an image appends the (at most 3) bytes after the last whole word, applies init/xorout and stores the CRC.
+// The message may start at any byte: the first word's bytes in front of it are masked to zero, which a zero-initialised CRC
+// register does not see.  The decoder's opt-in integrity check runs the same kernel over the files it reads (VERIFY).
 // About 3.3 thread-instructions per byte (4 table look-ups + 8 address instructions + 3 XORs per word).
 #include "kernels.cuh"
 #include "crc_math.cuh"
+#include "decode.cuh"
 #include <algorithm>
+#include <cstddef>
 
 namespace fpngb {
 
 constexpr uint32_t kCs2WarpWords = 2048;          // 8 KiB per warp
 constexpr uint32_t kCs2Warps = 8;                 // 64 KiB per CTA
 constexpr uint32_t kCs2CtaWords = kCs2WarpWords * kCs2Warps;
-constexpr uint32_t kCs2FirstWord = (kPngHeaderSize - 4u) / 4u;      // word 13 holds file bytes 52..55: bytes 52, 53 (IDAT length) are masked off
 
 __device__ uint32_t g2_f128b[4][256];             // byte k of (reg ^ word) advanced over 128 bytes
 __device__ uint32_t g2_byte[256];                 // plain byte table (tail bytes)
@@ -77,8 +80,16 @@ __device__ __forceinline__ uint32_t mul_nib(const uint32_t (*t)[16], uint32_t a)
 // grid (max CTAs per image, n images); only images with st.stored == want_stored (or all when want_stored < 0) are processed.
 // RAGGED: a 1-D grid over p.ragged, each image with the CTAs of its own max_encoded_size (crc_stream_ctas_for); its slot in p.out
 // is ImageDesc::out_ofs.
-template <bool RAGGED = false>
-__global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(std::conditional_t<RAGGED, RaggedParams<CrcParams>, CrcParams> p)
+// VERIFY: the decoder's check of a file it reads (decode.cuh, VerifyState): file blockIdx.y of p.files, whose message is "IDAT" +
+// idat_len data bytes from file byte idat_ofs + 4 (any alignment: ancillary chunks may precede IDAT); the last CTA compares the
+// CRC with the chunk's big-endian CRC field and sets the file's status to FPNG_DECODE_FAILED_HEADER_CRC32 when they differ.
+static_assert(offsetof(ImageState, tiles_done) == offsetof(ImageState, crc_acc) + 4 &&
+              offsetof(VerifyState, crc_done) == offsetof(VerifyState, crc_acc) + 4, "the CTA counter follows the CRC accumulator");
+template <bool RAGGED = false, bool VERIFY = false>
+using CrcStreamParams = std::conditional_t<VERIFY, VerifyParams, std::conditional_t<RAGGED, RaggedParams<CrcParams>, CrcParams>>;
+
+template <bool RAGGED = false, bool VERIFY = false>
+__global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStreamParams<RAGGED, VERIFY> p)
 {
     // one copy of the four slice tables (4 KiB).  Eight bank-disjoint copies (32 KiB, lanes l / 4 sharing a copy) were measured:
     // C2 0.380 -> 0.372 ms, but small files (one CTA per file) paid the 8x table fill (C2 G0 0.043 -> 0.064 ms): not kept.
@@ -86,28 +97,44 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(std::co
     __shared__ uint32_t s_part[kCs2Warps];
     uint32_t img = blockIdx.y, bx = blockIdx.x;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if constexpr (RAGGED) {
-        const uint32_t i = ragged_locate(p.ragged, blockIdx.x, bx);
-        p.st += i; p.out += p.ragged.desc[i].out_ofs;
-        img = 0;
+    // the message is bytes [m0, L) of the 4-byte aligned buffer file_base()
+    uint32_t m0, L;
+    [[maybe_unused]] ImageState* st = nullptr;
+    auto file_base = [&]() -> const uint8_t* {                               // recomputed where needed rather than kept live
+        if constexpr (VERIFY) return p.d_files + p.files[img].base;
+        else return p.out + (size_t)img * p.out_stride;
+    };
+    if constexpr (VERIFY) {
+        const FileDesc& fd = p.files[img];
+        if (fd.pre_status) return;                                           // never read: the walk or the argument checks failed
+        m0 = fd.idat_ofs + 4u; L = m0 + 4u + fd.idat_len;
+    } else {
+        if constexpr (RAGGED) {
+            const uint32_t i = ragged_locate(p.ragged, blockIdx.x, bx);
+            p.st += i; p.out += p.ragged.desc[i].out_ofs;
+            img = 0;
+        }
+        st = p.st + img;
+        if (p.stored_only && !st->stored) return;
+        m0 = kPngHeaderSize - 4u;                                            // the message starts at byte 54 ("IDAT")
+        L = kPngHeaderSize + st->zsize;                                      // end of the message (file offset)
     }
-    ImageState* st = p.st + img;
-    if (p.stored_only && !st->stored) return;
-    const uint32_t L = kPngHeaderSize + st->zsize;                           // end of the message (file offset); message starts at byte 54
-    const uint32_t wend = L >> 2;                                            // whole words [kCs2FirstWord, wend)
-    const uint32_t nwords = wend - kCs2FirstWord;
+    const uint32_t w0 = m0 >> 2;                                             // first word; its bytes before m0 are masked off
+    const uint32_t head_mask = 0xFFFFFFFFu << (8u * (m0 & 3u));
+    const uint32_t wend = L >> 2;                                            // whole words [w0, wend)
+    const uint32_t nwords = wend - w0;
     const uint32_t nctas = (nwords + kCs2CtaWords - 1) / kCs2CtaWords;
     if (bx >= nctas) return;
     for (uint32_t i = tid; i < 1024; i += blockDim.x) (&s_f[0][0])[i] = (&g2_f128b[0][0])[i];
     __syncthreads();
 
-    const uint32_t* fw = reinterpret_cast<const uint32_t*>(p.out + (size_t)img * p.out_stride);
+    const uint32_t* fw = reinterpret_cast<const uint32_t*>(file_base());
     // CTA b (counted from the END) covers words [wend - (b+1) * kCs2CtaWords, wend - b * kCs2CtaWords); warp m of it (from the end) 8 KiB
     const long long cta_end = (long long)wend - (long long)bx * kCs2CtaWords;
     const uint32_t m = kCs2Warps - 1u - warp;                                // warps in file order: warp 7 is the last chunk (m = 0)
     const long long chunk_end = cta_end - (long long)m * kCs2WarpWords, chunk_begin = chunk_end - kCs2WarpWords;
     uint32_t c = 0;
-    if (chunk_end > (long long)kCs2FirstWord) {
+    if (chunk_end > (long long)w0) {
         constexpr int kSteps = kCs2WarpWords / 32;                           // 64 lane steps
         constexpr int kBatch = 8;                                            // independent loads in flight per lane
 #pragma unroll 1
@@ -117,9 +144,9 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(std::co
             for (int q = 0; q < kBatch; q++) {
                 const long long j = chunk_begin + 32ll * (k0 + q) + lane;
                 uint32_t v = 0u;
-                if (j >= (long long)kCs2FirstWord) {
+                if (j >= (long long)w0) {
                     v = __ldg(fw + j);
-                    if (j == (long long)kCs2FirstWord) v &= 0xFFFF0000u;    // bytes 52, 53 are the chunk length field, not part of the message
+                    if (j == (long long)w0) v &= head_mask;                 // encoder: bytes 52, 53 are the chunk length field, not part of the message
                 }
                 w[q] = v;
             }
@@ -144,18 +171,27 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(std::co
         for (uint32_t u = 0; u < kCs2Warps; u++) acc ^= s_part[u];
         // bx CTAs (64 KiB each) follow this one before the last whole word
         acc = gf2_mulmod(acc, gf2_pow(c2_xpow2, 32ull * kCs2CtaWords * bx));
-        atomicXor(&st->crc_acc, acc);
+        // ctr[0]: the message's CRC accumulator, ctr[1]: its CTAs finished
+        uint32_t* ctr;
+        if constexpr (VERIFY) ctr = &p.vs[img].crc_acc; else ctr = &st->crc_acc;
+        atomicXor(ctr, acc);
         __threadfence();
-        const uint32_t done = atomicAdd(&st->tiles_done, 1u);
+        const uint32_t done = atomicAdd(ctr + 1, 1u);
         if (done == nctas - 1) {
             __threadfence();
-            uint32_t reg = atomicXor(&st->crc_acc, 0u);                      // register after all whole words (zero initial value)
-            const uint8_t* fb = p.out + (size_t)img * p.out_stride;
+            uint32_t reg = atomicXor(ctr, 0u);                               // register after all whole words (zero initial value)
+            const uint8_t* fb = file_base();
             for (uint32_t b = wend << 2; b < L; b++) reg = g2_byte[(reg ^ fb[b]) & 0xFFu] ^ (reg >> 8);
-            // initial value 0xFFFFFFFF advanced over the whole message (L - 54 bytes), final XOR
-            reg ^= gf2_mulmod(0xFFFFFFFFu, gf2_pow(c2_xpow2, 8ull * (L - (kPngHeaderSize - 4u)))) ^ 0xFFFFFFFFu;
-            uint8_t* q = p.out + (size_t)img * p.out_stride + L;
-            q[0] = (uint8_t)(reg >> 24); q[1] = (uint8_t)(reg >> 16); q[2] = (uint8_t)(reg >> 8); q[3] = (uint8_t)reg;
+            // initial value 0xFFFFFFFF advanced over the whole message (L - m0 bytes), final XOR
+            reg ^= gf2_mulmod(0xFFFFFFFFu, gf2_pow(c2_xpow2, 8ull * (L - m0))) ^ 0xFFFFFFFFu;
+            if constexpr (VERIFY) {
+                const uint8_t* q = fb + L;                                   // the chunk's CRC field
+                const uint32_t want = ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | q[3];
+                if (reg != want) p.state[img].status = 4u;                   // FPNG_DECODE_FAILED_HEADER_CRC32
+            } else {
+                uint8_t* q = p.out + (size_t)img * p.out_stride + L;
+                q[0] = (uint8_t)(reg >> 24); q[1] = (uint8_t)(reg >> 16); q[2] = (uint8_t)(reg >> 8); q[3] = (uint8_t)reg;
+            }
         }
     }
 }
@@ -273,6 +309,12 @@ void launch_crc_stream(const CrcParams& p, uint32_t n, size_t max_file_bytes, cu
 {
     dim3 grid(crc_stream_ctas_for(max_file_bytes), n);
     idat_crc_stream_kernel<false><<<grid, 32 * kCs2Warps, 0, s>>>(p);
+}
+
+void launch_idat_crc_verify(const VerifyParams& p, uint32_t n, size_t max_file_bytes, cudaStream_t s)
+{
+    dim3 grid(crc_stream_ctas_for(max_file_bytes), n);
+    idat_crc_stream_kernel<false, true><<<grid, 32 * kCs2Warps, 0, s>>>(p);
 }
 
 void launch_crc_stream_ragged(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s)

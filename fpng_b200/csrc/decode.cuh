@@ -36,7 +36,8 @@ __host__ __device__ __forceinline__ uint32_t delta_pitch(uint32_t w, uint32_t ch
 __host__ __device__ __forceinline__ uint32_t subs_for(uint32_t bytes) { return (uint32_t)(((uint64_t)bytes * 8 + 32) / kSubBits + 2); }
 
 struct DecodeState {
-    uint32_t status;                        // 0 ok, 1 -> FPNG_DECODE_NOT_FPNG
+    uint32_t status;                        // 0 ok, 1 -> FPNG_DECODE_NOT_FPNG; with verification on also the checksum kernels'
+                                            // FPNG_DECODE_FAILED_HEADER_CRC32 (4) and FPNGB_DECODE_ADLER_MISMATCH (102)
     uint32_t stored;                        // stored-block file
     unsigned long long token_start;         // bit offset (from the zlib stream start) of the first token
     unsigned long long out_bytes;           // filtered-stream bytes produced
@@ -65,7 +66,27 @@ struct OutStrides {
     size_t row, pixel, chan;                // interleaved (pixel = desired, chan = 1) or planar (pixel = 1); row 0: tight rows of each
                                             // file's own width (w * desired, the ragged call)
 };
-void launch_decode(const DecodeParams& p, const OutStrides& out, uint32_t n, uint32_t desired, cudaStream_t s);
+// Opt-in integrity check of every decode call (fpngb_set_decode_verify).  Two kernels read the file and the delta rows again:
+//   idat_crc_stream_kernel<false, true> (crc_stream_kernel.cu), after decode_prepare_kernel: the CRC-32 of "IDAT" + idat_len data
+//     bytes against the chunk's CRC field; a mismatch sets DecodeState::status to 4 for every file the walk passed, whatever the
+//     stream checks found, so the later kernels skip the file;
+//   decode_adler_kernel (decode_kernels.cu), after the write and stored kernels: the Adler-32 of the inflated stream against the
+//     stream's last four bytes; a mismatch sets status 102 before unfilter_kernel writes any pixel.
+// Their per-file accumulators, zeroed by one cudaMemsetAsync in front of the pipeline:
+struct VerifyState {
+    uint32_t crc_acc, crc_done;             // XOR of the CRC kernel's CTA contributions, CTAs finished
+    uint32_t adler_done, pad_;              // CTAs of the Adler kernel finished
+    unsigned long long s1, s2;              // sum x_i and sum i * x_i over the delta rows, each CTA's share reduced mod 65521
+};
+struct VerifyParams {
+    const uint8_t* d_files; const FileDesc* files; DecodeState* state; const uint8_t* delta;   // as in DecodeParams
+    VerifyState* vs;                        // [n]
+};
+// verify: the call's [n] accumulators, or nullptr (verification off: the pipeline is exactly the unverified one);
+// max_file_bytes: a bound of every file's size (the CRC kernel's grid)
+void launch_decode(const DecodeParams& p, const OutStrides& out, uint32_t n, uint32_t desired, cudaStream_t s,
+                   VerifyState* verify = nullptr, size_t max_file_bytes = 0);
+void launch_idat_crc_verify(const VerifyParams& p, uint32_t n, size_t max_file_bytes, cudaStream_t s);
 void decode_profile_enable(bool on);
 int decode_profile_read(float* ms, int n);
 unsigned long long decode_link_repairs(bool reset);

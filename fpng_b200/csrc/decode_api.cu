@@ -6,6 +6,7 @@
 #include "layout.h"
 #include "runtime.h"
 #include <string.h>
+#include <atomic>
 #include <vector>
 
 namespace fpngb {
@@ -13,9 +14,13 @@ namespace fpngb {
 static Buffer g_dec_ws;        // FileDesc[n] | DecodeState[n] | luts | delta scratch
 static Buffer g_dec_pin;       // pinned staging for the FileDesc upload / status download
 
+// fpngb_set_decode_verify: off at load; every decode call reads it once, under context().mu, when it enqueues
+static std::atomic<int> g_decode_verify{0};
+
 // Reserves the workspace of a decode call for n files, n_subs SubInfo records and delta_bytes of delta rows in all, orders it
-// after the previous call's kernels, and points p's workspace fields into it (p.files included).  Caller holds context().mu.
-static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes, cudaStream_t s, DecodeParams& p)
+// after the previous call's kernels, and points p's workspace fields into it (p.files included).  With verification on
+// (fpngb_set_decode_verify), *verify points to n VerifyState records behind the rest; else it is nullptr.  Caller holds context().mu.
+static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes, cudaStream_t s, DecodeParams& p, VerifyState** verify)
 {
     size_t o = 0;
     const size_t o_files = o; o = align_up(o + (size_t)n * sizeof(FileDesc), 256);
@@ -24,20 +29,23 @@ static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes
     const size_t o_fast = o; o = align_up(o + (size_t)n * kFastWords * 4, 256);
     const size_t o_subs = o; o = align_up(o + n_subs * sizeof(SubInfo), 256);
     const size_t o_delta = o; o = align_up(o + delta_bytes + 64, 256);
+    const bool verifying = g_decode_verify.load() != 0;
+    const size_t o_verify = o; if (verifying) o = align_up(o + (size_t)n * sizeof(VerifyState), 256);
     int rc = g_dec_ws.reserve(o); if (rc) return rc;
     rc = context().ws_acquire(s); if (rc) return rc;
     uint8_t* b = (uint8_t*)g_dec_ws.p;
     p.files = (const FileDesc*)(b + o_files); p.state = (DecodeState*)(b + o_state);
     p.luts = (uint32_t*)(b + o_luts); p.fast = (uint32_t*)(b + o_fast); p.subs = (SubInfo*)(b + o_subs);
     p.delta = b + o_delta;
+    *verify = verifying ? (VerifyState*)(b + o_verify) : nullptr;
     return 0;
 }
 // The same for n files of one shape whose IDAT chunks are at most max_idat bytes: file i's records and delta rows at i times the
 // per-file share (the bases the uniform calls put in FileDesc), and the launch grids of that shape.
 static int decode_workspace_uniform_locked(uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t max_idat, cudaStream_t s,
-                                           DecodeParams& p)
+                                           DecodeParams& p, VerifyState** verify)
 {
-    const int rc = decode_workspace_locked(n, (size_t)n * subs_for(max_idat), (size_t)n * delta_pitch(w, chans) * h, s, p);
+    const int rc = decode_workspace_locked(n, (size_t)n * subs_for(max_idat), (size_t)n * delta_pitch(w, chans) * h, s, p, verify);
     if (rc) return rc;
     p.max_w = w; p.max_h = h; p.max_subs = subs_for(max_idat); p.chans = chans;
     return 0;
@@ -82,7 +90,8 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     uint32_t max_idat = 0;
     for (uint32_t i = 0; i < n; i++) if (h_files[i].idat_len > max_idat) max_idat = h_files[i].idat_len;
     DecodeParams p{};
-    int rc = decode_workspace_uniform_locked(n, w, h, chans, max_idat, s, p); if (rc) return rc;
+    VerifyState* verify = nullptr;
+    int rc = decode_workspace_uniform_locked(n, w, h, chans, max_idat, s, p, &verify); if (rc) return rc;
     g_dec_pin.pinned = true;
     rc = g_dec_pin.reserve((size_t)n * sizeof(FileDesc)); if (rc) return rc;
     // the pinned staging buffer may still be in flight from the previous call on another stream: wait for it
@@ -99,10 +108,19 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     FPNGB_CUDA_OK(cudaMemcpyAsync((void*)p.files, g_dec_pin.p, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
     FPNGB_CUDA_OK(cudaEventRecord(staged, s));
     p.d_files = d_files; p.d_status = d_status;
-    launch_decode(p, set_output(p, d_out, out), n, desired, s);
-    count_launch(8);
+    // the CRC kernel's message ("IDAT" + stream) plus its misalignment stays within max_idat + 8 bytes
+    launch_decode(p, set_output(p, d_out, out), n, desired, s, verify, (size_t)max_idat + 8);
+    count_launch(verify ? 10 : 8);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
+}
+
+// A device status of a file the host walked: FPNG_DECODE_NOT_FPNG for every stream violation (fpng.cpp:3131-3136), and the
+// verify kernels' FPNG_DECODE_FAILED_HEADER_CRC32 / FPNGB_DECODE_ADLER_MISMATCH as they are.
+static int host_status(uint32_t s)
+{
+    if (s == FPNGB_DECODE_FAILED_HEADER_CRC32 || s == FPNGB_DECODE_ADLER_MISMATCH) return (int)s;
+    return s ? FPNGB_DECODE_NOT_FPNG : FPNGB_DECODE_SUCCESS;
 }
 
 // the host instantiation of the container walk (container.cuh)
@@ -182,7 +200,7 @@ int fpngb_decode_host(const void* file, uint32_t size, void* out, size_t out_cap
     uint32_t* h_status = (uint32_t*)c.pin_small.p;
     cudaMemcpyAsync(h_status, d_status, 4, cudaMemcpyDeviceToHost, s);
     if (cudaStreamSynchronize(s) != cudaSuccess) return FPNGB_DECODE_INVALID_ARG;
-    if (*h_status) return FPNGB_DECODE_NOT_FPNG;                                                        // fpng.cpp:3131-3136
+    if (*h_status) return host_status(*h_status);
     cudaMemcpyAsync(out, c.dev_out.p, need, cudaMemcpyDeviceToHost, s);
     if (cudaStreamSynchronize(s) != cudaSuccess) return FPNGB_DECODE_INVALID_ARG;
     return FPNGB_DECODE_SUCCESS;
@@ -250,7 +268,7 @@ int fpngb_decode_batch_host(const void* const* files, const uint32_t* sizes, uin
             if (cudaEventSynchronize(ev_out[sl]) != cudaSuccess) { result = FPNGB_ERR_INTERNAL; break; }
             const uint32_t pf = (k - kSlots) * per_chunk, pc = (pf + per_chunk <= m) ? per_chunk : m - pf;
             const uint32_t* hs = (const uint32_t*)((uint8_t*)c.pin_small.p + sl * align_up(per_chunk * 4, 256));
-            for (uint32_t j = 0; j < pc; j++) status[idx[pf + j]] = hs[j] ? FPNGB_DECODE_NOT_FPNG : FPNGB_DECODE_SUCCESS;
+            for (uint32_t j = 0; j < pc; j++) status[idx[pf + j]] = host_status(hs[j]);
         }
         uint8_t* din = (uint8_t*)c.dev_in.p + sl * slot_in;
         uint8_t* dout = (uint8_t*)c.dev_out.p + sl * slot_out;
@@ -277,14 +295,23 @@ int fpngb_decode_batch_host(const void* const* files, const uint32_t* sizes, uin
             const int sl = k % kSlots;
             const uint32_t pf = k * per_chunk, pc = (pf + per_chunk <= m) ? per_chunk : m - pf;
             const uint32_t* hs = (const uint32_t*)((uint8_t*)c.pin_small.p + sl * align_up(per_chunk * 4, 256));
-            for (uint32_t j = 0; j < pc; j++) status[idx[pf + j]] = hs[j] ? FPNGB_DECODE_NOT_FPNG : FPNGB_DECODE_SUCCESS;
+            for (uint32_t j = 0; j < pc; j++) status[idx[pf + j]] = host_status(hs[j]);
         }
         if (cudaGetLastError() != cudaSuccess) result = FPNGB_ERR_INTERNAL;
     }
     return result;
 }
 
-// per-kernel device times (ms) of the most recent decode call made while profiling was on: prepare, scan, link, write, stored, unfilter
+// per-kernel device times (ms) of the most recent decode call made while profiling was on: prepare, scan, link, write, stored, unfilter,
+// and for a verified call IDAT CRC and Adler-32
+FPNGB_API int fpngb_set_decode_verify(int on)
+{
+    std::lock_guard<std::mutex> lk(context().mu);        // a call in flight keeps the setting it read
+    g_decode_verify.store(on != 0);
+    return FPNGB_OK;
+}
+FPNGB_API int fpngb_get_decode_verify(void) { return g_decode_verify.load(); }
+
 FPNGB_API int fpngb_decode_profile_enable(int on) { decode_profile_enable(on != 0); return 0; }
 FPNGB_API int fpngb_decode_profile_read(float* ms, int n) { return decode_profile_read(ms, n); }
 // test hook: number of subsequences the link pass had to decode again since the last reset (synchronises the device)
@@ -332,15 +359,16 @@ int fpngb_decode_packed_device_strided(const void* d_base, const uint64_t* d_off
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     // an IDAT chunk is shorter than its file: max_file_size bounds the stream of every file that reaches the decode kernels
     DecodeParams p{};
-    rc = decode_workspace_uniform_locked(n, w, h, chans_in_file, max_file_size, s, p); if (rc) return rc;
+    VerifyState* verify = nullptr;
+    rc = decode_workspace_uniform_locked(n, w, h, chans_in_file, max_file_size, s, p, &verify); if (rc) return rc;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = w; wp.h = h; wp.chans = chans_in_file;
     wp.out_stride = out.image;
     launch_container_walk(wp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status;
-    launch_decode(p, set_output(p, (uint8_t*)d_out, out), n, desired_chans, s);
-    count_launch(9);
+    launch_decode(p, set_output(p, (uint8_t*)d_out, out), n, desired_chans, s, verify, max_file_size);
+    count_launch(verify ? 11 : 9);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
 }
@@ -395,7 +423,8 @@ int fpngb_decode_packed_ragged_device(const void* d_base, size_t base_bytes, con
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     DecodeParams p{};
-    int rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p); if (rc) return rc;
+    VerifyState* verify = nullptr;
+    int rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify); if (rc) return rc;
     p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
@@ -407,8 +436,8 @@ int fpngb_decode_packed_ragged_device(const void* d_base, size_t base_bytes, con
     pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
     launch_decode_place(pp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
-    launch_decode(p, OutStrides{0, desired_chans, 1}, n, desired_chans, s);
-    count_launch(11);
+    launch_decode(p, OutStrides{0, desired_chans, 1}, n, desired_chans, s, verify, max_file_size);
+    count_launch(verify ? 13 : 11);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
 }

@@ -13,6 +13,7 @@
 //   D3 unfilter_kernel         inverse PNG filter 2 = running sum down each byte column (fpng.cpp:2439-2466 fuses it into
 //                              the serial loop) + 24<->32bpp conversion (alpha 0xFF / dropped)
 //   D2' decode_stored_kernel   stored-block files (fpng.cpp:2107-2207)
+//   V2 decode_adler_kernel     opt-in (fpngb_set_decode_verify): zlib Adler-32 of the inflated stream from the delta rows
 // Every stream violation the reference rejects ends in status FPNG_DECODE_NOT_FPNG (fpng.cpp:3131-3136).
 #include "row_walk.cuh"
 #include "kernels.cuh"
@@ -1255,6 +1256,80 @@ __global__ void __launch_bounds__(256) decode_stored_kernel(DecodeParams p)
 }
 
 // ------------------------------------------------------------------------------------------------
+// V2: zlib Adler-32 of the inflated stream, read back from the delta rows (verification on only; decode.cuh, VerifyState).  It runs
+// after the write and stored kernels and before unfilter_kernel, so a file whose checksum does not match gets no pixel.
+// Adler-32 is linear in the byte positions: with N = h * (w*c + 1) bytes x_i at positions i = 0 .. N-1,
+//     A = 1 + sum x_i,     B = N + N * sum x_i - sum i * x_i     (mod 65521),
+// so any partition of the stream will do.  One warp per delta row: each lane sums the bytes of its 16-byte vectors and their
+// column-weighted sum (two dp4a per word), the CTA reduces, one atomic per CTA and file adds the shares (each reduced mod 65521),
+// and the file's last CTA adds the filter bytes in closed form -- 0 on the first scanline and 2 below it in compressed files, 0
+// everywhere in stored files, as the write and stored kernels have checked -- and compares with the stream's last four bytes.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t kAdlerRows = 8;                  // delta rows per CTA, one per warp
+
+__global__ void __launch_bounds__(32 * kAdlerRows) decode_adler_kernel(VerifyParams p)
+{
+    __shared__ unsigned long long s_s1[kAdlerRows], s_s2[kAdlerRows];
+    const uint32_t f = blockIdx.y, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    if (p.state[f].status) return;                  // the same for every CTA of the file: only the last one writes it
+    const FileDesc fd = p.files[f];
+    const uint32_t h = fd.h, bpl = fd.w * fd.chans;
+    const uint32_t nctas = (h + kAdlerRows - 1) / kAdlerRows;
+    if (blockIdx.x >= nctas) return;
+    const uint32_t y = blockIdx.x * kAdlerRows + warp;
+    unsigned long long s1 = 0, s2 = 0;
+    if (y < h) {
+        const uint4* row = reinterpret_cast<const uint4*>(p.delta + fd.delta_base + (size_t)y * fd.pitch);   // 16-byte aligned
+        const uint32_t nvec = (bpl + 15u) >> 4;
+        uint32_t sx = 0;                            // sum of the lane's bytes
+        unsigned long long sxc = 0;                 // sum of column * byte
+#pragma unroll 4
+        for (uint32_t v = lane; v < nvec; v += 32) {
+            uint4 q = __ldg(row + v);
+            const uint32_t rem = bpl - 16u * v;     // the row's pitch padding is not part of the stream
+            if (rem < 16u) {
+                uint32_t* w = &q.x;
+#pragma unroll
+                for (uint32_t k = 0; k < 4; k++) w[k] &= 4u * k >= rem ? 0u : (4u * k + 4u <= rem ? 0xFFFFFFFFu : (1u << (8u * (rem - 4u * k))) - 1u);
+            }
+            const uint32_t s = __dp4a(q.x, 0x01010101u, __dp4a(q.y, 0x01010101u, __dp4a(q.z, 0x01010101u, __dp4a(q.w, 0x01010101u, 0u))));
+            const uint32_t t = __dp4a(q.x, 0x03020100u, __dp4a(q.y, 0x07060504u, __dp4a(q.z, 0x0B0A0908u, __dp4a(q.w, 0x0F0E0D0Cu, 0u))));
+            sx += s;
+            sxc += (unsigned long long)(16u * v) * s + t;
+        }
+        // byte x of row y is at stream position y * (bpl + 1) + 1 + x
+        const unsigned long long pos0 = ((unsigned long long)y * (bpl + 1ull) + 1ull) % kAdlerMod;
+        s1 = sx % kAdlerMod;
+        s2 = (pos0 * s1 + sxc % kAdlerMod) % kAdlerMod;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) { s1 += __shfl_xor_sync(kFullMask, s1, o); s2 += __shfl_xor_sync(kFullMask, s2, o); }
+    if (lane == 0) { s_s1[warp] = s1; s_s2[warp] = s2; }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    s1 = 0; s2 = 0;
+    for (uint32_t k = 0; k < kAdlerRows; k++) { s1 += s_s1[k]; s2 += s_s2[k]; }
+    VerifyState* vs = p.vs + f;
+    atomicAdd(&vs->s1, s1 % kAdlerMod);
+    atomicAdd(&vs->s2, s2 % kAdlerMod);
+    __threadfence();
+    if (atomicAdd(&vs->adler_done, 1u) != nctas - 1) return;
+    __threadfence();
+    unsigned long long S1 = atomicAdd(&vs->s1, 0ull) % kAdlerMod, S2 = atomicAdd(&vs->s2, 0ull) % kAdlerMod;
+    if (!p.state[f].stored && h > 1) {               // filter byte 2 at position y * (bpl + 1) of every row y >= 1
+        S1 = (S1 + 2ull * (h - 1)) % kAdlerMod;
+        S2 = (S2 + (bpl + 1ull) % kAdlerMod * h % kAdlerMod * (h - 1) % kAdlerMod) % kAdlerMod;   // 2 * (bpl + 1) * h (h - 1) / 2
+    }
+    const unsigned long long N = ((unsigned long long)h * (bpl + 1ull)) % kAdlerMod;
+    const uint32_t A = (uint32_t)((1ull + S1) % kAdlerMod);
+    const uint32_t B = (uint32_t)((N + N * S1 % kAdlerMod + kAdlerMod - S2) % kAdlerMod);
+    const uint8_t* z = p.d_files + fd.base + fd.idat_ofs + 8;
+    const uint8_t* q = z + fd.idat_len - 4;          // the write and stored kernels checked that the stream ends there
+    const uint32_t want = ((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | q[3];
+    if (((B << 16) | A) != want) p.state[f].status = 102u;   // FPNGB_DECODE_ADLER_MISMATCH
+}
+
+// ------------------------------------------------------------------------------------------------
 // D3: inverse Up filter (running sum down the columns) + channel conversion.  One thread per group of 4 pixels.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t vadd4(uint32_t a, uint32_t b)
@@ -1386,26 +1461,31 @@ __global__ void decode_status_kernel(DecodeParams p, uint32_t n)
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f < n) {
         const uint32_t pre = p.files[f].pre_status;
-        p.d_status[f] = pre ? pre : (p.state[f].status ? 1u /*FPNG_DECODE_NOT_FPNG*/ : 0u);
+        p.d_status[f] = pre ? pre : p.state[f].status;   // 0, 1 (FPNG_DECODE_NOT_FPNG), or a verify kernel's 4 / 102
     }
 }
 
 // Optional per-kernel timing of the decode pipeline (bench.py): events recorded between the launches of the most recent
 // call while profiling is on; fpngb_decode_profile_read() returns the device times of prepare, scan, link, write, stored,
-// unfilter (ms).
+// unfilter (ms), and for a verified call also the IDAT CRC (slot 6) and Adler-32 (slot 7) kernels.  Events 0..6 bound the six
+// slots; a verified call also records event 7 after the CRC kernel (scan then starts there) and event 8 after the Adler kernel
+// (unfilter then starts there).
 static bool g_dec_profile = false;
-static cudaEvent_t g_dec_ev[8];
-static bool g_dec_ev_ready = false, g_dec_ev_valid = false;
+static cudaEvent_t g_dec_ev[9];
+static bool g_dec_ev_ready = false, g_dec_ev_valid = false, g_dec_ev_verify = false;
 void decode_profile_enable(bool on)
 {
     g_dec_profile = on;
-    if (on && !g_dec_ev_ready) { for (int i = 0; i < 8; i++) cudaEventCreate(&g_dec_ev[i]); g_dec_ev_ready = true; }
+    if (on && !g_dec_ev_ready) { for (int i = 0; i < 9; i++) cudaEventCreate(&g_dec_ev[i]); g_dec_ev_ready = true; }
 }
 int decode_profile_read(float* ms, int n)
 {
     if (!g_dec_ev_valid) return 0;
     cudaEventSynchronize(g_dec_ev[6]);
-    for (int i = 0; i < n && i < 6; i++) { ms[i] = 0.f; cudaEventElapsedTime(&ms[i], g_dec_ev[i], g_dec_ev[i + 1]); }
+    int from[8] = {0, 1, 2, 3, 4, 5, 1, 5}, to[8] = {1, 2, 3, 4, 5, 6, 7, 8};
+    if (g_dec_ev_verify) { from[1] = 7; from[5] = 8; }
+    const int slots = g_dec_ev_verify ? 8 : 6;
+    for (int i = 0; i < n && i < slots; i++) { ms[i] = 0.f; cudaEventElapsedTime(&ms[i], g_dec_ev[from[i]], g_dec_ev[to[i]]); }
     return 1;
 }
 #define DEC_MARK(i) do { if (g_dec_profile && g_dec_ev_ready) cudaEventRecord(g_dec_ev[i], s); } while (0)
@@ -1430,13 +1510,20 @@ bool decode_set_pre_roll(uint32_t bits)
     return true;
 }
 
-void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n, uint32_t desired, cudaStream_t s)
+void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n, uint32_t desired, cudaStream_t s, VerifyState* verify,
+                   size_t max_file_bytes)
 {
     DecodeParams p = params;
     p.pre_roll = g_dec_pre_roll;
+    const VerifyParams vp{p.d_files, p.files, p.state, p.delta, verify};
+    if (verify) cudaMemsetAsync(verify, 0, (size_t)n * sizeof(VerifyState), s);
     DEC_MARK(0);
     decode_prepare_kernel<<<n, 32, 0, s>>>(p);
     DEC_MARK(1);
+    if (verify) {                                   // after prepare (which resets the state), before anything decodes the stream
+        launch_idat_crc_verify(vp, n, max_file_bytes, s);
+        DEC_MARK(7);
+    }
     const uint32_t sub_blocks = (p.max_subs + kDecThreads - 1) / kDecThreads;
     dim3 gsub(sub_blocks, n);
     constexpr size_t kDecSmem = (kFastWords + kWinSmemWords) * 4;
@@ -1456,6 +1543,10 @@ void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n,
     dim3 gs((p.max_h + 7) / 8, n);
     decode_stored_kernel<<<gs, 256, 0, s>>>(p);
     DEC_MARK(5);
+    if (verify) {                                   // every delta row is final; no pixel is written yet
+        decode_adler_kernel<<<dim3((p.max_h + kAdlerRows - 1) / kAdlerRows, n), 32 * kAdlerRows, 0, s>>>(vp);
+        DEC_MARK(8);
+    }
     const uint32_t groups = (p.max_w + 3) / 4;
     dim3 gu((groups + 127) / 128, n);
     const bool planar = os.pixel == 1;
@@ -1469,7 +1560,7 @@ void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n,
     }
     decode_status_kernel<<<(n + 127) / 128, 128, 0, s>>>(p, n);
     DEC_MARK(6);
-    if (g_dec_profile && g_dec_ev_ready) g_dec_ev_valid = true;
+    if (g_dec_profile && g_dec_ev_ready) { g_dec_ev_valid = true; g_dec_ev_verify = verify != nullptr; }
 }
 
 }  // namespace fpngb

@@ -86,6 +86,7 @@ namespace fpng
         if (need > 0xFFFFFFFFull) return FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE;
         out.resize((size_t)need);
         st = fpngb_decode_host(pImage, image_size, out.data(), out.size(), &width, &height, &channels_in_file, desired_channels);
+        // a damaged file (fpngb_set_decode_verify: FPNG_DECODE_FAILED_HEADER_CRC32 / FPNGB_DECODE_ADLER_MISMATCH) is not handed to the fallback
         if (st == FPNG_DECODE_NOT_FPNG) return try_fallback(pImage, image_size, out, width, height, channels_in_file, desired_channels);
         return st;
     }

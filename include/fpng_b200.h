@@ -141,7 +141,8 @@ FPNGB_API int fpngb_decode_host(const void* file, uint32_t size, void* out, size
  *   file_sizes/idat_ofs/idat_len[i] : HOST arrays from the container walk (fpngb_get_info_ex) -- chunk parsing stays on
  *                               the host exactly where the reference does it (src/fpng.cpp:2930-3077)
  *   d_out + i*out_stride      : w*h*desired_chans pixels of file i
- *   d_status[i]               : FPNGB_DECODE_SUCCESS or FPNGB_DECODE_NOT_FPNG (device memory, n x uint32)
+ *   d_status[i]               : FPNGB_DECODE_SUCCESS or FPNGB_DECODE_NOT_FPNG (device memory, n x uint32), or with
+ *                               fpngb_set_decode_verify(1) also FPNGB_DECODE_FAILED_HEADER_CRC32 / FPNGB_DECODE_ADLER_MISMATCH
  * Enqueued on `stream` (NULL = the CUDA default stream); does not synchronise. */
 FPNGB_API int fpngb_decode_batch_device(const void* d_files, size_t file_stride, const uint32_t* file_sizes,
                                         const uint32_t* idat_ofs, const uint32_t* idat_len, uint32_t n,
@@ -306,6 +307,33 @@ typedef int (*fpngb_fallback_decoder)(const void* file, uint32_t size, uint32_t 
                                       void** pixels, uint32_t* w, uint32_t* h, uint32_t* chans_in_file);
 FPNGB_API void fpngb_set_fallback_decoder(fpngb_fallback_decoder fn, void* user);
 FPNGB_API fpngb_fallback_decoder fpngb_get_fallback_decoder(void** user);
+
+/* ---- opt-in integrity check of the decode (lodepng and pvpng check both sums by default; the reference skips them) ----------
+ * The decoder, like the reference, checks the CRC of IHDR and of every ancillary chunk but not the IDAT chunk's CRC-32, and never
+ * computes the zlib Adler-32.  A damaged file can then decode to wrong pixels with status 0 when the fpng stream rules still hold
+ * (a changed byte inside a stored block; a changed bit that swaps two literal codes of the same length).
+ * fpngb_set_decode_verify(1) turns on both checks, on the GPU, in every decode call: fpngb_decode_host, fpngb_decode_batch_host,
+ *   fpngb_decode_batch_device(_strided), fpngb_decode_packed_device(_strided), fpngb_decode_packed_ragged_device, and the C++
+ *   fpng::fpng_decode_memory / fpng_decode_file.  fpngb_get_info* are unchanged.  One process-wide switch (fpng_decode_memory has
+ *   the reference's signature and cannot take a flag), off at load; it may be set before fpngb_init.  A call reads it once,
+ *   under the library's lock, when it enqueues.  Default off keeps statuses and pixels those of the reference.
+ * Per file, after every earlier status (argument checks, the walk, FPNGB_DECODE_SHAPE_MISMATCH, DIMENSIONS_TOO_LARGE,
+ *   FPNGB_DECODE_OUT_OF_SPACE), in this order:
+ *     1. the CRC-32 of "IDAT" + the chunk's data against its CRC field: FPNGB_DECODE_FAILED_HEADER_CRC32 (4), the code the walk
+ *        gives every other chunk with a bad CRC.  It wins over the stream checks, so a damaged file never comes back as
+ *        FPNGB_DECODE_NOT_FPNG, which sends fpng_decode_memory's callers to their general-PNG fallback;
+ *     2. FPNGB_DECODE_NOT_FPNG from the stream, as without the check;
+ *     3. the Adler-32 of the inflated stream (filter bytes included) against the stream's last four bytes:
+ *        FPNGB_DECODE_ADLER_MISMATCH.
+ *   A file with status 4 or 102 gets none of its pixels written; the other files of the call decode as with the switch off.
+ *   The C++ wrappers do not call the fallback decoder for these two codes.
+ * Cost: two more kernels per call (the stream CRC kernel over every file, a pass over the delta rows before the pixels are
+ *   written) and one cudaMemsetAsync of 32 bytes per file; fpngb_launch_count grows by 2 per call (per chunk of
+ *   fpngb_decode_batch_host), and fpngb_decode_profile_read reports the two kernels in slots 6 (CRC) and 7 (Adler-32).
+ *   Still stream-ordered: no host synchronisation is added.  Returns FPNGB_OK; the getter returns 0 or 1. */
+enum { FPNGB_DECODE_ADLER_MISMATCH = 102 };   /* verified decode only: the zlib Adler-32 does not match the inflated stream */
+FPNGB_API int fpngb_set_decode_verify(int on);
+FPNGB_API int fpngb_get_decode_verify(void);
 
 /* Pins the calling thread to the CPUs of the NUMA node of the library's GPU (sysfs: the GPU's PCI device -> numa_node ->
  * cpulist), so that pinned buffers allocated afterwards and the thread that issues the H2D/D2H copies are local to the GPU's
