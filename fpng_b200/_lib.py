@@ -12,6 +12,11 @@ _lib = None
 u32p = C.POINTER(C.c_uint32)
 
 
+class PixelFormat(C.Structure):
+    """fpngb_pixel_format: the output type (FPNGB_DTYPE_*) and per-channel scale and bias of the *_typed decode calls"""
+    _fields_ = [("dtype", C.c_uint32), ("scale", C.c_float * 4), ("bias", C.c_float * 4)]
+
+
 def lib() -> C.CDLL:
     global _lib
     if _lib is not None:
@@ -67,6 +72,15 @@ def lib() -> C.CDLL:
     L.fpngb_decode_packed_ragged_device.restype = C.c_int
     L.fpngb_decode_packed_ragged_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p] + [C.c_uint32] * 5 + \
         [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.fpngb_decode_batch_device_typed.restype = C.c_int
+    L.fpngb_decode_batch_device_typed.argtypes = L.fpngb_decode_batch_device_strided.argtypes[:-2] + [C.POINTER(PixelFormat), C.c_void_p,
+                                                                                                   C.c_void_p]
+    L.fpngb_decode_packed_device_typed.restype = C.c_int
+    L.fpngb_decode_packed_device_typed.argtypes = L.fpngb_decode_packed_device_strided.argtypes[:-2] + [C.POINTER(PixelFormat), C.c_void_p,
+                                                                                                     C.c_void_p]
+    L.fpngb_decode_packed_ragged_device_typed.restype = C.c_int
+    L.fpngb_decode_packed_ragged_device_typed.argtypes = L.fpngb_decode_packed_ragged_device.argtypes[:-2] + [C.POINTER(PixelFormat),
+                                                                                                           C.c_void_p, C.c_void_p]
     L.fpngb_compact_batch_device.restype = C.c_int
     L.fpngb_compact_batch_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.fpngb_compact_packed_device.restype = C.c_int

@@ -12,7 +12,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import FpngB200Error, check, lib
+from ._lib import FpngB200Error, PixelFormat, check, lib
 
 FPNG_ENCODE_SLOWER = 1          # src/fpng.h:38
 FPNG_FORCE_UNCOMPRESSED = 2     # src/fpng.h:41
@@ -282,6 +282,75 @@ def _strided_out(out, n, h, w, desired_channels):
     return layout_strides(out.shape, out.stride())
 
 
+_DTYPE_CODES = {"float32": 1, "float16": 2, "bfloat16": 3}   # FPNGB_DTYPE_*
+
+
+def _out_dtype(out, dtype):
+    """the output dtype of a decode call: out's when given (dtype must then agree), else dtype, else torch.uint8"""
+    import torch
+
+    if out is not None:
+        if dtype is not None and dtype != out.dtype:
+            raise ValueError(f"dtype {dtype} differs from out.dtype {out.dtype}")
+        return out.dtype
+    return torch.uint8 if dtype is None else dtype
+
+
+def _per_channel(v, desired_channels, default, what):
+    if v is None:
+        return [default] * desired_channels
+    a = np.asarray(v.detach().cpu().numpy() if hasattr(v, "detach") else v, dtype=np.float32).reshape(-1)
+    if a.size == 1:
+        a = np.repeat(a, desired_channels)
+    if a.size != desired_channels:
+        raise ValueError(f"{what}: one value or one per output channel ({desired_channels}), got {a.size}")
+    return [float(x) for x in a]
+
+
+def _pixel_format(dtype, scale, bias, desired_channels):
+    """None for uint8 output (the uint8 calls, which take no scale or bias), else the fpngb_pixel_format of a float output:
+    scale defaults to 1 and bias to 0 per channel; a single value applies to every channel.  Values are rounded to float32."""
+    import torch
+
+    if dtype == torch.uint8:
+        if scale is not None or bias is not None:
+            raise ValueError("scale and bias apply to float32 / float16 / bfloat16 output only; uint8 pixels are written as decoded")
+        return None
+    code = _DTYPE_CODES.get(str(dtype).replace("torch.", ""))
+    if code is None:
+        raise ValueError(f"output dtype {dtype}: torch.uint8, float32, float16 or bfloat16")
+    fmt = PixelFormat()
+    fmt.dtype = code
+    fmt.scale[:desired_channels] = _per_channel(scale, desired_channels, 1.0, "scale")
+    fmt.bias[:desired_channels] = _per_channel(bias, desired_channels, 0.0, "bias")
+    return fmt
+
+
+def typed_layout(shape, strides, element_size):
+    """Byte strides (image_stride, row_pitch, pixel_stride, chan_stride) of an [n, h, w, chans] view whose elements are
+    element_size bytes, as the *_typed C calls take them: layout_strides applied to the element strides torch reports, then
+    multiplied by the element size.  NCHW float output is torch.empty(n, c, h, w, dtype=...).permute(0, 2, 3, 1)."""
+    return tuple(v * int(element_size) for v in layout_strides(shape, strides))
+
+
+def normalize_scale_bias(mean, std, max_value=255.0):
+    """The (scale, bias) pair, float32 arrays, for which the typed decode computes (x - mean) / std of x = v / max_value:
+    scale = 1 / (max_value * std) and bias = -mean / std, computed in float64 and then rounded to float32.  ImageNet:
+    normalize_scale_bias((0.485, 0.456, 0.406), (0.229, 0.224, 0.225)).
+
+    The decode computes v * scale + bias (two rounded fp32 operations), not torchvision's Normalize(mean, std)(v / 255), which
+    divides, subtracts and divides again; the results can therefore differ in the last bits."""
+    m = np.asarray(mean, dtype=np.float64).reshape(-1)
+    sd = np.asarray(std, dtype=np.float64).reshape(-1)
+    return (1.0 / (float(max_value) * sd)).astype(np.float32), (-m / sd).astype(np.float32)
+
+
+def _typed_out(out, n, h, w, desired_channels):
+    """the byte strides of a float `out` (any [n, h, w, desired_channels] view in one of the layouts of layout_strides)"""
+    assert out.is_cuda and tuple(out.shape) == (n, h, w, desired_channels), "out must be an [n, h, w, desired_channels] CUDA view"
+    return typed_layout(out.shape, out.stride(), out.element_size())
+
+
 def get_info_ex(data):
     """fpng_get_info plus (idat_ofs, idat_len): the host-side container walk (src/fpng.cpp:2930-3077)."""
     a = _u8(data)
@@ -316,17 +385,23 @@ def pack_files_for_device(files, device=None):
 
 
 def decode_batch_device(files_dev, sizes, idat_ofs, idat_len, w: int, h: int, chans_in_file: int, desired_channels: int,
-                        out=None, status=None, stream=None):
+                        out=None, status=None, stream=None, dtype=None, scale=None, bias=None):
     """Decode n fpng files resident on the device (tensor [n, stride] uint8). Returns (pixels [n, h, w, desired], status [n]).
     out may be any non-overlapping [n, h, w, desired] view in one of the two layouts of layout_strides, e.g.
-    torch.empty(n, desired, h, w).permute(0, 2, 3, 1) for NCHW pixels; the kernels write it in place."""
+    torch.empty(n, desired, h, w).permute(0, 2, 3, 1) for NCHW pixels; the kernels write it in place.
+    The output dtype is out.dtype when out is given, else dtype (default torch.uint8).  torch.float32 / float16 / bfloat16 store
+    T(v * scale[c] + bias[c]) for every uint8 value v of channel c, converted in the decoder's last kernel (scale defaults to 1,
+    bias to 0; one value or one per channel; normalize_scale_bias turns a mean / std into them).  uint8 output takes no scale
+    or bias (ValueError)."""
     import torch
 
     assert files_dev.is_cuda and files_dev.dtype == torch.uint8 and files_dev.dim() == 2 and files_dev.is_contiguous()
     n = files_dev.shape[0]
+    odt = _out_dtype(out, dtype)
+    fmt = _pixel_format(odt, scale, bias, desired_channels)
     if out is None:
-        out = torch.empty((n, h, w, desired_channels), dtype=torch.uint8, device=files_dev.device)
-    layout = _strided_out(out, n, h, w, desired_channels)
+        out = torch.empty((n, h, w, desired_channels), dtype=odt, device=files_dev.device)
+    layout = _strided_out(out, n, h, w, desired_channels) if fmt is None else _typed_out(out, n, h, w, desired_channels)
     if status is None:
         status = torch.empty((n,), dtype=torch.int32, device=files_dev.device)
     s = stream if stream is not None else torch.cuda.current_stream(files_dev.device).cuda_stream
@@ -334,7 +409,9 @@ def decode_batch_device(files_dev, sizes, idat_ofs, idat_len, w: int, h: int, ch
     idat_len = np.ascontiguousarray(idat_len, dtype=np.uint32)
     args = (files_dev.data_ptr(), files_dev.stride(0), sizes.ctypes.data_as(C.c_void_p), idat_ofs.ctypes.data_as(C.c_void_p),
             idat_len.ctypes.data_as(C.c_void_p), n, w, h, chans_in_file, desired_channels, out.data_ptr())
-    if layout is None:
+    if fmt is not None:
+        rc = lib().fpngb_decode_batch_device_typed(*args, *layout, C.byref(fmt), status.data_ptr(), s)
+    elif layout is None:
         rc = lib().fpngb_decode_batch_device(*args, h * w * desired_channels, status.data_ptr(), s)
     else:
         rc = lib().fpngb_decode_batch_device_strided(*args, *layout, status.data_ptr(), s)
@@ -375,7 +452,7 @@ def get_info_batch_device(data, offsets, sizes, stream=None):
 
 
 def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: int, desired_channels: int, max_file_size=None,
-                         out=None, status=None, stream=None):
+                         out=None, status=None, stream=None, dtype=None, scale=None, bias=None):
     """Decode the w x h x chans_in_file fpng files packed in device memory (same arguments as get_info_batch_device; every
     file 4-byte aligned).  The container walk runs on the device: no host synchronisation and no host copy.
     Returns (pixels uint8 [n, h, w, desired_channels], status int32 [n]); out may be a strided view as in decode_batch_device.  status[i] is fpng_decode_memory's code for file i,
@@ -383,23 +460,27 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
     max_file_size or an offset that is not a multiple of 4; pixels of files with a non-zero status are left untouched.
     max_file_size (bytes) bounds every file and sizes the decoder's workspace; the default, max_encoded_size(w, h,
     chans_in_file), holds for every file this library or the reference encoder writes.  A smaller bound known to the
-    caller saves workspace and launch overhead."""
+    caller saves workspace and launch overhead.  dtype, scale and bias as in decode_batch_device."""
     import torch
 
     n = _packed_args(data, offsets, sizes)
     if max_file_size is None:
         max_file_size = min(max_encoded_size(w, h, chans_in_file), 0xFFFFFFFF)
+    odt = _out_dtype(out, dtype)
+    fmt = _pixel_format(odt, scale, bias, desired_channels)
     if out is None:
-        out = torch.empty((n, h, w, desired_channels), dtype=torch.uint8, device=data.device)
+        out = torch.empty((n, h, w, desired_channels), dtype=odt, device=data.device)
     if status is None:
         status = torch.empty((n,), dtype=torch.int32, device=data.device)
-    layout = _strided_out(out, n, h, w, desired_channels)
+    layout = _strided_out(out, n, h, w, desired_channels) if fmt is None else _typed_out(out, n, h, w, desired_channels)
     assert layout is not None or out.numel() >= n * h * w * desired_channels
     assert status.is_cuda and status.dtype == torch.int32 and status.is_contiguous() and status.numel() >= n
     s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
     args = (data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, max_file_size, w, h, chans_in_file, desired_channels,
             out.data_ptr())
-    if layout is None:
+    if fmt is not None:
+        rc = lib().fpngb_decode_packed_device_typed(*args, *layout, C.byref(fmt), status.data_ptr(), s)
+    elif layout is None:
         rc = lib().fpngb_decode_packed_device(*args, h * w * desired_channels, status.data_ptr(), s)
     else:
         rc = lib().fpngb_decode_packed_device_strided(*args, *layout, status.data_ptr(), s)
@@ -410,9 +491,10 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
 FPNGB_DECODE_OUT_OF_SPACE = 101    # decode_packed_ragged_device only: the file's pixels do not fit in `out`
 
 
-def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h, stream):
-    """The bounds of decode_packed_ragged_device the caller left out, and the exact output size they give: one device walk
-    (get_info_batch_device) and one read-back of (info, sizes, offsets), which synchronises with the stream."""
+def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h, stream, element_size=1):
+    """The bounds of decode_packed_ragged_device the caller left out, and the exact output size in bytes they give for elements
+    of element_size bytes: one device walk (get_info_batch_device) and one read-back of (info, sizes, offsets), which
+    synchronises with the stream."""
     import torch
 
     info = get_info_batch_device(data, offsets, sizes, stream)
@@ -430,12 +512,12 @@ def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max
     px = w * h * desired_channels
     placed = (walked & (size <= max_file_size) & (ofs % 4 == 0) & (ofs + size <= data.numel()) & (w <= max_w) & (h <= max_h)
               & (px <= 0xFFFFFFFF))
-    total = int(((px[placed] + 15) // 16 * 16).sum())
+    total = int(((px[placed] * element_size + 15) // 16 * 16).sum())
     return max_file_size, max_w, max_h, total
 
 
 def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out=None, max_file_size=None, max_w=None, max_h=None,
-                                stream=None):
+                                stream=None, dtype=None, scale=None, bias=None):
     """Decode fpng files of ANY shapes and channel counts packed in device memory (the layout of get_info_batch_device; base_bytes
     is data.numel()) in one call, pixels placed back to back.  Returns (out uint8 [out_cap], out_offsets int64 [n + 1],
     info int32 [n, 6], status int32 [n]):
@@ -449,32 +531,40 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     With `out` (a flat, 16-byte aligned uint8 CUDA tensor) and all three bounds given, the call is stream-ordered: no host
     synchronisation.  Any of them that is None is computed from one get_info_batch_device and one read-back to the host, which
     waits for the stream: max_file_size, max_w and max_h become the largest size, width and height of the files the container
-    walk accepts, and out is allocated at the exact total.  Tight bounds save workspace and launch overhead."""
+    walk accepts, and out is allocated at the exact total.  Tight bounds save workspace and launch overhead.
+    dtype, scale and bias as in decode_batch_device: with a float output, out is a flat tensor of that dtype, file i takes
+    align_up(h*w*desired_channels*element_size, 16) bytes, and out_offsets stay in bytes (ragged_views converts them)."""
     import torch
 
     n = _packed_args(data, offsets, sizes)
     assert desired_channels in (3, 4), "desired_channels: 3 or 4"
+    odt = _out_dtype(out, dtype)
+    fmt = _pixel_format(odt, scale, bias, desired_channels)
+    es = torch.empty((), dtype=odt).element_size()
     if out is None or max_file_size is None or max_w is None or max_h is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
-                                                             stream)
+                                                             stream, es)
         if out is None:
-            out = torch.empty((max(total, 16),), dtype=torch.uint8, device=data.device)[:total]
-    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous(), "out: flat uint8 CUDA tensor"
+            out = torch.empty((max(total, 16) // es,), dtype=odt, device=data.device)[:total // es]
+    assert out.is_cuda and out.dtype == odt and out.is_contiguous() and out.dim() == 1, "out: flat CUDA tensor of the output dtype"
     out_offsets = torch.empty((n + 1,), dtype=torch.int64, device=data.device)
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
     status = torch.empty((n,), dtype=torch.int32, device=data.device)
     s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
-    rc = lib().fpngb_decode_packed_ragged_device(data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n,
-                                                 min(int(max_file_size), 0xFFFFFFFF), int(max_w), int(max_h), desired_channels,
-                                                 out.data_ptr(), out.numel(), out_offsets.data_ptr(), info.data_ptr(),
-                                                 status.data_ptr(), s)
+    args = (data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
+            int(max_h), desired_channels, out.data_ptr(), out.numel() * es, out_offsets.data_ptr(), info.data_ptr())
+    if fmt is None:
+        rc = lib().fpngb_decode_packed_ragged_device(*args, status.data_ptr(), s)
+    else:
+        rc = lib().fpngb_decode_packed_ragged_device_typed(*args, C.byref(fmt), status.data_ptr(), s)
     check(rc, "decode_packed_ragged_device")
     return out, out_offsets, info, status
 
 
 def ragged_views(out, out_offsets, info, status, desired_channels: int):
-    """Per file of a decode_packed_ragged_device result, an [h, w, desired_channels] view into `out`, or None when the file's
-    status is not 0.  Reads out_offsets, info and status back to the host, so it waits for the device."""
+    """Per file of a decode_packed_ragged_device result, an [h, w, desired_channels] view into `out` (any dtype: the byte offsets
+    become element offsets), or None when the file's status is not 0.  Reads out_offsets, info and status back to the host, so
+    it waits for the device."""
     offs = out_offsets.cpu().numpy()
     inf = info.cpu().numpy()
     st = status.cpu().numpy()
@@ -484,7 +574,7 @@ def ragged_views(out, out_offsets, info, status, desired_channels: int):
             views.append(None)
             continue
         w, h = int(inf[i, 1]), int(inf[i, 2])
-        o = int(offs[i])
+        o = int(offs[i]) // out.element_size()
         views.append(out[o:o + h * w * desired_channels].view(h, w, desired_channels))
     return views
 

@@ -89,7 +89,7 @@ __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams
         if (i < p.n) { fd = p.files[i]; placed = fd.pre_status == 0; }
         unsigned long long v[3] = {0ull, 0ull, 0ull};
         if (placed) {
-            v[0] = ((unsigned long long)fd.w * fd.h * p.desired + 15ull) & ~15ull;
+            v[0] = ((unsigned long long)fd.w * fd.h * p.px_bytes + 15ull) & ~15ull;
             v[1] = (unsigned long long)fd.h * fd.pitch;
             v[2] = subs_for(fd.file_size);
         }

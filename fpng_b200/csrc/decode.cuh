@@ -66,6 +66,12 @@ struct OutStrides {
     size_t row, pixel, chan;                // interleaved (pixel = desired, chan = 1) or planar (pixel = 1); row 0: tight rows of each
                                             // file's own width (w * desired, the ragged call)
 };
+// Typed output of the decode (fpngb_pixel_format, the *_typed calls): unfilter_typed_kernel stores every value v of output
+// channel c as T(__fadd_rn(__fmul_rn(float(v), scale[c]), bias[c])), T = float / __half / __nv_bfloat16 (dtype is the
+// FPNGB_DTYPE_* value).  A separate kernel argument, as OutStrides is, so that no other kernel's parameter block grows; the
+// OutStrides of a typed call are in bytes, with pixel == sizeof(T) for planar output.
+struct PixelAffine { float scale[4], bias[4]; };
+struct TypedOut { uint32_t dtype; PixelAffine aff; };
 // Opt-in integrity check of every decode call (fpngb_set_decode_verify).  Two kernels read the file and the delta rows again:
 //   idat_crc_stream_kernel<false, true> (crc_stream_kernel.cu), after decode_prepare_kernel: the CRC-32 of "IDAT" + idat_len data
 //     bytes against the chunk's CRC field; a mismatch sets DecodeState::status to 4 for every file the walk passed, whatever the
@@ -83,9 +89,12 @@ struct VerifyParams {
     VerifyState* vs;                        // [n]
 };
 // verify: the call's [n] accumulators, or nullptr (verification off: the pipeline is exactly the unverified one);
-// max_file_bytes: a bound of every file's size (the CRC kernel's grid)
+// max_file_bytes: a bound of every file's size (the CRC kernel's grid); typed: nullptr for uint8 pixels (unfilter_kernel), else the
+// output type and affine map of unfilter_typed_kernel, which takes the same launch slot
 void launch_decode(const DecodeParams& p, const OutStrides& out, uint32_t n, uint32_t desired, cudaStream_t s,
-                   VerifyState* verify = nullptr, size_t max_file_bytes = 0);
+                   VerifyState* verify = nullptr, size_t max_file_bytes = 0, const TypedOut* typed = nullptr);
+// unfilter_typed_kernel (decode_typed_kernels.cu) in launch_decode's unfilter slot, grid g
+void launch_unfilter_typed(const DecodeParams& p, const OutStrides& os, const TypedOut& t, uint32_t desired, dim3 g, cudaStream_t s);
 void launch_idat_crc_verify(const VerifyParams& p, uint32_t n, size_t max_file_bytes, cudaStream_t s);
 void decode_profile_enable(bool on);
 int decode_profile_read(float* ms, int n);
@@ -114,11 +123,12 @@ struct WalkParams {
 void launch_container_walk(const WalkParams& p, cudaStream_t s);
 
 // decode_place_kernel (container_kernels.cu), ragged call: one CTA places the files the walk accepted, in index order.  File i
-// takes align_up(w*h*desired, 16) output bytes, h * pitch delta bytes and subs_for(file_size) records; out_offsets[i] is the
+// takes align_up(w*h*px_bytes, 16) output bytes, h * pitch delta bytes and subs_for(file_size) records; out_offsets[i] is the
 // running output offset (a rejected file takes nothing), out_offsets[n] the total, with bit 63 set when it exceeds out_cap.
 // A file whose output, delta rows or records end past out_cap / delta_cap / sub_cap gets FPNGB_DECODE_OUT_OF_SPACE.
 struct PlaceParams {
-    FileDesc* files; uint32_t n, desired;
+    FileDesc* files; uint32_t n;
+    uint32_t px_bytes;                      // output bytes per pixel: desired * sizeof(T) (desired for uint8 pixels)
     unsigned long long out_cap, delta_cap, sub_cap;
     unsigned long long* out_offsets;        // [n + 1]
 };

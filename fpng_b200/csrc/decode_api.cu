@@ -5,6 +5,7 @@
 #include "container.cuh"
 #include "layout.h"
 #include "runtime.h"
+#include <math.h>
 #include <string.h>
 #include <atomic>
 #include <vector>
@@ -71,21 +72,42 @@ static int decode_shape_check(uint32_t w, uint32_t h, uint32_t chans_in_file, ui
     if ((uint64_t)w * h * desired_chans > 0xFFFFFFFFull) return FPNGB_ERR_BUFFER_TOO_SMALL;
     return FPNGB_OK;
 }
-// A strided output must be interleaved or planar, addressable, and no two pixels may share a byte.
+// A strided output of elem-byte elements (1: uint8 pixels) must be elem-aligned, interleaved or planar in elements, addressable,
+// and no two elements may share a byte.  L receives the byte strides.
 static int decode_output_check(const void* d_out, size_t image, size_t row, size_t pixel, size_t chan, uint32_t n, uint32_t w, uint32_t h,
-                               uint32_t desired, Layout& L)
+                               uint32_t desired, size_t elem, Layout& L)
 {
+    if ((uintptr_t)d_out % elem || image % elem || row % elem || pixel % elem || chan % elem) return FPNGB_ERR_ALIGNMENT;
     uint64_t last = 0;
-    if (!classify_layout(image, row, pixel, chan, n, h, w, desired, L) || !layout_disjoint(L, n, h, w, desired) ||
-        !layout_span(d_out, L, n, h, w, desired, last))
+    if (!classify_layout(image / elem, row / elem, pixel / elem, chan / elem, n, h, w, desired, L) || !layout_disjoint(L, n, h, w, desired))
         return FPNGB_ERR_INVALID_ARG;
+    L.image *= elem; L.row *= elem; L.pixel *= elem; L.chan *= elem;
+    if (!layout_span(d_out, L, n, h, w, desired, last) || last > UINT64_MAX - (uint64_t)(uintptr_t)d_out - (elem - 1))
+        return FPNGB_ERR_INVALID_ARG;
+    return FPNGB_OK;
+}
+
+// The output type of a *_typed call (desired is 3 or 4): FPNGB_ERR_INVALID_ARG for a NULL fmt, another dtype, or a scale or bias
+// in use that is not finite.  elem receives sizeof(T).
+static int typed_format(const fpngb_pixel_format* fmt, uint32_t desired, TypedOut& t, size_t& elem)
+{
+    if (!fmt || (fmt->dtype != FPNGB_DTYPE_FLOAT32 && fmt->dtype != FPNGB_DTYPE_FLOAT16 && fmt->dtype != FPNGB_DTYPE_BFLOAT16))
+        return FPNGB_ERR_INVALID_ARG;
+    t = TypedOut{};
+    t.dtype = fmt->dtype;
+    for (uint32_t c = 0; c < desired; c++) {
+        if (!isfinite(fmt->scale[c]) || !isfinite(fmt->bias[c])) return FPNGB_ERR_INVALID_ARG;
+        t.aff.scale[c] = fmt->scale[c]; t.aff.bias[c] = fmt->bias[c];
+    }
+    elem = fmt->dtype == FPNGB_DTYPE_FLOAT32 ? 4 : 2;
     return FPNGB_OK;
 }
 
 // Enqueue the decode pipeline for n files already resident on the device, file i at d_files + i * file_stride, described by host
 // FileDescs (their base and pre_status are set here).  Caller holds context().mu.
 static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const FileDesc* h_files, uint32_t n, uint32_t w, uint32_t h,
-                               uint32_t chans, uint32_t desired, uint8_t* d_out, const Layout& out, uint32_t* d_status, cudaStream_t s)
+                               uint32_t chans, uint32_t desired, uint8_t* d_out, const Layout& out, uint32_t* d_status, cudaStream_t s,
+                               const TypedOut* typed = nullptr)
 {
     uint32_t max_idat = 0;
     for (uint32_t i = 0; i < n; i++) if (h_files[i].idat_len > max_idat) max_idat = h_files[i].idat_len;
@@ -109,7 +131,7 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     FPNGB_CUDA_OK(cudaEventRecord(staged, s));
     p.d_files = d_files; p.d_status = d_status;
     // the CRC kernel's message ("IDAT" + stream) plus its misalignment stays within max_idat + 8 bytes
-    launch_decode(p, set_output(p, d_out, out), n, desired, s, verify, (size_t)max_idat + 8);
+    launch_decode(p, set_output(p, d_out, out), n, desired, s, verify, (size_t)max_idat + 8, typed);
     count_launch(verify ? 10 : 8);
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
@@ -132,6 +154,132 @@ int container_info(const uint8_t* f, uint32_t size, uint32_t* w, uint32_t* h, ui
     return container_walk(f, size, HostCrc{}, w, h, chans, idat_ofs, idat_len);
 }
 
+// The bodies of the device decode entry points: typed false is the uint8 call (fmt unused), true the *_typed one.
+static int decode_batch_device_impl(const void* d_files, size_t file_stride, const uint32_t* file_sizes, const uint32_t* idat_ofs,
+                                    const uint32_t* idat_len, uint32_t n, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                                    uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                    size_t out_pixel_stride, size_t out_chan_stride, bool typed, const fpngb_pixel_format* fmt,
+                                    uint32_t* d_status, void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_files || !file_sizes || !idat_ofs || !idat_len || !d_out || !d_status || n == 0 || n > 65535) return FPNGB_ERR_INVALID_ARG;
+    int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
+    TypedOut t{};
+    size_t elem = 1;
+    if (typed) { rc = typed_format(fmt, desired_chans, t, elem); if (rc) return rc; }
+    Layout out;
+    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, elem, out);
+    if (rc) return rc;
+    if (file_stride % 4 || (uintptr_t)d_files % 4) return FPNGB_ERR_ALIGNMENT;
+    std::vector<FileDesc> fds(n);
+    for (uint32_t i = 0; i < n; i++) {
+        if ((uint64_t)idat_ofs[i] + 8 + idat_len[i] + 4 > file_sizes[i] || file_sizes[i] > file_stride) return FPNGB_ERR_INVALID_ARG;
+        fds[i] = FileDesc{}; fds[i].file_size = file_sizes[i]; fds[i].idat_ofs = idat_ofs[i]; fds[i].idat_len = idat_len[i];
+    }
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    return decode_batch_locked((const uint8_t*)d_files, file_stride, fds.data(), n, w, h, chans_in_file, desired_chans, (uint8_t*)d_out,
+                               out, d_status, (cudaStream_t)stream, typed ? &t : nullptr);
+}
+
+static int decode_packed_device_impl(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
+                                     uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out,
+                                     size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride, size_t out_chan_stride,
+                                     bool typed, const fpngb_pixel_format* fmt, int32_t* d_status, void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_status || n == 0 || n > 65535 || !max_file_size) return FPNGB_ERR_INVALID_ARG;
+    int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
+    TypedOut t{};
+    size_t elem = 1;
+    if (typed) { rc = typed_format(fmt, desired_chans, t, elem); if (rc) return rc; }
+    Layout out;
+    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, elem, out);
+    if (rc) return rc;
+    if ((uintptr_t)d_base % 4) return FPNGB_ERR_ALIGNMENT;
+    const cudaStream_t s = (cudaStream_t)stream;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    // an IDAT chunk is shorter than its file: max_file_size bounds the stream of every file that reaches the decode kernels
+    DecodeParams p{};
+    VerifyState* verify = nullptr;
+    rc = decode_workspace_uniform_locked(n, w, h, chans_in_file, max_file_size, s, p, &verify); if (rc) return rc;
+    WalkParams wp{};
+    wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n;
+    wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = w; wp.h = h; wp.chans = chans_in_file;
+    wp.out_stride = out.image;
+    launch_container_walk(wp, s);
+    p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status;
+    launch_decode(p, set_output(p, (uint8_t*)d_out, out), n, desired_chans, s, verify, max_file_size, typed ? &t : nullptr);
+    count_launch(verify ? 11 : 9);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return context().ws_release(s);
+}
+
+// Workspace of the ragged call, from call arguments only (no host synchronisation).  Only files decode_place_kernel places and
+// that fit in out_cap are decoded; they are a prefix of the placed files, so for every one of them the sums below run over
+// decoded files alone.
+//   records:   subs_for(s) <= s/128 + 3 per file of s bytes; files that lie inside the buffer and do not overlap have sizes that
+//              sum to at most base_bytes, so base_bytes/128 + 3n records hold them all.  Every file also has s <= max_file_size.
+//   delta:     a file needs h * align_up(w*c, 16) <= (4/desired) * (w*h*desired) + 15h bytes, h <= max_h and h <= w*h, and the
+//              w*h*desired of the decoded files sum to at most out_cap.  Every file also needs at most max_h * pitch(max_w, 4).
+// A file whose range still ends past a bound (overlapping files) gets FPNGB_DECODE_OUT_OF_SPACE from decode_place_kernel.
+static unsigned long long sat_u64(unsigned __int128 v) { return v > ~0ull ? ~0ull : (unsigned long long)v; }
+static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired,
+                             size_t out_cap, unsigned long long& sub_cap, unsigned long long& delta_cap)
+{
+    typedef unsigned __int128 u128;
+    const u128 by_bytes = (u128)base_bytes / 128 + 3 * (u128)n, by_max = (u128)n * subs_for(max_file_size);
+    sub_cap = sat_u64(by_bytes < by_max ? by_bytes : by_max);
+    const u128 rows = (u128)n * max_h, rows_px = ((u128)out_cap + desired - 1) / desired;
+    const u128 by_out = ((u128)out_cap * 4 + desired - 1) / desired + 16 * (rows < rows_px ? rows : rows_px);
+    const u128 by_shape = rows * delta_pitch(max_w, 4);
+    delta_cap = sat_u64(by_out < by_shape ? by_out : by_shape);
+}
+
+static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                     uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
+                                     size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
+                                     int32_t* d_status, void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_out_offsets || !d_status || n == 0 || n > 65535 || !max_file_size ||
+        (desired_chans != 3 && desired_chans != 4) || !max_w || !max_h || max_w > (1u << 24) || max_h > (1u << 24))
+        return FPNGB_ERR_INVALID_ARG;
+    TypedOut t{};
+    size_t elem = 1;
+    if (typed) { const int rc = typed_format(fmt, desired_chans, t, elem); if (rc) return rc; }
+    if ((uintptr_t)d_base % 4 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    unsigned long long sub_cap = 0, delta_cap = 0;
+    // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
+    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, sub_cap, delta_cap);
+    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    const cudaStream_t s = (cudaStream_t)stream;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    DecodeParams p{};
+    VerifyState* verify = nullptr;
+    int rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify); if (rc) return rc;
+    p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
+    WalkParams wp{};
+    wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
+    wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
+    wp.base_bytes = base_bytes;
+    launch_container_walk(wp, s);
+    PlaceParams pp{};
+    pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * (uint32_t)elem;
+    pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
+    launch_decode_place(pp, s);
+    p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
+    launch_decode(p, OutStrides{0, desired_chans * elem, elem}, n, desired_chans, s, verify, max_file_size, typed ? &t : nullptr);
+    count_launch(verify ? 13 : 11);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return context().ws_release(s);
+}
+
 }  // namespace fpngb
 
 using namespace fpngb;
@@ -143,22 +291,18 @@ int fpngb_decode_batch_device_strided(const void* d_files, size_t file_stride, c
                                       uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
                                       size_t out_pixel_stride, size_t out_chan_stride, uint32_t* d_status, void* stream)
 {
-    Context& c = context();
-    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (!d_files || !file_sizes || !idat_ofs || !idat_len || !d_out || !d_status || n == 0 || n > 65535) return FPNGB_ERR_INVALID_ARG;
-    int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
-    Layout out;
-    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, out); if (rc) return rc;
-    if (file_stride % 4 || (uintptr_t)d_files % 4) return FPNGB_ERR_ALIGNMENT;
-    std::vector<FileDesc> fds(n);
-    for (uint32_t i = 0; i < n; i++) {
-        if ((uint64_t)idat_ofs[i] + 8 + idat_len[i] + 4 > file_sizes[i] || file_sizes[i] > file_stride) return FPNGB_ERR_INVALID_ARG;
-        fds[i] = FileDesc{}; fds[i].file_size = file_sizes[i]; fds[i].idat_ofs = idat_ofs[i]; fds[i].idat_len = idat_len[i];
-    }
-    std::lock_guard<std::mutex> lk(c.mu);
-    FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    return decode_batch_locked((const uint8_t*)d_files, file_stride, fds.data(), n, w, h, chans_in_file, desired_chans, (uint8_t*)d_out,
-                               out, d_status, (cudaStream_t)stream);
+    return decode_batch_device_impl(d_files, file_stride, file_sizes, idat_ofs, idat_len, n, w, h, chans_in_file, desired_chans, d_out,
+                                    out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, false, nullptr, d_status, stream);
+}
+
+int fpngb_decode_batch_device_typed(const void* d_files, size_t file_stride, const uint32_t* file_sizes, const uint32_t* idat_ofs,
+                                    const uint32_t* idat_len, uint32_t n, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                                    uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                    size_t out_pixel_stride, size_t out_chan_stride, const fpngb_pixel_format* fmt, uint32_t* d_status,
+                                    void* stream)
+{
+    return decode_batch_device_impl(d_files, file_stride, file_sizes, idat_ofs, idat_len, n, w, h, chans_in_file, desired_chans, d_out,
+                                    out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, true, fmt, d_status, stream);
 }
 
 int fpngb_decode_batch_device(const void* d_files, size_t file_stride, const uint32_t* file_sizes, const uint32_t* idat_ofs,
@@ -342,35 +486,23 @@ int fpngb_get_info_batch_device(const void* d_base, const uint64_t* d_offsets, c
     return FPNGB_OK;
 }
 
+
 int fpngb_decode_packed_device_strided(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
                                        uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out,
                                        size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride, size_t out_chan_stride,
                                        int32_t* d_status, void* stream)
 {
-    Context& c = context();
-    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_status || n == 0 || n > 65535 || !max_file_size) return FPNGB_ERR_INVALID_ARG;
-    int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
-    Layout out;
-    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, out); if (rc) return rc;
-    if ((uintptr_t)d_base % 4) return FPNGB_ERR_ALIGNMENT;
-    const cudaStream_t s = (cudaStream_t)stream;
-    std::lock_guard<std::mutex> lk(c.mu);
-    FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    // an IDAT chunk is shorter than its file: max_file_size bounds the stream of every file that reaches the decode kernels
-    DecodeParams p{};
-    VerifyState* verify = nullptr;
-    rc = decode_workspace_uniform_locked(n, w, h, chans_in_file, max_file_size, s, p, &verify); if (rc) return rc;
-    WalkParams wp{};
-    wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n;
-    wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = w; wp.h = h; wp.chans = chans_in_file;
-    wp.out_stride = out.image;
-    launch_container_walk(wp, s);
-    p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status;
-    launch_decode(p, set_output(p, (uint8_t*)d_out, out), n, desired_chans, s, verify, max_file_size);
-    count_launch(verify ? 11 : 9);
-    FPNGB_CUDA_OK(cudaGetLastError());
-    return context().ws_release(s);
+    return decode_packed_device_impl(d_base, d_offsets, d_sizes, n, max_file_size, w, h, chans_in_file, desired_chans, d_out, out_image_stride,
+                                     out_row_pitch, out_pixel_stride, out_chan_stride, false, nullptr, d_status, stream);
+}
+
+int fpngb_decode_packed_device_typed(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
+                                     uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans, void* d_out,
+                                     size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride, size_t out_chan_stride,
+                                     const fpngb_pixel_format* fmt, int32_t* d_status, void* stream)
+{
+    return decode_packed_device_impl(d_base, d_offsets, d_sizes, n, max_file_size, w, h, chans_in_file, desired_chans, d_out, out_image_stride,
+                                     out_row_pitch, out_pixel_stride, out_chan_stride, true, fmt, d_status, stream);
 }
 
 int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size,
@@ -385,61 +517,23 @@ int fpngb_decode_packed_device(const void* d_base, const uint64_t* d_offsets, co
                                               (size_t)w * desired_chans, desired_chans, 1, d_status, stream);
 }
 
-// Workspace of the ragged call, from call arguments only (no host synchronisation).  Only files decode_place_kernel places and
-// that fit in out_cap are decoded; they are a prefix of the placed files, so for every one of them the sums below run over
-// decoded files alone.
-//   records:   subs_for(s) <= s/128 + 3 per file of s bytes; files that lie inside the buffer and do not overlap have sizes that
-//              sum to at most base_bytes, so base_bytes/128 + 3n records hold them all.  Every file also has s <= max_file_size.
-//   delta:     a file needs h * align_up(w*c, 16) <= (4/desired) * (w*h*desired) + 15h bytes, h <= max_h and h <= w*h, and the
-//              w*h*desired of the decoded files sum to at most out_cap.  Every file also needs at most max_h * pitch(max_w, 4).
-// A file whose range still ends past a bound (overlapping files) gets FPNGB_DECODE_OUT_OF_SPACE from decode_place_kernel.
-static unsigned long long sat_u64(unsigned __int128 v) { return v > ~0ull ? ~0ull : (unsigned long long)v; }
-static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired,
-                             size_t out_cap, unsigned long long& sub_cap, unsigned long long& delta_cap)
-{
-    typedef unsigned __int128 u128;
-    const u128 by_bytes = (u128)base_bytes / 128 + 3 * (u128)n, by_max = (u128)n * subs_for(max_file_size);
-    sub_cap = sat_u64(by_bytes < by_max ? by_bytes : by_max);
-    const u128 rows = (u128)n * max_h, rows_px = ((u128)out_cap + desired - 1) / desired;
-    const u128 by_out = ((u128)out_cap * 4 + desired - 1) / desired + 16 * (rows < rows_px ? rows : rows_px);
-    const u128 by_shape = rows * delta_pitch(max_w, 4);
-    delta_cap = sat_u64(by_out < by_shape ? by_out : by_shape);
-}
+
 
 int fpngb_decode_packed_ragged_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                       uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                       size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, int32_t* d_status, void* stream)
 {
-    Context& c = context();
-    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_out_offsets || !d_status || n == 0 || n > 65535 || !max_file_size ||
-        (desired_chans != 3 && desired_chans != 4) || !max_w || !max_h || max_w > (1u << 24) || max_h > (1u << 24))
-        return FPNGB_ERR_INVALID_ARG;
-    if ((uintptr_t)d_base % 4 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
-    unsigned long long sub_cap = 0, delta_cap = 0;
-    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap, sub_cap, delta_cap);
-    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2) return FPNGB_ERR_BUFFER_TOO_SMALL;
-    const cudaStream_t s = (cudaStream_t)stream;
-    std::lock_guard<std::mutex> lk(c.mu);
-    FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    DecodeParams p{};
-    VerifyState* verify = nullptr;
-    int rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify); if (rc) return rc;
-    p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
-    WalkParams wp{};
-    wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
-    wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
-    wp.base_bytes = base_bytes;
-    launch_container_walk(wp, s);
-    PlaceParams pp{};
-    pp.files = (FileDesc*)p.files; pp.n = n; pp.desired = desired_chans;
-    pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
-    launch_decode_place(pp, s);
-    p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
-    launch_decode(p, OutStrides{0, desired_chans, 1}, n, desired_chans, s, verify, max_file_size);
-    count_launch(verify ? 13 : 11);
-    FPNGB_CUDA_OK(cudaGetLastError());
-    return context().ws_release(s);
+    return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
+                                     d_out_offsets, d_info, false, nullptr, d_status, stream);
+}
+
+int fpngb_decode_packed_ragged_device_typed(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
+                                            uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans,
+                                            void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info,
+                                            const fpngb_pixel_format* fmt, int32_t* d_status, void* stream)
+{
+    return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
+                                     d_out_offsets, d_info, true, fmt, d_status, stream);
 }
 
 }  // extern "C"

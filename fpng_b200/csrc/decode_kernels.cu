@@ -11,13 +11,15 @@
 //                              counts places every subsequence in the filtered stream and a last decode writes the delta
 //                              bytes (literals) / replicates the previous delta pixel (RLE matches, fpng.cpp:2289-2388)
 //   D3 unfilter_kernel         inverse PNG filter 2 = running sum down each byte column (fpng.cpp:2439-2466 fuses it into
-//                              the serial loop) + 24<->32bpp conversion (alpha 0xFF / dropped)
+//                              the serial loop) + 24<->32bpp conversion (alpha 0xFF / dropped); for the *_typed calls
+//                              unfilter_typed_kernel (decode_typed_kernels.cu) in the same slot, storing float / half / bf16
 //   D2' decode_stored_kernel   stored-block files (fpng.cpp:2107-2207)
 //   V2 decode_adler_kernel     opt-in (fpngb_set_decode_verify): zlib Adler-32 of the inflated stream from the delta rows
 // Every stream violation the reference rejects ends in status FPNG_DECODE_NOT_FPNG (fpng.cpp:3131-3136).
 #include "row_walk.cuh"
 #include "kernels.cuh"
 #include "decode.cuh"
+#include "unfilter.cuh"
 
 namespace fpngb {
 
@@ -1332,12 +1334,6 @@ __global__ void __launch_bounds__(32 * kAdlerRows) decode_adler_kernel(VerifyPar
 // ------------------------------------------------------------------------------------------------
 // D3: inverse Up filter (running sum down the columns) + channel conversion.  One thread per group of 4 pixels.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t vadd4(uint32_t a, uint32_t b)
-{
-    const uint32_t s = (a & 0x7F7F7F7Fu) + (b & 0x7F7F7F7Fu);
-    return s ^ ((a ^ b) & 0x80808080u);
-}
-
 // the 4 pixels of o[] (DST interleaved channels) as one 32-bit word per channel plane
 template <int DST>
 __device__ __forceinline__ void planes_of(const uint32_t (&o)[DST], uint32_t (&pl)[DST])
@@ -1384,39 +1380,13 @@ __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p, OutStride
     constexpr int kRowsAhead = 8;                  // independent loads in flight per thread (8 rows x 12-16 bytes: enough bytes in flight at 256 files)
     for (uint32_t y0 = 0; y0 < h; y0 += kRowsAhead) {
         uint32_t dd[kRowsAhead][SRC];
-#pragma unroll
-        for (int j = 0; j < kRowsAhead; j++) {
-            const uint32_t y = min(y0 + j, h - 1);
-            const uint8_t* dr = delta + (size_t)y * pitch;
-            if (full) {
-#pragma unroll
-                for (int i = 0; i < SRC; i++) dd[j][i] = __ldg(reinterpret_cast<const uint32_t*>(dr + 4 * i));   // pitch % 16 == 0 and x0*SRC % 4 == 0
-            } else {
-#pragma unroll
-                for (int i = 0; i < SRC; i++) { dd[j][i] = 0; for (int b = 0; b < 4; b++) if ((uint32_t)(4 * i + b) < npx * SRC) dd[j][i] |= (uint32_t)dr[4 * i + b] << (8 * b); }
-            }
-        }
+        load_delta_rows<SRC>(delta, pitch, y0, h, full, npx, dd);
 #pragma unroll
         for (int j = 0; j < kRowsAhead; j++) {
             const uint32_t y = y0 + j;
             if (y >= h) break;
-#pragma unroll
-            for (int i = 0; i < SRC; i++) acc[i] = summing ? vadd4(acc[i], dd[j][i]) : dd[j][i];
-            // repack to DST channels
             uint32_t o[DST];
-            if (SRC == DST) {
-#pragma unroll
-                for (int i = 0; i < DST; i++) o[i] = acc[i];
-            } else if (SRC == 3) {   // 24 -> 32 bpp, alpha 0xFF (fpng.cpp:2331)
-                o[0] = (acc[0] & 0x00FFFFFFu) | 0xFF000000u;
-                o[1] = __byte_perm(acc[0], acc[1], 0x4543) | 0xFF000000u;
-                o[2] = __byte_perm(acc[1], acc[2], 0x4432) | 0xFF000000u;
-                o[DST - 1] = (acc[2] >> 8) | 0xFF000000u;
-            } else {                 // 32 -> 24 bpp, alpha dropped (fpng.cpp:2684-2721)
-                o[0] = __byte_perm(acc[0], acc[1], 0x4210);
-                o[1] = __byte_perm(acc[1], acc[2], 0x5421);
-                o[DST - 1] = __byte_perm(acc[2], acc[SRC - 1], 0x6542);
-            }
+            unfilter_row<SRC, DST>(acc, dd[j], summing, o);
             uint8_t* orow = out + (size_t)y * out_pitch;
             if (PLANAR) {
                 // one word per plane when every plane row is 4-byte aligned (x0 % 4 == 0), else bytes
@@ -1455,6 +1425,7 @@ __global__ void __launch_bounds__(128) unfilter_kernel(DecodeParams p, OutStride
         }
     }
 }
+
 
 __global__ void decode_status_kernel(DecodeParams p, uint32_t n)
 {
@@ -1511,7 +1482,7 @@ bool decode_set_pre_roll(uint32_t bits)
 }
 
 void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n, uint32_t desired, cudaStream_t s, VerifyState* verify,
-                   size_t max_file_bytes)
+                   size_t max_file_bytes, const TypedOut* typed)
 {
     DecodeParams p = params;
     p.pre_roll = g_dec_pre_roll;
@@ -1550,8 +1521,9 @@ void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n,
     const uint32_t groups = (p.max_w + 3) / 4;
     dim3 gu((groups + 127) / 128, n);
     const bool planar = os.pixel == 1;
+    if (typed) launch_unfilter_typed(p, os, *typed, desired, gu, s);
     // one instantiation per channel count in the call (a mixed call launches both; each skips the other's files)
-    for (uint32_t src = 3; src <= 4; src++) {
+    for (uint32_t src = 3; src <= 4 && !typed; src++) {
         if (p.chans && p.chans != src) continue;
         if (src == 3 && desired == 3) { if (planar) unfilter_kernel<3, 3, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 3, false><<<gu, 128, 0, s>>>(p, os); }
         else if (src == 3) { if (planar) unfilter_kernel<3, 4, true><<<gu, 128, 0, s>>>(p, os); else unfilter_kernel<3, 4, false><<<gu, 128, 0, s>>>(p, os); }

@@ -1,0 +1,143 @@
+// fpng_b200/csrc/decode_typed_kernels.cu -- D3 typed: the unfilter pass of the *_typed decode calls (include/fpng_b200.h,
+// fpngb_pixel_format).  unfilter_kernel's running sum (unfilter.cuh) with every value converted in registers and stored as float32,
+// float16 or bfloat16: no uint8 buffer and no extra pass over the pixels.  v * scale + bias is two separately rounded fp32
+// operations (never an FMA: what numpy and torch eager compute for x * s + b), then round to nearest even into T (overflow to
+// +-inf, as torch's .to()).  Its own translation unit, so that the uint8 decode kernels compile exactly as they did.
+#include "decode.cuh"
+#include "unfilter.cuh"
+#include "../../include/fpng_b200.h"
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+namespace fpngb {
+
+template <typename T> __device__ __forceinline__ uint32_t typed_bits(float v);
+template <> __device__ __forceinline__ uint32_t typed_bits<float>(float v) { return __float_as_uint(v); }
+template <> __device__ __forceinline__ uint32_t typed_bits<__half>(float v) { return __half_as_ushort(__float2half_rn(v)); }
+template <> __device__ __forceinline__ uint32_t typed_bits<__nv_bfloat16>(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
+
+// byte k of the interleaved pixel bytes o[] (k = pixel * DST + channel), mapped to channel c and converted
+template <typename T, int DST>
+__device__ __forceinline__ uint32_t typed_value(const uint32_t (&o)[DST], int k, int c, const PixelAffine& pa)
+{
+    const float v = __uint2float_rn((o[k >> 2] >> (8 * (k & 3))) & 0xFFu);
+    return typed_bits<T>(__fadd_rn(__fmul_rn(v, pa.scale[c]), pa.bias[c]));
+}
+
+__device__ __forceinline__ void store_elem(uint8_t* a, uint32_t bits, int size)
+{
+    if (size == 4) *reinterpret_cast<uint32_t*>(a) = bits;
+    else *reinterpret_cast<uint16_t*>(a) = (uint16_t)bits;
+}
+
+// NE contiguous elements of T (bit patterns e[]) at a, which is sizeof(T)-aligned: the widest stores the address allows, 16, then 8,
+// then 4 bytes, else 2-byte elements.  NE * sizeof(T) is a multiple of 8 for every group shape here (4 pixels x 3 or 4 channels
+// interleaved, 4 values of one plane).
+template <typename T, int NE>
+__device__ __forceinline__ void store_elems(uint8_t* a, const uint32_t (&e)[NE])
+{
+    constexpr int ES = sizeof(T), NW = NE * ES / 4;
+    static_assert(NE * ES % 8 == 0, "whole 8-byte units");
+    uint32_t wd[NW];
+#pragma unroll
+    for (int k = 0; k < NW; k++) {
+        if constexpr (ES == 4) wd[k] = e[k];
+        else wd[k] = e[2 * k] | (e[2 * k + 1] << 16);
+    }
+    const uint32_t mis = (uint32_t)((uintptr_t)a & 15u);
+    if (mis == 0u) {
+#pragma unroll
+        for (int k = 0; k + 4 <= NW; k += 4) *reinterpret_cast<uint4*>(a + 4 * k) = make_uint4(wd[k], wd[k + 1], wd[k + 2], wd[k + 3]);
+        if (NW % 4) *reinterpret_cast<uint2*>(a + 4 * (NW - 2)) = make_uint2(wd[NW - 2], wd[NW - 1]);
+    } else if ((mis & 7u) == 0u) {
+#pragma unroll
+        for (int k = 0; k < NW; k += 2) *reinterpret_cast<uint2*>(a + 4 * k) = make_uint2(wd[k], wd[k + 1]);
+    } else if ((mis & 3u) == 0u) {
+#pragma unroll
+        for (int k = 0; k < NW; k++) *reinterpret_cast<uint32_t*>(a + 4 * k) = wd[k];
+    } else {
+#pragma unroll
+        for (int k = 0; k < NE; k++) store_elem(a + ES * k, e[k], ES);
+    }
+}
+
+// OutStrides in bytes: interleaved rows (pixel = DST * sizeof(T)) at any pitch, or planar (pixel = sizeof(T)); row 0: tight rows.
+// All output addressing is 64-bit: one file's typed pixels may pass 4 GiB.
+template <int SRC, int DST, bool PLANAR, typename T>
+__global__ void __launch_bounds__(128) unfilter_typed_kernel(DecodeParams p, OutStrides os, PixelAffine pa)
+{
+    constexpr int ES = sizeof(T);
+    const uint32_t f = blockIdx.y;
+    const DecodeState st = p.state[f];
+    if (st.status) return;
+    const FileDesc& fd = p.files[f];
+    if (fd.chans != SRC) return;                                                // the same for the whole CTA
+    const uint32_t w = fd.w, h = fd.h, pitch = fd.pitch;
+    const uint32_t x0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;            // first pixel of the thread's group
+    if (x0 >= w) return;
+    const uint32_t npx = min(4u, w - x0);
+    const bool full = npx == 4;
+    const uint8_t* delta = p.delta + fd.delta_base + (size_t)x0 * SRC;
+    uint8_t* out = p.d_out + fd.out_base + (size_t)x0 * (PLANAR ? 1u : DST) * ES;
+    const size_t out_pitch = os.row ? os.row : (size_t)w * DST * ES, cs = os.chan;
+    uint32_t acc[SRC];
+#pragma unroll
+    for (int i = 0; i < SRC; i++) acc[i] = 0;
+    const bool summing = !st.stored;
+    constexpr int kRowsAhead = 8;
+    for (uint32_t y0 = 0; y0 < h; y0 += kRowsAhead) {
+        uint32_t dd[kRowsAhead][SRC];
+        load_delta_rows<SRC>(delta, pitch, y0, h, full, npx, dd);
+#pragma unroll
+        for (int j = 0; j < kRowsAhead; j++) {
+            const uint32_t y = y0 + j;
+            if (y >= h) break;
+            uint32_t o[DST];
+            unfilter_row<SRC, DST>(acc, dd[j], summing, o);
+            uint8_t* orow = out + (size_t)y * out_pitch;
+            if (PLANAR) {                                                       // 4 * sizeof(T) contiguous bytes per plane
+#pragma unroll
+                for (int c = 0; c < DST; c++) {
+                    uint32_t e[4];
+#pragma unroll
+                    for (int q = 0; q < 4; q++) e[q] = typed_value<T>(o, q * DST + c, c, pa);
+                    uint8_t* a = orow + c * cs;
+                    if (full) store_elems<T>(a, e);
+                    else for (uint32_t q = 0; q < npx; q++) store_elem(a + ES * q, e[q], ES);
+                }
+            } else {                                                            // 4 * DST * sizeof(T) contiguous bytes
+                uint32_t e[4 * DST];
+#pragma unroll
+                for (int k = 0; k < 4 * DST; k++) e[k] = typed_value<T>(o, k, k % DST, pa);
+                if (full) store_elems<T>(orow, e);
+                else {
+#pragma unroll
+                    for (int k = 0; k < 4 * DST; k++) if ((uint32_t)k < npx * DST) store_elem(orow + ES * k, e[k], ES);
+                }
+            }
+        }
+    }
+}
+
+// one instantiation per source channel count in the call, as for unfilter_kernel
+template <typename T>
+static void launch_typed(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t desired, dim3 g, cudaStream_t s)
+{
+    const bool planar = os.pixel == sizeof(T);
+    for (uint32_t src = 3; src <= 4; src++) {
+        if (p.chans && p.chans != src) continue;
+        if (src == 3 && desired == 3) { if (planar) unfilter_typed_kernel<3, 3, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<3, 3, false, T><<<g, 128, 0, s>>>(p, os, pa); }
+        else if (src == 3) { if (planar) unfilter_typed_kernel<3, 4, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<3, 4, false, T><<<g, 128, 0, s>>>(p, os, pa); }
+        else if (desired == 3) { if (planar) unfilter_typed_kernel<4, 3, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<4, 3, false, T><<<g, 128, 0, s>>>(p, os, pa); }
+        else { if (planar) unfilter_typed_kernel<4, 4, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<4, 4, false, T><<<g, 128, 0, s>>>(p, os, pa); }
+    }
+}
+
+void launch_unfilter_typed(const DecodeParams& p, const OutStrides& os, const TypedOut& t, uint32_t desired, dim3 g, cudaStream_t s)
+{
+    if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_typed<float>(p, os, t.aff, desired, g, s);
+    else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_typed<__half>(p, os, t.aff, desired, g, s);
+    else launch_typed<__nv_bfloat16>(p, os, t.aff, desired, g, s);
+}
+
+}  // namespace fpngb

@@ -335,6 +335,46 @@ enum { FPNGB_DECODE_ADLER_MISMATCH = 102 };   /* verified decode only: the zlib 
 FPNGB_API int fpngb_set_decode_verify(int on);
 FPNGB_API int fpngb_get_decode_verify(void);
 
+/* ---- typed decode output: float32 / float16 / bfloat16 pixels with a per-channel scale and bias ------------------------------
+ * The *_typed calls decode exactly as their uint8 twins and store, for output channel c (0 .. desired_chans-1, counted after
+ * the 3 <-> 4 conversion) and v the uint8 value the twin would write (alpha 255 when a 3-channel file is decoded to 4):
+ *     out = T( (float)v * scale[c] + bias[c] )
+ *   The multiply and the add are two separately rounded fp32 operations (never contracted to an FMA: what numpy and torch eager
+ *   compute for x * s + b); T is float32, float16 or bfloat16, converted with round to nearest even, overflow to +-inf (as
+ *   torch's .to()).  The conversion runs in the decoder's last kernel, which holds each final pixel in registers: no extra pass
+ *   and no uint8 buffer.  Entries of scale / bias at index >= desired_chans are ignored.
+ *   Statuses and their order, the verify mode (a file with status 4 or 102 gets no element written), the rule that a failed file's
+ *   output is left untouched, the launch count and stream ordering (no host synchronisation) are the uint8 twin's.
+ * Call-level checks, in addition to the twin's (a rejected call enqueues nothing and writes nothing):
+ *   FPNGB_ERR_INVALID_ARG for a NULL fmt, a dtype other than the three below (uint8 output is the twin itself), or a scale or
+ *   bias entry that is not finite (in use: index < desired_chans).
+ * fpngb_decode_batch_device_typed / fpngb_decode_packed_device_typed: the arguments of the *_strided twin plus fmt.  All strides
+ *   stay in BYTES: element (i, y, x, c) at d_out + i*out_image_stride + y*out_row_pitch + x*out_pixel_stride + c*out_chan_stride.
+ *   d_out and every stride must be a multiple of sizeof(T), else FPNGB_ERR_ALIGNMENT; divided by sizeof(T), the strides must form
+ *   a non-overlapping interleaved or planar layout of "Pixel layouts" above (pixel_stride == desired_chans * sizeof(T) or
+ *   == sizeof(T)), else FPNGB_ERR_INVALID_ARG.
+ * fpngb_decode_packed_ragged_device_typed: the arguments of fpngb_decode_packed_ragged_device plus fmt.  File i takes
+ *   align_up(w*h*desired_chans*sizeof(T), 16) bytes; d_out_offsets and out_cap are in bytes.  The w*h*desired_chans > 0xFFFFFFFF
+ *   rule (FPNGB_DECODE_FAILED_DIMENSIONS_TOO_LARGE) is unchanged, so one file's typed output may pass 4 GiB. */
+enum { FPNGB_DTYPE_FLOAT32 = 1, FPNGB_DTYPE_FLOAT16 = 2, FPNGB_DTYPE_BFLOAT16 = 3 };
+typedef struct { uint32_t dtype; float scale[4]; float bias[4]; } fpngb_pixel_format;   /* entries >= desired_chans ignored */
+FPNGB_API int fpngb_decode_batch_device_typed(const void* d_files, size_t file_stride, const uint32_t* file_sizes,
+                                              const uint32_t* idat_ofs, const uint32_t* idat_len, uint32_t n,
+                                              uint32_t w, uint32_t h, uint32_t chans_in_file, uint32_t desired_chans,
+                                              void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                              size_t out_pixel_stride, size_t out_chan_stride, const fpngb_pixel_format* fmt,
+                                              uint32_t* d_status, void* stream);
+FPNGB_API int fpngb_decode_packed_device_typed(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                               uint32_t max_file_size, uint32_t w, uint32_t h, uint32_t chans_in_file,
+                                               uint32_t desired_chans, void* d_out, size_t out_image_stride, size_t out_row_pitch,
+                                               size_t out_pixel_stride, size_t out_chan_stride, const fpngb_pixel_format* fmt,
+                                               int32_t* d_status, void* stream);
+FPNGB_API int fpngb_decode_packed_ragged_device_typed(const void* d_base, size_t base_bytes, const uint64_t* d_offsets,
+                                                      const uint32_t* d_sizes, uint32_t n, uint32_t max_file_size, uint32_t max_w,
+                                                      uint32_t max_h, uint32_t desired_chans, void* d_out, size_t out_cap,
+                                                      uint64_t* d_out_offsets /* n+1 */, uint32_t* d_info /* n*6 or NULL */,
+                                                      const fpngb_pixel_format* fmt, int32_t* d_status, void* stream);
+
 /* Pins the calling thread to the CPUs of the NUMA node of the library's GPU (sysfs: the GPU's PCI device -> numa_node ->
  * cpulist), so that pinned buffers allocated afterwards and the thread that issues the H2D/D2H copies are local to the GPU's
  * PCIe root port.  Call once per rank after fpngb_init(), before allocating staging memory.  Returns the node, or -1 if the
