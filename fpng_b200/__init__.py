@@ -16,5 +16,5 @@ from .api import (  # noqa: F401
     FPNGB_DECODE_OUT_OF_SPACE, decode_packed_ragged_device, ragged_views,
     encode_ragged_device, ragged_slot_offsets, compact_packed_device,
     FPNGB_DECODE_ADLER_MISMATCH, set_decode_verify, decode_verify,
-    normalize_scale_bias, typed_layout,
+    normalize_scale_bias, denormalize_scale_bias, typed_layout,
 )

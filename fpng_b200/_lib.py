@@ -13,7 +13,7 @@ u32p = C.POINTER(C.c_uint32)
 
 
 class PixelFormat(C.Structure):
-    """fpngb_pixel_format: the output type (FPNGB_DTYPE_*) and per-channel scale and bias of the *_typed decode calls"""
+    """fpngb_pixel_format: the element type (FPNGB_DTYPE_*) and per-channel scale and bias of the *_typed decode and encode calls"""
     _fields_ = [("dtype", C.c_uint32), ("scale", C.c_float * 4), ("bias", C.c_float * 4)]
 
 
@@ -81,6 +81,13 @@ def lib() -> C.CDLL:
     L.fpngb_decode_packed_ragged_device_typed.restype = C.c_int
     L.fpngb_decode_packed_ragged_device_typed.argtypes = L.fpngb_decode_packed_ragged_device.argtypes[:-2] + [C.POINTER(PixelFormat),
                                                                                                            C.c_void_p, C.c_void_p]
+    L.fpngb_encode_batch_device_typed.restype = C.c_int
+    L.fpngb_encode_batch_device_typed.argtypes = [C.c_void_p] + [C.c_size_t] * 4 + [C.c_uint32] * 4 + [C.POINTER(PixelFormat), C.c_uint32,
+                                                                                                   C.c_void_p, C.c_size_t, C.c_void_p,
+                                                                                                   C.c_void_p]
+    L.fpngb_encode_ragged_device_typed.restype = C.c_int
+    L.fpngb_encode_ragged_device_typed.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PixelFormat), C.c_uint32,
+                                                   C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     L.fpngb_compact_batch_device.restype = C.c_int
     L.fpngb_compact_batch_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
     L.fpngb_compact_packed_device.restype = C.c_int

@@ -169,20 +169,43 @@ def layout_strides(shape, strides):
     return image, row, pixel, chan
 
 
-def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=None):
+def _input_format(dtype, scale, bias, chans, what):
+    """None for uint8 input (the uint8 calls: no scale or bias), else the fpngb_pixel_format of a float32 / float16 / bfloat16
+    input (scale defaults to 1, bias to 0; one value or one per channel).  ValueError for any other dtype."""
+    import torch
+
+    if dtype == torch.uint8:
+        if scale is not None or bias is not None:
+            raise ValueError(f"{what}: scale and bias apply to float32 / float16 / bfloat16 input only; uint8 pixels are encoded as they are")
+        return None
+    if _DTYPE_CODES.get(str(dtype).replace("torch.", "")) is None:
+        raise ValueError(f"{what}: input dtype {dtype}: torch.uint8, float32, float16 or bfloat16")
+    return _pixel_format(dtype, scale, bias, chans)
+
+
+def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=None, scale=None, bias=None):
     """Encode a batch of equally sized device-resident images.
 
-    images: torch.uint8 CUDA tensor [n, h, w, chans]: contiguous, or any view in one of the two layouts of layout_strides --
-    e.g. x_nchw.permute(0, 2, 3, 1), a crop canvas[:, y0:y1, x0:x1, :] or img.expand(n, -1, -1, -1) -- which is encoded in
-    place, without a copy.  Returns (out [n, stride] uint8, sizes [n] int32 holding uint32 file sizes) on the same device;
-    kernels are enqueued on the current torch stream (or `stream`), not synchronised.
+    images: CUDA tensor [n, h, w, chans]: contiguous, or any view in one of the two layouts of layout_strides -- e.g.
+    x_nchw.permute(0, 2, 3, 1), a crop canvas[:, y0:y1, x0:x1, :] or img.expand(n, -1, -1, -1) -- which is read in place,
+    without a copy.  torch.uint8 pixels are encoded as they are.  torch.float32 / float16 / bfloat16 elements x of channel c
+    are encoded as the bytes nan_to_num(x.float() * scale[c] + bias[c], nan=0).round().clamp(0, 255), rounding half to even,
+    converted on the GPU (scale defaults to 1, bias to 0; one value or one per channel; denormalize_scale_bias inverts a
+    normalisation): a model's NCHW output in [-1, 1] is encode_batch_device(x.permute(0, 2, 3, 1), scale=127.5, bias=127.5).
+    uint8 input takes no scale or bias and other dtypes are refused (ValueError).  Returns (out [n, stride] uint8, sizes [n]
+    int32 holding uint32 file sizes) on the same device; kernels are enqueued on the current torch stream (or `stream`), not
+    synchronised.
     """
     import torch
 
-    assert images.is_cuda and images.dtype == torch.uint8 and images.dim() == 4
+    assert images.dim() == 4
     n, h, w, c = images.shape
+    fmt = _input_format(images.dtype, scale, bias, c, "encode_batch_device")
+    assert images.is_cuda
     strided = not images.is_contiguous()
-    if strided:
+    if fmt is not None:
+        layout = typed_layout(images.shape, images.stride(), images.element_size())
+    elif strided:
         layout = layout_strides(images.shape, images.stride())
     stride = (max_encoded_size(w, h, c) + 15) // 16 * 16
     if out is None:
@@ -190,7 +213,10 @@ def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=Non
     if sizes is None:
         sizes = torch.empty((n,), dtype=torch.int32, device=images.device)
     s = stream if stream is not None else torch.cuda.current_stream(images.device).cuda_stream
-    if strided:
+    if fmt is not None:
+        rc = lib().fpngb_encode_batch_device_typed(images.data_ptr(), *layout, n, w, h, c, C.byref(fmt), flags, out.data_ptr(),
+                                                   out.stride(0), sizes.data_ptr(), s)
+    elif strided:
         rc = lib().fpngb_encode_batch_device_strided(images.data_ptr(), *layout, n, w, h, c, flags, out.data_ptr(), out.stride(0),
                                                      sizes.data_ptr(), s)
     else:
@@ -209,12 +235,15 @@ def ragged_slot_offsets(shapes):
     return ofs
 
 
-def encode_ragged_device(images, flags: int = 0, out=None, stream=None):
+def encode_ragged_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None):
     """Encode device images of ANY shapes, channel counts and layouts in one call (fpngb_encode_ragged_device).
 
-    images: list of torch.uint8 CUDA tensors [h, w, chans] (chans 3 or 4), each contiguous or any view in one of the two layouts of
+    images: list of CUDA tensors [h, w, chans] (chans 3 or 4), each contiguous or any view in one of the two layouts of
     layout_strides (HWC rows at any pitch, e.g. a crop, or CHW planes, e.g. x_chw.permute(1, 2, 0)); the same tensor may appear
-    more than once.  Any other layout raises FpngB200Error (invalid argument).  Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]): file i is the sizes[i] bytes at
+    more than once.  Any other layout raises FpngB200Error (invalid argument).  The images are all torch.uint8, or all one of
+    float32 / float16 / bfloat16, converted as in encode_batch_device with scale and bias (one value or one per channel, up to
+    the largest channel count of the list); a mixed list raises ValueError.  Returns (out uint8 [total], offsets int64 [n + 1],
+    sizes int32 [n]): file i is the sizes[i] bytes at
     out[offsets[i]:], offsets being ragged_slot_offsets of the shapes and offsets[n] the total -- the (data, offsets, sizes)
     decode_packed_ragged_device takes.  out, if given, is a flat 16-byte aligned uint8 CUDA tensor of at least the total; no byte
     of it past the total is written.  Kernels are enqueued on the current torch stream (or `stream`), with no host
@@ -224,15 +253,21 @@ def encode_ragged_device(images, flags: int = 0, out=None, stream=None):
     # the per-image work here is the host cost of the call: attribute reads only; the layout rules are checked by the C call
     # (an unsupported layout raises FpngB200Error "invalid argument")
     n = len(images)
-    u8 = torch.uint8
+    dtype = images[0].dtype if n else torch.uint8
+    mixed = {t.dtype for t in images} - {dtype}
+    if mixed:
+        raise ValueError(f"encode_ragged_device: the images are all uint8 or all one float dtype, got {dtype} and {mixed.pop()}")
     ptrs, dims, strides = [], [], []
     for t in images:
-        assert t.is_cuda and t.dtype == u8 and t.dim() == 3, "images: [h, w, chans] uint8 CUDA tensors"
+        assert t.is_cuda and t.dim() == 3, "images: [h, w, chans] CUDA tensors"
         h, w, c = t.shape
         ptrs.append(t.data_ptr()); dims.append((w, h, c)); strides.append(t.stride())
     ptrs = np.array(ptrs, dtype=np.uint64)
     dims = np.array(dims, dtype=np.uint32).reshape(n, 3)
     strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
+    fmt = _input_format(dtype, scale, bias, int(dims[:, 2].max()) if n else 3, "encode_ragged_device")
+    if fmt is not None:
+        strides = strides * np.uint64(images[0].element_size())
     device = images[0].device if n else torch.device("cuda")
     if out is None:
         slot = {}
@@ -245,9 +280,14 @@ def encode_ragged_device(images, flags: int = 0, out=None, stream=None):
     offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
     sizes = torch.empty((n,), dtype=torch.int32, device=device)
     s = stream if stream is not None else torch.cuda.current_stream(device).cuda_stream
-    rc = lib().fpngb_encode_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
-                                          strides.ctypes.data_as(C.c_void_p), flags, out.data_ptr(), out.numel(),
-                                          offsets.data_ptr(), sizes.data_ptr(), s)
+    if fmt is not None:
+        rc = lib().fpngb_encode_ragged_device_typed(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
+                                                    strides.ctypes.data_as(C.c_void_p), C.byref(fmt), flags, out.data_ptr(),
+                                                    out.numel(), offsets.data_ptr(), sizes.data_ptr(), s)
+    else:
+        rc = lib().fpngb_encode_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
+                                              strides.ctypes.data_as(C.c_void_p), flags, out.data_ptr(), out.numel(),
+                                              offsets.data_ptr(), sizes.data_ptr(), s)
     check(rc, "encode_ragged_device")
     return out, offsets, sizes
 
@@ -343,6 +383,17 @@ def normalize_scale_bias(mean, std, max_value=255.0):
     m = np.asarray(mean, dtype=np.float64).reshape(-1)
     sd = np.asarray(std, dtype=np.float64).reshape(-1)
     return (1.0 / (float(max_value) * sd)).astype(np.float32), (-m / sd).astype(np.float32)
+
+
+def denormalize_scale_bias(mean, std, max_value=255.0):
+    """The (scale, bias) pair, float32 arrays, that the typed encode applies to a normalised tensor x = (v / max_value - mean) / std
+    to get back v: scale = max_value * std and bias = max_value * mean, computed in float64 and then rounded to float32 -- the
+    inverse of normalize_scale_bias.  The encode rounds x * scale + bias half to even and clamps it to [0, 255], so a decode with
+    normalize_scale_bias(mean, std) followed by an encode with these values gives back the bytes wherever the float type keeps
+    enough precision (bfloat16 with CLIP's mean and std misses one value in 768)."""
+    m = np.asarray(mean, dtype=np.float64).reshape(-1)
+    sd = np.asarray(std, dtype=np.float64).reshape(-1)
+    return (float(max_value) * sd).astype(np.float32), (float(max_value) * m).astype(np.float32)
 
 
 def _typed_out(out, n, h, w, desired_channels):

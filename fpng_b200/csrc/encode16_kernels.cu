@@ -802,28 +802,4 @@ void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint
     FPNGB_LAUNCH16(pack_rows16_kernel, true, pack16_smem, ctas, 32 * kPack16Rows, p, rows_per_warp);
 }
 
-// ------------------------------------------------------------------------------------------------
-// Strided input for the encoders that read tight interleaved rows only (the generic 4-pixel kernels, the single-pass
-// encoder): one copy into a contiguous [n][h][w * chans] buffer, then the unchanged path.  One CTA per scanline (grid-stride).
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) gather_pixels_kernel(GatherParams p)
-{
-    const uint32_t bpl = p.w * p.chans;
-    for (unsigned long long r = blockIdx.x; r < (unsigned long long)p.n * p.h; r += gridDim.x) {
-        const unsigned long long img = r / p.h, y = r - img * p.h;
-        const uint8_t* src = p.src + img * p.image_stride + y * p.row_pitch;
-        uint8_t* dst = p.dst + r * bpl;
-        for (uint32_t i = threadIdx.x; i < bpl; i += blockDim.x) {
-            const uint32_t x = i / p.chans, c = i - x * p.chans;
-            dst[i] = __ldg(src + (size_t)x * p.pixel_stride + (size_t)c * p.chan_stride);
-        }
-    }
-}
-
-void launch_gather_pixels(const GatherParams& p, cudaStream_t s)
-{
-    const unsigned long long rows = (unsigned long long)p.n * p.h;
-    gather_pixels_kernel<<<(uint32_t)min(rows, 65536ull), 256, 0, s>>>(p);
-}
-
 }  // namespace fpngb

@@ -14,6 +14,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <math.h>
 #include <mutex>
 #include <new>
 #include <sched.h>
@@ -152,28 +153,46 @@ static std::mutex g_init_mu;
 Context& context() { return g_ctx; }
 
 // Optional per-kernel timing with CUDA events on the launching stream (bench.py's roofline numbers).
-enum ProfSlot { kProfHist = 0, kProfHuff, kProfScan, kProfOffsets, kProfFused, kProfFinish, kProfPack, kProfAdler, kProfCrc, kProfSlots };
-struct ProfSet { cudaEvent_t ev[kProfSlots + 1]; cudaEvent_t crc_start; bool used[kProfSlots]; bool crc_side; uint64_t call; };
+// kProfConvert: the conversion pre-pass (convert_pixels_kernel), which runs before the first slot and has its own start event.
+enum ProfSlot { kProfHist = 0, kProfHuff, kProfScan, kProfOffsets, kProfFused, kProfFinish, kProfPack, kProfAdler, kProfCrc, kProfConvert,
+                kProfSlots };
+struct ProfSet { cudaEvent_t ev[kProfSlots + 1]; cudaEvent_t crc_start, conv_start; bool used[kProfSlots]; bool crc_side; uint64_t call; };
 static uint64_t g_prof_call = 0;                // encode calls seen while profiling (a chunked call owns several ProfSets)
 static bool g_profile = false;
 static std::vector<ProfSet*> g_prof_sets;      // one per encode call since the last read
 static std::vector<ProfSet*> g_prof_free;
+static ProfSet* g_prof_conv = nullptr;         // a set whose conversion slot is recorded; the next prof_begin takes it over
 
-static ProfSet* prof_begin(cudaStream_t s)
+static ProfSet* prof_alloc()
 {
-    if (!g_profile) return nullptr;
     ProfSet* ps;
     if (!g_prof_free.empty()) { ps = g_prof_free.back(); g_prof_free.pop_back(); }
     else {
         ps = new ProfSet();
         for (int i = 0; i <= kProfSlots; i++) if (cudaEventCreate(&ps->ev[i]) != cudaSuccess) { delete ps; return nullptr; }
-        if (cudaEventCreate(&ps->crc_start) != cudaSuccess) { delete ps; return nullptr; }
+        if (cudaEventCreate(&ps->crc_start) != cudaSuccess || cudaEventCreate(&ps->conv_start) != cudaSuccess) { delete ps; return nullptr; }
     }
-    ps->crc_side = false; ps->call = g_prof_call;
+    ps->crc_side = false;
     for (int i = 0; i < kProfSlots; i++) ps->used[i] = false;
+    return ps;
+}
+
+static ProfSet* prof_begin(cudaStream_t s)
+{
+    if (!g_profile) return nullptr;
+    ProfSet* ps = g_prof_conv ? g_prof_conv : prof_alloc();
+    g_prof_conv = nullptr;
+    if (!ps) return nullptr;
+    ps->call = g_prof_call;
     cudaEventRecord(ps->ev[0], s);
     g_prof_sets.push_back(ps);
     return ps;
+}
+
+// a conversion slot no encode took over (the call failed after the pre-pass) is dropped
+static void prof_drop_conv()
+{
+    if (g_prof_conv) { g_prof_free.push_back(g_prof_conv); g_prof_conv = nullptr; }
 }
 // records the end of slot `slot`; slots must be closed in increasing order, skipped slots stay unused
 static void prof_mark(ProfSet* ps, int slot, cudaStream_t s)
@@ -181,6 +200,18 @@ static void prof_mark(ProfSet* ps, int slot, cudaStream_t s)
     if (!ps) return;
     cudaEventRecord(ps->ev[slot + 1], s);
     ps->used[slot] = true;
+}
+
+// One launch of the conversion pre-pass into tight uint8 rows (dtype 0: the uint8 copy), profiled in slot kProfConvert of the
+// encode that follows it on the stream.
+static void convert_enqueue(const ConvertParams& cp, uint32_t dtype, int layout, cudaStream_t s)
+{
+    prof_drop_conv();
+    ProfSet* ps = g_profile ? prof_alloc() : nullptr;
+    if (ps) cudaEventRecord(ps->conv_start, s);
+    launch_convert_pixels(cp, dtype, layout, s);
+    count_launch(1);
+    if (ps) { prof_mark(ps, kProfConvert, s); g_prof_conv = ps; }
 }
 
 struct Workspace {
@@ -272,7 +303,7 @@ static void make_png_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t chans
 //
 // The input layout (layout.h) is image_stride / row_pitch and, for planar images, chan_stride (0: interleaved rows).  The 16-pixel
 // scan and pack kernels read every layout in place; the generic kernels and the single-pass encoder read tight interleaved rows
-// only, so a strided batch bound for them is first copied into the workspace by gather_pixels_kernel.
+// only, so a strided batch bound for them is first copied into the workspace by the uint8 instantiation of convert_pixels_kernel.
 static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image_stride, uint32_t row_pitch, size_t chan_stride,
                                uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, uint8_t* d_out, size_t out_stride,
                                uint32_t* d_sizes, cudaStream_t s)
@@ -299,9 +330,11 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
     rc = c.ws_acquire(s);
     if (rc) return rc;
     if (gather) {
-        GatherParams gp{d_pixels, image_stride, row_pitch, chan_stride ? 1u : chans, chan_stride ? chan_stride : 1u, ws.gather, n, w, h, chans};
-        launch_gather_pixels(gp, s);
-        count_launch(1);
+        ConvertParams gp{};
+        const uint32_t ctas = convert_ctas_per_image(w, h);
+        gp.one = ConvDesc{d_pixels, image_stride, row_pitch, chan_stride, 0, 0, n, w, h, chans, ctas, chan_stride ? 1u : 0u};
+        gp.count = 1; gp.total_ctas = (unsigned long long)n * ctas; gp.dst = ws.gather;
+        convert_enqueue(gp, 0, chan_stride ? kConvPlanar : kConvInterleaved, s);
         d_pixels = ws.gather; image_stride = bytes_per_image; row_pitch = w * chans; chan_stride = 0;
     }
     const int mode = pick_load_mode(d_pixels, image_stride, w, chans);
@@ -694,27 +727,78 @@ int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_
                                              d_sizes, stream);
 }
 
-int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
-                               void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+// The element type of a *_typed encode call: FPNGB_ERR_INVALID_ARG for a NULL fmt or a dtype other than the three float types.
+static int typed_dtype(const fpngb_pixel_format* fmt, size_t& es)
+{
+    if (!fmt || (fmt->dtype != FPNGB_DTYPE_FLOAT32 && fmt->dtype != FPNGB_DTYPE_FLOAT16 && fmt->dtype != FPNGB_DTYPE_BFLOAT16))
+        return FPNGB_ERR_INVALID_ARG;
+    es = fmt->dtype == FPNGB_DTYPE_FLOAT32 ? 4 : 2;
+    return FPNGB_OK;
+}
+
+// scale and bias of the channels in use (index < chans): FPNGB_ERR_INVALID_ARG for an entry that is not finite
+static int typed_affine(const fpngb_pixel_format* fmt, uint32_t chans, ConvertParams& cp)
+{
+    for (uint32_t c = 0; c < chans && c < 4; c++) {
+        if (!isfinite(fmt->scale[c]) || !isfinite(fmt->bias[c])) return FPNGB_ERR_INVALID_ARG;
+        cp.scale[c] = fmt->scale[c]; cp.bias[c] = fmt->bias[c];
+    }
+    return FPNGB_OK;
+}
+
+// The byte layout L of a typed input: FPNGB_ERR_ALIGNMENT unless the base and every stride are multiples of es; divided by es, the
+// strides must form an interleaved or planar layout of "Pixel layouts" (size-1 dimensions canonicalised) whose last element lies
+// inside the address space, else FPNGB_ERR_INVALID_ARG.  No row-pitch limit: the conversion pre-pass addresses with 64 bits.
+static int typed_layout(const void* base, uint64_t image, uint64_t row, uint64_t pixel, uint64_t chan, uint32_t n, uint32_t h, uint32_t w,
+                        uint32_t chans, size_t es, Layout& L)
+{
+    if ((uintptr_t)base % es || image % es || row % es || pixel % es || chan % es) return FPNGB_ERR_ALIGNMENT;
+    Layout E;
+    if (!classify_layout(image / es, row / es, pixel / es, chan / es, n, h, w, chans, E)) return FPNGB_ERR_INVALID_ARG;
+    const uint64_t lim = UINT64_MAX / es;
+    if (E.image > lim || E.row > lim || E.pixel > lim || E.chan > lim) return FPNGB_ERR_INVALID_ARG;
+    L = Layout{E.image * es, E.row * es, E.pixel * es, E.chan * es, E.planar};
+    uint64_t last = 0;
+    if (!layout_span(base, L, n, h, w, chans, last) || last > UINT64_MAX - (uint64_t)(uintptr_t)base - (es - 1)) return FPNGB_ERR_INVALID_ARG;
+    return FPNGB_OK;
+}
+
+// Body of fpngb_encode_ragged_device (fmt NULL) and fpngb_encode_ragged_device_typed (typed: fmt required).
+static int encode_ragged_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
+                              const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
+                              uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    size_t es = 1;
+    if (typed) { const int rc = typed_dtype(fmt, es); if (rc) return rc; }
     if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
     // every image on its own: the layout rules of the strided batch call for a batch of one
     std::vector<RaggedImage> im(n);
+    std::vector<Layout> src(typed ? n : 0);
     uint64_t total = 0;
+    uint32_t max_chans = 0;
     for (uint32_t i = 0; i < n; i++) {
         const uint32_t w = dims[3 * i], h = dims[3 * i + 1], chans = dims[3 * i + 2];
         if (!pixels[i] || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
-        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans, pixel = strides ? strides[3 * i + 1] : chans;
-        const uint64_t chan = strides ? strides[3 * i + 2] : 1;
+        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans * es, pixel = strides ? strides[3 * i + 1] : chans * es;
+        const uint64_t chan = strides ? strides[3 * i + 2] : es;
         Layout L;
-        uint64_t last = 0;
-        if (!classify_layout(0, row, pixel, chan, 1, h, w, chans, L) || L.row > 0xFFFFFFFFull ||
-            !layout_span((const void*)(uintptr_t)pixels[i], L, 1, h, w, chans, last))
-            return FPNGB_ERR_INVALID_ARG;
+        if (typed) {
+            const int rc = typed_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, chan, 1, h, w, chans, es, L);
+            if (rc) return rc;
+            src[i] = L;
+        } else {
+            uint64_t last = 0;
+            if (!classify_layout(0, row, pixel, chan, 1, h, w, chans, L) || L.row > 0xFFFFFFFFull ||
+                !layout_span((const void*)(uintptr_t)pixels[i], L, 1, h, w, chans, last))
+                return FPNGB_ERR_INVALID_ARG;
+        }
         im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
         total += align_up(max_encoded_size(w, h, chans), 16);
+        max_chans = std::max(max_chans, chans);
     }
+    ConvertParams cp{};
+    if (typed) { const int rc = typed_affine(fmt, max_chans, cp); if (rc) return rc; }
     if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
     if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
     Context& c = g_ctx;
@@ -722,6 +806,42 @@ int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     cudaStream_t s = (cudaStream_t)stream;
     uint8_t* out = (uint8_t*)d_out;
+
+    // staging: d_out_offsets (n + 1), then the descriptor table and work lists, then (typed) the conversion descriptors
+    const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
+    const size_t conv_stage = align_up(ofs_bytes + align_up((size_t)n * sizeof(ImageDesc), 16) + (size_t)n * 5 * 4, 16);
+    StageSlot* sl = nullptr;
+    int rc = ragged_stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
+    if (rc) return rc;
+    uint8_t* stage = (uint8_t*)sl->buf.p;
+
+    if (typed) {
+        // the conversion buffer: image i's tight uint8 rows at a 16-byte aligned offset, then the descriptor table; one launch
+        // converts every image, and from here on the call is the uint8 call on those rows
+        std::vector<uint64_t> at(n);
+        uint64_t bytes = 0;
+        for (uint32_t i = 0; i < n; i++) { at[i] = bytes; bytes += align_up((uint64_t)im[i].w * im[i].h * im[i].chans, 16); }
+        const uint64_t desc_at = align_up(bytes, 256);
+        rc = c.conv.reserve(desc_at + (size_t)n * sizeof(ConvDesc));
+        if (rc) return rc;
+        uint8_t* cb = (uint8_t*)c.conv.p;
+        ConvDesc* hd = (ConvDesc*)(stage + conv_stage);
+        unsigned long long ctas = 0;
+        uint32_t planar = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            RaggedImage& r = im[i];
+            const uint32_t per = convert_ctas_per_image(r.w, r.h);
+            hd[i] = ConvDesc{r.pixels, 0, src[i].row, src[i].chan, at[i], ctas, 1, r.w, r.h, r.chans, per, src[i].planar ? 1u : 0u};
+            ctas += per;
+            planar += hd[i].planar;
+            r.pixels = cb + at[i]; r.row = (uint64_t)r.w * r.chans; r.chan = 0;
+        }
+        rc = c.ws_acquire(s);
+        if (rc) return rc;
+        FPNGB_CUDA_OK(cudaMemcpyAsync(cb + desc_at, hd, (size_t)n * sizeof(ConvDesc), cudaMemcpyHostToDevice, s));
+        cp.one = hd[0]; cp.desc = (const ConvDesc*)(cb + desc_at); cp.count = n; cp.total_ctas = ctas; cp.dst = cb;
+        convert_enqueue(cp, fmt->dtype, planar == 0 ? kConvInterleaved : planar == n ? kConvPlanar : kConvAny, s);
+    }
 
     // images the 16-pixel kernels do not take (RGBA 1-pass under a table whose one-pixel-match rule is live, or FPNGB_FORCE_GENERIC)
     // go through the uniform pipeline one at a time, into their slots
@@ -733,18 +853,12 @@ int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_
         const RaggedImage& r = im[i];
         if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
             const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
-            const int rc = encode_batch_locked(c, r.pixels, (size_t)r.h * r.row, (uint32_t)r.row, r.chan, 1, r.w, r.h, r.chans, flags,
-                                               out + r.slot, slot, d_sizes + i, s);
-            if (rc) return rc;
+            rc = encode_batch_locked(c, r.pixels, (size_t)r.h * r.row, (uint32_t)r.row, r.chan, 1, r.w, r.h, r.chans, flags,
+                                     out + r.slot, slot, d_sizes + i, s);
+            if (rc) { prof_drop_conv(); cudaEventRecord(sl->ev, s); return rc; }
         } else ids.push_back(i);
     }
 
-    // staging: d_out_offsets (n + 1), then the descriptor table and work lists
-    const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
-    StageSlot* sl = nullptr;
-    int rc = ragged_stage_slot(ofs_bytes + align_up((size_t)n * sizeof(ImageDesc), 16) + (size_t)n * 5 * 4, &sl);
-    if (rc) return rc;
-    uint8_t* stage = (uint8_t*)sl->buf.p;
     uint64_t* h_ofs = (uint64_t*)stage;
     for (uint32_t i = 0; i < n; i++) h_ofs[i] = im[i].slot;
     h_ofs[n] = total;
@@ -753,8 +867,58 @@ int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_
         rc = encode_ragged_locked(c, im, ids, flags, out, d_sizes, s, stage + ofs_bytes);
         if (rc) { cudaEventRecord(sl->ev, s); return rc; }
     }
+    prof_drop_conv();
     FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
     return FPNGB_OK;
+}
+
+int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
+                               void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    return encode_ragged_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                     const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
+                                     uint32_t* d_sizes, void* stream)
+{
+    return encode_ragged_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+int fpngb_encode_batch_device_typed(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride,
+                                    uint32_t n, uint32_t w, uint32_t h, uint32_t chans, const fpngb_pixel_format* fmt, uint32_t flags,
+                                    void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    size_t es = 0;
+    int rc = typed_dtype(fmt, es);
+    if (rc) return rc;
+    if (!d_pixels || !d_out || !d_sizes || n == 0 || n > 65535 || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
+    ConvertParams cp{};
+    rc = typed_affine(fmt, chans, cp);
+    if (rc) return rc;
+    Layout L;
+    rc = typed_layout(d_pixels, image_stride, row_pitch, pixel_stride, chan_stride, n, h, w, chans, es, L);
+    if (rc) return rc;
+    if (out_stride < max_encoded_size(w, h, chans)) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    if (out_stride % 16 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    Context& c = g_ctx;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const size_t image_bytes = (size_t)w * h * chans;
+    rc = c.conv.reserve((size_t)n * image_bytes);
+    if (rc) return rc;
+    rc = c.ws_acquire(s);
+    if (rc) return rc;
+    const uint32_t ctas = convert_ctas_per_image(w, h);
+    cp.one = ConvDesc{(const uint8_t*)d_pixels, L.image, L.row, L.chan, 0, 0, n, w, h, chans, ctas, L.planar ? 1u : 0u};
+    cp.count = 1; cp.total_ctas = (unsigned long long)n * ctas; cp.dst = (uint8_t*)c.conv.p;
+    convert_enqueue(cp, fmt->dtype, L.planar ? kConvPlanar : kConvInterleaved, s);
+    rc = encode_batch_locked(c, (const uint8_t*)c.conv.p, image_bytes, w * chans, 0, n, w, h, chans, flags, (uint8_t*)d_out, out_stride,
+                             d_sizes, s);
+    prof_drop_conv();
+    return rc;
 }
 
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)
@@ -860,7 +1024,9 @@ int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
 }
 
 // Per-kernel device times (ms) averaged over the encode calls since the last read; slots in ProfSlot order:
-// hist, huffman, scan, offsets, pack, adler, crc.  Returns the number of calls averaged.
+// hist, huffman, scan, offsets, fused, finish, pack, adler, crc, conversion pre-pass (slot 9: the *_typed calls, and the uint8 copy of a
+// strided batch bound for the generic or single-pass encoder).  A caller asking for 9 slots gets the first nine.  Returns the number
+// of calls averaged.
 FPNGB_API int fpngb_profile_enable(int on)
 {
     std::lock_guard<std::mutex> lk(g_ctx.mu);
@@ -880,9 +1046,11 @@ FPNGB_API int fpngb_profile_read(float* ms, int nslots)
             float t = 0;
             cudaEventSynchronize(ps->ev[i + 1]);
             // the CRC of a chunk may run on the side stream, overlapped with the next chunk: its own start event brackets it
-            cudaEvent_t from = (i == kProfCrc && ps->crc_side) ? ps->crc_start : ps->ev[last];
+            // and the conversion pre-pass, which runs before slot 0 opens
+            const bool own_start = (i == kProfCrc && ps->crc_side) || i == kProfConvert;
+            cudaEvent_t from = i == kProfConvert ? ps->conv_start : own_start ? ps->crc_start : ps->ev[last];
             if (cudaEventElapsedTime(&t, from, ps->ev[i + 1]) == cudaSuccess) sum[i] += t;
-            if (!(i == kProfCrc && ps->crc_side)) last = i + 1;
+            if (!own_start) last = i + 1;
         }
         if (ps->call < first_call) first_call = ps->call;
         if (ps->call > last_call) last_call = ps->call;

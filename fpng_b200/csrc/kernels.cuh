@@ -166,13 +166,30 @@ void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint
 void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s);
 void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s);
 
-// strided input -> contiguous [n][h][w * chans] (encode16_kernels.cu)
-struct GatherParams {
-    const uint8_t* src; size_t image_stride, row_pitch, pixel_stride, chan_stride;
-    uint8_t* dst;
+// Conversion pre-pass (encode_typed_kernels.cu): strided input of T -> tight uint8 HWC rows.  One descriptor is an image, or with
+// n > 1 a batch of n images of one shape: element (i, y, x, c) at src + i*image + y*row + x*pixel + c*chan bytes, where pixel is
+// chans * sizeof(T) (interleaved) or sizeof(T) (planar), goes to byte dst + ((i*h + y)*w + x)*chans + c of ConvertParams::dst.
+struct ConvDesc {
+    const uint8_t* src;
+    unsigned long long image, row, chan;          // byte strides (chan: the plane stride of a planar image)
+    unsigned long long dst;                       // byte offset of image 0's tight rows
+    unsigned long long cta_start;                 // first CTA of the descriptor in the launch
     uint32_t n, w, h, chans;
+    uint32_t ctas_per_image;                      // convert_ctas_per_image(w, h)
+    uint32_t planar;
 };
-void launch_gather_pixels(const GatherParams& p, cudaStream_t s);
+struct ConvertParams {
+    ConvDesc one;                                 // count == 1: the only descriptor, passed by value
+    const ConvDesc* desc;                         // count > 1: device table, ascending cta_start
+    uint32_t count;
+    unsigned long long total_ctas;
+    uint8_t* dst;
+    float scale[4], bias[4];                      // per channel (the uint8 copy ignores them)
+};
+enum { kConvInterleaved = 0, kConvPlanar = 1, kConvAny = 2 };   // kConvAny: per descriptor (ConvDesc::planar)
+uint32_t convert_ctas_per_image(uint32_t w, uint32_t h);
+// dtype: an FPNGB_DTYPE_* value, or 0 for the uint8 copy (kConvInterleaved or kConvPlanar only)
+void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, cudaStream_t s);
 
 void launch_scan(const ScanParams& p, uint32_t n, uint32_t chans, int mode, bool hist, cudaStream_t s);
 bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans);

@@ -375,6 +375,39 @@ FPNGB_API int fpngb_decode_packed_ragged_device_typed(const void* d_base, size_t
                                                       uint64_t* d_out_offsets /* n+1 */, uint32_t* d_info /* n*6 or NULL */,
                                                       const fpngb_pixel_format* fmt, int32_t* d_status, void* stream);
 
+/* ---- typed encode input: float32 / float16 / bfloat16 pixels with a per-channel scale and bias, rounded to 8 bits ------------
+ * The *_typed encode calls take the input as elements x of T (fmt->dtype: float32, float16 or bfloat16) and encode, for channel c,
+ * the uint8 value
+ *     f = (float)x                                        exact for all three types
+ *     y = (f * scale[c]) + bias[c]                        two separately rounded fp32 operations, never an FMA
+ *     q = NaN(y) ? 0 : clamp(round_half_to_even(y), 0, 255)
+ *   so +-inf and out-of-range values saturate to 255 or 0.  In torch: torch.nan_to_num(x.float() * s + b, nan=0.0).round()
+ *   .clamp(0, 255).to(torch.uint8).  The written file is byte-identical to what fpngb_encode_batch_device writes for the uint8
+ *   image q, for every flag.  Rounding is half to even only; torchvision's save_image adds 0.5 and truncates, which differs on
+ *   exact ties (x.5) alone.  Here scale and bias act on the input: the inverse of a typed decode's normalisation is
+ *   scale = max_value * std, bias = max_value * mean.  Entries at an index >= the image's channel count are ignored.
+ *   How: one conversion kernel reads the input once and writes tight uint8 rows into a library-owned device buffer of
+ *   sum(w*h*chans) bytes (grow-only, kept between calls); the uint8 pipeline then encodes that buffer.  Each call adds that one
+ *   launch to the uint8 call's, and fpngb_profile_read reports the conversion kernel in slot 9.
+ * Call-level checks, in addition to the uint8 twin's (a rejected call enqueues nothing and writes nothing):
+ *   FPNGB_ERR_INVALID_ARG for a NULL fmt, a dtype other than the three above, or a scale or bias entry in use (index < chans; for
+ *   the ragged call, < the largest chans of the call) that is not finite;
+ *   FPNGB_ERR_ALIGNMENT unless the pixel address(es) and every stride are multiples of sizeof(T);
+ *   FPNGB_ERR_INVALID_ARG unless the strides divided by sizeof(T) form an interleaved or planar layout of "Pixel layouts" (pixel
+ *   stride chans * sizeof(T), channel stride sizeof(T); or pixel stride sizeof(T)), size-1 dimensions canonicalised.  Inputs may
+ *   overlap (stride 0 included).  All input addressing is 64-bit: no row-pitch limit, and one image's input may pass 4 GiB.
+ * fpngb_encode_batch_device_typed: the arguments of fpngb_encode_batch_device_strided plus fmt; strides in BYTES.
+ * fpngb_encode_ragged_device_typed: the arguments of fpngb_encode_ragged_device plus fmt; strides (or NULL for tight HWC rows of
+ *   T) in BYTES.  One launch converts every image of the call (its descriptors go up with the call's other tables through the
+ *   pinned staging ring).  Slots, d_out_offsets, d_sizes, fallbacks, stream ordering with no host synchronisation: the uint8 call's. */
+FPNGB_API int fpngb_encode_batch_device_typed(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride,
+                                              size_t chan_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans,
+                                              const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_stride,
+                                              uint32_t* d_sizes, void* stream);
+FPNGB_API int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                               const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap,
+                                               uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
+
 /* Pins the calling thread to the CPUs of the NUMA node of the library's GPU (sysfs: the GPU's PCI device -> numa_node ->
  * cpulist), so that pinned buffers allocated afterwards and the thread that issues the H2D/D2H copies are local to the GPU's
  * PCIe root port.  Call once per rank after fpngb_init(), before allocating staging memory.  Returns the node, or -1 if the
