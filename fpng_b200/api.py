@@ -169,18 +169,45 @@ def layout_strides(shape, strides):
     return image, row, pixel, chan
 
 
-def _input_format(dtype, scale, bias, chans, what):
-    """None for uint8 input (the uint8 calls: no scale or bias), else the fpngb_pixel_format of a float32 / float16 / bfloat16
-    input (scale defaults to 1, bias to 0; one value or one per channel).  ValueError for any other dtype."""
+def _layout(t, shape):
+    """The byte strides (image_stride, row_pitch, pixel_stride, chan_stride) of the C calls for t, an [n, h, w, chans] array of
+    the given shape: those of tight rows for a contiguous tensor, else those of a view of that shape in one of the layouts of
+    layout_strides.  ValueError for a view of another shape or layout."""
+    if t.is_contiguous():
+        n, h, w, c = (int(v) for v in shape)
+        es = t.element_size()
+        return h * w * c * es, w * c * es, c * es, es
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError(f"a non-contiguous view must have shape {tuple(shape)}, got {tuple(t.shape)}")
+    return typed_layout(t.shape, t.stride(), t.element_size())
+
+
+def _check_arg(t, name, device, dtype, entries=0, row_bytes=None, view=False):
+    """ValueError unless t, the tensor a caller passed as `name`, is a CUDA tensor on `device` of `dtype` that holds what the call
+    writes there: with row_bytes (an encode's out), at least `entries` rows of row_bytes with unit stride within a row; with view
+    (a decode's pixels), a non-contiguous view, whose shape and layout _layout checks, or else a contiguous tensor of at least
+    `entries` elements, as for every other tensor."""
     import torch
 
-    if dtype == torch.uint8:
-        if scale is not None or bias is not None:
-            raise ValueError(f"{what}: scale and bias apply to float32 / float16 / bfloat16 input only; uint8 pixels are encoded as they are")
-        return None
-    if _DTYPE_CODES.get(str(dtype).replace("torch.", "")) is None:
-        raise ValueError(f"{what}: input dtype {dtype}: torch.uint8, float32, float16 or bfloat16")
-    return _pixel_format(dtype, scale, bias, chans)
+    if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device != device:
+        raise ValueError(f"{name}: a CUDA tensor on {device} is needed")
+    if t.dtype != dtype:
+        raise ValueError(f"{name}: dtype {t.dtype}, {dtype} is needed")
+    if row_bytes is not None:
+        ok = t.dim() == 2 and t.shape[0] >= entries and t.shape[1] >= row_bytes and (t.stride(1) == 1 or t.shape[1] == 1)
+        want = f"at least [{entries}, {row_bytes}] with unit stride within a row"
+    else:
+        ok = (view and not t.is_contiguous()) or (t.is_contiguous() and t.numel() >= entries)
+        want = f"a contiguous tensor of at least {entries} elements" + (" or an [n, h, w, c] view" if view else "")
+    if not ok:
+        raise ValueError(f"{name}: shape {tuple(t.shape)} with strides {t.stride()}: {want} is needed")
+
+
+def _stream(stream, device):
+    """the stream a call enqueues on: `stream` (a cudaStream_t handle) when given, else the current torch stream of device"""
+    import torch
+
+    return stream if stream is not None else torch.cuda.current_stream(device).cuda_stream
 
 
 def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=None, scale=None, bias=None):
@@ -200,28 +227,19 @@ def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=Non
 
     assert images.dim() == 4
     n, h, w, c = images.shape
-    fmt = _input_format(images.dtype, scale, bias, c, "encode_batch_device")
+    fmt = _pixel_format(images.dtype, scale, bias, c, "encode_batch_device")
     assert images.is_cuda
-    strided = not images.is_contiguous()
-    if fmt is not None:
-        layout = typed_layout(images.shape, images.stride(), images.element_size())
-    elif strided:
-        layout = layout_strides(images.shape, images.stride())
-    stride = (max_encoded_size(w, h, c) + 15) // 16 * 16
+    layout = _layout(images, images.shape)
+    cap = max_encoded_size(w, h, c)
     if out is None:
-        out = torch.empty((n, stride), dtype=torch.uint8, device=images.device)
+        out = torch.empty((n, (cap + 15) // 16 * 16), dtype=torch.uint8, device=images.device)
     if sizes is None:
         sizes = torch.empty((n,), dtype=torch.int32, device=images.device)
-    s = stream if stream is not None else torch.cuda.current_stream(images.device).cuda_stream
-    if fmt is not None:
-        rc = lib().fpngb_encode_batch_device_typed(images.data_ptr(), *layout, n, w, h, c, C.byref(fmt), flags, out.data_ptr(),
-                                                   out.stride(0), sizes.data_ptr(), s)
-    elif strided:
-        rc = lib().fpngb_encode_batch_device_strided(images.data_ptr(), *layout, n, w, h, c, flags, out.data_ptr(), out.stride(0),
-                                                     sizes.data_ptr(), s)
-    else:
-        rc = lib().fpngb_encode_batch_device(images.data_ptr(), h * w * c, n, w, h, c, flags, out.data_ptr(), out.stride(0),
-                                             sizes.data_ptr(), s)
+    _check_arg(out, "out", images.device, torch.uint8, n, row_bytes=cap)
+    _check_arg(sizes, "sizes", images.device, torch.int32, n)
+    args = (images.data_ptr(), *layout, n, w, h, c) + ((C.byref(fmt),) if fmt is not None else ())
+    rc = (lib().fpngb_encode_batch_device_strided if fmt is None else lib().fpngb_encode_batch_device_typed)(
+        *args, flags, out.data_ptr(), out.stride(0), sizes.data_ptr(), _stream(stream, images.device))
     check(rc, "encode_batch_device")
     return out, sizes
 
@@ -265,7 +283,7 @@ def encode_ragged_device(images, flags: int = 0, out=None, stream=None, scale=No
     ptrs = np.array(ptrs, dtype=np.uint64)
     dims = np.array(dims, dtype=np.uint32).reshape(n, 3)
     strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
-    fmt = _input_format(dtype, scale, bias, int(dims[:, 2].max()) if n else 3, "encode_ragged_device")
+    fmt = _pixel_format(dtype, scale, bias, int(dims[:, 2].max()) if n else 3, "encode_ragged_device")
     if fmt is not None:
         strides = strides * np.uint64(images[0].element_size())
     device = images[0].device if n else torch.device("cuda")
@@ -276,10 +294,10 @@ def encode_ragged_device(images, flags: int = 0, out=None, stream=None, scale=No
                 slot[key] = (max_encoded_size(*key) + 15) // 16 * 16
         total = sum(slot[key] for key in map(tuple, dims.tolist()))
         out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
-    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous(), "out: flat uint8 CUDA tensor"
+    _check_arg(out, "out", device, torch.uint8)
     offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
     sizes = torch.empty((n,), dtype=torch.int32, device=device)
-    s = stream if stream is not None else torch.cuda.current_stream(device).cuda_stream
+    s = _stream(stream, device)
     if fmt is not None:
         rc = lib().fpngb_encode_ragged_device_typed(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
                                                     strides.ctypes.data_as(C.c_void_p), C.byref(fmt), flags, out.data_ptr(),
@@ -303,23 +321,12 @@ def compact_packed_device(data, offsets, sizes, out=None, stream=None):
     n = _packed_args(data, offsets, sizes)
     if out is None:
         out = torch.empty((max(data.numel(), 16),), dtype=torch.uint8, device=data.device)
-    assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous(), "out: flat uint8 CUDA tensor"
+    _check_arg(out, "out", data.device, torch.uint8)
     dst_offsets = torch.empty((n + 1,), dtype=torch.int64, device=data.device)
-    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    s = _stream(stream, data.device)
     check(lib().fpngb_compact_packed_device(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, out.data_ptr(), out.numel(),
                                             dst_offsets.data_ptr(), s), "compact_packed_device")
     return out, dst_offsets
-
-
-def _strided_out(out, n, h, w, desired_channels):
-    """The layout of a caller's non-contiguous `out` view (layout_strides), or None for a contiguous one."""
-    import torch
-
-    assert out.is_cuda and out.dtype == torch.uint8
-    if out.is_contiguous():
-        return None
-    assert tuple(out.shape) == (n, h, w, desired_channels), "a non-contiguous out must be an [n, h, w, desired_channels] view"
-    return layout_strides(out.shape, out.stride())
 
 
 _DTYPE_CODES = {"float32": 1, "float16": 2, "bfloat16": 3}   # FPNGB_DTYPE_*
@@ -347,22 +354,23 @@ def _per_channel(v, desired_channels, default, what):
     return [float(x) for x in a]
 
 
-def _pixel_format(dtype, scale, bias, desired_channels):
-    """None for uint8 output (the uint8 calls, which take no scale or bias), else the fpngb_pixel_format of a float output:
-    scale defaults to 1 and bias to 0 per channel; a single value applies to every channel.  Values are rounded to float32."""
+def _pixel_format(dtype, scale, bias, chans, what="pixel format"):
+    """None for uint8 pixels (the uint8 calls, which take no scale or bias), else the fpngb_pixel_format of float32 / float16 /
+    bfloat16 pixels of chans channels: scale defaults to 1 and bias to 0 per channel; a single value applies to every channel.
+    Values are rounded to float32.  ValueError for any other dtype."""
     import torch
 
     if dtype == torch.uint8:
         if scale is not None or bias is not None:
-            raise ValueError("scale and bias apply to float32 / float16 / bfloat16 output only; uint8 pixels are written as decoded")
+            raise ValueError(f"{what}: scale and bias apply to float32 / float16 / bfloat16 pixels only; uint8 pixels are taken as they are")
         return None
     code = _DTYPE_CODES.get(str(dtype).replace("torch.", ""))
     if code is None:
-        raise ValueError(f"output dtype {dtype}: torch.uint8, float32, float16 or bfloat16")
+        raise ValueError(f"{what}: dtype {dtype}: torch.uint8, float32, float16 or bfloat16")
     fmt = PixelFormat()
     fmt.dtype = code
-    fmt.scale[:desired_channels] = _per_channel(scale, desired_channels, 1.0, "scale")
-    fmt.bias[:desired_channels] = _per_channel(bias, desired_channels, 0.0, "bias")
+    fmt.scale[:chans] = _per_channel(scale, chans, 1.0, "scale")
+    fmt.bias[:chans] = _per_channel(bias, chans, 0.0, "bias")
     return fmt
 
 
@@ -394,12 +402,6 @@ def denormalize_scale_bias(mean, std, max_value=255.0):
     m = np.asarray(mean, dtype=np.float64).reshape(-1)
     sd = np.asarray(std, dtype=np.float64).reshape(-1)
     return (float(max_value) * sd).astype(np.float32), (float(max_value) * m).astype(np.float32)
-
-
-def _typed_out(out, n, h, w, desired_channels):
-    """the byte strides of a float `out` (any [n, h, w, desired_channels] view in one of the layouts of layout_strides)"""
-    assert out.is_cuda and tuple(out.shape) == (n, h, w, desired_channels), "out must be an [n, h, w, desired_channels] CUDA view"
-    return typed_layout(out.shape, out.stride(), out.element_size())
 
 
 def get_info_ex(data):
@@ -447,25 +449,23 @@ def decode_batch_device(files_dev, sizes, idat_ofs, idat_len, w: int, h: int, ch
     import torch
 
     assert files_dev.is_cuda and files_dev.dtype == torch.uint8 and files_dev.dim() == 2 and files_dev.is_contiguous()
-    n = files_dev.shape[0]
+    n, dev = files_dev.shape[0], files_dev.device
     odt = _out_dtype(out, dtype)
-    fmt = _pixel_format(odt, scale, bias, desired_channels)
+    fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_batch_device")
+    shape = (n, h, w, desired_channels)
     if out is None:
-        out = torch.empty((n, h, w, desired_channels), dtype=odt, device=files_dev.device)
-    layout = _strided_out(out, n, h, w, desired_channels) if fmt is None else _typed_out(out, n, h, w, desired_channels)
+        out = torch.empty(shape, dtype=odt, device=dev)
     if status is None:
-        status = torch.empty((n,), dtype=torch.int32, device=files_dev.device)
-    s = stream if stream is not None else torch.cuda.current_stream(files_dev.device).cuda_stream
+        status = torch.empty((n,), dtype=torch.int32, device=dev)
+    _check_arg(out, "out", dev, odt, n * h * w * desired_channels, view=True)
+    _check_arg(status, "status", dev, torch.int32, n)
     sizes = np.ascontiguousarray(sizes, dtype=np.uint32); idat_ofs = np.ascontiguousarray(idat_ofs, dtype=np.uint32)
     idat_len = np.ascontiguousarray(idat_len, dtype=np.uint32)
     args = (files_dev.data_ptr(), files_dev.stride(0), sizes.ctypes.data_as(C.c_void_p), idat_ofs.ctypes.data_as(C.c_void_p),
-            idat_len.ctypes.data_as(C.c_void_p), n, w, h, chans_in_file, desired_channels, out.data_ptr())
-    if fmt is not None:
-        rc = lib().fpngb_decode_batch_device_typed(*args, *layout, C.byref(fmt), status.data_ptr(), s)
-    elif layout is None:
-        rc = lib().fpngb_decode_batch_device(*args, h * w * desired_channels, status.data_ptr(), s)
-    else:
-        rc = lib().fpngb_decode_batch_device_strided(*args, *layout, status.data_ptr(), s)
+            idat_len.ctypes.data_as(C.c_void_p), n, w, h, chans_in_file, desired_channels, out.data_ptr(), *_layout(out, shape))
+    args += (C.byref(fmt),) if fmt is not None else ()
+    rc = (lib().fpngb_decode_batch_device_strided if fmt is None else lib().fpngb_decode_batch_device_typed)(
+        *args, status.data_ptr(), _stream(stream, dev))
     check(rc, "decode_batch_device")
     return out, status
 
@@ -496,7 +496,7 @@ def get_info_batch_device(data, offsets, sizes, stream=None):
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
     if n == 0:
         return info
-    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    s = _stream(stream, data.device)
     check(lib().fpngb_get_info_batch_device(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, info.data_ptr(), s),
           "get_info_batch_device")
     return info
@@ -518,23 +518,19 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
     if max_file_size is None:
         max_file_size = min(max_encoded_size(w, h, chans_in_file), 0xFFFFFFFF)
     odt = _out_dtype(out, dtype)
-    fmt = _pixel_format(odt, scale, bias, desired_channels)
+    fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_device")
+    shape = (n, h, w, desired_channels)
     if out is None:
-        out = torch.empty((n, h, w, desired_channels), dtype=odt, device=data.device)
+        out = torch.empty(shape, dtype=odt, device=data.device)
     if status is None:
         status = torch.empty((n,), dtype=torch.int32, device=data.device)
-    layout = _strided_out(out, n, h, w, desired_channels) if fmt is None else _typed_out(out, n, h, w, desired_channels)
-    assert layout is not None or out.numel() >= n * h * w * desired_channels
-    assert status.is_cuda and status.dtype == torch.int32 and status.is_contiguous() and status.numel() >= n
-    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    _check_arg(out, "out", data.device, odt, n * h * w * desired_channels, view=True)
+    _check_arg(status, "status", data.device, torch.int32, n)
     args = (data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, max_file_size, w, h, chans_in_file, desired_channels,
-            out.data_ptr())
-    if fmt is not None:
-        rc = lib().fpngb_decode_packed_device_typed(*args, *layout, C.byref(fmt), status.data_ptr(), s)
-    elif layout is None:
-        rc = lib().fpngb_decode_packed_device(*args, h * w * desired_channels, status.data_ptr(), s)
-    else:
-        rc = lib().fpngb_decode_packed_device_strided(*args, *layout, status.data_ptr(), s)
+            out.data_ptr(), *_layout(out, shape))
+    args += (C.byref(fmt),) if fmt is not None else ()
+    rc = (lib().fpngb_decode_packed_device_strided if fmt is None else lib().fpngb_decode_packed_device_typed)(
+        *args, status.data_ptr(), _stream(stream, data.device))
     check(rc, "decode_packed_device")
     return out, status
 
@@ -590,18 +586,18 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     n = _packed_args(data, offsets, sizes)
     assert desired_channels in (3, 4), "desired_channels: 3 or 4"
     odt = _out_dtype(out, dtype)
-    fmt = _pixel_format(odt, scale, bias, desired_channels)
+    fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_ragged_device")
     es = torch.empty((), dtype=odt).element_size()
     if out is None or max_file_size is None or max_w is None or max_h is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
                                                              stream, es)
         if out is None:
             out = torch.empty((max(total, 16) // es,), dtype=odt, device=data.device)[:total // es]
-    assert out.is_cuda and out.dtype == odt and out.is_contiguous() and out.dim() == 1, "out: flat CUDA tensor of the output dtype"
+    _check_arg(out, "out", data.device, odt)
     out_offsets = torch.empty((n + 1,), dtype=torch.int64, device=data.device)
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
     status = torch.empty((n,), dtype=torch.int32, device=data.device)
-    s = stream if stream is not None else torch.cuda.current_stream(data.device).cuda_stream
+    s = _stream(stream, data.device)
     args = (data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
             int(max_h), desired_channels, out.data_ptr(), out.numel() * es, out_offsets.data_ptr(), info.data_ptr())
     if fmt is None:
@@ -686,7 +682,7 @@ def train_accumulate_device(images, counts=None, stream=None):
     n, h, w, c = images.shape
     if counts is None:
         counts = np.zeros(288, dtype=np.uint64)
-    s = stream if stream is not None else torch.cuda.current_stream(images.device).cuda_stream
+    s = _stream(stream, images.device)
     check(lib().fpngb_train_accumulate_device(images.data_ptr(), h * w * c, n, w, h, c, counts.ctypes.data_as(C.c_void_p), s), "train_accumulate_device")
     return counts
 

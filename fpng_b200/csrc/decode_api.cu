@@ -5,7 +5,6 @@
 #include "container.cuh"
 #include "layout.h"
 #include "runtime.h"
-#include <math.h>
 #include <string.h>
 #include <atomic>
 #include <vector>
@@ -13,7 +12,6 @@
 namespace fpngb {
 
 static Buffer g_dec_ws;        // FileDesc[n] | DecodeState[n] | luts | delta scratch
-static Buffer g_dec_pin;       // pinned staging for the FileDesc upload / status download
 
 // fpngb_set_decode_verify: off at load; every decode call reads it once, under context().mu, when it enqueues
 static std::atomic<int> g_decode_verify{0};
@@ -58,10 +56,6 @@ static OutStrides set_output(DecodeParams& p, uint8_t* d_out, const Layout& L)
     p.d_out = d_out;
     return OutStrides{L.row, L.pixel, L.chan};
 }
-static Layout tight_output(uint32_t w, uint32_t h, uint32_t desired, size_t out_stride)
-{
-    return Layout{out_stride, (uint64_t)w * desired, desired, 1, false};
-}
 
 // Call-level checks shared by the device decode entry points: counts, channels and the container's shape limits
 // (fpng.cpp:2966-2971: keeps w * chans and the scratch pitch inside 32 bits).
@@ -72,34 +66,15 @@ static int decode_shape_check(uint32_t w, uint32_t h, uint32_t chans_in_file, ui
     if ((uint64_t)w * h * desired_chans > 0xFFFFFFFFull) return FPNGB_ERR_BUFFER_TOO_SMALL;
     return FPNGB_OK;
 }
-// A strided output of elem-byte elements (1: uint8 pixels) must be elem-aligned, interleaved or planar in elements, addressable,
-// and no two elements may share a byte.  L receives the byte strides.
-static int decode_output_check(const void* d_out, size_t image, size_t row, size_t pixel, size_t chan, uint32_t n, uint32_t w, uint32_t h,
-                               uint32_t desired, size_t elem, Layout& L)
+// The output format of a device decode call as the decode kernels take it: uint8 (typed false, fmt unused) or the *_typed call's
+// fmt.  elem receives the bytes per element.
+static int decode_format(bool typed, const fpngb_pixel_format* fmt, uint32_t desired, TypedOut& t, uint32_t& elem)
 {
-    if ((uintptr_t)d_out % elem || image % elem || row % elem || pixel % elem || chan % elem) return FPNGB_ERR_ALIGNMENT;
-    uint64_t last = 0;
-    if (!classify_layout(image / elem, row / elem, pixel / elem, chan / elem, n, h, w, desired, L) || !layout_disjoint(L, n, h, w, desired))
-        return FPNGB_ERR_INVALID_ARG;
-    L.image *= elem; L.row *= elem; L.pixel *= elem; L.chan *= elem;
-    if (!layout_span(d_out, L, n, h, w, desired, last) || last > UINT64_MAX - (uint64_t)(uintptr_t)d_out - (elem - 1))
-        return FPNGB_ERR_INVALID_ARG;
-    return FPNGB_OK;
-}
-
-// The output type of a *_typed call (desired is 3 or 4): FPNGB_ERR_INVALID_ARG for a NULL fmt, another dtype, or a scale or bias
-// in use that is not finite.  elem receives sizeof(T).
-static int typed_format(const fpngb_pixel_format* fmt, uint32_t desired, TypedOut& t, size_t& elem)
-{
-    if (!fmt || (fmt->dtype != FPNGB_DTYPE_FLOAT32 && fmt->dtype != FPNGB_DTYPE_FLOAT16 && fmt->dtype != FPNGB_DTYPE_BFLOAT16))
-        return FPNGB_ERR_INVALID_ARG;
-    t = TypedOut{};
-    t.dtype = fmt->dtype;
-    for (uint32_t c = 0; c < desired; c++) {
-        if (!isfinite(fmt->scale[c]) || !isfinite(fmt->bias[c])) return FPNGB_ERR_INVALID_ARG;
-        t.aff.scale[c] = fmt->scale[c]; t.aff.bias[c] = fmt->bias[c];
-    }
-    elem = fmt->dtype == FPNGB_DTYPE_FLOAT32 ? 4 : 2;
+    PixelFormat f = uint8_format();
+    if (typed) { const int rc = parse_format(fmt, desired, f); if (rc) return rc; }
+    t = TypedOut{f.dtype, {}};
+    memcpy(t.aff.scale, f.scale, sizeof f.scale); memcpy(t.aff.bias, f.bias, sizeof f.bias);
+    elem = f.elem;
     return FPNGB_OK;
 }
 
@@ -114,21 +89,17 @@ static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const
     DecodeParams p{};
     VerifyState* verify = nullptr;
     int rc = decode_workspace_uniform_locked(n, w, h, chans, max_idat, s, p, &verify); if (rc) return rc;
-    g_dec_pin.pinned = true;
-    rc = g_dec_pin.reserve((size_t)n * sizeof(FileDesc)); if (rc) return rc;
-    // the pinned staging buffer may still be in flight from the previous call on another stream: wait for it
-    static cudaEvent_t staged = nullptr;
-    if (!staged) FPNGB_CUDA_OK(cudaEventCreateWithFlags(&staged, cudaEventDisableTiming));
-    else FPNGB_CUDA_OK(cudaEventSynchronize(staged));
-    FileDesc* staging = (FileDesc*)g_dec_pin.p;
+    StageSlot* sl = nullptr;
+    rc = context().stage_slot((size_t)n * sizeof(FileDesc), &sl); if (rc) return rc;
+    FileDesc* staging = (FileDesc*)sl->buf.p;
     for (uint32_t i = 0; i < n; i++) {
         FileDesc& fd = staging[i];
         fd = h_files[i]; fd.base = (unsigned long long)i * file_stride; fd.pre_status = 0;
         fd.w = w; fd.h = h; fd.chans = chans; fd.pitch = delta_pitch(w, chans);
         fd.delta_base = (unsigned long long)i * fd.pitch * h; fd.out_base = (unsigned long long)i * out.image; fd.sub_base = (unsigned long long)i * p.max_subs;
     }
-    FPNGB_CUDA_OK(cudaMemcpyAsync((void*)p.files, g_dec_pin.p, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
-    FPNGB_CUDA_OK(cudaEventRecord(staged, s));
+    FPNGB_CUDA_OK(cudaMemcpyAsync((void*)p.files, staging, (size_t)n * sizeof(FileDesc), cudaMemcpyHostToDevice, s));
+    FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
     p.d_files = d_files; p.d_status = d_status;
     // the CRC kernel's message ("IDAT" + stream) plus its misalignment stays within max_idat + 8 bytes
     launch_decode(p, set_output(p, d_out, out), n, desired, s, verify, (size_t)max_idat + 8, typed);
@@ -165,11 +136,11 @@ static int decode_batch_device_impl(const void* d_files, size_t file_stride, con
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_files || !file_sizes || !idat_ofs || !idat_len || !d_out || !d_status || n == 0 || n > 65535) return FPNGB_ERR_INVALID_ARG;
     int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
-    TypedOut t{};
-    size_t elem = 1;
-    if (typed) { rc = typed_format(fmt, desired_chans, t, elem); if (rc) return rc; }
+    TypedOut t;
+    uint32_t elem;
+    rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
     Layout out;
-    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, elem, out);
+    rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, h, w, desired_chans, elem, true, out);
     if (rc) return rc;
     if (file_stride % 4 || (uintptr_t)d_files % 4) return FPNGB_ERR_ALIGNMENT;
     std::vector<FileDesc> fds(n);
@@ -192,11 +163,11 @@ static int decode_packed_device_impl(const void* d_base, const uint64_t* d_offse
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_base || !d_offsets || !d_sizes || !d_out || !d_status || n == 0 || n > 65535 || !max_file_size) return FPNGB_ERR_INVALID_ARG;
     int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
-    TypedOut t{};
-    size_t elem = 1;
-    if (typed) { rc = typed_format(fmt, desired_chans, t, elem); if (rc) return rc; }
+    TypedOut t;
+    uint32_t elem;
+    rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
     Layout out;
-    rc = decode_output_check(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, w, h, desired_chans, elem, out);
+    rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, h, w, desired_chans, elem, true, out);
     if (rc) return rc;
     if ((uintptr_t)d_base % 4) return FPNGB_ERR_ALIGNMENT;
     const cudaStream_t s = (cudaStream_t)stream;
@@ -249,9 +220,9 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     if (!d_base || !d_offsets || !d_sizes || !d_out || !d_out_offsets || !d_status || n == 0 || n > 65535 || !max_file_size ||
         (desired_chans != 3 && desired_chans != 4) || !max_w || !max_h || max_w > (1u << 24) || max_h > (1u << 24))
         return FPNGB_ERR_INVALID_ARG;
-    TypedOut t{};
-    size_t elem = 1;
-    if (typed) { const int rc = typed_format(fmt, desired_chans, t, elem); if (rc) return rc; }
+    TypedOut t;
+    uint32_t elem;
+    int rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
     if ((uintptr_t)d_base % 4 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
     unsigned long long sub_cap = 0, delta_cap = 0;
     // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
@@ -262,7 +233,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     DecodeParams p{};
     VerifyState* verify = nullptr;
-    int rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify); if (rc) return rc;
+    rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify); if (rc) return rc;
     p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
@@ -270,7 +241,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     wp.base_bytes = base_bytes;
     launch_container_walk(wp, s);
     PlaceParams pp{};
-    pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * (uint32_t)elem;
+    pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem;
     pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
     launch_decode_place(pp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
@@ -339,7 +310,7 @@ int fpngb_decode_host(const void* file, uint32_t size, void* out, size_t out_cap
     cudaMemcpyAsync(c.dev_in.p, file, size, cudaMemcpyHostToDevice, s);
     FileDesc fd{}; fd.file_size = size; fd.idat_ofs = idat_ofs; fd.idat_len = idat_len;
     if (decode_batch_locked((const uint8_t*)c.dev_in.p, fstride, &fd, 1, ww, hh, cc, desired, (uint8_t*)c.dev_out.p,
-                            tight_output(ww, hh, desired, align_up(need, 16)), d_status, s))
+                            tight_layout(ww, desired, align_up(need, 16)), d_status, s))
         return FPNGB_DECODE_INVALID_ARG;
     uint32_t* h_status = (uint32_t*)c.pin_small.p;
     cudaMemcpyAsync(h_status, d_status, 4, cudaMemcpyDeviceToHost, s);
@@ -424,7 +395,7 @@ int fpngb_decode_batch_host(const void* const* files, const uint32_t* sizes, uin
         }
         cudaEventRecord(ev_in[sl], c.copy_in);
         cudaStreamWaitEvent(c.stream, ev_in[sl], 0);
-        rc = decode_batch_locked(din, fstride, cf.data(), cnt, W, H, C, desired, dout, tight_output(W, H, desired, pstride), dst, c.stream);
+        rc = decode_batch_locked(din, fstride, cf.data(), cnt, W, H, C, desired, dout, tight_layout(W, desired, pstride), dst, c.stream);
         if (rc) { result = rc; break; }
         cudaEventRecord(ev_done[sl], c.stream);
         cudaStreamWaitEvent(c.copy_out, ev_done[sl], 0);

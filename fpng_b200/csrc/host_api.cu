@@ -14,9 +14,7 @@
 
 #include <algorithm>
 #include <atomic>
-#include <math.h>
 #include <mutex>
-#include <new>
 #include <sched.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -202,14 +200,28 @@ static void prof_mark(ProfSet* ps, int slot, cudaStream_t s)
     ps->used[slot] = true;
 }
 
-// One launch of the conversion pre-pass into tight uint8 rows (dtype 0: the uint8 copy), profiled in slot kProfConvert of the
-// encode that follows it on the stream.
-static void convert_enqueue(const ConvertParams& cp, uint32_t dtype, int layout, cudaStream_t s)
+// The conversion descriptor of n images of one shape in byte layout L whose tight uint8 rows go to byte dst of the conversion
+// buffer, converted by the CTAs from cta_start on.
+static ConvDesc conv_desc(const uint8_t* src, const Layout& L, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint64_t dst,
+                          uint64_t cta_start)
 {
+    return ConvDesc{src, L.image, L.row, L.chan, dst, cta_start, n, w, h, chans, convert_ctas_per_image(w, h), L.planar ? 1u : 0u};
+}
+
+// One launch of the conversion pre-pass over the count descriptors hd (ascending cta_start; for count > 1 also uploaded to d_desc)
+// into tight uint8 rows at dst, the uint8 copy for f.dtype 0.  Profiled in slot kProfConvert of the encode that follows it on the stream.
+static void convert_enqueue(const ConvDesc* hd, uint32_t count, const ConvDesc* d_desc, const PixelFormat& f, uint8_t* dst, cudaStream_t s)
+{
+    ConvertParams cp{};
+    cp.one = hd[0]; cp.desc = d_desc; cp.count = count; cp.dst = dst;
+    cp.total_ctas = hd[count - 1].cta_start + (unsigned long long)hd[count - 1].n * hd[count - 1].ctas_per_image;
+    memcpy(cp.scale, f.scale, sizeof cp.scale); memcpy(cp.bias, f.bias, sizeof cp.bias);
+    uint32_t planar = 0;
+    for (uint32_t i = 0; i < count; i++) planar += hd[i].planar;
     prof_drop_conv();
     ProfSet* ps = g_profile ? prof_alloc() : nullptr;
     if (ps) cudaEventRecord(ps->conv_start, s);
-    launch_convert_pixels(cp, dtype, layout, s);
+    launch_convert_pixels(cp, f.dtype, planar == 0 ? kConvInterleaved : planar == count ? kConvPlanar : kConvAny, s);
     count_launch(1);
     if (ps) { prof_mark(ps, kProfConvert, s); g_prof_conv = ps; }
 }
@@ -219,12 +231,10 @@ struct Workspace {
     uint2* lane_ofs; uint32_t lane_ofs_pitch;
     void* fused_desc;
     uint32_t* row_crc;
-    uint8_t* gather;                            // contiguous copy of a strided batch (encoders without layout support)
 };
 
 
-static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, bool two_pass, Workspace& w, bool fused = false,
-                           size_t gather_bytes = 0)
+static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, bool two_pass, Workspace& w, bool fused = false)
 {
     const size_t rows = (size_t)n * h;
     const uint32_t lane_pitch = ((width + 511u) / 512u) * 32u;       // one uint2 per 16-pixel group, whole warp steps
@@ -238,7 +248,6 @@ static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, b
     const size_t o_lane = o; o = align_up(o + (fused ? 0 : rows * lane_pitch * 8), 256);
     const size_t o_desc = o; o = align_up(o + (fused ? fused_desc_bytes(n, width, h) : 0), 256);
     const size_t o_rcrc = o; o = align_up(o + (fused ? 0 : rows * 4), 256);
-    const size_t o_gather = o; o = align_up(o + gather_bytes, 256);
     int rc = c.ws.reserve(o);
     if (rc) return rc;
     uint8_t* b = (uint8_t*)c.ws.p;
@@ -247,7 +256,6 @@ static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, b
     w.st = (ImageState*)(b + o_st); w.hist = (uint32_t*)(b + o_hist); w.books = (CodeBook*)(b + o_books);
     w.lane_ofs = (uint2*)(b + o_lane); w.lane_ofs_pitch = lane_pitch;
     w.fused_desc = b + o_desc;
-    w.gather = b + o_gather;
     return 0;
 }
 
@@ -301,12 +309,12 @@ static void make_png_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t chans
 //    and writes the file once, byte-identical output, measured slower than the two-kernel path because it is bound by
 //    instruction issue, not by HBM.
 //
-// The input layout (layout.h) is image_stride / row_pitch and, for planar images, chan_stride (0: interleaved rows).  The 16-pixel
-// scan and pack kernels read every layout in place; the generic kernels and the single-pass encoder read tight interleaved rows
-// only, so a strided batch bound for them is first copied into the workspace by the uint8 instantiation of convert_pixels_kernel.
-static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image_stride, uint32_t row_pitch, size_t chan_stride,
-                               uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, uint8_t* d_out, size_t out_stride,
-                               uint32_t* d_sizes, cudaStream_t s)
+// The input is n images of format f at src in byte layout L (layout.h; a uint8 row pitch fits in 32 bits).  The 16-pixel scan and
+// pack kernels read every uint8 layout in place.  The conversion pre-pass (convert_pixels_kernel) first writes tight uint8 rows into
+// c.conv for a float input, and for a uint8 input that is not tight interleaved but bound for the generic kernels or the single-pass
+// encoder, which read tight interleaved rows only.  Rows already in c.conv are tight uint8, so they are never converted again.
+static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, const PixelFormat& f, uint32_t n, uint32_t w, uint32_t h,
+                               uint32_t chans, uint32_t flags, uint8_t* d_out, size_t out_stride, uint32_t* d_sizes, cudaStream_t s)
 {
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
     // second-generation kernels (16 pixels per lane, coalesced 128-bit loads) whenever every scanline is 16-byte aligned;
@@ -321,22 +329,18 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
     const bool v2 = !force_generic && !lit1_rule;
     const bool want_fused = g_fused_mode == 1 || (g_fused_mode < 0 && env_fused);
     const bool fused = want_fused && !force_generic && !lit1_rule && !(flags & FPNGB_FORCE_UNCOMPRESSED) &&
-                       fused_eligible(d_pixels, image_stride, w, h, chans, n);
-    const bool gather = (!v2 || fused) && (chan_stride != 0 || row_pitch != w * chans);
-    const size_t bytes_per_image = (size_t)w * h * chans;
+                       fused_eligible(src, L.image, w, h, chans, n);
+    const bool convert = f.dtype != 0 || ((!v2 || fused) && (L.planar || L.row != (uint64_t)w * chans));
+    const size_t image_bytes = (size_t)w * h * chans;
     Workspace ws;
-    int rc = carve_workspace(c, n, h, w, two_pass, ws, fused, gather ? n * bytes_per_image : 0);
+    int rc = carve_workspace(c, n, h, w, two_pass, ws, fused);
     if (rc) return rc;
+    if (convert) { rc = c.conv.reserve((size_t)n * image_bytes); if (rc) return rc; }
     rc = c.ws_acquire(s);
     if (rc) return rc;
-    if (gather) {
-        ConvertParams gp{};
-        const uint32_t ctas = convert_ctas_per_image(w, h);
-        gp.one = ConvDesc{d_pixels, image_stride, row_pitch, chan_stride, 0, 0, n, w, h, chans, ctas, chan_stride ? 1u : 0u};
-        gp.count = 1; gp.total_ctas = (unsigned long long)n * ctas; gp.dst = ws.gather;
-        convert_enqueue(gp, 0, chan_stride ? kConvPlanar : kConvInterleaved, s);
-        d_pixels = ws.gather; image_stride = bytes_per_image; row_pitch = w * chans; chan_stride = 0;
-    }
+    const uint8_t* d_pixels = convert ? (const uint8_t*)c.conv.p : src;
+    const size_t image_stride = convert ? image_bytes : L.image, chan_stride = convert || !L.planar ? 0 : L.chan;
+    const uint32_t row_pitch = convert ? w * chans : (uint32_t)L.row;
     const int mode = pick_load_mode(d_pixels, image_stride, w, chans);
     const CodeBook* books0 = two_pass ? ws.books : c.d_static_books + (chans == 4 ? 1 : 0);
     const uint32_t book_stride = two_pass ? 1u : 0u;
@@ -350,6 +354,11 @@ static int encode_batch_locked(Context& c, const uint8_t* d_pixels, size_t image
     if (nchunks > 1) {
         if (!c.side) FPNGB_CUDA_OK(cudaStreamCreateWithFlags(&c.side, cudaStreamNonBlocking));
         for (int i = 0; i < 5; i++) if (!c.side_ev[i]) FPNGB_CUDA_OK(cudaEventCreateWithFlags(&c.side_ev[i], cudaEventDisableTiming));
+    }
+    // nothing can fail between the pre-pass and the first chunk's prof_begin, which takes over its profile slot
+    if (convert) {
+        const ConvDesc d = conv_desc(src, L, n, w, h, chans, 0, 0);
+        convert_enqueue(&d, 1, nullptr, f, (uint8_t*)c.conv.p, s);
     }
     for (uint32_t k = 0; k < nchunks; k++) {
         const uint32_t i0 = (uint32_t)((uint64_t)n * k / nchunks), i1 = (uint32_t)((uint64_t)n * (k + 1) / nchunks), cnt = i1 - i0;
@@ -455,28 +464,6 @@ struct RaggedImage {
     uint32_t w, h, chans;
     uint64_t slot;                                      // offset of its slot in d_out
 };
-
-// Pinned staging of the descriptor table: a ring of buffers, each reused only once the copy that last read it has completed
-// (cudaEventQuery), so that a call never waits on the stream.
-struct StageSlot { Buffer buf; cudaEvent_t ev = nullptr; };
-static std::vector<StageSlot*> g_ragged_stage;
-
-static int ragged_stage_slot(size_t bytes, StageSlot** out)
-{
-    StageSlot* sl = nullptr;
-    for (StageSlot* x : g_ragged_stage) if (x->buf.cap >= bytes && cudaEventQuery(x->ev) == cudaSuccess) { sl = x; break; }
-    if (!sl) {
-        sl = new (std::nothrow) StageSlot();
-        if (!sl) return FPNGB_ERR_INTERNAL;
-        sl->buf.pinned = true;
-        FPNGB_CUDA_OK(cudaEventCreateWithFlags(&sl->ev, cudaEventDisableTiming));
-        g_ragged_stage.push_back(sl);
-    }
-    const int rc = sl->buf.reserve(bytes);
-    if (rc) return rc;
-    *out = sl;
-    return 0;
-}
 
 static bool force_generic_env()
 {
@@ -694,27 +681,43 @@ FPNGB_API int fpngb_debug_static_table(uint32_t chans, uint8_t* sizes, uint16_t*
     return FPNGB_OK;
 }
 
-int fpngb_encode_batch_device_strided(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride,
-                                      uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* d_out, size_t out_stride,
-                                      uint32_t* d_sizes, void* stream)
+// Body of fpngb_encode_batch_device_strided (typed false, fmt unused) and fpngb_encode_batch_device_typed (fmt required).
+static int encode_batch_impl(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride, uint32_t n,
+                             uint32_t w, uint32_t h, uint32_t chans, bool typed, const fpngb_pixel_format* fmt, uint32_t flags, void* d_out,
+                             size_t out_stride, uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (!d_pixels || !d_out || !d_sizes || n == 0 || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
-    // any interleaved or planar layout, overlapping ones included (the pixels are only read); the kernels take a 32-bit row pitch
+    PixelFormat f = uint8_format();
+    if (typed) { const int rc = parse_format(fmt, chans, f); if (rc) return rc; }
+    if (!d_pixels || !d_out || !d_sizes || n == 0 || n > 65535 || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
+    // any interleaved or planar layout, overlapping ones included (the pixels are only read)
     Layout L;
-    uint64_t last = 0;
-    if (!classify_layout(image_stride, row_pitch, pixel_stride, chan_stride, n, h, w, chans, L) || L.row > 0xFFFFFFFFull ||
-        !layout_span(d_pixels, L, n, h, w, chans, last))
-        return FPNGB_ERR_INVALID_ARG;
+    const int rc = check_layout(d_pixels, image_stride, row_pitch, pixel_stride, chan_stride, n, h, w, chans, f.elem, false, L);
+    if (rc) return rc;
+    if (!typed && L.row > 0xFFFFFFFFull) return FPNGB_ERR_INVALID_ARG;      // the uint8 kernels take a 32-bit row pitch
     if (out_stride < max_encoded_size(w, h, chans)) return FPNGB_ERR_BUFFER_TOO_SMALL;
     if (out_stride % 16 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
-    if (n > 65535) return FPNGB_ERR_INVALID_ARG;
     Context& c = g_ctx;
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     cudaStream_t s = (cudaStream_t)stream;      // NULL = the CUDA default stream, exactly as the caller passed it
-    return encode_batch_locked(c, (const uint8_t*)d_pixels, L.image, (uint32_t)L.row, L.planar ? L.chan : 0, n, w, h, chans, flags,
-                               (uint8_t*)d_out, out_stride, d_sizes, s);
+    return encode_batch_locked(c, (const uint8_t*)d_pixels, L, f, n, w, h, chans, flags, (uint8_t*)d_out, out_stride, d_sizes, s);
+}
+
+int fpngb_encode_batch_device_strided(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride,
+                                      uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* d_out, size_t out_stride,
+                                      uint32_t* d_sizes, void* stream)
+{
+    return encode_batch_impl(d_pixels, image_stride, row_pitch, pixel_stride, chan_stride, n, w, h, chans, false, nullptr, flags, d_out,
+                             out_stride, d_sizes, stream);
+}
+
+int fpngb_encode_batch_device_typed(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride,
+                                    uint32_t n, uint32_t w, uint32_t h, uint32_t chans, const fpngb_pixel_format* fmt, uint32_t flags,
+                                    void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream)
+{
+    return encode_batch_impl(d_pixels, image_stride, row_pitch, pixel_stride, chan_stride, n, w, h, chans, true, fmt, flags, d_out,
+                             out_stride, d_sizes, stream);
 }
 
 int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans,
@@ -727,78 +730,37 @@ int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_
                                              d_sizes, stream);
 }
 
-// The element type of a *_typed encode call: FPNGB_ERR_INVALID_ARG for a NULL fmt or a dtype other than the three float types.
-static int typed_dtype(const fpngb_pixel_format* fmt, size_t& es)
-{
-    if (!fmt || (fmt->dtype != FPNGB_DTYPE_FLOAT32 && fmt->dtype != FPNGB_DTYPE_FLOAT16 && fmt->dtype != FPNGB_DTYPE_BFLOAT16))
-        return FPNGB_ERR_INVALID_ARG;
-    es = fmt->dtype == FPNGB_DTYPE_FLOAT32 ? 4 : 2;
-    return FPNGB_OK;
-}
-
-// scale and bias of the channels in use (index < chans): FPNGB_ERR_INVALID_ARG for an entry that is not finite
-static int typed_affine(const fpngb_pixel_format* fmt, uint32_t chans, ConvertParams& cp)
-{
-    for (uint32_t c = 0; c < chans && c < 4; c++) {
-        if (!isfinite(fmt->scale[c]) || !isfinite(fmt->bias[c])) return FPNGB_ERR_INVALID_ARG;
-        cp.scale[c] = fmt->scale[c]; cp.bias[c] = fmt->bias[c];
-    }
-    return FPNGB_OK;
-}
-
-// The byte layout L of a typed input: FPNGB_ERR_ALIGNMENT unless the base and every stride are multiples of es; divided by es, the
-// strides must form an interleaved or planar layout of "Pixel layouts" (size-1 dimensions canonicalised) whose last element lies
-// inside the address space, else FPNGB_ERR_INVALID_ARG.  No row-pitch limit: the conversion pre-pass addresses with 64 bits.
-static int typed_layout(const void* base, uint64_t image, uint64_t row, uint64_t pixel, uint64_t chan, uint32_t n, uint32_t h, uint32_t w,
-                        uint32_t chans, size_t es, Layout& L)
-{
-    if ((uintptr_t)base % es || image % es || row % es || pixel % es || chan % es) return FPNGB_ERR_ALIGNMENT;
-    Layout E;
-    if (!classify_layout(image / es, row / es, pixel / es, chan / es, n, h, w, chans, E)) return FPNGB_ERR_INVALID_ARG;
-    const uint64_t lim = UINT64_MAX / es;
-    if (E.image > lim || E.row > lim || E.pixel > lim || E.chan > lim) return FPNGB_ERR_INVALID_ARG;
-    L = Layout{E.image * es, E.row * es, E.pixel * es, E.chan * es, E.planar};
-    uint64_t last = 0;
-    if (!layout_span(base, L, n, h, w, chans, last) || last > UINT64_MAX - (uint64_t)(uintptr_t)base - (es - 1)) return FPNGB_ERR_INVALID_ARG;
-    return FPNGB_OK;
-}
-
-// Body of fpngb_encode_ragged_device (fmt NULL) and fpngb_encode_ragged_device_typed (typed: fmt required).
+// Body of fpngb_encode_ragged_device (typed false, fmt unused) and fpngb_encode_ragged_device_typed (fmt required).
 static int encode_ragged_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
                               const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
                               uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    size_t es = 1;
-    if (typed) { const int rc = typed_dtype(fmt, es); if (rc) return rc; }
     if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
-    // every image on its own: the layout rules of the strided batch call for a batch of one
+    PixelFormat f = uint8_format();
+    if (typed) {                                        // scale and bias are in use up to the largest channel count
+        uint32_t max_chans = 0;
+        for (uint32_t i = 0; i < n; i++) max_chans = std::max(max_chans, dims[3 * i + 2]);
+        const int rc = parse_format(fmt, max_chans, f);
+        if (rc) return rc;
+    }
+    // every image on its own: the layout rules of the batch call for a batch of one
     std::vector<RaggedImage> im(n);
-    std::vector<Layout> src(typed ? n : 0);
+    std::vector<Layout> src(n);
     uint64_t total = 0;
-    uint32_t max_chans = 0;
     for (uint32_t i = 0; i < n; i++) {
         const uint32_t w = dims[3 * i], h = dims[3 * i + 1], chans = dims[3 * i + 2];
         if (!pixels[i] || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
+        const uint64_t es = f.elem;
         const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans * es, pixel = strides ? strides[3 * i + 1] : chans * es;
         const uint64_t chan = strides ? strides[3 * i + 2] : es;
-        Layout L;
-        if (typed) {
-            const int rc = typed_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, chan, 1, h, w, chans, es, L);
-            if (rc) return rc;
-            src[i] = L;
-        } else {
-            uint64_t last = 0;
-            if (!classify_layout(0, row, pixel, chan, 1, h, w, chans, L) || L.row > 0xFFFFFFFFull ||
-                !layout_span((const void*)(uintptr_t)pixels[i], L, 1, h, w, chans, last))
-                return FPNGB_ERR_INVALID_ARG;
-        }
+        Layout& L = src[i];
+        const int rc = check_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, chan, 1, h, w, chans, f.elem, false, L);
+        if (rc) return rc;
+        if (!typed && L.row > 0xFFFFFFFFull) return FPNGB_ERR_INVALID_ARG;  // the uint8 kernels take a 32-bit row pitch
         im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
         total += align_up(max_encoded_size(w, h, chans), 16);
-        max_chans = std::max(max_chans, chans);
     }
-    ConvertParams cp{};
-    if (typed) { const int rc = typed_affine(fmt, max_chans, cp); if (rc) return rc; }
     if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
     if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
     Context& c = g_ctx;
@@ -811,7 +773,7 @@ static int encode_ragged_impl(uint32_t n, const uint64_t* pixels, const uint32_t
     const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
     const size_t conv_stage = align_up(ofs_bytes + align_up((size_t)n * sizeof(ImageDesc), 16) + (size_t)n * 5 * 4, 16);
     StageSlot* sl = nullptr;
-    int rc = ragged_stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
+    int rc = c.stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
     if (rc) return rc;
     uint8_t* stage = (uint8_t*)sl->buf.p;
 
@@ -827,20 +789,17 @@ static int encode_ragged_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         uint8_t* cb = (uint8_t*)c.conv.p;
         ConvDesc* hd = (ConvDesc*)(stage + conv_stage);
         unsigned long long ctas = 0;
-        uint32_t planar = 0;
         for (uint32_t i = 0; i < n; i++) {
             RaggedImage& r = im[i];
-            const uint32_t per = convert_ctas_per_image(r.w, r.h);
-            hd[i] = ConvDesc{r.pixels, 0, src[i].row, src[i].chan, at[i], ctas, 1, r.w, r.h, r.chans, per, src[i].planar ? 1u : 0u};
-            ctas += per;
-            planar += hd[i].planar;
+            hd[i] = conv_desc(r.pixels, src[i], 1, r.w, r.h, r.chans, at[i], ctas);
+            ctas += hd[i].ctas_per_image;
             r.pixels = cb + at[i]; r.row = (uint64_t)r.w * r.chans; r.chan = 0;
+            src[i] = tight_layout(r.w, r.chans, r.h * r.row);
         }
         rc = c.ws_acquire(s);
         if (rc) return rc;
         FPNGB_CUDA_OK(cudaMemcpyAsync(cb + desc_at, hd, (size_t)n * sizeof(ConvDesc), cudaMemcpyHostToDevice, s));
-        cp.one = hd[0]; cp.desc = (const ConvDesc*)(cb + desc_at); cp.count = n; cp.total_ctas = ctas; cp.dst = cb;
-        convert_enqueue(cp, fmt->dtype, planar == 0 ? kConvInterleaved : planar == n ? kConvPlanar : kConvAny, s);
+        convert_enqueue(hd, n, (const ConvDesc*)(cb + desc_at), f, cb, s);
     }
 
     // images the 16-pixel kernels do not take (RGBA 1-pass under a table whose one-pixel-match rule is live, or FPNGB_FORCE_GENERIC)
@@ -853,8 +812,7 @@ static int encode_ragged_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         const RaggedImage& r = im[i];
         if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
             const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
-            rc = encode_batch_locked(c, r.pixels, (size_t)r.h * r.row, (uint32_t)r.row, r.chan, 1, r.w, r.h, r.chans, flags,
-                                     out + r.slot, slot, d_sizes + i, s);
+            rc = encode_batch_locked(c, r.pixels, src[i], uint8_format(), 1, r.w, r.h, r.chans, flags, out + r.slot, slot, d_sizes + i, s);
             if (rc) { prof_drop_conv(); cudaEventRecord(sl->ev, s); return rc; }
         } else ids.push_back(i);
     }
@@ -885,42 +843,6 @@ int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const u
     return encode_ragged_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
 }
 
-int fpngb_encode_batch_device_typed(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride, size_t chan_stride,
-                                    uint32_t n, uint32_t w, uint32_t h, uint32_t chans, const fpngb_pixel_format* fmt, uint32_t flags,
-                                    void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream)
-{
-    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    size_t es = 0;
-    int rc = typed_dtype(fmt, es);
-    if (rc) return rc;
-    if (!d_pixels || !d_out || !d_sizes || n == 0 || n > 65535 || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
-    ConvertParams cp{};
-    rc = typed_affine(fmt, chans, cp);
-    if (rc) return rc;
-    Layout L;
-    rc = typed_layout(d_pixels, image_stride, row_pitch, pixel_stride, chan_stride, n, h, w, chans, es, L);
-    if (rc) return rc;
-    if (out_stride < max_encoded_size(w, h, chans)) return FPNGB_ERR_BUFFER_TOO_SMALL;
-    if (out_stride % 16 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
-    Context& c = g_ctx;
-    std::lock_guard<std::mutex> lk(c.mu);
-    FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    cudaStream_t s = (cudaStream_t)stream;
-    const size_t image_bytes = (size_t)w * h * chans;
-    rc = c.conv.reserve((size_t)n * image_bytes);
-    if (rc) return rc;
-    rc = c.ws_acquire(s);
-    if (rc) return rc;
-    const uint32_t ctas = convert_ctas_per_image(w, h);
-    cp.one = ConvDesc{(const uint8_t*)d_pixels, L.image, L.row, L.chan, 0, 0, n, w, h, chans, ctas, L.planar ? 1u : 0u};
-    cp.count = 1; cp.total_ctas = (unsigned long long)n * ctas; cp.dst = (uint8_t*)c.conv.p;
-    convert_enqueue(cp, fmt->dtype, L.planar ? kConvPlanar : kConvInterleaved, s);
-    rc = encode_batch_locked(c, (const uint8_t*)c.conv.p, image_bytes, w * chans, 0, n, w, h, chans, flags, (uint8_t*)d_out, out_stride,
-                             d_sizes, s);
-    prof_drop_conv();
-    return rc;
-}
-
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)
 {
     if (out_size) *out_size = 0;
@@ -937,7 +859,8 @@ int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans
     uint32_t* d_size = (uint32_t*)((uint8_t*)c.dev_out.p + stride);
     cudaStream_t s = c.stream;
     FPNGB_CUDA_OK(cudaMemcpyAsync(c.dev_in.p, pixels, in_bytes, cudaMemcpyHostToDevice, s));
-    rc = encode_batch_locked(c, (const uint8_t*)c.dev_in.p, in_bytes, w * chans, 0, 1, w, h, chans, flags, (uint8_t*)c.dev_out.p, stride, d_size, s);
+    rc = encode_batch_locked(c, (const uint8_t*)c.dev_in.p, tight_layout(w, chans, in_bytes), uint8_format(), 1, w, h, chans, flags,
+                             (uint8_t*)c.dev_out.p, stride, d_size, s);
     if (rc) return rc;
     uint32_t* h_size = (uint32_t*)c.pin_small.p;
     FPNGB_CUDA_OK(cudaMemcpyAsync(h_size, d_size, 4, cudaMemcpyDeviceToHost, s));
@@ -1009,7 +932,7 @@ int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
         if (e != cudaSuccess) { result = 1000 + (int)e; break; }
         cudaEventRecord(ev_in[sl], c.copy_in);
         cudaStreamWaitEvent(c.stream, ev_in[sl], 0);
-        rc = encode_batch_locked(c, din, in_bytes, w * chans, 0, cnt, w, h, chans, flags, dout, dstride, dsz, c.stream);
+        rc = encode_batch_locked(c, din, tight_layout(w, chans, in_bytes), uint8_format(), cnt, w, h, chans, flags, dout, dstride, dsz, c.stream);
         if (rc) { result = rc; break; }
         cudaEventRecord(ev_done[sl], c.stream);
         cudaStreamWaitEvent(c.copy_out, ev_done[sl], 0);

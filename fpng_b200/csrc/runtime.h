@@ -1,7 +1,10 @@
 // fpng_b200/csrc/runtime.h -- host runtime state shared by host_api.cu and decode_api.cu.
 #pragma once
+#include "../../include/fpng_b200.h"
 #include "common.cuh"
 #include <mutex>
+#include <new>
+#include <vector>
 
 namespace fpngb {
 
@@ -17,6 +20,10 @@ struct Buffer {
         return 0;
     }
 };
+
+// One pinned buffer of the staging ring for host-built tables that a call uploads (descriptor tables, offsets).  The caller
+// records ev on the stream after the copies that read buf.
+struct StageSlot { Buffer buf; cudaEvent_t ev = nullptr; };
 
 struct Context {
     int device = -1;
@@ -49,6 +56,25 @@ struct Context {
     {
         FPNGB_CUDA_OK(cudaEventRecord(ws_done, s));
         ws_stream = s; ws_busy = true;
+        return 0;
+    }
+    // A staging slot of at least `bytes`: one whose last copy has completed (cudaEventQuery), else a new one, so that a call never
+    // waits on the host for an earlier call's upload.  Slots live as long as the process.
+    std::vector<StageSlot*> stage;
+    int stage_slot(size_t bytes, StageSlot** out)
+    {
+        StageSlot* sl = nullptr;
+        for (StageSlot* x : stage) if (x->buf.cap >= bytes && cudaEventQuery(x->ev) == cudaSuccess) { sl = x; break; }
+        if (!sl) {
+            sl = new (std::nothrow) StageSlot();
+            if (!sl) return FPNGB_ERR_INTERNAL;
+            sl->buf.pinned = true;
+            FPNGB_CUDA_OK(cudaEventCreateWithFlags(&sl->ev, cudaEventDisableTiming));
+            stage.push_back(sl);
+        }
+        const int rc = sl->buf.reserve(bytes);
+        if (rc) return rc;
+        *out = sl;
         return 0;
     }
 };
