@@ -17,4 +17,5 @@ from .api import (  # noqa: F401
     encode_ragged_device, ragged_slot_offsets, compact_packed_device,
     FPNGB_DECODE_ADLER_MISMATCH, set_decode_verify, decode_verify,
     normalize_scale_bias, denormalize_scale_bias, typed_layout,
+    FPNGB_DECODE_BAD_CROP, FPNGB_RESIZE_ANTIALIAS, decode_packed_resized_device,
 )

@@ -626,6 +626,62 @@ def ragged_views(out, out_offsets, info, status, desired_channels: int):
     return views
 
 
+FPNGB_DECODE_BAD_CROP = 103        # decode_packed_resized_device only: the file's crop box is empty or not inside the image
+FPNGB_RESIZE_ANTIALIAS = 1
+
+
+def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: int, boxes=None, antialias=True, out=None, dtype=None,
+                                 scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None):
+    """Decode fpng files of ANY shapes packed in device memory (the layout of decode_packed_ragged_device) into one batch of a fixed
+    size = (H, W): file i is cropped to boxes[i] and resized with F.interpolate's bilinear rule (align_corners=False, antialias as
+    given) on the GPU, then stored as decode_batch_device stores its pixels (uint8, rounded half to even and clamped, or dtype with
+    scale and bias).  Returns (out [n, H, W, desired_channels], info int32 [n, 6], status int32 [n]).
+      * boxes: None (whole images) or an int32 CUDA tensor [n, 4] of (top, left, height, width), torchvision's resized_crop order;
+      * out: any non-overlapping [n, H, W, C] view in one of the layouts of layout_strides, e.g. torch.empty(n, C, H, W,
+        dtype=torch.bfloat16).permute(0, 2, 3, 1) for NCHW; by default a contiguous [n, H, W, C] tensor;
+      * status[i] is decode_packed_ragged_device's code, or FPNGB_DECODE_BAD_CROP for a box that is empty or not inside the image;
+        the output slice of a file whose status is not 0 is left untouched;
+      * pixel_cap bounds the bytes of uint8 pixels the call decodes before resizing (align_up(w*h*desired_channels, 16) per file),
+        as out's size does in decode_packed_ragged_device: files past it get FPNGB_DECODE_OUT_OF_SPACE.
+    With max_file_size, max_w, max_h and pixel_cap all given, the call is stream-ordered: no host synchronisation.  Any of them
+    that is None is computed by decode_packed_ragged_device's rule: one get_info_batch_device and one read-back to the host, which
+    waits for the stream; pixel_cap then becomes the exact size of the decodable files."""
+    import torch
+
+    if desired_channels not in (3, 4):
+        raise ValueError(f"decode_packed_resized_device: desired_channels {desired_channels}: 3 or 4")
+    H, W = (int(v) for v in size)
+    if not (1 <= H <= 1 << 24 and 1 <= W <= 1 << 24):
+        raise ValueError(f"decode_packed_resized_device: size {tuple(size)}: each side in 1 .. 2^24")
+    odt = _out_dtype(out, dtype)
+    fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
+    if boxes is not None:
+        if not isinstance(boxes, torch.Tensor) or not boxes.is_cuda or boxes.device != data.device:
+            raise ValueError(f"boxes: a CUDA tensor on {data.device} is needed")
+        n = sizes.shape[0]
+        if boxes.dtype != torch.int32 or tuple(boxes.shape) != (n, 4) or not boxes.is_contiguous():
+            raise ValueError(f"boxes: dtype {boxes.dtype}, shape {tuple(boxes.shape)}: a contiguous int32 [{n}, 4] tensor is needed")
+    n = _packed_args(data, offsets, sizes)
+    shape = (n, H, W, desired_channels)
+    if out is None:
+        out = torch.empty(shape, dtype=odt, device=data.device)
+    _check_arg(out, "out", data.device, odt, n * H * W * desired_channels, view=True)
+    if max_file_size is None or max_w is None or max_h is None or pixel_cap is None:
+        max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
+                                                             stream)
+        if pixel_cap is None:
+            pixel_cap = total
+    info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
+    status = torch.empty((n,), dtype=torch.int32, device=data.device)
+    rc = lib().fpngb_decode_packed_resized_device(
+        data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
+        int(max_h), int(pixel_cap), None if boxes is None else boxes.data_ptr(), W, H, desired_channels,
+        FPNGB_RESIZE_ANTIALIAS if antialias else 0, None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape),
+        info.data_ptr(), status.data_ptr(), _stream(stream, data.device))
+    check(rc, "decode_packed_resized_device")
+    return out, info, status
+
+
 def decode_batch_host(file_ptrs, sizes, desired_channels: int, out, out_stride: int):
     """Pipelined host-buffer batch decode (fpngb_decode_batch_host).  file_ptrs: array of host addresses (uint64), sizes:
     uint32 array, out: host buffer (numpy uint8 / pinned torch tensor) with out_stride bytes per image.

@@ -54,6 +54,11 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
         if (!pre && ragged) {
             if (w > p.w || h > p.h) pre = FPNGB_DECODE_SHAPE_MISMATCH;
             else if ((unsigned long long)w * h * p.desired > 0xFFFFFFFFull) pre = FPNGB_DECODE_FAILED_DIMENSIONS_TOO_LARGE;   // fpng.cpp:3103-3105
+            else if (p.boxes) {                                                     // the resized call's crop box
+                const int32_t* b = p.boxes + (size_t)i * 4;
+                const long long top = b[0], left = b[1], bh = b[2], bw = b[3];
+                if (bh < 1 || bw < 1 || top < 0 || left < 0 || top + bh > h || left + bw > w) pre = FPNGB_DECODE_BAD_CROP;
+            }
         } else if (!pre && (w != p.w || h != p.h || c != p.chans)) pre = FPNGB_DECODE_SHAPE_MISMATCH;
         FileDesc fd;
         fd.base = ofs; fd.file_size = size; fd.idat_ofs = pre ? 0u : io; fd.idat_len = pre ? 0u : il; fd.pre_status = pre;

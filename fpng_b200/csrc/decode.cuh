@@ -109,7 +109,8 @@ bool decode_set_pre_roll(uint32_t bits);    // DecodeParams::pre_roll of later c
 //   uniform call (chans != 0): FPNGB_DECODE_SHAPE_MISMATCH when a valid file is not w x h x chans; the workspace bases are
 //     i * (h * delta_pitch(w, chans)), i * out_stride and i * subs_for(max_file_size);
 //   ragged call (chans == 0): the walk runs only when the argument checks pass; FPNGB_DECODE_SHAPE_MISMATCH when the file is
-//     wider than w or taller than h, FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE when w * h * desired > 0xFFFFFFFF; the bases are
+//     wider than w or taller than h, FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE when w * h * desired > 0xFFFFFFFF, then, for the
+//     resized call (boxes != nullptr), FPNGB_DECODE_BAD_CROP when the file's box is empty or not inside the image; the bases are
 //     set by decode_place_kernel.
 struct WalkParams {
     const uint8_t* base; const unsigned long long* offsets; const uint32_t* sizes; uint32_t n;
@@ -119,6 +120,7 @@ struct WalkParams {
     uint32_t desired;                       // ragged call: output channels
     unsigned long long base_bytes;          // ragged call: length of the buffer behind base
     unsigned long long out_stride;          // uniform call: output bytes per file
+    const int32_t* boxes;                   // resized call: [n][4] {top, left, height, width}, or nullptr (whole images)
 };
 void launch_container_walk(const WalkParams& p, cudaStream_t s);
 
@@ -133,5 +135,22 @@ struct PlaceParams {
     unsigned long long* out_offsets;        // [n + 1]
 };
 void launch_decode_place(const PlaceParams& p, cudaStream_t s);
+
+// decode_resize_kernel (decode_resize_kernels.cu), resized call: after the ragged pipeline has decoded every file into tight uint8
+// HWC rows (pitch w * desired) at px + px_offsets[f], crops file f to its box and resizes it to out_h x out_w with the bilinear
+// rule of fpngb_decode_packed_resized_device, then stores T(r * scale[c] + bias[c]) (float types) or round_u8(r) (dtype 0).
+// Files whose d_status is not 0 are skipped.  Output strides in bytes: element (f, y, x, c) at d_out + f*image + y*row + x*pixel
+// + c*chan, interleaved (pixel = desired * sizeof(T)) or planar (pixel = sizeof(T)).
+struct ResizeParams {
+    const uint8_t* px; const unsigned long long* px_offsets;   // the ragged decode's pixels and their placement
+    const FileDesc* files; const int32_t* d_status;
+    const int32_t* boxes;                   // [n][4] {top, left, height, width}, or nullptr (whole images)
+    uint8_t* d_out;
+    unsigned long long image, row, pixel, chan;
+    uint32_t out_w, out_h, antialias;
+};
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t n, uint32_t desired, cudaStream_t s);
+// profiling (fpngb_decode_profile_read): the end of the kernel enqueued right behind launch_decode, reported in slot 8
+void decode_profile_mark_resize(cudaStream_t s);
 
 }  // namespace fpngb

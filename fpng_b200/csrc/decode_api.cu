@@ -18,8 +18,10 @@ static std::atomic<int> g_decode_verify{0};
 
 // Reserves the workspace of a decode call for n files, n_subs SubInfo records and delta_bytes of delta rows in all, orders it
 // after the previous call's kernels, and points p's workspace fields into it (p.files included).  With verification on
-// (fpngb_set_decode_verify), *verify points to n VerifyState records behind the rest; else it is nullptr.  Caller holds context().mu.
-static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes, cudaStream_t s, DecodeParams& p, VerifyState** verify)
+// (fpngb_set_decode_verify), *verify points to n VerifyState records behind the rest; else it is nullptr.  extra_bytes more (the
+// resized call's uint8 pixels and their offsets) go last, at *extra (256-byte aligned).  Caller holds context().mu.
+static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes, cudaStream_t s, DecodeParams& p, VerifyState** verify,
+                                   size_t extra_bytes = 0, uint8_t** extra = nullptr)
 {
     size_t o = 0;
     const size_t o_files = o; o = align_up(o + (size_t)n * sizeof(FileDesc), 256);
@@ -30,6 +32,7 @@ static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes
     const size_t o_delta = o; o = align_up(o + delta_bytes + 64, 256);
     const bool verifying = g_decode_verify.load() != 0;
     const size_t o_verify = o; if (verifying) o = align_up(o + (size_t)n * sizeof(VerifyState), 256);
+    const size_t o_extra = o; o += extra_bytes;
     int rc = g_dec_ws.reserve(o); if (rc) return rc;
     rc = context().ws_acquire(s); if (rc) return rc;
     uint8_t* b = (uint8_t*)g_dec_ws.p;
@@ -37,6 +40,7 @@ static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes
     p.luts = (uint32_t*)(b + o_luts); p.fast = (uint32_t*)(b + o_fast); p.subs = (SubInfo*)(b + o_subs);
     p.delta = b + o_delta;
     *verify = verifying ? (VerifyState*)(b + o_verify) : nullptr;
+    if (extra) *extra = b + o_extra;
     return 0;
 }
 // The same for n files of one shape whose IDAT chunks are at most max_idat bytes: file i's records and delta rows at i times the
@@ -210,35 +214,47 @@ static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_si
     delta_cap = sat_u64(by_out < by_shape ? by_out : by_shape);
 }
 
+// The resize step of fpngb_decode_packed_resized_device: its checked output and arguments.
+struct ResizeOut {
+    const int32_t* boxes; uint32_t out_w, out_h, flags;
+    uint8_t* d_out; Layout out; TypedOut t;
+};
+
+// The ragged pipeline: walk, place, decode.  With rz (the resized call), the uint8 pixels and their offsets go to the decode
+// workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes, and the
+// resize kernel runs behind the decode, before the workspace is released.
 static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
-                                     int32_t* d_status, void* stream)
+                                     int32_t* d_status, void* stream, const ResizeOut* rz = nullptr)
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (!d_base || !d_offsets || !d_sizes || !d_out || !d_out_offsets || !d_status || n == 0 || n > 65535 || !max_file_size ||
+    if (!d_base || !d_offsets || !d_sizes || (!rz && (!d_out || !d_out_offsets)) || !d_status || n == 0 || n > 65535 || !max_file_size ||
         (desired_chans != 3 && desired_chans != 4) || !max_w || !max_h || max_w > (1u << 24) || max_h > (1u << 24))
         return FPNGB_ERR_INVALID_ARG;
     TypedOut t;
     uint32_t elem;
     int rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
-    if ((uintptr_t)d_base % 4 || (uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    if ((uintptr_t)d_base % 4 || (!rz && (uintptr_t)d_out % 16)) return FPNGB_ERR_ALIGNMENT;
     unsigned long long sub_cap = 0, delta_cap = 0;
     // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
     ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, sub_cap, delta_cap);
-    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2 || (rz && out_cap > SIZE_MAX / 2)) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    const size_t offsets_bytes = align_up(((size_t)n + 1) * sizeof(uint64_t), 256);
     const cudaStream_t s = (cudaStream_t)stream;
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     DecodeParams p{};
     VerifyState* verify = nullptr;
-    rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify); if (rc) return rc;
+    uint8_t* extra = nullptr;
+    rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify, rz ? offsets_bytes + out_cap : 0, &extra); if (rc) return rc;
+    if (rz) { d_out_offsets = (uint64_t*)extra; d_out = extra + offsets_bytes; }
     p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
-    wp.base_bytes = base_bytes;
+    wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr;
     launch_container_walk(wp, s);
     PlaceParams pp{};
     pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem;
@@ -246,7 +262,16 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     launch_decode_place(pp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
     launch_decode(p, OutStrides{0, desired_chans * elem, elem}, n, desired_chans, s, verify, max_file_size, typed ? &t : nullptr);
-    count_launch(verify ? 13 : 11);
+    if (rz) {
+        ResizeParams rp{};
+        rp.px = (const uint8_t*)d_out; rp.px_offsets = (const unsigned long long*)d_out_offsets; rp.files = p.files; rp.d_status = d_status;
+        rp.boxes = rz->boxes; rp.d_out = rz->d_out;
+        rp.image = rz->out.image; rp.row = rz->out.row; rp.pixel = rz->out.pixel; rp.chan = rz->out.chan;
+        rp.out_w = rz->out_w; rp.out_h = rz->out_h; rp.antialias = rz->flags & FPNGB_RESIZE_ANTIALIAS;
+        launch_decode_resize(rp, rz->t, n, desired_chans, s);
+        decode_profile_mark_resize(s);
+    }
+    count_launch((verify ? 13 : 11) + (rz ? 1 : 0));
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
 }
@@ -505,6 +530,27 @@ int fpngb_decode_packed_ragged_device_typed(const void* d_base, size_t base_byte
 {
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
                                      d_out_offsets, d_info, true, fmt, d_status, stream);
+}
+
+int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                       uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap, const int32_t* d_boxes,
+                                       uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags, const fpngb_pixel_format* fmt,
+                                       void* d_out, size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride,
+                                       size_t out_chan_stride, uint32_t* d_info, int32_t* d_status, void* stream)
+{
+    if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_out || n == 0 || n > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
+        (desired_chans != 3 && desired_chans != 4) || (flags & ~(uint32_t)FPNGB_RESIZE_ANTIALIAS))
+        return FPNGB_ERR_INVALID_ARG;
+    ResizeOut rz{};
+    rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
+    uint32_t elem;
+    int rc = decode_format(fmt != nullptr, fmt, desired_chans, rz.t, elem); if (rc) return rc;
+    rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, out_h, out_w, desired_chans, elem, true,
+                      rz.out);
+    if (rc) return rc;
+    return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
+                                     nullptr, d_info, false, nullptr, d_status, stream, &rz);
 }
 
 }  // extern "C"

@@ -5,16 +5,10 @@
 // +-inf, as torch's .to()).  Its own translation unit, so that the uint8 decode kernels compile exactly as they did.
 #include "decode.cuh"
 #include "unfilter.cuh"
+#include "typed_store.cuh"
 #include "../../include/fpng_b200.h"
-#include <cuda_bf16.h>
-#include <cuda_fp16.h>
 
 namespace fpngb {
-
-template <typename T> __device__ __forceinline__ uint32_t typed_bits(float v);
-template <> __device__ __forceinline__ uint32_t typed_bits<float>(float v) { return __float_as_uint(v); }
-template <> __device__ __forceinline__ uint32_t typed_bits<__half>(float v) { return __half_as_ushort(__float2half_rn(v)); }
-template <> __device__ __forceinline__ uint32_t typed_bits<__nv_bfloat16>(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
 
 // byte k of the interleaved pixel bytes o[] (k = pixel * DST + channel), mapped to channel c and converted
 template <typename T, int DST>
@@ -22,43 +16,6 @@ __device__ __forceinline__ uint32_t typed_value(const uint32_t (&o)[DST], int k,
 {
     const float v = __uint2float_rn((o[k >> 2] >> (8 * (k & 3))) & 0xFFu);
     return typed_bits<T>(__fadd_rn(__fmul_rn(v, pa.scale[c]), pa.bias[c]));
-}
-
-__device__ __forceinline__ void store_elem(uint8_t* a, uint32_t bits, int size)
-{
-    if (size == 4) *reinterpret_cast<uint32_t*>(a) = bits;
-    else *reinterpret_cast<uint16_t*>(a) = (uint16_t)bits;
-}
-
-// NE contiguous elements of T (bit patterns e[]) at a, which is sizeof(T)-aligned: the widest stores the address allows, 16, then 8,
-// then 4 bytes, else 2-byte elements.  NE * sizeof(T) is a multiple of 8 for every group shape here (4 pixels x 3 or 4 channels
-// interleaved, 4 values of one plane).
-template <typename T, int NE>
-__device__ __forceinline__ void store_elems(uint8_t* a, const uint32_t (&e)[NE])
-{
-    constexpr int ES = sizeof(T), NW = NE * ES / 4;
-    static_assert(NE * ES % 8 == 0, "whole 8-byte units");
-    uint32_t wd[NW];
-#pragma unroll
-    for (int k = 0; k < NW; k++) {
-        if constexpr (ES == 4) wd[k] = e[k];
-        else wd[k] = e[2 * k] | (e[2 * k + 1] << 16);
-    }
-    const uint32_t mis = (uint32_t)((uintptr_t)a & 15u);
-    if (mis == 0u) {
-#pragma unroll
-        for (int k = 0; k + 4 <= NW; k += 4) *reinterpret_cast<uint4*>(a + 4 * k) = make_uint4(wd[k], wd[k + 1], wd[k + 2], wd[k + 3]);
-        if (NW % 4) *reinterpret_cast<uint2*>(a + 4 * (NW - 2)) = make_uint2(wd[NW - 2], wd[NW - 1]);
-    } else if ((mis & 7u) == 0u) {
-#pragma unroll
-        for (int k = 0; k < NW; k += 2) *reinterpret_cast<uint2*>(a + 4 * k) = make_uint2(wd[k], wd[k + 1]);
-    } else if ((mis & 3u) == 0u) {
-#pragma unroll
-        for (int k = 0; k < NW; k++) *reinterpret_cast<uint32_t*>(a + 4 * k) = wd[k];
-    } else {
-#pragma unroll
-        for (int k = 0; k < NE; k++) store_elem(a + ES * k, e[k], ES);
-    }
 }
 
 // OutStrides in bytes: interleaved rows (pixel = DST * sizeof(T)) at any pitch, or planar (pixel = sizeof(T)); row 0: tight rows.

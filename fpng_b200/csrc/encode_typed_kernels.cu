@@ -13,6 +13,7 @@
 // elements at row ends).  The CTAs of a launch cover one or more descriptors; a CTA finds its descriptor by a binary search over
 // their CTA prefix, as ragged_locate does.  All input addressing is 64-bit.
 #include "kernels.cuh"
+#include "typed_store.cuh"
 #include "../../include/fpng_b200.h"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -33,10 +34,7 @@ __device__ __forceinline__ uint32_t quantize(uint32_t bits, float scale, float b
     if constexpr (sizeof(T) == 1) {
         return bits;
     } else {
-        const float y = __fadd_rn(__fmul_rn(elem_to_float<T>(bits), scale), bias);
-        unsigned short q;
-        asm("cvt.rni.sat.u8.f32 %0, %1;" : "=h"(q) : "f"(y));
-        return q;
+        return round_u8(__fadd_rn(__fmul_rn(elem_to_float<T>(bits), scale), bias));
     }
 }
 

@@ -375,6 +375,51 @@ FPNGB_API int fpngb_decode_packed_ragged_device_typed(const void* d_base, size_t
                                                       uint64_t* d_out_offsets /* n+1 */, uint32_t* d_info /* n*6 or NULL */,
                                                       const fpngb_pixel_format* fmt, int32_t* d_status, void* stream);
 
+/* ---- resized decode: packed files of any shapes into one fixed-size batch, with a per-file crop box ---------------------------
+ * fpngb_decode_packed_resized_device decodes the packed files of fpngb_decode_packed_ragged_device, crops file i to its box
+ *   d_boxes[i*4 + 0..3] = {top, left, height, width} (device int32; d_boxes NULL: the whole image), resizes the crop to
+ *   out_h x out_w with torch's bilinear rule (F.interpolate(mode="bilinear", align_corners=False, antialias=...)) and stores
+ *   the batch [n, out_h, out_w, desired_chans]: element (i, y, x, c) at d_out + i*out_image_stride + y*out_row_pitch +
+ *   x*out_pixel_stride + c*out_chan_stride, any non-overlapping interleaved or planar layout of "Pixel layouts" (NCHW included).
+ * The resize rule, per axis, for a crop length `in`, an output length `out` and output index i; all fp32, as torch's CUDA kernel
+ *   (ATen/native/cuda/UpSample.cuh, upsample_antialias::_compute_weights_span / _compute_weights, bilinear filter):
+ *     scale   = (float)in / (float)out
+ *     aa      = (flags & FPNGB_RESIZE_ANTIALIAS) && scale >= 1
+ *     support = aa ? scale : 1;   invscale = aa ? 1 / scale : 1
+ *     center  = scale * (i + 0.5f)
+ *     xmin    = max((int)(center - support + 0.5f), 0)          (truncation, as torch)
+ *     xsize   = min((int)(center + support + 0.5f), in) - xmin
+ *     w_j     = tri((j + xmin - center + 0.5f) * invscale), j < xsize, tri(t) = max(0, 1 - |t|); then w_j /= sum(w) if the sum != 0
+ *   With support 1 these are exactly the taps and weights of F.interpolate(mode="bilinear", align_corners=False, antialias=False),
+ *   edges included.  The resampled value is r = sum_y wy * sum_x wx * p(top + ymin + y, left + xmin + x, c) in fp32, in any
+ *   order, where p is the uint8 value fpngb_decode_packed_ragged_device writes (alpha 255 when a 3-channel file is decoded to 4).
+ *   Stored: T(__fadd_rn(__fmul_rn(r, scale[c]), bias[c])) for a float fmt (the rule of the *_typed decodes), or, with fmt NULL,
+ *   the uint8 cvt.rni.sat.u8.f32(r) (round half to even, clamp to [0, 255]: the typed encode's quantiser).
+ * Input: the arguments, bounds (max_file_size, max_w, max_h) and per-file rules of fpngb_decode_packed_ragged_device, and the
+ *   verify switch.  pixel_cap bounds the bytes of decoded uint8 pixels the call holds, the sum of align_up(w*h*desired_chans, 16)
+ *   over the files it decodes (the ragged call's out_cap; the library keeps these pixels in its own grow-only workspace).
+ * Per-file statuses in d_status, in this order, each only when the earlier ones passed: the ragged call's argument checks; the
+ *   walk (d_info as in the ragged call); FPNGB_DECODE_SHAPE_MISMATCH, then FPNGB_DECODE_FAILED_DIMENSIONS_TOO_LARGE;
+ *   FPNGB_DECODE_BAD_CROP when height or width < 1, top or left < 0, top + height > h or left + width > w (such a file takes
+ *   no space and is not decoded); FPNGB_DECODE_OUT_OF_SPACE for a placed file past pixel_cap (the files that fit are a prefix of
+ *   the placed ones); the decode (with verify on: 4, then FPNG_DECODE_NOT_FPNG, then 102).  The output slice of a file whose
+ *   status is not 0 is left untouched.
+ * Call-level checks (a rejected call enqueues nothing and writes nothing): FPNGB_ERR_INVALID_ARG for n == 0 or n > 65535, a NULL
+ *   d_base / d_offsets / d_sizes / d_out / d_status, max_file_size == 0, max_w or max_h outside 1..2^24, out_w or out_h outside
+ *   1..2^24, desired_chans other than 3 or 4, unknown flags bits, a bad fmt (as the *_typed calls) or a bad layout;
+ *   FPNGB_ERR_ALIGNMENT unless d_base % 4 == 0 and d_out and every stride are multiples of the element size.
+ * Stream-ordered, no host synchronisation: the ragged pipeline plus one resize kernel, 12 launches (14 with verify on);
+ *   fpngb_decode_profile_read reports the resize kernel in slot 8 (slots 6 and 7 are 0 with verify off). */
+enum { FPNGB_RESIZE_ANTIALIAS = 1 };
+enum { FPNGB_DECODE_BAD_CROP = 103 };   /* resized decode only: the file's crop box is empty or not inside the image */
+FPNGB_API int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
+                                                 uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap,
+                                                 const int32_t* d_boxes /* n x {top, left, height, width}, device, or NULL = whole image */,
+                                                 uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags,
+                                                 const fpngb_pixel_format* fmt /* NULL = uint8 */,
+                                                 void* d_out, size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride,
+                                                 size_t out_chan_stride, uint32_t* d_info /* n*6 or NULL */, int32_t* d_status, void* stream);
+
 /* ---- typed encode input: float32 / float16 / bfloat16 pixels with a per-channel scale and bias, rounded to 8 bits ------------
  * The *_typed encode calls take the input as elements x of T (fmt->dtype: float32, float16 or bfloat16) and encode, for channel c,
  * the uint8 value
