@@ -7,10 +7,9 @@
 namespace fpngb {
 
 constexpr int kScan16Rows = 8;                   // warps (scanlines) per CTA, scan
-#ifndef FPNGB_PACK_WARPS
-#define FPNGB_PACK_WARPS 7
-#endif
-constexpr int kPack16Rows = FPNGB_PACK_WARPS;    // warps per CTA, pack (larger staging buffers)
+// warps (scanline sequences) per CTA, pack: 8 for RGB, 7 for RGBA.  Shared memory per warp (tiles + staging) sets the CTAs per SM:
+// RGB 4 x 7 or 3 x 8 warps, RGBA 3 x 7 or 2 x 8.  RGB runs faster with 8 (H100 at 700 W, C2: pack 1.54 against 1.64 ms, DESIGN 4.1).
+__host__ __device__ constexpr int pack16_warps(int chans) { return chans == 4 ? 7 : 8; }
 constexpr uint32_t kRowsPerWarp16 = 5;           // consecutive scanlines per warp (pack kernel) on large batches: amortises the CTA prologue and
                                                  // lets a scanline's first tile be prefetched during the previous scanline's last step
 // small jobs (a single image) keep one scanline per warp so that the grid still fills the GPU
@@ -289,38 +288,6 @@ __device__ __forceinline__ void sts_u32(uint32_t saddr, uint32_t v) { asm volati
 __device__ __forceinline__ void reds_or_u32(uint32_t saddr, uint32_t v) { asm volatile("red.shared.or.b32 [%0], %1;\n" :: "r"(saddr), "r"(v)); }
 __device__ __forceinline__ uint32_t lds_u32(uint32_t saddr) { uint32_t v; asm("ld.shared.u32 %0, [%1];\n" : "=r"(v) : "r"(saddr)); return v; }
 
-// FPNGB_PACK_MUL (A/B build, default off): the stager shifts by MULTIPLYING.  The pack kernel is bound by the ALU pipe (LOP3 / SHF /
-// IADD3 / ISETP: ncu 76 % active, math-pipe-throttle the top stall) while the FMA pipe is mostly idle, so with the fill level kept as
-// m = 2^n, "cur | code << n" becomes code * m + cur (IMAD; the operands never overlap, so + is |), the spill IMAD.HI, the new level
-// m * 2^len (its high word is non-zero exactly when the word is complete) and a pair of codes c0 + c1 * 2^l0; the tables then hold
-// 2^size instead of size.  Byte-exact, but measured slower than shift + OR: the wide / high
-// multiplies make the FMA pipe the new limiter.
-#ifndef FPNGB_PACK_MUL
-#define FPNGB_PACK_MUL 0
-#endif
-#if FPNGB_PACK_MUL
-struct BitStager16 {
-    uint32_t cur;               // the word being filled
-    uint32_t m;                 // 2^n, n = valid bits in it (n < 32)
-    uint32_t dst;               // shared-memory address of the staging word it goes to
-    __device__ __forceinline__ void begin(uint32_t stage_saddr, uint32_t bitpos, uint32_t seed)
-    {
-        cur = seed; m = 1u << (bitpos & 31u); dst = stage_saddr + ((bitpos >> 5) << 2);
-    }
-    // append a code of `len` bits given as pw = 2^len (len <= 24, code < pw); pw == 1 (code == 0) is a no-op
-    __device__ __forceinline__ void put_pow(uint32_t code, uint32_t pw)
-    {
-        const uint32_t lo = code * m + cur;                             // cur < m and code * m is a multiple of m: + is |
-        const uint32_t hi = __umulhi(code, m);                          // bits that spill into the next word
-        const uint32_t mlo = m * pw, mhi = __umulhi(m, pw);             // 2^(n + len): the high word is set iff the word is complete
-        if (mhi) { sts_u32(dst, lo); dst += 4u; cur = hi; m = mhi; }    // this lane owns bit 31 of the word: plain store
-        else { cur = lo; m = mlo; }
-    }
-    __device__ __forceinline__ void put(uint32_t code, uint32_t len) { put_pow(code, 1u << len); }
-    // after a warp barrier: the partial last word is shared with the next lane's first word
-    __device__ __forceinline__ void end() { if (cur) reds_or_u32(dst, cur); }
-};
-#else
 struct BitStager16 {
     uint32_t cur, n;            // word being filled (n < 32 valid bits)
     uint32_t dst;               // shared-memory address of the staging word `cur` goes to
@@ -340,7 +307,6 @@ struct BitStager16 {
     // after a warp barrier: the partial last word is shared with the next lane's first word
     __device__ __forceinline__ void end() { if (cur) reds_or_u32(dst, cur); }
 };
-#endif
 
 __device__ __forceinline__ void put_pair16(BitStager16& bs, uint32_t a, uint32_t b)   // two table entries (len << 16 | code), <= 24 bits
 {
@@ -353,89 +319,51 @@ __device__ __forceinline__ void put_match16(BitStager16& bs, uint32_t s_match_sa
     bs.put(m & 0xFFFFFFu, m >> 24);
 }
 
-// FPNGB_PACK_LIT64: the all-literal path fetches (code, size) register pairs with one 64-bit shared load per byte instead of a
-// packed 32-bit entry whose fields have to be shifted / masked apart (2 ALU instructions less per literal; the pack kernel is
-// ALU-pipe bound).  The 8-byte table sits directly below the 4-byte one in shared memory.
-#ifndef FPNGB_PACK_LIT64
-#define FPNGB_PACK_LIT64 1
-#endif
-#if FPNGB_PACK_LIT64
+// Literal codes come as (code, size) register pairs from one 64-bit shared load per byte, instead of a packed 32-bit entry whose
+// fields have to be shifted / masked apart (2 ALU instructions less per literal; the pack kernel is ALU-pipe bound).  The 8-byte
+// table [512][2] sits directly below the 4-byte one in shared memory; its upper half is all zero: a "null" entry of 0 bits, which
+// switches a pixel's literals off without a branch.
 __device__ __forceinline__ uint2 lds_u64(uint32_t saddr) { uint2 v; asm("ld.shared.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "r"(saddr)); return v; }
-// FPNGB_PACK_OFS_FMA: the byte offset of a table entry as "extract the byte (one ALU-pipe instruction), multiply by 8 (IMAD with a
-// constant-bank operand, FMA pipe)" instead of shift + mask (two ALU-pipe instructions); only where no null-half bit is OR-ed in.
-// Measured slightly faster than shift + mask; =0 restores shift + mask.
-#ifndef FPNGB_PACK_OFS_FMA
-#define FPNGB_PACK_OFS_FMA 1
-#endif
 template <int POS>
 __device__ __forceinline__ uint32_t lit_off16x8(uint32_t w, uint32_t nb8)
 {
     const uint32_t x = POS == 0 ? (w << 3) : (POS == 1 ? (w >> 5) : (POS == 2 ? (w >> 13) : (w >> 21)));
     return (x & 0x7F8u) | nb8;
 }
+// the all-literal path's offset: "extract the byte (one ALU-pipe instruction), multiply by 8 (IMAD with a constant-bank operand,
+// FMA pipe)" instead of shift + mask (two ALU-pipe instructions).  Measured on an H100 (700 W) as fast as shift + mask (C2 pack
+// 1.636-1.646 against 1.642 ms); kept for its lower ALU-pipe count.
 template <int POS>
 __device__ __forceinline__ uint32_t lit_off16x8_plain(uint32_t w)
 {
-#if FPNGB_PACK_OFS_FMA
     const uint32_t b = POS == 0 ? (w & 0xFFu) : (POS == 1 ? byte1(w) : (POS == 2 ? byte2(w) : (w >> 24)));
     return b * c_fma_k[5];
-#else
-    return lit_off16x8<POS>(w, 0u);
-#endif
 }
-#endif
 
-// byte offset of the literal-table entry of byte POS of word w, OR-ed with `nb` (0, or 0x400 = the all-zero upper half of
-// the table: a "null" entry of 0 bits, used to switch a pixel's literals off without a branch)
+// byte offset of the packed 32-bit (size << 16 | code) entry of byte POS of word w
 template <int POS>
-__device__ __forceinline__ uint32_t lit_off16(uint32_t w, uint32_t nb)
+__device__ __forceinline__ uint32_t lit_off16(uint32_t w)
 {
     const uint32_t x = POS == 0 ? (w << 2) : (POS == 1 ? (w >> 6) : (POS == 2 ? (w >> 14) : (w >> 22)));
-    return (x & 0x3FCu) | nb;                                            // one LOP3
+    return x & 0x3FCu;
 }
 
 template <int CHANS>
 __device__ __forceinline__ void put_literal16(BitStager16& bs, uint32_t s_lit_saddr, uint32_t px)
 {
-    put_pair16(bs, lds_u32(s_lit_saddr + lit_off16<0>(px, 0u)), lds_u32(s_lit_saddr + lit_off16<1>(px, 0u)));
-    if (CHANS == 4) put_pair16(bs, lds_u32(s_lit_saddr + lit_off16<2>(px, 0u)), lds_u32(s_lit_saddr + lit_off16<3>(px, 0u)));
-    else { const uint32_t c2 = lds_u32(s_lit_saddr + lit_off16<2>(px, 0u)); bs.put(c2 & 0xFFFFu, c2 >> 16); }
+    put_pair16(bs, lds_u32(s_lit_saddr + lit_off16<0>(px)), lds_u32(s_lit_saddr + lit_off16<1>(px)));
+    if (CHANS == 4) put_pair16(bs, lds_u32(s_lit_saddr + lit_off16<2>(px)), lds_u32(s_lit_saddr + lit_off16<3>(px)));
+    else { const uint32_t c2 = lds_u32(s_lit_saddr + lit_off16<2>(px)); bs.put(c2 & 0xFFFFu, c2 >> 16); }
 }
 
-// the 4 literal codes of one 32-bit word of filtered bytes, in byte order, as two <= 24-bit puts (kPlain: nb == 0, the all-literal path)
-template <bool kPlain = false>
-__device__ __forceinline__ void put_word16(BitStager16& bs, uint32_t s_lit_saddr, uint32_t w, uint32_t nb)
+// the 4 literal codes of one 32-bit word of filtered bytes, in byte order, as two <= 24-bit puts (the all-literal path)
+__device__ __forceinline__ void put_word16(BitStager16& bs, uint32_t s_lit_saddr, uint32_t w)
 {
-#if FPNGB_PACK_LIT64
-    const uint32_t l64 = s_lit_saddr - 4096u, nb8 = nb << 1;
-    uint2 f0, f1, f2, f3;
-    if (kPlain) {
-        f0 = lds_u64(l64 + lit_off16x8_plain<0>(w)); f1 = lds_u64(l64 + lit_off16x8_plain<1>(w));
-        f2 = lds_u64(l64 + lit_off16x8_plain<2>(w)); f3 = lds_u64(l64 + lit_off16x8_plain<3>(w));
-    } else {
-        f0 = lds_u64(l64 + lit_off16x8<0>(w, nb8)); f1 = lds_u64(l64 + lit_off16x8<1>(w, nb8));
-        f2 = lds_u64(l64 + lit_off16x8<2>(w, nb8)); f3 = lds_u64(l64 + lit_off16x8<3>(w, nb8));
-    }
-#if FPNGB_PACK_MUL
-    bs.put_pow(f0.x + f1.x * f0.y, f0.y * f1.y);                         // the table holds (code, 2^size)
-    bs.put_pow(f2.x + f3.x * f2.y, f2.y * f3.y);
-#else
+    const uint32_t l64 = s_lit_saddr - 4096u;
+    const uint2 f0 = lds_u64(l64 + lit_off16x8_plain<0>(w)), f1 = lds_u64(l64 + lit_off16x8_plain<1>(w));
+    const uint2 f2 = lds_u64(l64 + lit_off16x8_plain<2>(w)), f3 = lds_u64(l64 + lit_off16x8_plain<3>(w));
     bs.put(f0.x | (f1.x << f0.y), f0.y + f1.y);
     bs.put(f2.x | (f3.x << f2.y), f2.y + f3.y);
-#endif
-    return;
-#endif
-    const uint32_t e0 = lds_u32(s_lit_saddr + lit_off16<0>(w, nb)), e1 = lds_u32(s_lit_saddr + lit_off16<1>(w, nb));
-    const uint32_t e2 = lds_u32(s_lit_saddr + lit_off16<2>(w, nb)), e3 = lds_u32(s_lit_saddr + lit_off16<3>(w, nb));
-    put_pair16(bs, e0, e1);
-    put_pair16(bs, e2, e3);
-}
-
-// entry of byte B (0..23) of a half's 6 RGB words
-template <int B>
-__device__ __forceinline__ uint32_t lit_entry_rgb16(uint32_t s_lit_saddr, const uint32_t (&hw)[6], uint32_t nb)
-{
-    return lds_u32(s_lit_saddr + lit_off16<B & 3>(hw[B >> 2], nb));
 }
 
 // pending run length before pixel kk (0..16) of a lane, from its equality mask and the run entering the lane
@@ -455,8 +383,49 @@ __device__ __forceinline__ void put_event16(BitStager16& bs, uint32_t s_match_sa
     if (len) put_match16(bs, s_match_saddr, len);
 }
 
+// the literal codes of word J (0 .. kHalfWords-1) of a mixed half: one 64-bit (code, size) load per byte, each byte's entry taken
+// from the table's null half when its pixel is not a literal, two codes per put.  A token event goes before its pixel's first byte:
+// for RGB that byte can sit inside the word, and only then (rare: a run ends or reaches M in this word) the word is put code by
+// code with the match token in between.
+__device__ __forceinline__ uint32_t null_ofs8(uint32_t nl, int k) { return (nl << (11 - k)) & 0x800u; }   // bit k of nl -> 0x800 (k <= 7)
+template <int CHANS, int J, uint32_t M>
+__device__ __forceinline__ void put_mixed_word16(BitStager16& bs, uint32_t lit_s, uint32_t match_s, uint32_t w, uint32_t nl, uint32_t ev8,
+                                                 uint32_t eqm, uint32_t r_in, uint32_t kbase)
+{
+    constexpr int kFirst = 4 * J / CHANS;                              // pixel of byte 0
+    constexpr int kIn = (4 * J + 3) / CHANS;                           // pixel of byte 3: starts inside the word iff kIn != kFirst (RGB)
+    constexpr int kSplit = CHANS * kIn - 4 * J;                        // its first byte (1..3)
+    const uint32_t l64 = lit_s - 4096u;
+    const uint2 f0 = lds_u64(l64 + lit_off16x8<0>(w, null_ofs8(nl, kFirst)));
+    const uint2 f1 = lds_u64(l64 + lit_off16x8<1>(w, null_ofs8(nl, (4 * J + 1) / CHANS)));
+    const uint2 f2 = lds_u64(l64 + lit_off16x8<2>(w, null_ofs8(nl, (4 * J + 2) / CHANS)));
+    const uint2 f3 = lds_u64(l64 + lit_off16x8<3>(w, null_ofs8(nl, kIn)));
+    if (CHANS * kFirst == 4 * J && (ev8 & (1u << kFirst))) put_event16<M>(bs, match_s, eqm, r_in, kbase + kFirst);
+    if (kIn != kFirst && (ev8 & (1u << kIn))) {
+        const uint2 f[4] = {f0, f1, f2, f3};
+#pragma unroll
+        for (int b = 0; b < 4; b++) {
+            if (b == kSplit) put_event16<M>(bs, match_s, eqm, r_in, kbase + kIn);
+            bs.put(f[b].x, f[b].y);
+        }
+        return;
+    }
+    bs.put(f0.x | (f1.x << f0.y), f0.y + f1.y);
+    bs.put(f2.x | (f3.x << f2.y), f2.y + f3.y);
+}
+// words J.. of a mixed half (hw: its 2 * CHANS filtered words; nl: bit k set when pixel k is not a literal)
+template <int CHANS, uint32_t M, int J = 0>
+__device__ __forceinline__ void put_mixed_half16(BitStager16& bs, uint32_t lit_s, uint32_t match_s, const uint32_t (&hw)[2 * CHANS], uint32_t nl,
+                                                 uint32_t ev8, uint32_t eqm, uint32_t r_in, uint32_t kbase)
+{
+    put_mixed_word16<CHANS, J, M>(bs, lit_s, match_s, hw[J], nl, ev8, eqm, r_in, kbase);
+    if constexpr (J + 1 < 2 * CHANS) put_mixed_half16<CHANS, M, J + 1>(bs, lit_s, match_s, hw, nl, ev8, eqm, r_in, kbase);
+}
+
 // one Horner step of the in-kernel CRC: the register (XOR-ed with the lane's previous word) advanced over 128 bytes, then the next
-// word (slice tables [4][256] at shared address crc_s; byte extraction with PRMT so that each look-up address is one LEA)
+// word (slice tables [4][256] at shared address crc_s; byte extraction with PRMT so that each look-up address is one LEA).
+// Nibble tables [8][16] (every look-up conflict free: 1 instead of ~3 wavefronts) measured slower: the 8 extra ALU instructions
+// per word cost more than the bank conflicts (DESIGN 4.1).
 __device__ __forceinline__ uint32_t crc_step16(uint32_t crc_s, uint32_t cx, uint32_t v)
 {
     const uint32_t b0 = cx & 0xFFu, b1 = __byte_perm(cx, 0u, 0x4441), b2 = __byte_perm(cx, 0u, 0x4442), b3 = cx >> 24;
@@ -464,7 +433,7 @@ __device__ __forceinline__ uint32_t crc_step16(uint32_t crc_s, uint32_t cx, uint
 }
 
 template <int CHANS, int LOAD, bool RAGGED = false>
-__global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(std::conditional_t<RAGGED, RaggedParams<PackParams>, PackParams> p,
+__global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(std::conditional_t<RAGGED, RaggedParams<PackParams>, PackParams> p,
                                                                        uint32_t rows_per_warp)
 {
     using WK = typename Loader16<CHANS, LOAD>::type;
@@ -477,14 +446,11 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(std::cond
     if (p.stored_only && !p.st[img].stored) return;     // after the fused encoder only stored-block images are left to write
     constexpr uint32_t M = max_match_pixels(CHANS);
     constexpr int kHalfWords = 2 * CHANS;        // filtered words of 8 pixels
+    constexpr int kPack16Rows = pack16_warps(CHANS);
     extern __shared__ __align__(16) uint8_t dyn_smem[];
-#if FPNGB_PACK_LIT64
     uint32_t* s_lit64 = reinterpret_cast<uint32_t*>(dyn_smem + kPack16Rows * WK::kWarpBytes);   // [512][2]: (code, size) + null half
-    uint32_t* s_lit = s_lit64 + 1024;                // [512]: 256 packed entries + 256 zeros
-#else
-    uint32_t* s_lit = reinterpret_cast<uint32_t*>(dyn_smem + kPack16Rows * WK::kWarpBytes);   // [512]: 256 entries + 256 zeros
-#endif
-    uint32_t* s_match = s_lit + 512;
+    uint32_t* s_lit = s_lit64 + 1024;                // [256]: packed entries (size << 16 | code)
+    uint32_t* s_match = s_lit + 256;
     uint32_t* s_stage_all = s_match + 88;
     uint32_t* s_crc = s_stage_all + kPack16Rows * stage16_words<CHANS>();              // [4][256] CRC slice tables (row_crc only)
 
@@ -505,14 +471,8 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(std::cond
     }
     for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) {
         const uint32_t e = book->lit[i];
-        s_lit[i] = e; s_lit[256 + i] = 0u;
-#if FPNGB_PACK_LIT64
-#if FPNGB_PACK_MUL
-        s_lit64[2 * i] = e & 0xFFFFu; s_lit64[2 * i + 1] = 1u << (e >> 16); s_lit64[512 + 2 * i] = 0u; s_lit64[512 + 2 * i + 1] = 1u;   // (code, 2^size); null: 2^0
-#else
+        s_lit[i] = e;
         s_lit64[2 * i] = e & 0xFFFFu; s_lit64[2 * i + 1] = e >> 16; s_lit64[512 + 2 * i] = 0u; s_lit64[512 + 2 * i + 1] = 0u;
-#endif
-#endif
     }
     if (threadIdx.x < 88) s_match[threadIdx.x] = book->match[threadIdx.x];
     if (do_crc) for (uint32_t i = threadIdx.x; i < 1024; i += blockDim.x) s_crc[i] = __ldg(p.crc_f128b + i);
@@ -598,38 +558,14 @@ __global__ void __launch_bounds__(32 * kPack16Rows) pack_rows16_kernel(std::cond
             if (__all_sync(kFullMask, lit8 == 0xFFu && ev8 == 0u)) {
                 // (1) all 256 pixels are literals, no run pending (noisy rows): the filtered bytes in order, two codes per put
 #pragma unroll
-                for (int j = 0; j < kHalfWords; j++) put_word16<true>(bs, lit_s, hw[j], 0u);
+                for (int j = 0; j < kHalfWords; j++) put_word16(bs, lit_s, hw[j]);
             } else if (__all_sync(kFullMask, lit8 == 0u)) {
                 // (2) no literal at all (inside long runs): only a run reaching M emits a token
                 if (ev8) put_match16(bs, match_s, M);
             } else if (__reduce_add_sync(kFullMask, (uint32_t)__popc(lit8)) >= 16u) {
-                // (3) mixed: straight-line literal emission for every pixel, switched off per pixel through the table's null
-                //     half; the rare run tokens are inserted by a per-pixel event check
-                const uint32_t nl = ~lit8;
-#pragma unroll
-                for (int k = 0; k < 8; k++) {
-                    if (ev8 & (1u << k)) put_event16<M>(bs, match_s, eqm, r_in, 8u * h + k);
-                    const uint32_t nb = (k <= 10 ? (nl << (10 - k)) : (nl >> (k - 10))) & 0x400u;
-                    if (CHANS == 4) put_word16(bs, lit_s, hw[k], nb);
-                    else {
-                        uint32_t e0, e1, e2;
-                        // bytes 3k .. 3k+2 of the half's 24 filtered bytes
-                        const uint32_t* hp = hw;
-                        switch (k) {                                     // compile-time after unrolling
-                        default:
-                        case 0: e0 = lds_u32(lit_s + lit_off16<0>(hp[0], nb)); e1 = lds_u32(lit_s + lit_off16<1>(hp[0], nb)); e2 = lds_u32(lit_s + lit_off16<2>(hp[0], nb)); break;
-                        case 1: e0 = lds_u32(lit_s + lit_off16<3>(hp[0], nb)); e1 = lds_u32(lit_s + lit_off16<0>(hp[1], nb)); e2 = lds_u32(lit_s + lit_off16<1>(hp[1], nb)); break;
-                        case 2: e0 = lds_u32(lit_s + lit_off16<2>(hp[1], nb)); e1 = lds_u32(lit_s + lit_off16<3>(hp[1], nb)); e2 = lds_u32(lit_s + lit_off16<0>(hp[2], nb)); break;
-                        case 3: e0 = lds_u32(lit_s + lit_off16<1>(hp[2], nb)); e1 = lds_u32(lit_s + lit_off16<2>(hp[2], nb)); e2 = lds_u32(lit_s + lit_off16<3>(hp[2], nb)); break;
-                        case 4: e0 = lds_u32(lit_s + lit_off16<0>(hp[3], nb)); e1 = lds_u32(lit_s + lit_off16<1>(hp[3], nb)); e2 = lds_u32(lit_s + lit_off16<2>(hp[3], nb)); break;
-                        case 5: e0 = lds_u32(lit_s + lit_off16<3>(hp[3], nb)); e1 = lds_u32(lit_s + lit_off16<0>(hp[4], nb)); e2 = lds_u32(lit_s + lit_off16<1>(hp[4], nb)); break;
-                        case 6: e0 = lds_u32(lit_s + lit_off16<2>(hp[4], nb)); e1 = lds_u32(lit_s + lit_off16<3>(hp[4], nb)); e2 = lds_u32(lit_s + lit_off16<0>(hp[5], nb)); break;
-                        case 7: e0 = lds_u32(lit_s + lit_off16<1>(hp[5], nb)); e1 = lds_u32(lit_s + lit_off16<2>(hp[5], nb)); e2 = lds_u32(lit_s + lit_off16<3>(hp[5], nb)); break;
-                        }
-                        put_pair16(bs, e0, e1);
-                        bs.put(e2 & 0xFFFFu, e2 >> 16);
-                    }
-                }
+                // (3) mixed: the all-literal emission word by word, each byte switched off through the table's null half when
+                //     its pixel is not a literal; the rare run tokens are inserted by a per-word event check
+                put_mixed_half16<CHANS, M>(bs, lit_s, match_s, hw, ~lit8, ev8, eqm, r_in, 8u * h);
             } else {
                 // (4) sparse literals (RLE-dominated rows): per-pixel token walk, 4 pixels at a time
                 uint32_t r = run_before16<M>(eqm, r_in, 8u * h);
@@ -735,7 +671,7 @@ template <class P> static int load16_mode(const P& p, uint32_t chans)
 template <int CHANS, int LOAD> constexpr size_t scan16_smem() { return kScan16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + 256 + 96; }
 template <int CHANS, int LOAD> constexpr size_t pack16_smem()
 {
-    return kPack16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + ((FPNGB_PACK_LIT64 ? 1024 : 0) + 512 + 88 + kPack16Rows * stage16_words<CHANS>() + 1024) * 4;
+    return pack16_warps(CHANS) * Loader16<CHANS, LOAD>::type::kWarpBytes + (1024 + 256 + 88 + pack16_warps(CHANS) * stage16_words<CHANS>() + 1024) * 4;
 }
 template <int CHANS, int LOAD> constexpr size_t hist16_smem() { return kScan16Rows * Loader16<CHANS, LOAD>::type::kWarpBytes + kScan16Rows * 288 * 4; }
 
@@ -773,9 +709,9 @@ void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t
 void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
 {
     const int load = load16_mode(p, chans);
-    const uint32_t rpw = rows_per_warp16(n, p.h), rows_per_cta = kPack16Rows * rpw;
+    const uint32_t rpw = rows_per_warp16(n, p.h), rows_per_cta = pack16_warps(chans) * rpw;
     dim3 grid((p.h + rows_per_cta - 1) / rows_per_cta, n);
-    FPNGB_LAUNCH16(pack_rows16_kernel, false, pack16_smem, grid, 32 * kPack16Rows, p, rpw);
+    FPNGB_LAUNCH16(pack_rows16_kernel, false, pack16_smem, grid, 32 * pack16_warps(chans), p, rpw);
 }
 
 // Ragged launches: one per (chans, loader) class, over the class's CTAs (the host sums them per image: ceil(h / rows per CTA)).
@@ -785,7 +721,7 @@ uint32_t pack16_rows_per_warp(size_t total_rows)
     if (g_rows_per_warp_override) return g_rows_per_warp_override;
     return total_rows >= (size_t)sm_count() * 64u * kRowsPerWarp16 ? kRowsPerWarp16 : 1u;
 }
-uint32_t pack16_rows_per_cta(uint32_t rows_per_warp) { return kPack16Rows * rows_per_warp; }
+uint32_t pack16_rows_per_cta(uint32_t rows_per_warp, uint32_t chans) { return pack16_warps(chans) * rows_per_warp; }
 
 void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s)
 {
@@ -799,7 +735,7 @@ void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint
 
 void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s)
 {
-    FPNGB_LAUNCH16(pack_rows16_kernel, true, pack16_smem, ctas, 32 * kPack16Rows, p, rows_per_warp);
+    FPNGB_LAUNCH16(pack_rows16_kernel, true, pack16_smem, ctas, 32 * pack16_warps(chans), p, rows_per_warp);
 }
 
 }  // namespace fpngb

@@ -482,7 +482,7 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
     size_t rows = 0, lanes = 0;
     for (uint32_t k : ids) { rows += im[k].h; lanes += (size_t)im[k].h * (((im[k].w + 511u) / 512u) * 32u); }
-    const uint32_t rpw = pack16_rows_per_warp(rows), pack_rows = pack16_rows_per_cta(rpw), scan_rows = scan16_rows_per_cta();
+    const uint32_t rpw = pack16_rows_per_warp(rows), scan_rows = scan16_rows_per_cta();
     // class of an image: (chans == 4) * 3 + loader, the loader by the uniform launch's rule for one image
     constexpr int kClasses = 6;
     std::vector<uint32_t> cls(m);
@@ -538,6 +538,7 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
         const uint32_t k = cls[j], q = fill[k]++;
         l_img[q] = j;
         l_scan[q] = (uint32_t)cls_scan_ctas[k]; cls_scan_ctas[k] += (r.h + scan_rows - 1) / scan_rows;
+        const uint32_t pack_rows = pack16_rows_per_cta(rpw, r.chans);
         l_pack[q] = (uint32_t)cls_pack_ctas[k]; cls_pack_ctas[k] += (r.h + pack_rows - 1) / pack_rows;
         l_crc_img[j] = j; l_crc[j] = (uint32_t)crc_ctas; crc_ctas += crc_stream_ctas_for(max_encoded_size(r.w, r.h, r.chans));
         max_split = std::max(max_split, row_crc_split_for(r.h));

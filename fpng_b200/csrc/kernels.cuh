@@ -161,7 +161,7 @@ void launch_huffman_build_ragged(const HuffParams& p, uint32_t n, cudaStream_t s
 enum { kLoad16Staged = 0, kLoad16Direct = 1, kLoad16Planar = 2 };
 uint32_t scan16_rows_per_cta();
 uint32_t pack16_rows_per_warp(size_t total_rows);        // the uniform launch's rule for a batch of that many scanlines
-uint32_t pack16_rows_per_cta(uint32_t rows_per_warp);
+uint32_t pack16_rows_per_cta(uint32_t rows_per_warp, uint32_t chans);
 void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s);
 void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s);
 void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s);
