@@ -18,4 +18,5 @@ from .api import (  # noqa: F401
     FPNGB_DECODE_ADLER_MISMATCH, set_decode_verify, decode_verify,
     normalize_scale_bias, denormalize_scale_bias, typed_layout,
     FPNGB_DECODE_BAD_CROP, FPNGB_RESIZE_ANTIALIAS, decode_packed_resized_device,
+    FPNGB_DECODE_UNSUPPORTED_PNG, FPNGB_RESIZE_ANY_PNG, get_png_info,
 )

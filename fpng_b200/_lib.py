@@ -81,6 +81,12 @@ def lib() -> C.CDLL:
     L.fpngb_decode_packed_ragged_device_typed.restype = C.c_int
     L.fpngb_decode_packed_ragged_device_typed.argtypes = L.fpngb_decode_packed_ragged_device.argtypes[:-2] + [C.POINTER(PixelFormat),
                                                                                                            C.c_void_p, C.c_void_p]
+    L.fpngb_decode_packed_png_device.restype = C.c_int
+    L.fpngb_decode_packed_png_device.argtypes = L.fpngb_decode_packed_ragged_device_typed.argtypes
+    L.fpngb_get_png_info_batch_device.restype = C.c_int
+    L.fpngb_get_png_info_batch_device.argtypes = L.fpngb_get_info_batch_device.argtypes
+    L.fpngb_get_png_info.restype = C.c_int
+    L.fpngb_get_png_info.argtypes = L.fpngb_get_info_ex.argtypes
     L.fpngb_decode_packed_resized_device.restype = C.c_int
     L.fpngb_decode_packed_resized_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p] + [C.c_uint32] * 4 + \
         [C.c_size_t, C.c_void_p] + [C.c_uint32] * 4 + [C.POINTER(PixelFormat), C.c_void_p] + [C.c_size_t] * 4 + [C.c_void_p] * 3

@@ -4,6 +4,7 @@
 // per file: a file has a handful of chunks, and the only long loop is the CRC of an ancillary chunk, which one thread
 // computes byte by byte from a 256-entry table in constant memory.
 #include "container.cuh"
+#include "png_walk.cuh"
 #include "decode.cuh"
 #include "crc_math.cuh"
 
@@ -31,7 +32,10 @@ struct DeviceCrc {
     }
 };
 
-__global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
+// kAny (the any-PNG calls): files container_walk rejects with FPNGB_DECODE_NOT_FPNG are walked again by png_walk; a general file that
+// passes every check of the call gets pre_status kPngPending and, with png != nullptr, its PngDesc (decode.cuh)
+template <bool kAny>
+__global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDesc* png)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n) return;
@@ -42,7 +46,9 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
     // decode kernels' word reads; the ragged call also keeps every file inside the buffer and walks only files that pass
     const bool bad_arg = !size || (p.files && (size > p.max_file_size || (ofs & 3ull) || (ragged && (ofs > p.base_bytes || size > p.base_bytes - ofs))));
     uint32_t st, w = 0, h = 0, c = 0, io = 0, il = 0;
+    bool general = false;
     if (!size || (ragged && bad_arg)) st = FPNGB_DECODE_INVALID_ARG;
+    else if (kAny) st = any_png_walk(p.base + ofs, size, DeviceCrc{}, &w, &h, &c, &io, &il, &general);
     else st = container_walk(p.base + ofs, size, DeviceCrc{}, &w, &h, &c, &io, &il);
     if (p.info) {
         uint32_t* o = p.info + (size_t)i * 6;
@@ -60,6 +66,9 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
                 if (bh < 1 || bw < 1 || top < 0 || left < 0 || top + bh > h || left + bw > w) pre = FPNGB_DECODE_BAD_CROP;
             }
         } else if (!pre && (w != p.w || h != p.h || c != p.chans)) pre = FPNGB_DECODE_SHAPE_MISMATCH;
+        if (kAny && !pre && general) pre = kPngPending;
+        if (kAny && png) png[i] = PngDesc{0ull, pre == kPngPending ? il : 0u, 0u};
+        if (kAny && pre == kPngPending) pre = 0;                                // placed as any file; marked again below
         FileDesc fd;
         fd.base = ofs; fd.file_size = size; fd.idat_ofs = pre ? 0u : io; fd.idat_len = pre ? 0u : il; fd.pre_status = pre;
         if (ragged) {
@@ -70,37 +79,53 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p)
             fd.delta_base = (unsigned long long)i * fd.pitch * p.h; fd.out_base = i * p.out_stride;
             fd.sub_base = (unsigned long long)i * subs_for(p.max_file_size);
         }
+        if (kAny && general && !pre) fd.pre_status = kPngPending;
         p.files[i] = fd;
     }
 }
 
 void launch_container_walk(const WalkParams& p, cudaStream_t s)
 {
-    container_walk_kernel<<<(p.n + 127) / 128, 128, 0, s>>>(p);
+    container_walk_kernel<false><<<(p.n + 127) / 128, 128, 0, s>>>(p, nullptr);
+}
+void launch_container_walk_any(const WalkParams& p, PngDesc* png, cudaStream_t s)
+{
+    container_walk_kernel<true><<<(p.n + 127) / 128, 128, 0, s>>>(p, png);
 }
 
 // One CTA: exclusive scans of the output bytes, delta bytes and records of the accepted files, kPlaceThreads files per round.
+// kAny: general files (pre_status kPngPending) are placed too, with their inflated rows in the delta bytes, no records, and a
+// fourth scan of their gathered zlib bytes (z_cap).
 constexpr uint32_t kPlaceThreads = 1024;
-__global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams p)
+template <bool kAny>
+__global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams p, PngDesc* png, unsigned long long z_cap)
 {
-    __shared__ unsigned long long s_warp[3][kPlaceThreads / 32];
-    __shared__ unsigned long long s_carry[3];
+    constexpr int K = kAny ? 4 : 3;
+    __shared__ unsigned long long s_warp[K][kPlaceThreads / 32];
+    __shared__ unsigned long long s_carry[K];
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    if (tid < 3) s_carry[tid] = 0;
+    if (tid < K) s_carry[tid] = 0;
     for (uint32_t first = 0; first < p.n; first += kPlaceThreads) {
         const uint32_t i = first + tid;
         FileDesc fd{};
-        bool placed = false;
-        if (i < p.n) { fd = p.files[i]; placed = fd.pre_status == 0; }
-        unsigned long long v[3] = {0ull, 0ull, 0ull};
+        bool placed = false, general = false;
+        if (i < p.n) { fd = p.files[i]; general = kAny && fd.pre_status == kPngPending; placed = fd.pre_status == 0 || general; }
+        unsigned long long v[K];
+#pragma unroll
+        for (int k = 0; k < K; k++) v[k] = 0ull;
         if (placed) {
             v[0] = ((unsigned long long)fd.w * fd.h * p.px_bytes + 15ull) & ~15ull;
-            v[1] = (unsigned long long)fd.h * fd.pitch;
-            v[2] = subs_for(fd.file_size);
+            if (general) {
+                v[1] = ((unsigned long long)fd.h * (1ull + (unsigned long long)fd.w * fd.chans) + 15ull) & ~15ull;
+                v[K - 1] = ((unsigned long long)png[i].zlen + 15ull) & ~15ull;
+            } else {
+                v[1] = (unsigned long long)fd.h * fd.pitch;
+                v[2] = subs_for(fd.file_size);
+            }
         }
-        unsigned long long x[3];
+        unsigned long long x[K];
 #pragma unroll
-        for (int k = 0; k < 3; k++) {                      // inclusive warp scan, then the warp totals
+        for (int k = 0; k < K; k++) {                      // inclusive warp scan, then the warp totals
             x[k] = v[k];
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, x[k], o); if (lane >= (uint32_t)o) x[k] += u; }
@@ -109,7 +134,7 @@ __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams
         __syncthreads();
         if (warp == 0) {                                   // exclusive scan of the warp totals, carry of the earlier rounds in front
 #pragma unroll
-            for (int k = 0; k < 3; k++) {
+            for (int k = 0; k < K; k++) {
                 unsigned long long t = s_warp[k][lane];
 #pragma unroll
                 for (int o = 1; o < 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xFFFFFFFFu, t, o); if (lane >= (uint32_t)o) t += u; }
@@ -117,18 +142,23 @@ __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams
             }
         }
         __syncthreads();
-        unsigned long long at[3];
+        unsigned long long at[K];
 #pragma unroll
-        for (int k = 0; k < 3; k++) at[k] = s_warp[k][warp] + x[k] - v[k];
+        for (int k = 0; k < K; k++) at[k] = s_warp[k][warp] + x[k] - v[k];
         if (i < p.n) {
             p.out_offsets[i] = at[0];
             if (placed) {
                 FileDesc* d = p.files + i;
-                if (at[0] + v[0] > p.out_cap || at[1] + v[1] > p.delta_cap || at[2] + v[2] > p.sub_cap) d->pre_status = FPNGB_DECODE_OUT_OF_SPACE;
-                else { d->out_base = at[0]; d->delta_base = at[1]; d->sub_base = at[2]; }
+                if (at[0] + v[0] > p.out_cap || at[1] + v[1] > p.delta_cap || at[2] + v[2] > p.sub_cap ||
+                    (kAny && at[K - 1] + v[K - 1] > z_cap))
+                    d->pre_status = FPNGB_DECODE_OUT_OF_SPACE;
+                else {
+                    d->out_base = at[0]; d->delta_base = at[1]; d->sub_base = at[2];
+                    if (general) png[i].zofs = at[K - 1];
+                }
             }
         }
-        if (tid == kPlaceThreads - 1) for (int k = 0; k < 3; k++) s_carry[k] = at[k] + v[k];
+        if (tid == kPlaceThreads - 1) for (int k = 0; k < K; k++) s_carry[k] = at[k] + v[k];
         __syncthreads();
     }
     if (tid == 0) p.out_offsets[p.n] = s_carry[0] | (s_carry[0] > p.out_cap ? 1ull << 63 : 0ull);
@@ -136,7 +166,11 @@ __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams
 
 void launch_decode_place(const PlaceParams& p, cudaStream_t s)
 {
-    decode_place_kernel<<<1, kPlaceThreads, 0, s>>>(p);
+    decode_place_kernel<false><<<1, kPlaceThreads, 0, s>>>(p, nullptr, 0ull);
+}
+void launch_decode_place_any(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s)
+{
+    decode_place_kernel<true><<<1, kPlaceThreads, 0, s>>>(p, png, z_cap);
 }
 
 }  // namespace fpngb

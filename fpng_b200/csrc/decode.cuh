@@ -136,6 +136,31 @@ struct PlaceParams {
 };
 void launch_decode_place(const PlaceParams& p, cudaStream_t s);
 
+// ---- general PNG files (fpngb_decode_packed_png_device, FPNGB_RESIZE_ANY_PNG; png_walk.cuh) ----
+// The any-PNG walk gives a general file that passes every check the internal pre_status kPngPending: no fpng kernel touches it and
+// decode_status_kernel writes that marker to d_status, which png_unfilter_kernel, launched behind it, overwrites with the file's
+// final status.  decode_place_kernel<true> places general files like any file (align_up(w*h*px_bytes, 16) output bytes), takes
+// align_up(h * (1 + w*chans), 16) delta bytes for the inflated rows (FileDesc::delta_base) and no records, and allots the gathered
+// IDAT bytes (PngDesc::zofs) from a fourth scan bounded by z_cap.
+constexpr uint32_t kPngPending = 0x7FFFFFF0u;
+struct PngDesc {
+    unsigned long long zofs;                // byte offset of the file's gathered zlib stream from PngParams::z (a multiple of 16)
+    uint32_t zlen;                          // its length: the sum of the IDAT data lengths
+    uint32_t status;                        // 0 until the gather (4) or inflate (8, 102) kernels find an error
+};
+struct PngParams {
+    const uint8_t* d_files; const FileDesc* files; PngDesc* png;
+    uint8_t* z;                             // gathered zlib streams
+    uint8_t* rows;                          // inflated rows: file f at rows + files[f].delta_base (the decode's delta region)
+    uint8_t* d_out; uint32_t* d_status;     // pixels as the ragged decode places them (tight HWC rows at d_out + files[f].out_base)
+    uint32_t n, desired, verify;
+};
+// container_walk_kernel<true> (png != nullptr only with files != nullptr) and decode_place_kernel<true>, z_cap the gathered bytes
+void launch_container_walk_any(const WalkParams& p, PngDesc* png, cudaStream_t s);
+void launch_decode_place_any(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s);
+// gather, inflate and unfilter of the general files (three launches; grids from n alone), behind launch_decode
+void launch_png_decode(const PngParams& p, const TypedOut* typed, cudaStream_t s);
+
 // decode_resize_kernel (decode_resize_kernels.cu), resized call: after the ragged pipeline has decoded every file into tight uint8
 // HWC rows (pitch w * desired) at px + px_offsets[f], crops file f to its box and resizes it to out_h x out_w with the bilinear
 // rule of fpngb_decode_packed_resized_device, then stores T(r * scale[c] + bias[c]) (float types) or round_u8(r) (dtype 0).

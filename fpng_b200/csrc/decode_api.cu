@@ -3,6 +3,7 @@
 #include "kernels.cuh"
 #include "decode.cuh"
 #include "container.cuh"
+#include "png_walk.cuh"
 #include "layout.h"
 #include "runtime.h"
 #include <string.h>
@@ -19,9 +20,10 @@ static std::atomic<int> g_decode_verify{0};
 // Reserves the workspace of a decode call for n files, n_subs SubInfo records and delta_bytes of delta rows in all, orders it
 // after the previous call's kernels, and points p's workspace fields into it (p.files included).  With verification on
 // (fpngb_set_decode_verify), *verify points to n VerifyState records behind the rest; else it is nullptr.  extra_bytes more (the
-// resized call's uint8 pixels and their offsets) go last, at *extra (256-byte aligned).  Caller holds context().mu.
+// resized call's uint8 pixels and their offsets) go last, at *extra (256-byte aligned), and png_bytes more (the any-PNG calls'
+// PngDesc records and gathered streams) behind them, at *png (256-byte aligned).  Caller holds context().mu.
 static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes, cudaStream_t s, DecodeParams& p, VerifyState** verify,
-                                   size_t extra_bytes = 0, uint8_t** extra = nullptr)
+                                   size_t extra_bytes = 0, uint8_t** extra = nullptr, size_t png_bytes = 0, uint8_t** png = nullptr)
 {
     size_t o = 0;
     const size_t o_files = o; o = align_up(o + (size_t)n * sizeof(FileDesc), 256);
@@ -33,6 +35,7 @@ static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes
     const bool verifying = g_decode_verify.load() != 0;
     const size_t o_verify = o; if (verifying) o = align_up(o + (size_t)n * sizeof(VerifyState), 256);
     const size_t o_extra = o; o += extra_bytes;
+    const size_t o_png = png_bytes ? (o = align_up(o, 256)) : o; o += png_bytes;
     int rc = g_dec_ws.reserve(o); if (rc) return rc;
     rc = context().ws_acquire(s); if (rc) return rc;
     uint8_t* b = (uint8_t*)g_dec_ws.p;
@@ -41,6 +44,7 @@ static int decode_workspace_locked(uint32_t n, size_t n_subs, size_t delta_bytes
     p.delta = b + o_delta;
     *verify = verifying ? (VerifyState*)(b + o_verify) : nullptr;
     if (extra) *extra = b + o_extra;
+    if (png) *png = b + o_png;
     return 0;
 }
 // The same for n files of one shape whose IDAT chunks are at most max_idat bytes: file i's records and delta rows at i times the
@@ -200,18 +204,25 @@ static int decode_packed_device_impl(const void* d_base, const uint64_t* d_offse
 //              sum to at most base_bytes, so base_bytes/128 + 3n records hold them all.  Every file also has s <= max_file_size.
 //   delta:     a file needs h * align_up(w*c, 16) <= (4/desired) * (w*h*desired) + 15h bytes, h <= max_h and h <= w*h, and the
 //              w*h*desired of the decoded files sum to at most out_cap.  Every file also needs at most max_h * pitch(max_w, 4).
+//   any-PNG calls: a general file's inflated rows take align_up(h * (1 + w*c), 16) <= 4*w*h + 16h delta bytes (c <= 4, h >= 1), inside
+//              the same bound from out_cap; from the shape, h * (delta_pitch(w, 4) + 16) per file.  Its gathered stream takes
+//              align_up(zlen, 16) bytes, zlen < its size: at most base_bytes + 16n for files that do not overlap, and
+//              align_up(max_file_size, 16) each.
 // A file whose range still ends past a bound (overlapping files) gets FPNGB_DECODE_OUT_OF_SPACE from decode_place_kernel.
 static unsigned long long sat_u64(unsigned __int128 v) { return v > ~0ull ? ~0ull : (unsigned long long)v; }
 static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired,
-                             size_t out_cap, unsigned long long& sub_cap, unsigned long long& delta_cap)
+                             size_t out_cap, bool any_png, unsigned long long& sub_cap, unsigned long long& delta_cap,
+                             unsigned long long& z_cap)
 {
     typedef unsigned __int128 u128;
     const u128 by_bytes = (u128)base_bytes / 128 + 3 * (u128)n, by_max = (u128)n * subs_for(max_file_size);
     sub_cap = sat_u64(by_bytes < by_max ? by_bytes : by_max);
     const u128 rows = (u128)n * max_h, rows_px = ((u128)out_cap + desired - 1) / desired;
     const u128 by_out = ((u128)out_cap * 4 + desired - 1) / desired + 16 * (rows < rows_px ? rows : rows_px);
-    const u128 by_shape = rows * delta_pitch(max_w, 4);
+    const u128 by_shape = rows * (delta_pitch(max_w, 4) + (any_png ? 16u : 0u));
     delta_cap = sat_u64(by_out < by_shape ? by_out : by_shape);
+    const u128 z_bytes = (u128)base_bytes + 16 * (u128)n, z_max = (u128)n * align_up((size_t)max_file_size, 16);
+    z_cap = any_png ? sat_u64(z_bytes < z_max ? z_bytes : z_max) : 0ull;
 }
 
 // The resize step of fpngb_decode_packed_resized_device: its checked output and arguments.
@@ -222,11 +233,12 @@ struct ResizeOut {
 
 // The ragged pipeline: walk, place, decode.  With rz (the resized call), the uint8 pixels and their offsets go to the decode
 // workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes, and the
-// resize kernel runs behind the decode, before the workspace is released.
+// resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
+// general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc).
 static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
-                                     int32_t* d_status, void* stream, const ResizeOut* rz = nullptr)
+                                     int32_t* d_status, void* stream, const ResizeOut* rz = nullptr, bool any_png = false)
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
@@ -237,10 +249,12 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     uint32_t elem;
     int rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
     if ((uintptr_t)d_base % 4 || (!rz && (uintptr_t)d_out % 16)) return FPNGB_ERR_ALIGNMENT;
-    unsigned long long sub_cap = 0, delta_cap = 0;
+    unsigned long long sub_cap = 0, delta_cap = 0, z_cap = 0;
     // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
-    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, sub_cap, delta_cap);
-    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2 || (rz && out_cap > SIZE_MAX / 2)) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, any_png, sub_cap, delta_cap, z_cap);
+    if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2 || (rz && out_cap > SIZE_MAX / 2) || z_cap > SIZE_MAX / 4)
+        return FPNGB_ERR_BUFFER_TOO_SMALL;
+    const size_t png_desc_bytes = any_png ? align_up((size_t)n * sizeof(PngDesc), 256) : 0;
     const size_t offsets_bytes = align_up(((size_t)n + 1) * sizeof(uint64_t), 256);
     const cudaStream_t s = (cudaStream_t)stream;
     std::lock_guard<std::mutex> lk(c.mu);
@@ -248,20 +262,31 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     DecodeParams p{};
     VerifyState* verify = nullptr;
     uint8_t* extra = nullptr;
-    rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify, rz ? offsets_bytes + out_cap : 0, &extra); if (rc) return rc;
+    uint8_t* png = nullptr;
+    rc = decode_workspace_locked(n, sub_cap, delta_cap, s, p, &verify, rz ? offsets_bytes + out_cap : 0, &extra,
+                                 any_png ? png_desc_bytes + z_cap : 0, &png);
+    if (rc) return rc;
     if (rz) { d_out_offsets = (uint64_t*)extra; d_out = extra + offsets_bytes; }
     p.max_w = max_w; p.max_h = max_h; p.max_subs = subs_for(max_file_size); p.chans = 0;
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
     wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr;
-    launch_container_walk(wp, s);
+    if (any_png) launch_container_walk_any(wp, (PngDesc*)png, s);
+    else launch_container_walk(wp, s);
     PlaceParams pp{};
     pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem;
     pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
-    launch_decode_place(pp, s);
+    if (any_png) launch_decode_place_any(pp, (PngDesc*)png, z_cap, s);
+    else launch_decode_place(pp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
     launch_decode(p, OutStrides{0, desired_chans * elem, elem}, n, desired_chans, s, verify, max_file_size, typed ? &t : nullptr);
+    if (any_png) {                                  // behind decode_status_kernel: the general files' final statuses
+        PngParams q{};
+        q.d_files = (const uint8_t*)d_base; q.files = p.files; q.png = (PngDesc*)png; q.z = png + png_desc_bytes; q.rows = p.delta;
+        q.d_out = (uint8_t*)d_out; q.d_status = (uint32_t*)d_status; q.n = n; q.desired = desired_chans; q.verify = verify != nullptr;
+        launch_png_decode(q, typed ? &t : nullptr, s);
+    }
     if (rz) {
         ResizeParams rp{};
         rp.px = (const uint8_t*)d_out; rp.px_offsets = (const unsigned long long*)d_out_offsets; rp.files = p.files; rp.d_status = d_status;
@@ -271,7 +296,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         launch_decode_resize(rp, rz->t, n, desired_chans, s);
         decode_profile_mark_resize(s);
     }
-    count_launch((verify ? 13 : 11) + (rz ? 1 : 0));
+    count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0));
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
 }
@@ -540,7 +565,7 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
 {
     if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_out || n == 0 || n > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
-        (desired_chans != 3 && desired_chans != 4) || (flags & ~(uint32_t)FPNGB_RESIZE_ANTIALIAS))
+        (desired_chans != 3 && desired_chans != 4) || (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG)))
         return FPNGB_ERR_INVALID_ARG;
     ResizeOut rz{};
     rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
@@ -550,7 +575,39 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
                       rz.out);
     if (rc) return rc;
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
-                                     nullptr, d_info, false, nullptr, d_status, stream, &rz);
+                                     nullptr, d_info, false, nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0);
+}
+
+int fpngb_decode_packed_png_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                   uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
+                                   size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, const fpngb_pixel_format* fmt,
+                                   int32_t* d_status, void* stream)
+{
+    return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
+                                     d_out_offsets, d_info, fmt != nullptr, fmt, d_status, stream, nullptr, true);
+}
+
+int fpngb_get_png_info_batch_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t* d_info,
+                                    void* stream)
+{
+    Context& c = context();
+    if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (!d_base || !d_offsets || !d_sizes || !d_info || n == 0) return FPNGB_ERR_INVALID_ARG;
+    WalkParams p{};
+    p.base = (const uint8_t*)d_base; p.offsets = (const unsigned long long*)d_offsets; p.sizes = d_sizes; p.n = n; p.info = d_info;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    launch_container_walk_any(p, nullptr, (cudaStream_t)stream);
+    count_launch(1);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return FPNGB_OK;
+}
+
+int fpngb_get_png_info(const void* file, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs, uint32_t* idat_len)
+{
+    if (!file || !w || !h || !chans || !idat_ofs || !idat_len) return FPNGB_DECODE_INVALID_ARG;
+    bool general;
+    return any_png_walk((const uint8_t*)file, size, HostCrc{}, w, h, chans, idat_ofs, idat_len, &general);
 }
 
 }  // extern "C"

@@ -420,6 +420,51 @@ FPNGB_API int fpngb_decode_packed_resized_device(const void* d_base, size_t base
                                                  void* d_out, size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride,
                                                  size_t out_chan_stride, uint32_t* d_info /* n*6 or NULL */, int32_t* d_status, void* stream);
 
+/* ---- general PNG files (any writer) in the packed ragged and resized decodes ---------------------------------------------------
+ * The fpng decode reads only files fpng wrote; every other PNG gets FPNGB_DECODE_NOT_FPNG.  The calls below also decode, on the GPU,
+ * the PNGs image datasets hold: 8-bit, non-interlaced gray, gray+alpha, RGB and RGBA, from any zlib stream, any mix of the five row
+ * filters.  Files the fpng walk accepts take the fpng kernels unchanged; files it rejects with FPNGB_DECODE_NOT_FPNG go to the
+ * general walk (the "general files"):
+ *   * signature, IHDR length and CRC, the dimension limits, chunk framing and ancillary-chunk CRCs as the fpng walk;
+ *   * IHDR must say bit depth 8, color type 0 / 2 / 4 / 6, compression 0, filter method 0, interlace 0, else
+ *     FPNGB_DECODE_UNSUPPORTED_PNG (palette, 16-bit, sub-byte depths, Adam7): route such files to a host decoder;
+ *   * FPNGB_DECODE_UNSUPPORTED_PNG also for a critical chunk other than IHDR / PLTE / IDAT / IEND, a second IHDR, a PLTE in a gray
+ *     file and a tRNS chunk in a color type 0 or 2 file (whatever desired_chans is); a PLTE in an RGB / RGBA file and every other
+ *     ancillary chunk are ignored;
+ *   * the IDAT chunks must be consecutive (FPNGB_DECODE_FAILED_CHUNK_PARSING); zero-length ones are legal; no IDAT or fewer than 2
+ *     data bytes in all: FPNGB_DECODE_FAILED_INVALID_IDAT.
+ *   Info row of a general file: {0, w, h, chans (1 gray, 2 gray+alpha, 3, 4), offset of the first IDAT chunk, sum of the IDAT data
+ *   lengths}.  fpng-written files keep fpngb_get_info_ex's row.
+ * Stream of a general file (the IDAT payloads concatenated): the zlib header must have CM 8, CINFO <= 7, a correct FCHECK and no
+ *   preset dictionary, the Deflate data must be accepted by zlib's inflate up to the end of its final block, inflate to exactly
+ *   h * (1 + w * chans) bytes, and every row's filter byte must be <= 4; anything else gives FPNGB_DECODE_FAILED_INVALID_IDAT.
+ *   Bytes after the final block are read only with verify on: then, in this order, a bad CRC on any IDAT chunk gives
+ *   FPNGB_DECODE_FAILED_HEADER_CRC32 (before any stream check) and a missing or wrong Adler-32 FPNGB_DECODE_ADLER_MISMATCH.
+ * Channels: gray Y -> (Y, Y, Y[, 255]); gray+alpha -> (Y, Y, Y[, A]); RGB -> alpha 255 when desired is 4; RGBA -> alpha dropped
+ *   when desired is 3 (PIL's convert("RGB") / convert("RGBA")).  Typed output as for fpng files.
+ * A file with an fdEC chunk that the fpng walk accepts but whose stream breaks the fpng rules keeps FPNGB_DECODE_NOT_FPNG.
+ *
+ * fpngb_decode_packed_png_device: fpngb_decode_packed_ragged_device (fmt NULL) or its _typed twin (fmt not NULL) with general files
+ *   decoded too.  Same arguments, placement (a general file takes align_up(w*h*desired_chans*elem, 16) bytes, tight HWC rows),
+ *   statuses and workspace rules; the workspace also holds each general file's gathered IDAT bytes (at most base_bytes + 16 n for
+ *   files that do not overlap) and its inflated rows (inside the delta-row bound).  Three launches more than the ragged call: 14
+ *   (16 with verify on).  Stream-ordered, no host synchronisation.
+ * fpngb_decode_packed_resized_device with flags & FPNGB_RESIZE_ANY_PNG: the same for the resized call (15 launches, 17 verified);
+ *   the crop boxes are checked against the general files' w and h.
+ * fpngb_get_info_batch_device with the general rules: fpngb_get_png_info_batch_device (one launch).
+ * fpngb_get_png_info: the same walk on the host (arguments as fpngb_get_info_ex). */
+enum { FPNGB_DECODE_UNSUPPORTED_PNG = 104 };  /* any-PNG decode: a well-formed PNG this decoder does not read (palette, 16-bit, ...) */
+enum { FPNGB_RESIZE_ANY_PNG = 4 };   /* bit 2: flags 2 stays an unknown bit, rejected as before */
+FPNGB_API int fpngb_decode_packed_png_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
+                                             uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans,
+                                             void* d_out, size_t out_cap, uint64_t* d_out_offsets /* n+1 */,
+                                             uint32_t* d_info /* n*6 or NULL */, const fpngb_pixel_format* fmt /* NULL = uint8 */,
+                                             int32_t* d_status, void* stream);
+FPNGB_API int fpngb_get_png_info_batch_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                              uint32_t* d_info, void* stream);
+FPNGB_API int fpngb_get_png_info(const void* file, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs,
+                                 uint32_t* idat_len);
+
 /* ---- typed encode input: float32 / float16 / bfloat16 pixels with a per-channel scale and bias, rounded to 8 bits ------------
  * The *_typed encode calls take the input as elements x of T (fmt->dtype: float32, float16 or bfloat16) and encode, for channel c,
  * the uint8 value
