@@ -87,6 +87,15 @@ def lib() -> C.CDLL:
     L.fpngb_get_png_info_batch_device.argtypes = L.fpngb_get_info_batch_device.argtypes
     L.fpngb_get_png_info.restype = C.c_int
     L.fpngb_get_png_info.argtypes = L.fpngb_get_info_ex.argtypes
+    L.fpngb_decode_packed_png_device_ex.restype = C.c_int
+    L.fpngb_decode_packed_png_device_ex.argtypes = L.fpngb_decode_packed_ragged_device.argtypes[:-2] + [C.c_uint32, C.POINTER(PixelFormat),
+                                                                                                     C.c_void_p, C.c_void_p]
+    L.fpngb_get_png_info_batch_device_ex.restype = C.c_int
+    L.fpngb_get_png_info_batch_device_ex.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
+    L.fpngb_get_png_info_ex.restype = C.c_int
+    L.fpngb_get_png_info_ex.argtypes = L.fpngb_get_info_ex.argtypes[:2] + [C.c_uint32] + L.fpngb_get_info_ex.argtypes[2:]
+    L.fpngb_debug_png_raw_len.restype = C.c_uint64
+    L.fpngb_debug_png_raw_len.argtypes = [C.c_uint32] * 4
     L.fpngb_decode_packed_resized_device.restype = C.c_int
     L.fpngb_decode_packed_resized_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p] + [C.c_uint32] * 4 + \
         [C.c_size_t, C.c_void_p] + [C.c_uint32] * 4 + [C.POINTER(PixelFormat), C.c_void_p] + [C.c_size_t] * 4 + [C.c_void_p] * 3

@@ -413,17 +413,25 @@ def get_info_ex(data):
 
 
 FPNGB_DECODE_UNSUPPORTED_PNG = 104   # any_png decodes: a well-formed PNG the GPU decoder does not read (palette, 16-bit, Adam7, tRNS)
+FPNGB_PNG_ALL_FORMATS = 1            # all_formats=True: palette, 1/2/4/16-bit, color-keyed and Adam7 files decode too
 
 
-def get_png_info(data):
+def get_png_info(data, all_formats=False):
     """get_info_ex with the general-PNG rules of the any_png decodes: fpng files give get_info_ex's row, files the fpng walk
     rejects with FPNG_DECODE_NOT_FPNG are walked again as general PNGs (include/fpng_b200.h): status 0 with the file's own
     channel count (1 gray, 2 gray+alpha, 3, 4), the offset of the first IDAT chunk and the sum of the IDAT data lengths, or
-    FPNGB_DECODE_UNSUPPORTED_PNG / a walk error."""
+    FPNGB_DECODE_UNSUPPORTED_PNG / a walk error.  all_formats=True applies the walk rules of FPNGB_PNG_ALL_FORMATS: palette,
+    1/2/4/16-bit, tRNS and Adam7 files pass too (chans: palette 3, a tRNS chunk in gray / RGB / palette files adds alpha)."""
     a = _u8(data)
     w, h, c, o, l = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32()
-    st = lib().fpngb_get_png_info(a.ctypes.data_as(C.c_void_p), a.size, C.byref(w), C.byref(h), C.byref(c), C.byref(o), C.byref(l))
+    st = lib().fpngb_get_png_info_ex(a.ctypes.data_as(C.c_void_p), a.size, FPNGB_PNG_ALL_FORMATS if all_formats else 0, C.byref(w),
+                                     C.byref(h), C.byref(c), C.byref(o), C.byref(l))
     return st, w.value, h.value, c.value, o.value, l.value
+
+
+def _all_formats_check(any_png, all_formats, fn):
+    if all_formats and not any_png:
+        raise ValueError(f"{fn}: all_formats=True needs any_png=True")
 
 
 def pack_files_for_device(files, device=None):
@@ -498,21 +506,27 @@ def _packed_args(data, offsets, sizes):
     return n
 
 
-def get_info_batch_device(data, offsets, sizes, stream=None, any_png=False):
+def get_info_batch_device(data, offsets, sizes, stream=None, any_png=False, all_formats=False):
     """Container walk on the device of the files packed in `data` (file i: sizes[i] bytes at offsets[i]) -- the layout of
     dist.compact and of the gather window.  data: flat uint8 CUDA tensor, offsets: int64 CUDA tensor (>= n entries),
     sizes: int32 CUDA tensor [n] (uint32 values; 0 = no file).  Returns an int32 CUDA tensor [n, 6]: per file
-    (status, w, h, chans, idat_ofs, idat_len) as get_info_ex (any_png: as get_png_info).  Enqueued on the current torch stream
-    (or `stream`); no host synchronisation."""
+    (status, w, h, chans, idat_ofs, idat_len) as get_info_ex (any_png: as get_png_info, with all_formats as get_png_info's).
+    Enqueued on the current torch stream (or `stream`); no host synchronisation."""
     import torch
 
+    _all_formats_check(any_png, all_formats, "get_info_batch_device")
     n = _packed_args(data, offsets, sizes)
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
     if n == 0:
         return info
     s = _stream(stream, data.device)
-    fn = lib().fpngb_get_png_info_batch_device if any_png else lib().fpngb_get_info_batch_device
-    check(fn(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, info.data_ptr(), s), "get_info_batch_device")
+    if all_formats:
+        rc = lib().fpngb_get_png_info_batch_device_ex(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, FPNGB_PNG_ALL_FORMATS,
+                                                      info.data_ptr(), s)
+    else:
+        fn = lib().fpngb_get_png_info_batch_device if any_png else lib().fpngb_get_info_batch_device
+        rc = fn(data.data_ptr(), offsets.data_ptr(), sizes.data_ptr(), n, info.data_ptr(), s)
+    check(rc, "get_info_batch_device")
     return info
 
 
@@ -552,13 +566,14 @@ def decode_packed_device(data, offsets, sizes, w: int, h: int, chans_in_file: in
 FPNGB_DECODE_OUT_OF_SPACE = 101    # decode_packed_ragged_device only: the file's pixels do not fit in `out`
 
 
-def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h, stream, element_size=1, any_png=False):
+def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h, stream, element_size=1, any_png=False,
+                   all_formats=False):
     """The bounds of decode_packed_ragged_device the caller left out, and the exact output size in bytes they give for elements
     of element_size bytes: one device walk (get_info_batch_device) and one read-back of (info, sizes, offsets), which
     synchronises with the stream."""
     import torch
 
-    info = get_info_batch_device(data, offsets, sizes, stream, any_png=any_png)
+    info = get_info_batch_device(data, offsets, sizes, stream, any_png=any_png, all_formats=all_formats)
     if stream is not None:
         torch.cuda.ExternalStream(stream, device=data.device).synchronize()
     t = torch.cat([info.long(), (sizes.long() & 0xFFFFFFFF)[:, None], offsets[:n, None]], 1).cpu().numpy()
@@ -578,7 +593,7 @@ def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max
 
 
 def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out=None, max_file_size=None, max_w=None, max_h=None,
-                                stream=None, dtype=None, scale=None, bias=None, any_png=False):
+                                stream=None, dtype=None, scale=None, bias=None, any_png=False, all_formats=False):
     """Decode fpng files of ANY shapes and channel counts packed in device memory (the layout of get_info_batch_device; base_bytes
     is data.numel()) in one call, pixels placed back to back.  Returns (out uint8 [out_cap], out_offsets int64 [n + 1],
     info int32 [n, 6], status int32 [n]):
@@ -597,9 +612,13 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     align_up(h*w*desired_channels*element_size, 16) bytes, and out_offsets stay in bytes (ragged_views converts them).
     any_png=True also decodes, on the GPU, the 8-bit non-interlaced gray, gray+alpha, RGB and RGBA PNGs of any other writer
     (fpngb_decode_packed_png_device): their info rows are get_png_info's, their statuses 0, FPNGB_DECODE_UNSUPPORTED_PNG, a walk
-    error or FPNG_DECODE_FAILED_INVALID_IDAT for a bad stream; fpng files decode exactly as without it."""
+    error or FPNG_DECODE_FAILED_INVALID_IDAT for a bad stream; fpng files decode exactly as without it.
+    all_formats=True (with any_png=True, else ValueError) also decodes palette, 1/2/4-bit gray, 16-bit, color-keyed (tRNS) and
+    Adam7-interlaced files (FPNGB_PNG_ALL_FORMATS; pixel rules in include/fpng_b200.h): sub-byte gray scaled to 0..255, 16-bit
+    samples as their high byte (typed output: s / 257), palette entries with tRNS alpha, a color key as alpha 0."""
     import torch
 
+    _all_formats_check(any_png, all_formats, "decode_packed_ragged_device")
     n = _packed_args(data, offsets, sizes)
     assert desired_channels in (3, 4), "desired_channels: 3 or 4"
     odt = _out_dtype(out, dtype)
@@ -607,7 +626,7 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     es = torch.empty((), dtype=odt).element_size()
     if out is None or max_file_size is None or max_w is None or max_h is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
-                                                             stream, es, any_png)
+                                                             stream, es, any_png, all_formats)
         if out is None:
             out = torch.empty((max(total, 16) // es,), dtype=odt, device=data.device)[:total // es]
     _check_arg(out, "out", data.device, odt)
@@ -617,7 +636,10 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     s = _stream(stream, data.device)
     args = (data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
             int(max_h), desired_channels, out.data_ptr(), out.numel() * es, out_offsets.data_ptr(), info.data_ptr())
-    if any_png:
+    if all_formats:
+        rc = lib().fpngb_decode_packed_png_device_ex(*args, FPNGB_PNG_ALL_FORMATS, None if fmt is None else C.byref(fmt),
+                                                     status.data_ptr(), s)
+    elif any_png:
         rc = lib().fpngb_decode_packed_png_device(*args, None if fmt is None else C.byref(fmt), status.data_ptr(), s)
     elif fmt is None:
         rc = lib().fpngb_decode_packed_ragged_device(*args, status.data_ptr(), s)
@@ -648,11 +670,12 @@ def ragged_views(out, out_offsets, info, status, desired_channels: int):
 FPNGB_DECODE_BAD_CROP = 103        # decode_packed_resized_device only: the file's crop box is empty or not inside the image
 FPNGB_RESIZE_ANTIALIAS = 1
 FPNGB_RESIZE_ANY_PNG = 4
+FPNGB_RESIZE_ALL_PNG_FORMATS = 8
 
 
 def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: int, boxes=None, antialias=True, out=None, dtype=None,
                                  scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None,
-                                 any_png=False):
+                                 any_png=False, all_formats=False):
     """Decode fpng files of ANY shapes packed in device memory (the layout of decode_packed_ragged_device) into one batch of a fixed
     size = (H, W): file i is cropped to boxes[i] and resized with F.interpolate's bilinear rule (align_corners=False, antialias as
     given) on the GPU, then stored as decode_batch_device stores its pixels (uint8, rounded half to even and clamped, or dtype with
@@ -667,9 +690,12 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     With max_file_size, max_w, max_h and pixel_cap all given, the call is stream-ordered: no host synchronisation.  Any of them
     that is None is computed by decode_packed_ragged_device's rule: one get_info_batch_device and one read-back to the host, which
     waits for the stream; pixel_cap then becomes the exact size of the decodable files.
-    any_png=True decodes general PNGs too, as decode_packed_ragged_device(any_png=True) does (FPNGB_RESIZE_ANY_PNG)."""
+    any_png=True decodes general PNGs too, as decode_packed_ragged_device(any_png=True) does (FPNGB_RESIZE_ANY_PNG), and
+    all_formats=True (with any_png=True, else ValueError) every PNG format as there (FPNGB_RESIZE_ALL_PNG_FORMATS); the resize
+    reads the uint8 values, so a 16-bit file is resized from its high bytes."""
     import torch
 
+    _all_formats_check(any_png, all_formats, "decode_packed_resized_device")
     if desired_channels not in (3, 4):
         raise ValueError(f"decode_packed_resized_device: desired_channels {desired_channels}: 3 or 4")
     H, W = (int(v) for v in size)
@@ -690,7 +716,7 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     _check_arg(out, "out", data.device, odt, n * H * W * desired_channels, view=True)
     if max_file_size is None or max_w is None or max_h is None or pixel_cap is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
-                                                             stream, any_png=any_png)
+                                                             stream, any_png=any_png, all_formats=all_formats)
         if pixel_cap is None:
             pixel_cap = total
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
@@ -698,7 +724,8 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     rc = lib().fpngb_decode_packed_resized_device(
         data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
         int(max_h), int(pixel_cap), None if boxes is None else boxes.data_ptr(), W, H, desired_channels,
-        (FPNGB_RESIZE_ANTIALIAS if antialias else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0), None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape),
+        (FPNGB_RESIZE_ANTIALIAS if antialias else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
+        (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0), None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape),
         info.data_ptr(), status.data_ptr(), _stream(stream, data.device))
     check(rc, "decode_packed_resized_device")
     return out, info, status

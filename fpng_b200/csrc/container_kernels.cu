@@ -32,10 +32,11 @@ struct DeviceCrc {
     }
 };
 
-// kAny (the any-PNG calls): files container_walk rejects with FPNGB_DECODE_NOT_FPNG are walked again by png_walk; a general file that
-// passes every check of the call gets pre_status kPngPending and, with png != nullptr, its PngDesc (decode.cuh)
+// kAny (the any-PNG calls): files container_walk rejects with FPNGB_DECODE_NOT_FPNG are walked again by png_walk (with `flags`); a
+// general file that passes every check of the call gets pre_status kPngPending (kPngPendingExt for the files png_walk marks ext)
+// and, with png != nullptr, its PngDesc (decode.cuh)
 template <bool kAny>
-__global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDesc* png)
+__global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDesc* png, uint32_t flags)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n) return;
@@ -47,8 +48,9 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDe
     const bool bad_arg = !size || (p.files && (size > p.max_file_size || (ofs & 3ull) || (ragged && (ofs > p.base_bytes || size > p.base_bytes - ofs))));
     uint32_t st, w = 0, h = 0, c = 0, io = 0, il = 0;
     bool general = false;
+    PngFormat fm{};
     if (!size || (ragged && bad_arg)) st = FPNGB_DECODE_INVALID_ARG;
-    else if (kAny) st = any_png_walk(p.base + ofs, size, DeviceCrc{}, &w, &h, &c, &io, &il, &general);
+    else if (kAny) st = any_png_walk(p.base + ofs, size, DeviceCrc{}, flags, &w, &h, &c, &io, &il, &general, &fm);
     else st = container_walk(p.base + ofs, size, DeviceCrc{}, &w, &h, &c, &io, &il);
     if (p.info) {
         uint32_t* o = p.info + (size_t)i * 6;
@@ -67,7 +69,12 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDe
             }
         } else if (!pre && (w != p.w || h != p.h || c != p.chans)) pre = FPNGB_DECODE_SHAPE_MISMATCH;
         if (kAny && !pre && general) pre = kPngPending;
-        if (kAny && png) png[i] = PngDesc{0ull, pre == kPngPending ? il : 0u, 0u};
+        if (kAny && png) {
+            const bool ok = pre == kPngPending, ext = ok && fm.ext;
+            png[i] = ext ? PngDesc{0ull, il, 0u, fm.raw_len, fm.depth, fm.type, fm.interlace, fm.plte_ofs, fm.plte_n, fm.trns_ofs,
+                                   fm.trns_len, 0u}
+                         : PngDesc{0ull, ok ? il : 0u, 0u};
+        }
         if (kAny && pre == kPngPending) pre = 0;                                // placed as any file; marked again below
         FileDesc fd;
         fd.base = ofs; fd.file_size = size; fd.idat_ofs = pre ? 0u : io; fd.idat_len = pre ? 0u : il; fd.pre_status = pre;
@@ -79,23 +86,23 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDe
             fd.delta_base = (unsigned long long)i * fd.pitch * p.h; fd.out_base = i * p.out_stride;
             fd.sub_base = (unsigned long long)i * subs_for(p.max_file_size);
         }
-        if (kAny && general && !pre) fd.pre_status = kPngPending;
+        if (kAny && general && !pre) fd.pre_status = fm.ext ? kPngPendingExt : kPngPending;
         p.files[i] = fd;
     }
 }
 
 void launch_container_walk(const WalkParams& p, cudaStream_t s)
 {
-    container_walk_kernel<false><<<(p.n + 127) / 128, 128, 0, s>>>(p, nullptr);
+    container_walk_kernel<false><<<(p.n + 127) / 128, 128, 0, s>>>(p, nullptr, 0u);
 }
-void launch_container_walk_any(const WalkParams& p, PngDesc* png, cudaStream_t s)
+void launch_container_walk_any(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s)
 {
-    container_walk_kernel<true><<<(p.n + 127) / 128, 128, 0, s>>>(p, png);
+    container_walk_kernel<true><<<(p.n + 127) / 128, 128, 0, s>>>(p, png, flags);
 }
 
 // One CTA: exclusive scans of the output bytes, delta bytes and records of the accepted files, kPlaceThreads files per round.
-// kAny: general files (pre_status kPngPending) are placed too, with their inflated rows in the delta bytes, no records, and a
-// fourth scan of their gathered zlib bytes (z_cap).
+// kAny: general files (pre_status kPngPending or kPngPendingExt) are placed too, with their inflated rows in the delta bytes (an
+// ext file's PngDesc::raw_len), no records, and a fourth scan of their gathered zlib bytes (z_cap).
 constexpr uint32_t kPlaceThreads = 1024;
 template <bool kAny>
 __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams p, PngDesc* png, unsigned long long z_cap)
@@ -109,14 +116,16 @@ __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams
         const uint32_t i = first + tid;
         FileDesc fd{};
         bool placed = false, general = false;
-        if (i < p.n) { fd = p.files[i]; general = kAny && fd.pre_status == kPngPending; placed = fd.pre_status == 0 || general; }
+        if (i < p.n) { fd = p.files[i]; general = kAny && png_pending(fd.pre_status); placed = fd.pre_status == 0 || general; }
         unsigned long long v[K];
 #pragma unroll
         for (int k = 0; k < K; k++) v[k] = 0ull;
         if (placed) {
             v[0] = ((unsigned long long)fd.w * fd.h * p.px_bytes + 15ull) & ~15ull;
             if (general) {
-                v[1] = ((unsigned long long)fd.h * (1ull + (unsigned long long)fd.w * fd.chans) + 15ull) & ~15ull;
+                const unsigned long long raw = fd.pre_status == kPngPendingExt ? png[i].raw_len
+                                                                               : (unsigned long long)fd.h * (1ull + (unsigned long long)fd.w * fd.chans);
+                v[1] = (raw + 15ull) & ~15ull;
                 v[K - 1] = ((unsigned long long)png[i].zlen + 15ull) & ~15ull;
             } else {
                 v[1] = (unsigned long long)fd.h * fd.pitch;

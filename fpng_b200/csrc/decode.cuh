@@ -142,12 +142,24 @@ void launch_decode_place(const PlaceParams& p, cudaStream_t s);
 // final status.  decode_place_kernel<true> places general files like any file (align_up(w*h*px_bytes, 16) output bytes), takes
 // align_up(h * (1 + w*chans), 16) delta bytes for the inflated rows (FileDesc::delta_base) and no records, and allots the gathered
 // IDAT bytes (PngDesc::zofs) from a fourth scan bounded by z_cap.
+// With FPNGB_PNG_ALL_FORMATS the files png_unfilter_kernel does not read (palette, depth != 8, a color key, Adam7: the "ext" files)
+// get kPngPendingExt instead: gather, inflate and place take both markers, png_unfilter_kernel skips them, and png_unfilter_ext_kernel
+// writes their final status.  An ext file's inflated bytes are PngDesc::raw_len (delta bytes align_up(raw_len, 16)).
 constexpr uint32_t kPngPending = 0x7FFFFFF0u;
+constexpr uint32_t kPngPendingExt = 0x7FFFFFF1u;
+__host__ __device__ __forceinline__ bool png_pending(uint32_t pre) { return pre == kPngPending || pre == kPngPendingExt; }
 struct PngDesc {
     unsigned long long zofs;                // byte offset of the file's gathered zlib stream from PngParams::z (a multiple of 16)
     uint32_t zlen;                          // its length: the sum of the IDAT data lengths
     uint32_t status;                        // 0 until the gather (4) or inflate (8, 102) kernels find an error
+    // ext files only (png_walk.cuh's PngFormat; 0 for the others)
+    unsigned long long raw_len;             // inflated bytes, every Adam7 pass and filter byte included
+    uint32_t depth, type, interlace;        // IHDR bit depth, color type, interlace method
+    uint32_t plte_ofs, plte_n;              // PLTE data: offset from the file's first byte, entries
+    uint32_t trns_ofs, trns_len;            // tRNS data: offset from the file's first byte (0: none), bytes
+    uint32_t pad_;
 };
+static_assert(sizeof(PngDesc) == 56, "PngDesc");
 struct PngParams {
     const uint8_t* d_files; const FileDesc* files; PngDesc* png;
     uint8_t* z;                             // gathered zlib streams
@@ -155,11 +167,13 @@ struct PngParams {
     uint8_t* d_out; uint32_t* d_status;     // pixels as the ragged decode places them (tight HWC rows at d_out + files[f].out_base)
     uint32_t n, desired, verify;
 };
-// container_walk_kernel<true> (png != nullptr only with files != nullptr) and decode_place_kernel<true>, z_cap the gathered bytes
-void launch_container_walk_any(const WalkParams& p, PngDesc* png, cudaStream_t s);
+// container_walk_kernel<true> (png != nullptr only with files != nullptr; flags: png_walk's) and decode_place_kernel<true>, z_cap
+// the gathered bytes
+void launch_container_walk_any(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s);
 void launch_decode_place_any(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s);
-// gather, inflate and unfilter of the general files (three launches; grids from n alone), behind launch_decode
-void launch_png_decode(const PngParams& p, const TypedOut* typed, cudaStream_t s);
+// gather, inflate and unfilter of the general files (three launches, four with FPNGB_PNG_ALL_FORMATS in flags; grids from n alone),
+// behind launch_decode
+void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags, cudaStream_t s);
 
 // decode_resize_kernel (decode_resize_kernels.cu), resized call: after the ragged pipeline has decoded every file into tight uint8
 // HWC rows (pitch w * desired) at px + px_offsets[f], crops file f to its box and resizes it to out_h x out_w with the bilinear

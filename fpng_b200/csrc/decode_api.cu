@@ -208,18 +208,26 @@ static int decode_packed_device_impl(const void* d_base, const uint64_t* d_offse
 //              the same bound from out_cap; from the shape, h * (delta_pitch(w, 4) + 16) per file.  Its gathered stream takes
 //              align_up(zlen, 16) bytes, zlen < its size: at most base_bytes + 16n for files that do not overlap, and
 //              align_up(max_file_size, 16) each.
+//   all formats (FPNGB_PNG_ALL_FORMATS): an ext file of b <= 64 bits per pixel inflates to the rows of its passes, each of
+//              1 + ceil(pw*b/8) bytes.  For b >= 8 the data bytes of all rows sum to w*h*b/8 <= 8wh; for b < 8 a row holds at most
+//              pw bytes, so at most wh in all.  One filter byte per pass row: interlace 0 has h rows; Adam7's seven passes have
+//              ceil(h/8) + ceil(h/8) + ceil((h-4)/8) + ceil(h/4) + ceil((h-2)/4) + ceil(h/2) + ceil((h-1)/2) <= 15h/8 + 6 rows, the
+//              "2h + 6" Adam7 adds.  So align_up(raw_len, 16) <= 8wh + 2h + 21 <= 8wh + 32h (h >= 1): the bound from out_cap is
+//              out_cap*8/desired + 32 * min(rows, rows_px), and from the shape h * (8w + 32) per file.  Both also bound the 8-bit
+//              general and fpng files (4wh + 16h, and h * (delta_pitch(w, 4) + 16) <= h * (8w + 32)).  Flag off: the bounds above.
 // A file whose range still ends past a bound (overlapping files) gets FPNGB_DECODE_OUT_OF_SPACE from decode_place_kernel.
 static unsigned long long sat_u64(unsigned __int128 v) { return v > ~0ull ? ~0ull : (unsigned long long)v; }
 static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired,
-                             size_t out_cap, bool any_png, unsigned long long& sub_cap, unsigned long long& delta_cap,
-                             unsigned long long& z_cap)
+                             size_t out_cap, bool any_png, bool all_formats, unsigned long long& sub_cap,
+                             unsigned long long& delta_cap, unsigned long long& z_cap)
 {
     typedef unsigned __int128 u128;
     const u128 by_bytes = (u128)base_bytes / 128 + 3 * (u128)n, by_max = (u128)n * subs_for(max_file_size);
     sub_cap = sat_u64(by_bytes < by_max ? by_bytes : by_max);
     const u128 rows = (u128)n * max_h, rows_px = ((u128)out_cap + desired - 1) / desired;
-    const u128 by_out = ((u128)out_cap * 4 + desired - 1) / desired + 16 * (rows < rows_px ? rows : rows_px);
-    const u128 by_shape = rows * (delta_pitch(max_w, 4) + (any_png ? 16u : 0u));
+    const u128 px_bytes = all_formats ? 8 : 4, row_bytes = all_formats ? 32 : 16;
+    const u128 by_out = ((u128)out_cap * px_bytes + desired - 1) / desired + row_bytes * (rows < rows_px ? rows : rows_px);
+    const u128 by_shape = rows * (all_formats ? 8 * (u128)max_w + 32 : (u128)(delta_pitch(max_w, 4) + (any_png ? 16u : 0u)));
     delta_cap = sat_u64(by_out < by_shape ? by_out : by_shape);
     const u128 z_bytes = (u128)base_bytes + 16 * (u128)n, z_max = (u128)n * align_up((size_t)max_file_size, 16);
     z_cap = any_png ? sat_u64(z_bytes < z_max ? z_bytes : z_max) : 0ull;
@@ -234,11 +242,13 @@ struct ResizeOut {
 // The ragged pipeline: walk, place, decode.  With rz (the resized call), the uint8 pixels and their offsets go to the decode
 // workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes, and the
 // resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
-// general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc).
+// general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc); png_flags: png_walk's flags
+// (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel).
 static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
-                                     int32_t* d_status, void* stream, const ResizeOut* rz = nullptr, bool any_png = false)
+                                     int32_t* d_status, void* stream, const ResizeOut* rz = nullptr, bool any_png = false,
+                                     uint32_t png_flags = 0)
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
@@ -251,7 +261,9 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     if ((uintptr_t)d_base % 4 || (!rz && (uintptr_t)d_out % 16)) return FPNGB_ERR_ALIGNMENT;
     unsigned long long sub_cap = 0, delta_cap = 0, z_cap = 0;
     // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
-    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, any_png, sub_cap, delta_cap, z_cap);
+    const bool all_formats = any_png && (png_flags & FPNGB_PNG_ALL_FORMATS);
+    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, any_png, all_formats, sub_cap, delta_cap,
+                     z_cap);
     if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2 || (rz && out_cap > SIZE_MAX / 2) || z_cap > SIZE_MAX / 4)
         return FPNGB_ERR_BUFFER_TOO_SMALL;
     const size_t png_desc_bytes = any_png ? align_up((size_t)n * sizeof(PngDesc), 256) : 0;
@@ -272,7 +284,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
     wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr;
-    if (any_png) launch_container_walk_any(wp, (PngDesc*)png, s);
+    if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags, s);
     else launch_container_walk(wp, s);
     PlaceParams pp{};
     pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem;
@@ -285,7 +297,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         PngParams q{};
         q.d_files = (const uint8_t*)d_base; q.files = p.files; q.png = (PngDesc*)png; q.z = png + png_desc_bytes; q.rows = p.delta;
         q.d_out = (uint8_t*)d_out; q.d_status = (uint32_t*)d_status; q.n = n; q.desired = desired_chans; q.verify = verify != nullptr;
-        launch_png_decode(q, typed ? &t : nullptr, s);
+        launch_png_decode(q, typed ? &t : nullptr, png_flags, s);
     }
     if (rz) {
         ResizeParams rp{};
@@ -296,7 +308,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         launch_decode_resize(rp, rz->t, n, desired_chans, s);
         decode_profile_mark_resize(s);
     }
-    count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0));
+    count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0) + (all_formats ? 1 : 0));
     FPNGB_CUDA_OK(cudaGetLastError());
     return context().ws_release(s);
 }
@@ -565,7 +577,9 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
 {
     if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (!d_out || n == 0 || n > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
-        (desired_chans != 3 && desired_chans != 4) || (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG)))
+        (desired_chans != 3 && desired_chans != 4) ||
+        (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS)) ||
+        ((flags & FPNGB_RESIZE_ALL_PNG_FORMATS) && !(flags & FPNGB_RESIZE_ANY_PNG)))
         return FPNGB_ERR_INVALID_ARG;
     ResizeOut rz{};
     rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
@@ -575,7 +589,18 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
                       rz.out);
     if (rc) return rc;
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
-                                     nullptr, d_info, false, nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0);
+                                     nullptr, d_info, false, nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
+                                     (flags & FPNGB_RESIZE_ALL_PNG_FORMATS) ? (uint32_t)FPNGB_PNG_ALL_FORMATS : 0u);
+}
+
+int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
+                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, uint32_t flags,
+                                      const fpngb_pixel_format* fmt, int32_t* d_status, void* stream)
+{
+    if (flags & ~(uint32_t)FPNGB_PNG_ALL_FORMATS) return context().ready ? FPNGB_ERR_INVALID_ARG : FPNGB_ERR_NOT_INITIALIZED;
+    return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
+                                     d_out_offsets, d_info, fmt != nullptr, fmt, d_status, stream, nullptr, true, flags);
 }
 
 int fpngb_decode_packed_png_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
@@ -583,31 +608,49 @@ int fpngb_decode_packed_png_device(const void* d_base, size_t base_bytes, const 
                                    size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, const fpngb_pixel_format* fmt,
                                    int32_t* d_status, void* stream)
 {
-    return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
-                                     d_out_offsets, d_info, fmt != nullptr, fmt, d_status, stream, nullptr, true);
+    return fpngb_decode_packed_png_device_ex(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out,
+                                             out_cap, d_out_offsets, d_info, 0u, fmt, d_status, stream);
 }
 
-int fpngb_get_png_info_batch_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t* d_info,
-                                    void* stream)
+int fpngb_get_png_info_batch_device_ex(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t flags,
+                                       uint32_t* d_info, void* stream)
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (!d_base || !d_offsets || !d_sizes || !d_info || n == 0) return FPNGB_ERR_INVALID_ARG;
+    if (!d_base || !d_offsets || !d_sizes || !d_info || n == 0 || (flags & ~(uint32_t)FPNGB_PNG_ALL_FORMATS)) return FPNGB_ERR_INVALID_ARG;
     WalkParams p{};
     p.base = (const uint8_t*)d_base; p.offsets = (const unsigned long long*)d_offsets; p.sizes = d_sizes; p.n = n; p.info = d_info;
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    launch_container_walk_any(p, nullptr, (cudaStream_t)stream);
+    launch_container_walk_any(p, nullptr, flags, (cudaStream_t)stream);
     count_launch(1);
     FPNGB_CUDA_OK(cudaGetLastError());
     return FPNGB_OK;
 }
 
+int fpngb_get_png_info_batch_device(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n, uint32_t* d_info,
+                                    void* stream)
+{
+    return fpngb_get_png_info_batch_device_ex(d_base, d_offsets, d_sizes, n, 0u, d_info, stream);
+}
+
+int fpngb_get_png_info_ex(const void* file, uint32_t size, uint32_t flags, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs,
+                          uint32_t* idat_len)
+{
+    if (!file || !w || !h || !chans || !idat_ofs || !idat_len || (flags & ~(uint32_t)FPNGB_PNG_ALL_FORMATS)) return FPNGB_DECODE_INVALID_ARG;
+    bool general;
+    PngFormat fm;
+    return any_png_walk((const uint8_t*)file, size, HostCrc{}, flags, w, h, chans, idat_ofs, idat_len, &general, &fm);
+}
+
 int fpngb_get_png_info(const void* file, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs, uint32_t* idat_len)
 {
-    if (!file || !w || !h || !chans || !idat_ofs || !idat_len) return FPNGB_DECODE_INVALID_ARG;
-    bool general;
-    return any_png_walk((const uint8_t*)file, size, HostCrc{}, w, h, chans, idat_ofs, idat_len, &general);
+    return fpngb_get_png_info_ex(file, size, 0u, w, h, chans, idat_ofs, idat_len);
+}
+
+uint64_t fpngb_debug_png_raw_len(uint32_t w, uint32_t h, uint32_t bits_per_pixel, uint32_t interlace)
+{
+    return png_raw_len(w, h, bits_per_pixel, interlace);
 }
 
 }  // extern "C"

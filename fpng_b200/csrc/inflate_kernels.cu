@@ -14,7 +14,8 @@
 //   code with one code of length 1, or no distance codes), HLIT > 286, HDIST > 30, a repeat with no previous length or past the
 //   end, no end-of-block code, lit/len 286 / 287, distance 30 / 31, a distance before the start of the stream, a stored length
 //   whose complement does not match, block type 3, and input ending before the final block does: FAILED_INVALID_IDAT.  So are
-//   a bad zlib header, an inflated size other than h * (1 + w*chans) and a filter byte above 4.  With verify on the Adler-32 of the
+//   a bad zlib header, an inflated size other than h * (1 + w*chans) (PngDesc::raw_len for the ext files of FPNGB_PNG_ALL_FORMATS)
+//   and a filter byte above 4 (checked here for 8-bit files, by png_unfilter_ext_kernel for ext files).  With verify on the Adler-32 of the
 //   inflated bytes (per-lane sums and the closed form of decode_adler_kernel) is checked against the four bytes behind the final
 //   block: FPNGB_DECODE_ADLER_MISMATCH when they differ or are missing.
 #include "decode.cuh"
@@ -67,7 +68,7 @@ __global__ void __launch_bounds__(kGatherThreads) png_gather_kernel(PngParams p)
     __shared__ uint32_t s_red[kGatherThreads / 32];
     const uint32_t f = blockIdx.x, tid = threadIdx.x;
     const FileDesc fd = p.files[f];
-    if (fd.pre_status != kPngPending) return;                               // the same for the whole CTA
+    if (!png_pending(fd.pre_status)) return;                               // the same for the whole CTA
     if (p.verify) {
         for (uint32_t i = tid; i < 256 + 32; i += kGatherThreads) (&s_tab.byte[0])[i] = (&c_png_crc.byte[0])[i];
         __syncthreads();
@@ -227,13 +228,14 @@ __global__ void __launch_bounds__(32 * kInflateWarps) png_inflate_kernel(PngPara
     const uint32_t f = blockIdx.x * kInflateWarps + warp;
     if (f >= p.n) return;
     const FileDesc fd = p.files[f];
-    if (fd.pre_status != kPngPending) return;
+    if (!png_pending(fd.pre_status)) return;
+    const bool ext = fd.pre_status == kPngPendingExt;
     const PngDesc pd = p.png[f];
     if (pd.status) return;                                                  // a bad IDAT CRC (verify)
     InflateSmem& sm = s_all[warp];
     uint8_t* out = p.rows + fd.delta_base;
     const uint32_t stride = fd.w * fd.chans + 1u;
-    const unsigned long long N = (unsigned long long)fd.h * stride;
+    const unsigned long long N = ext ? pd.raw_len : (unsigned long long)fd.h * stride;
     BitReader br;
     br.z = reinterpret_cast<const uint32_t*>(p.z + pd.zofs); br.win = sm.win;
     br.zlen = pd.zlen; br.padded = (pd.zlen + 3u) & ~3u; br.pos = 0; br.bc = 0; br.bb = 0;
@@ -350,7 +352,7 @@ __global__ void __launch_bounds__(32 * kInflateWarps) png_inflate_kernel(PngPara
     }
     if (!err && (o != N || br.past())) err = true;
     __syncwarp();
-    if (!err) {                                                             // filter bytes
+    if (!err && !ext) {                                                     // filter bytes (ext files: png_unfilter_ext_kernel)
         bool bad = false;
         for (uint32_t y = lane; y < fd.h; y += 32) bad |= out[(size_t)y * stride] > 4;
         err = __any_sync(0xFFFFFFFFu, bad);

@@ -427,7 +427,8 @@ FPNGB_API int fpngb_decode_packed_resized_device(const void* d_base, size_t base
  * general walk (the "general files"):
  *   * signature, IHDR length and CRC, the dimension limits, chunk framing and ancillary-chunk CRCs as the fpng walk;
  *   * IHDR must say bit depth 8, color type 0 / 2 / 4 / 6, compression 0, filter method 0, interlace 0, else
- *     FPNGB_DECODE_UNSUPPORTED_PNG (palette, 16-bit, sub-byte depths, Adam7): route such files to a host decoder;
+ *     FPNGB_DECODE_UNSUPPORTED_PNG (palette, 16-bit, sub-byte depths, Adam7): route such files to a host decoder, or decode them
+ *     on the GPU too with FPNGB_PNG_ALL_FORMATS (below);
  *   * FPNGB_DECODE_UNSUPPORTED_PNG also for a critical chunk other than IHDR / PLTE / IDAT / IEND, a second IHDR, a PLTE in a gray
  *     file and a tRNS chunk in a color type 0 or 2 file (whatever desired_chans is); a PLTE in an RGB / RGBA file and every other
  *     ancillary chunk are ignored;
@@ -464,6 +465,62 @@ FPNGB_API int fpngb_get_png_info_batch_device(const void* d_base, const uint64_t
                                               uint32_t* d_info, void* stream);
 FPNGB_API int fpngb_get_png_info(const void* file, uint32_t size, uint32_t* w, uint32_t* h, uint32_t* chans, uint32_t* idat_ofs,
                                  uint32_t* idat_len);
+
+/* ---- every PNG format in the any-PNG decodes (opt-in: FPNGB_PNG_ALL_FORMATS, FPNGB_RESIZE_ALL_PNG_FORMATS) -----------------------
+ * With the flag the general walk also accepts palette, 1/2/4-bit gray, 16-bit, color-keyed (tRNS) and Adam7-interlaced files, and
+ * the decode calls decode them on the GPU.  Without it every call behaves as above, FPNGB_DECODE_UNSUPPORTED_PNG included.
+ * Walk rules with the flag (host and device):
+ *   * IHDR (color type: bit depths) 0: 1, 2, 4, 8, 16; 2: 8, 16; 3: 1, 2, 4, 8; 4: 8, 16; 6: 8, 16; interlace 0 or 1; compression
+ *     and filter method 0.  Any other IHDR: FPNGB_DECODE_UNSUPPORTED_PNG.
+ *   * PLTE: color type 3 needs exactly one, before the first IDAT, with a length that is a nonzero multiple of 3 and at most 768;
+ *     missing, empty, bad length, a second one or one after IDAT: FPNGB_DECODE_FAILED_CHUNK_PARSING.  In a gray file
+ *     FPNGB_DECODE_UNSUPPORTED_PNG, in an RGB / RGBA file ignored, as without the flag.
+ *   * tRNS: at most one, before the first IDAT, in color type 3 after PLTE; length 2 (type 0), 6 (type 2), at most the palette's
+ *     entry count (type 3); any violation: FPNGB_DECODE_FAILED_CHUNK_PARSING.  Ignored in types 4 and 6, as without the flag.
+ *   * Unknown critical chunks and a second IHDR: FPNGB_DECODE_UNSUPPORTED_PNG.  Framing, CRC and IDAT-run rules as above.
+ *   * Info row: {0, w, h, chans, idat_ofs, idat_len}, chans: gray 1 (2 with tRNS), gray+alpha 2, RGB 3 (4 with tRNS), RGBA 4,
+ *     palette 3 (4 with tRNS).  Files fpng wrote keep fpngb_get_info_ex's row and the fpng kernels.
+ *   * Inflated size: h * (1 + ceil(w * bits_per_pixel / 8)) without interlace; with Adam7 the sum of that expression over the 7
+ *     passes, skipping passes of width or height 0.  Any other size, or a filter byte above 4 in any row of any pass:
+ *     FPNGB_DECODE_FAILED_INVALID_IDAT.  With verify on the order of the checks is unchanged: 4, then 8, then 102.
+ * Pixel rules (the uint8 value of each output channel):
+ *   * gray below 8 bits: Y = s * 255 / (2^d - 1), i.e. s * 255, * 85 or * 17 for d = 1, 2, 4 (libpng's expand, PIL, stb_image);
+ *     the padding bits at the end of a row are ignored;
+ *   * 16-bit samples: the high byte, s >> 8 (PIL, stb_image, lodepng, libpng's strip_16);
+ *   * palette: index i < entry count gives PLTE[i], a larger index (0, 0, 0) (libpng, lodepng; no error); alpha tRNS[i] when i is
+ *     below the tRNS length, else 255;
+ *   * color key (tRNS in types 0 and 2): alpha 0 when the raw samples equal the key, else 255; the comparison uses full samples
+ *     (16 bits in 16-bit files), so a key with bits above the depth never matches;
+ *   * then the channel mapping above to desired_chans 3 / 4, applied to the expanded gray / gray+alpha / RGB / RGBA pixel;
+ *   * Adam7: every pass pixel lands at its full-image position.
+ * Typed output: T(v * scale[c] + bias[c]) as for 8-bit files, v the uint8 value above, except for a 16-bit sample (color or alpha):
+ *   there v = s / 257.0f, rounded to nearest (torch's s.float() / 257), so the 8-bit-calibrated normalize_scale_bias stays valid,
+ *   257 * k decodes to exactly k, and round(v * 257) == s in float32 for every s.  A color-key alpha and an added alpha are 0 or
+ *   255.
+ * The resized call resamples the uint8 values above: a 16-bit file is resized from its high bytes.
+ * Kernels: one more launch than the any-PNG call without the flag (a warp-per-file unfilter of these files): 15 for the ragged call
+ *   (17 with verify on), 16 for the resized call (18).  8-bit gray / gray+alpha / RGB / RGBA files without tRNS or Adam7 take the
+ *   kernels of the call without the flag and decode to the same bytes.
+ * fpngb_decode_packed_png_device_ex: fpngb_decode_packed_png_device with flags (0 or FPNGB_PNG_ALL_FORMATS; other bits:
+ *   FPNGB_ERR_INVALID_ARG).  fpngb_decode_packed_png_device is this call with flags 0.
+ * fpngb_decode_packed_resized_device: FPNGB_RESIZE_ALL_PNG_FORMATS is valid only together with FPNGB_RESIZE_ANY_PNG (alone:
+ *   FPNGB_ERR_INVALID_ARG).  Bit value 2 stays unknown.
+ * fpngb_get_png_info_batch_device_ex / fpngb_get_png_info_ex: the device and host walks with flags (unknown bits: the device call
+ *   returns FPNGB_ERR_INVALID_ARG, the host walk FPNGB_DECODE_INVALID_ARG, as for its other argument errors).  Without the _ex
+ *   they run with flags 0. */
+enum { FPNGB_PNG_ALL_FORMATS = 1 };
+enum { FPNGB_RESIZE_ALL_PNG_FORMATS = 8 };
+FPNGB_API int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
+                                                uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans,
+                                                void* d_out, size_t out_cap, uint64_t* d_out_offsets /* n+1 */,
+                                                uint32_t* d_info /* n*6 or NULL */, uint32_t flags,
+                                                const fpngb_pixel_format* fmt /* NULL = uint8 */, int32_t* d_status, void* stream);
+FPNGB_API int fpngb_get_png_info_batch_device_ex(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                                 uint32_t flags, uint32_t* d_info, void* stream);
+FPNGB_API int fpngb_get_png_info_ex(const void* file, uint32_t size, uint32_t flags, uint32_t* w, uint32_t* h, uint32_t* chans,
+                                    uint32_t* idat_ofs, uint32_t* idat_len);
+/* test hook: png_raw_len, the inflated size above, of a w x h file of bits_per_pixel bits (1..64) and interlace method 0 / 1 */
+FPNGB_API uint64_t fpngb_debug_png_raw_len(uint32_t w, uint32_t h, uint32_t bits_per_pixel, uint32_t interlace);
 
 /* ---- typed encode input: float32 / float16 / bfloat16 pixels with a per-channel scale and bias, rounded to 8 bits ------------
  * The *_typed encode calls take the input as elements x of T (fmt->dtype: float32, float16 or bfloat16) and encode, for channel c,
