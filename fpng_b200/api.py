@@ -310,6 +310,55 @@ def encode_ragged_device(images, flags: int = 0, out=None, stream=None, scale=No
     return out, offsets, sizes
 
 
+def png_slot_offsets(shapes):
+    """The slot offsets of encode_png_device for images of the given (h, w, chans, depth) shapes: the exclusive prefix of
+    max_encoded_size(w, h, chans * depth // 8) rounded up to 16 bytes, in index order, with the total as the last of the n + 1
+    entries."""
+    ofs = np.zeros(len(shapes) + 1, dtype=np.int64)
+    for i, (h, w, c, depth) in enumerate(shapes):
+        ofs[i + 1] = ofs[i] + (max_encoded_size(int(w), int(h), int(c) * int(depth) // 8) + 15) // 16 * 16
+    return ofs
+
+
+def encode_png_device(images, flags: int = 0, out=None, stream=None):
+    """Encode device images of 1 to 4 channels, uint8 or uint16, to PNG in one call (fpngb_encode_png_ragged_device).
+
+    images: list of CUDA tensors [h, w, c], c from 1 to 4, torch.uint8 (8-bit samples) or torch.uint16 (16-bit samples, written
+    losslessly: depth maps, sensor frames), each contiguous or a view in one of the layouts of layout_strides (HWC rows at any
+    pitch, e.g. a crop, or CHW planes, e.g. x_chw.permute(1, 2, 0)).  uint8 images with 3 or 4 channels become fpng files,
+    byte-identical to encode_ragged_device's with the same flags; the others (masks, mattes, gray+alpha, 16-bit) become PNG files
+    with a per-row filter choice and a Huffman code built per image (include/fpng_b200.h).  Other dtypes raise ValueError.
+    Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]) as encode_ragged_device does, offsets being
+    png_slot_offsets of the shapes -- the (data, offsets, sizes) that decode_packed_ragged_device(any_png=True,
+    all_formats=True) reads.  Kernels are enqueued on the current torch stream (or `stream`), with no host synchronisation."""
+    import torch
+
+    n = len(images)
+    ptrs, dims, strides = [], [], []
+    for t in images:
+        if t.dtype not in (torch.uint8, torch.uint16):
+            raise ValueError(f"encode_png_device: torch.uint8 or torch.uint16 images are needed, got {t.dtype}")
+        assert t.is_cuda and t.dim() == 3, "images: [h, w, c] CUDA tensors"
+        h, w, c = t.shape
+        es = t.element_size()
+        ptrs.append(t.data_ptr()); dims.append((w, h, c, 8 * es)); strides.append(tuple(v * es for v in t.stride()))
+    ptrs = np.array(ptrs, dtype=np.uint64)
+    dims = np.array(dims, dtype=np.uint32).reshape(n, 4)
+    strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
+    device = images[0].device if n else torch.device("cuda")
+    if out is None:
+        total = int(png_slot_offsets([(h, w, c, d) for (w, h, c, d) in dims.tolist()])[-1])
+        out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
+    _check_arg(out, "out", device, torch.uint8)
+    offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
+    sizes = torch.empty((n,), dtype=torch.int32, device=device)
+    rc = lib().fpngb_encode_png_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
+                                              strides.ctypes.data_as(C.c_void_p), flags, out.data_ptr(), out.numel(),
+                                              offsets.data_ptr(), sizes.data_ptr(), _stream(stream, device))
+    check(rc, "encode_png_device")
+    return out, offsets, sizes
+
+
 def compact_packed_device(data, offsets, sizes, out=None, stream=None):
     """Pack the files of a packed device buffer (file i: sizes[i] bytes at data[offsets[i]:], every offset a multiple of 16, e.g.
     an encode_ragged_device result) back to back, each starting 16-byte aligned (fpngb_compact_packed_device).  Returns

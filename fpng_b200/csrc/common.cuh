@@ -11,6 +11,7 @@
 namespace fpngb {
 
 constexpr uint32_t kPngHeaderSize = 58;      // sig(8) IHDR(25) fdEC(17) IDAT len+type(8): fpng.cpp:1701,1770-1783
+constexpr uint32_t kPngEncHeaderSize = 41;  // fpngb_encode_png_ragged_device's files: sig(8) IHDR(25) IDAT len+type(8), no fdEC
 constexpr uint32_t kPngTrailerSize = 16;     // IDAT crc(4) + IEND(12): fpng.cpp:1794
 constexpr uint32_t kZlibBitBase = kPngHeaderSize * 8;   // file-bit coordinate of zlib bit 0
 constexpr uint32_t kAdlerMod = 65521;

@@ -88,7 +88,8 @@ static_assert(offsetof(ImageState, tiles_done) == offsetof(ImageState, crc_acc) 
 template <bool RAGGED = false, bool VERIFY = false>
 using CrcStreamParams = std::conditional_t<VERIFY, VerifyParams, std::conditional_t<RAGGED, RaggedParams<CrcParams>, CrcParams>>;
 
-template <bool RAGGED = false, bool VERIFY = false>
+// MSG_AT: the message starts at byte p.msg_start of the file (the 41-byte header of png_encode_kernels.cu: 37) instead of byte 54
+template <bool RAGGED = false, bool VERIFY = false, bool MSG_AT = false>
 __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStreamParams<RAGGED, VERIFY> p)
 {
     // one copy of the four slice tables (4 KiB).  Eight bank-disjoint copies (32 KiB, lanes l / 4 sharing a copy) were measured:
@@ -116,8 +117,8 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStre
         }
         st = p.st + img;
         if (p.stored_only && !st->stored) return;
-        m0 = kPngHeaderSize - 4u;                                            // the message starts at byte 54 ("IDAT")
-        L = kPngHeaderSize + st->zsize;                                      // end of the message (file offset)
+        m0 = MSG_AT ? p.msg_start : kPngHeaderSize - 4u;                     // the message starts at byte 54 ("IDAT")
+        L = m0 + 4u + st->zsize;                                             // end of the message (file offset)
     }
     const uint32_t w0 = m0 >> 2;                                             // first word; its bytes before m0 are masked off
     const uint32_t head_mask = 0xFFFFFFFFu << (8u * (m0 & 3u));
@@ -320,6 +321,11 @@ void launch_idat_crc_verify(const VerifyParams& p, uint32_t n, size_t max_file_b
 void launch_crc_stream_ragged(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s)
 {
     idat_crc_stream_kernel<true><<<total_ctas, 32 * kCs2Warps, 0, s>>>(p);
+}
+
+void launch_crc_stream_png(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s)
+{
+    idat_crc_stream_kernel<true, false, true><<<total_ctas, 32 * kCs2Warps, 0, s>>>(p);
 }
 
 }  // namespace fpngb

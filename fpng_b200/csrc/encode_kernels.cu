@@ -141,23 +141,6 @@ __global__ void __launch_bounds__(kScanThreads) row_scan_kernel(ScanParams p)
 // ------------------------------------------------------------------------------------------------
 // K2: offsets + container
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long block_excl_scan_u64(unsigned long long v, unsigned long long* s_warp, unsigned long long& total)
-{
-    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    unsigned long long s = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned long long n = __shfl_up_sync(kFullMask, s, o);
-        if (lane >= (uint32_t)o) s += n;
-    }
-    if (lane == 31) s_warp[warp] = s;
-    __syncthreads();
-    unsigned long long base = 0, tot = 0;
-    for (uint32_t i = 0; i < nwarps; i++) { const unsigned long long x = s_warp[i]; if (i < warp) base += x; tot += x; }
-    __syncthreads();
-    total = tot;
-    return base + s - v;
-}
 
 __device__ __forceinline__ void store_be32(uint8_t* p, uint32_t v)
 {
@@ -414,7 +397,8 @@ __global__ void __launch_bounds__(kPackThreads) pack_rows_kernel(PackParams p)
 // ------------------------------------------------------------------------------------------------
 // K3b: Adler-32 combine.  State after row r: a' = a + S1_r, b' = b + n*a + S2_r  (mod 65521), start (1, 0).
 // ------------------------------------------------------------------------------------------------
-template <bool RAGGED = false>
+// ZLIB_AT: the file offset of the zlib stream (kPngEncHeaderSize for the files of png_encode_kernels.cu)
+template <bool RAGGED = false, uint32_t ZLIB_AT = kPngHeaderSize>
 __global__ void __launch_bounds__(kOffsetsThreads) adler_finalize_kernel(AdlerParams p)
 {
     __shared__ unsigned long long s_red[3][kOffsetsThreads / 32];
@@ -445,7 +429,7 @@ __global__ void __launch_bounds__(kOffsetsThreads) adler_finalize_kernel(AdlerPa
         const unsigned long long b = (S2 % kAdlerMod + n * before) % kAdlerMod;
         const uint32_t adler = (uint32_t)((b << 16) | a);
         const ImageState st = p.st[img];
-        store_be32(p.out + (size_t)img * p.out_stride + kPngHeaderSize + st.zsize - 4u, adler);
+        store_be32(p.out + (size_t)img * p.out_stride + ZLIB_AT + st.zsize - 4u, adler);
         p.st[img].adler = adler;
     }
 }
@@ -486,6 +470,11 @@ void launch_offsets_ragged(const OffsetsParams& p, uint32_t n, cudaStream_t s)
 void launch_adler_finalize_ragged(const AdlerParams& p, uint32_t n, cudaStream_t s)
 {
     adler_finalize_kernel<true><<<n, kOffsetsThreads, 0, s>>>(p);
+}
+
+void launch_adler_finalize_png(const AdlerParams& p, uint32_t n, cudaStream_t s)
+{
+    adler_finalize_kernel<true, kPngEncHeaderSize><<<n, kOffsetsThreads, 0, s>>>(p);
 }
 
 void launch_pack(const PackParams& p, uint32_t n, uint32_t chans, int mode, cudaStream_t s)

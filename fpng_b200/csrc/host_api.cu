@@ -609,6 +609,139 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
     return c.ws_release(s);
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// PNG encode of the images fpng does not write (fpngb_encode_png_ragged_device): gray, gray+alpha and 16-bit.
+// ---------------------------------------------------------------------------------------------------------
+// The 41-byte container header of these files: signature, IHDR (depth 8 or 16, color type 0, 4, 2 or 6), and the IDAT length
+// (patched per image on the device) and type.
+static void make_png_enc_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t chans, uint32_t depth)
+{
+    static const uint8_t sig[8] = {0x89, 'P', 'N', 'G', 0x0D, 0x0A, 0x1A, 0x0A};
+    static const uint8_t color_type[4] = {0, 4, 2, 6};
+    memset(hdr, 0, kPngEncHeaderSize);
+    memcpy(hdr, sig, 8);
+    hdr[11] = 13; memcpy(hdr + 12, "IHDR", 4);
+    for (int i = 0; i < 4; i++) { hdr[16 + i] = (uint8_t)(w >> (24 - 8 * i)); hdr[20 + i] = (uint8_t)(h >> (24 - 8 * i)); }
+    hdr[24] = (uint8_t)depth; hdr[25] = color_type[chans - 1];
+    const uint32_t c = host_crc32(hdr + 12, 17, 0);
+    for (int i = 0; i < 4; i++) hdr[29 + i] = (uint8_t)(c >> (24 - 8 * i));
+    memcpy(hdr + 37, "IDAT", 4);
+}
+
+// the (bytes per pixel, depth) classes of the PNG row kernels: gray8, GA8, gray16, GA16, RGB16, RGBA16
+constexpr int kPngClasses = 6;
+static const uint32_t kPngClassBpp[kPngClasses] = {1, 2, 2, 4, 6, 8}, kPngClassDepth[kPngClasses] = {8, 8, 16, 16, 16, 16};
+static int png_class(uint32_t bpp, uint32_t depth)
+{
+    for (int k = 0; k < kPngClasses; k++) if (kPngClassBpp[k] == bpp && kPngClassDepth[k] == depth) return k;
+    return -1;
+}
+
+// bytes of the descriptor table and work lists encode_png_locked stages for m images
+static size_t png_table_bytes(size_t m) { return align_up(m * sizeof(ImageDesc), 16) + m * 4 * 4; }
+
+// Enqueues the PNG pipeline for images im[k] (k in `ids`, depth[k] bits per sample) into their slots.  Caller holds ctx.mu.
+// Launches: per non-empty (bytes per pixel, depth) class a filter/histogram, a row-size and a pack kernel, then four per-image
+// kernels: Huffman build, offsets, Adler-32, stream CRC.  own_call: no fpng pipeline ran in this call (a new profile call).
+static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, const std::vector<uint32_t>& depth, const std::vector<uint32_t>& ids,
+                             uint32_t flags, uint8_t* d_out, uint32_t* d_sizes, cudaStream_t s, uint8_t* stage, bool own_call)
+{
+    const uint32_t m = (uint32_t)ids.size();
+    const uint32_t rpc = png_rows_per_cta();
+    size_t rows = 0;
+    std::vector<int> cls(m);
+    uint32_t cls_count[kPngClasses] = {0};
+    for (uint32_t j = 0; j < m; j++) {
+        const RaggedImage& r = im[ids[j]];
+        rows += r.h;
+        cls[j] = png_class(r.chans * depth[ids[j]] / 8, depth[ids[j]]);
+        cls_count[cls[j]]++;
+    }
+    const size_t table = png_table_bytes(m);
+    size_t o = 0;
+    const size_t o_bits = o; o = align_up(o + rows * 4, 256);
+    const size_t o_ofs = o; o = align_up(o + rows * 8, 256);
+    const size_t o_adl = o; o = align_up(o + rows * 8, 256);
+    const size_t o_filt = o; o = align_up(o + rows, 256);
+    const size_t o_st = o; o = align_up(o + (size_t)m * sizeof(ImageState), 256);
+    const size_t o_hist = o; o = align_up(o + (size_t)m * 288 * 4, 256);
+    const size_t o_books = o; o = align_up(o + (size_t)m * sizeof(CodeBook), 256);
+    const size_t o_table = o; o = align_up(o + table, 256);
+    int rc = c.ws.reserve(o);
+    if (rc) return rc;
+    rc = c.ws_acquire(s);
+    if (rc) return rc;
+    uint8_t* b = (uint8_t*)c.ws.p;
+    PngEncParams p{};
+    p.row_bits = (uint32_t*)(b + o_bits); p.row_ofs = (unsigned long long*)(b + o_ofs); p.row_adler = (uint2*)(b + o_adl);
+    p.row_filter = b + o_filt; p.st = (ImageState*)(b + o_st); p.hist = (uint32_t*)(b + o_hist);
+    CodeBook* books = (CodeBook*)(b + o_books);
+    const ImageDesc* d_desc = (const ImageDesc*)(b + o_table);
+    p.out = d_out; p.sizes = d_sizes; p.flags = flags; p.desc = d_desc;
+
+    // the table in staging: ImageDesc[m] | row-kernel img[] and CTA prefix[] per class, in class order | crc img[], crc prefix[]
+    ImageDesc* desc = (ImageDesc*)stage;
+    uint32_t* lists = (uint32_t*)(stage + align_up((size_t)m * sizeof(ImageDesc), 16));
+    uint32_t* l_img = lists; uint32_t* l_cta = lists + m; uint32_t* l_crc_img = lists + 2 * m; uint32_t* l_crc = lists + 3 * m;
+    uint32_t cls_first[kPngClasses], fill[kPngClasses];
+    for (int k = 0, acc = 0; k < kPngClasses; k++) { cls_first[k] = fill[k] = acc; acc += cls_count[k]; }
+    uint64_t cls_ctas[kPngClasses] = {0}, crc_ctas = 0;
+    size_t row_base = 0;
+    for (uint32_t j = 0; j < m; j++) {
+        const RaggedImage& r = im[ids[j]];
+        const uint32_t bpp = r.chans * depth[ids[j]] / 8;
+        ImageDesc& d = desc[j];
+        memset(&d, 0, sizeof d);
+        d.pixels = r.pixels; d.chan_stride = r.chan; d.row_base = row_base; d.out_ofs = r.slot; d.book = books + j;
+        d.row_pitch = (uint32_t)r.row; d.w = r.w; d.h = r.h; d.chans = bpp; d.index = ids[j];
+        make_png_enc_header(d.png_header, r.w, r.h, r.chans, depth[ids[j]]);
+        row_base += r.h;
+        const int k = cls[j];
+        const uint32_t q = fill[k]++;
+        l_img[q] = j; l_cta[q] = (uint32_t)cls_ctas[k]; cls_ctas[k] += (r.h + rpc - 1) / rpc;
+        l_crc_img[j] = j; l_crc[j] = (uint32_t)crc_ctas; crc_ctas += crc_stream_ctas_for(max_encoded_size(r.w, r.h, bpp));
+    }
+    for (int k = 0; k < kPngClasses; k++) if (cls_ctas[k] > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
+    if (crc_ctas > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
+    FPNGB_CUDA_OK(cudaMemcpyAsync((void*)d_desc, stage, table, cudaMemcpyHostToDevice, s));
+    const uint32_t* d_lists = (const uint32_t*)((const uint8_t*)d_desc + align_up((size_t)m * sizeof(ImageDesc), 16));
+    if (g_profile && own_call) g_prof_call++;
+    ProfSet* ps = prof_begin(s);
+    uint64_t launches = 0;
+    auto rows_pass = [&](int mode) {
+        for (int k = 0; k < kPngClasses; k++) {
+            if (!cls_count[k]) continue;
+            p.ragged = RaggedWork{d_desc, d_lists + cls_first[k], d_lists + m + cls_first[k], cls_count[k]};
+            launch_png_rows(p, (uint32_t)cls_ctas[k], kPngClassBpp[k], kPngClassDepth[k], mode, s);
+            launches++;
+        }
+    };
+
+    FPNGB_CUDA_OK(cudaMemsetAsync(p.hist, 0, (size_t)m * 288 * 4, s));
+    rows_pass(0);
+    prof_mark(ps, kProfHist, s);
+    HuffParams hp{p.hist, books, 0u, 0u, d_desc};
+    launch_huffman_build_png(hp, m, s);
+    prof_mark(ps, kProfHuff, s);
+    rows_pass(1);
+    prof_mark(ps, kProfScan, s);
+    launch_png_offsets(p, m, s);
+    prof_mark(ps, kProfOffsets, s);
+    rows_pass(2);
+    prof_mark(ps, kProfPack, s);
+    AdlerParams ap{p.row_adler, p.st, d_out, 0, 0, 0, 0, d_desc};
+    launch_adler_finalize_png(ap, m, s);
+    prof_mark(ps, kProfAdler, s);
+    RaggedParams<CrcParams> cp{};
+    cp.out = d_out; cp.st = p.st; cp.msg_start = kPngEncHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu; cp.stored_only = 0u;
+    cp.ragged = RaggedWork{d_desc, d_lists + 2 * (size_t)m, d_lists + 3 * (size_t)m, m};
+    launch_crc_stream_png(cp, (uint32_t)crc_ctas, s);
+    prof_mark(ps, kProfCrc, s);
+    count_launch(launches + 4);
+    FPNGB_CUDA_OK(cudaGetLastError());
+    return c.ws_release(s);
+}
+
 }  // namespace fpngb
 
 using namespace fpngb;
@@ -842,6 +975,80 @@ int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const u
                                      uint32_t* d_sizes, void* stream)
 {
     return encode_ragged_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
+                                   void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
+    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
+    std::vector<RaggedImage> im(n);
+    std::vector<Layout> src(n);
+    std::vector<uint32_t> depth(n), fpng_ids, png_ids;
+    uint64_t total = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t w = dims[4 * i], h = dims[4 * i + 1], chans = dims[4 * i + 2], dep = dims[4 * i + 3];
+        if (!pixels[i] || (dep != 8 && dep != 16) || chans < 1 || chans > 4) return FPNGB_ERR_INVALID_ARG;
+        const uint32_t es = dep / 8, bpp = chans * es;
+        const bool fpng = dep == 8 && chans >= 3;                        // fpng's files, as fpngb_encode_ragged_device writes them
+        if (fpng ? !valid_dims(w, h, chans)
+                 : (w < 1 || h < 1 || w > (1u << 24) || h > (1u << 24) || max_encoded_size(w, h, bpp) > 0x7FFFFFFFull))
+            return FPNGB_ERR_INVALID_ARG;                                 // one IDAT chunk must hold the stored file
+        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * bpp, pixel = strides ? strides[3 * i + 1] : bpp;
+        const uint64_t chan = (strides && chans > 1) ? strides[3 * i + 2] : es;   // a single channel's stride addresses nothing
+        Layout& L = src[i];
+        const int rc = check_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, chan, 1, h, w, chans, es, false, L);
+        if (rc) return rc;
+        if (L.row > 0xFFFFFFFFull) return FPNGB_ERR_INVALID_ARG;          // the kernels take a 32-bit row pitch
+        im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
+        depth[i] = dep;
+        (fpng ? fpng_ids : png_ids).push_back(i);
+        total += align_up(max_encoded_size(w, h, bpp), 16);
+    }
+    if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    Context& c = g_ctx;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    cudaStream_t s = (cudaStream_t)stream;
+    uint8_t* out = (uint8_t*)d_out;
+
+    // staging: d_out_offsets (n + 1), then the fpng images' table and work lists, then the PNG images' table and work lists
+    const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
+    const size_t fpng_table = align_up(align_up(fpng_ids.size() * sizeof(ImageDesc), 16) + fpng_ids.size() * 5 * 4, 16);
+    StageSlot* sl = nullptr;
+    int rc = c.stage_slot(ofs_bytes + fpng_table + png_table_bytes(png_ids.size()), &sl);
+    if (rc) return rc;
+    uint8_t* stage = (uint8_t*)sl->buf.p;
+    uint64_t* h_ofs = (uint64_t*)stage;
+    for (uint32_t i = 0; i < n; i++) h_ofs[i] = im[i].slot;
+    h_ofs[n] = total;
+    FPNGB_CUDA_OK(cudaMemcpyAsync(d_out_offsets, h_ofs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+
+    // the fpng images take fpngb_encode_ragged_device's route: the ragged pipeline, or the uniform one image by image where the
+    // 16-pixel kernels do not apply
+    const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
+    const bool lit1_rgba = !two_pass && c.h_static_books[1].lit1_rule;
+    std::vector<uint32_t> ids;
+    for (uint32_t i : fpng_ids) {
+        const RaggedImage& r = im[i];
+        if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
+            const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
+            rc = encode_batch_locked(c, r.pixels, src[i], uint8_format(), 1, r.w, r.h, r.chans, flags, out + r.slot, slot, d_sizes + i, s);
+            if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+        } else ids.push_back(i);
+    }
+    if (!ids.empty()) {
+        rc = encode_ragged_locked(c, im, ids, flags, out, d_sizes, s, stage + ofs_bytes);
+        if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+    }
+    if (!png_ids.empty()) {
+        rc = encode_png_locked(c, im, depth, png_ids, flags, out, d_sizes, s, stage + ofs_bytes + fpng_table, fpng_ids.empty());
+        if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+    }
+    FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
+    return FPNGB_OK;
 }
 
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)

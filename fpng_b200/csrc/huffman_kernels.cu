@@ -112,7 +112,10 @@ struct DevBitWriter {
 };
 
 // RAGGED: the channel count is image blockIdx.x's (p.desc) instead of the call's
-template <bool RAGGED = false>
+// PNG: the books of fpngb_encode_png_ragged_device, where p.desc's chans is B, the bytes per pixel.  The distance table is
+//   {d(B): 1 bit, d(B) + 1: 1 bit} with d(B) + 2 codes (d(B) the distance code of distance B; for B = 3, 4 fpng's table), and
+//   match[j] holds length symbol 257 + j as code | size << 16 (j < 29) instead of fpng's matches in pixels
+template <bool RAGGED = false, bool PNG = false>
 __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
 {
     __shared__ HuffScratch s;
@@ -154,10 +157,11 @@ __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
 
     // --- header (lane 0): the distance table is always {chans-1: 1 bit, chans: 1 bit} (fpng.cpp:1096-1098)
     if (lane == 0) {
-        int nlit = 286, ndist = (int)chans + 1;
+        const int dsym = PNG ? (chans <= 4 ? (int)chans - 1 : (chans <= 6 ? 4 : 5)) : (int)chans - 1;
+        int nlit = 286, ndist = dsym + 2;
         while (nlit > 257 && !s_size0[nlit - 1]) nlit--;
         for (int i = 0; i < nlit; i++) s.seq[i] = s_size0[i];
-        for (int i = 0; i < ndist; i++) s.seq[nlit + i] = (i == (int)chans - 1 || i == (int)chans) ? 1 : 0;
+        for (int i = 0; i < ndist; i++) s.seq[nlit + i] = (i == dsym || i == dsym + 1) ? 1 : 0;
         const int totalc = nlit + ndist;
         uint16_t cnt2[19];
         for (int i = 0; i < 19; i++) cnt2[i] = 0;
@@ -220,6 +224,13 @@ __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
     for (uint32_t i = lane; i < kMaxHdrBytes; i += 32) cb->hdr[i] = (uint8_t)(s.hdr_words[i >> 2] >> (8 * (i & 3)));
     for (uint32_t v = lane; v < 256; v += 32) { cb->lit[v] = s_code0[v] | ((uint32_t)s_size0[v] << 16); cb->lit_size[v] = s_size0[v]; }
     for (uint32_t i = lane; i < 288; i += 32) cb->sym_size[i] = s_size0[i];
+    if constexpr (PNG) {
+        for (uint32_t j = lane; j < 88; j += 32) {
+            cb->match[j] = j < 29 ? s_code0[257 + j] | ((uint32_t)s_size0[257 + j] << 16) : 0u;
+            cb->match_bits[j] = 0;
+        }
+        return;
+    }
     const uint32_t M = max_match_pixels(chans);
     for (uint32_t n = lane; n < 88; n += 32) {
         uint32_t m = 0, tb = 0;
@@ -242,6 +253,11 @@ void launch_huffman_build(const HuffParams& p, uint32_t n, cudaStream_t s)
 void launch_huffman_build_ragged(const HuffParams& p, uint32_t n, cudaStream_t s)
 {
     huffman_build_kernel<true><<<n, 32, 0, s>>>(p);
+}
+
+void launch_huffman_build_png(const HuffParams& p, uint32_t n, cudaStream_t s)
+{
+    huffman_build_kernel<true, true><<<n, 32, 0, s>>>(p);
 }
 
 }  // namespace fpngb

@@ -130,6 +130,27 @@ struct HuffParams {
     const ImageDesc* desc;                        // ragged kernel: the channel count of image blockIdx.x
 };
 
+// fpngb_encode_png_ragged_device (png_encode_kernels.cu): the images are ImageDesc entries whose chans is B, the bytes per pixel,
+// whose png_header holds the 41-byte container header (the sample depth at byte 24), and whose chan_stride is the plane stride of
+// a planar image (0: interleaved).  One block of parameters for every kernel of the pipeline.
+struct PngEncParams {
+    ImageState* st;                               // [m]
+    uint32_t* hist;                               // [m * 288]
+    uint8_t* row_filter;                          // [rows] filter type of each scanline
+    uint32_t* row_bits;                           // [rows] code bits of each scanline, its filter byte included
+    unsigned long long* row_ofs;                  // [rows] file bit offset of each scanline
+    uint2* row_adler;                             // [rows] (S1, S2) of the scanline as written
+    uint8_t* out; uint32_t* sizes; uint32_t flags;
+    const ImageDesc* desc;                        // the images (offsets kernel: image blockIdx.x)
+    RaggedWork ragged;                            // the images and CTA map of a row-kernel launch
+};
+uint32_t png_rows_per_cta();
+// mode 0: filter choice + histogram, 1: row bits, 2: pack; one launch over the images of one (bpp, depth) class
+void launch_png_rows(const PngEncParams& p, uint32_t ctas, uint32_t bpp, uint32_t depth, int mode, cudaStream_t s);
+void launch_png_offsets(const PngEncParams& p, uint32_t n, cudaStream_t s);
+void launch_huffman_build_png(const HuffParams& p, uint32_t n, cudaStream_t s);
+void launch_adler_finalize_png(const AdlerParams& p, uint32_t n, cudaStream_t s);
+
 // opt in to > 48 KiB of dynamic shared memory (per kernel instantiation, once per process)
 #define FPNGB_SET_SMEM(kernel, bytes) do { static bool done_ = false; \
     if (!done_) { cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(bytes)); done_ = true; } } while (0)
@@ -152,6 +173,7 @@ int crc_stream_table_ptrs(const uint32_t** f128b, const uint32_t** lane_mul);
 uint32_t crc_stream_ctas_for(size_t max_file_bytes);     // CTAs of the stream CRC kernel for a file of at most that many bytes
 uint32_t row_crc_split_for(uint32_t h);                   // CTAs of the scanline-CRC combine for an image of h scanlines
 void launch_crc_stream_ragged(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s);
+void launch_crc_stream_png(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s);   // message from p.msg_start
 void launch_row_crc_combine_ragged(const RowCrcParams& p, uint32_t n, uint32_t max_split, cudaStream_t s);
 void launch_offsets_ragged(const OffsetsParams& p, uint32_t n, cudaStream_t s);
 void launch_adler_finalize_ragged(const AdlerParams& p, uint32_t n, cudaStream_t s);

@@ -194,6 +194,25 @@ __device__ __forceinline__ uint32_t warp_excl_scan_u32(uint32_t v, uint32_t lane
     return s - v;
 }
 
+// exclusive prefix of v over the block (blockDim.x a multiple of 32, s_warp one entry per warp); total: the block sum
+__device__ __forceinline__ unsigned long long block_excl_scan_u64(unsigned long long v, unsigned long long* s_warp, unsigned long long& total)
+{
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    unsigned long long s = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long n = __shfl_up_sync(kFullMask, s, o);
+        if (lane >= (uint32_t)o) s += n;
+    }
+    if (lane == 31) s_warp[warp] = s;
+    __syncthreads();
+    unsigned long long base = 0, tot = 0;
+    for (uint32_t i = 0; i < nwarps; i++) { const unsigned long long x = s_warp[i]; if (i < warp) base += x; tot += x; }
+    __syncthreads();
+    total = tot;
+    return base + s - v;
+}
+
 // Source bytes of a stored row, in PNG byte order: byte i of an interleaved scanline, or of a planar one (channel i % CHANS
 // of pixel i / CHANS, planes chan_stride bytes apart)
 struct RowBytes {

@@ -121,6 +121,37 @@ FPNGB_API int fpngb_encode_batch_device_strided(const void* d_pixels, size_t ima
 FPNGB_API int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
                                          void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
 
+/* fpngb_encode_png_ragged_device: encodes n device images of 1 to 4 channels and 8 or 16 bits per sample to PNG, in one call and
+ *   into the packed layout of fpngb_encode_ragged_device: segmentation masks and mattes (gray8), gray+alpha, depth maps and
+ *   16-bit sensor frames (gray16), and 16-bit gray+alpha, RGB and RGBA.
+ *     pixels   HOST array of n device addresses
+ *     dims     HOST array of n x {w, h, chans, depth}: chans 1..4, depth 8 (uint8 samples) or 16 (native little-endian uint16)
+ *     strides  HOST array of n x {row_pitch, pixel_stride, chan_stride} in bytes, or NULL for tight HWC rows; the layouts of
+ *              "Pixel layouts" above with elements of depth / 8 bytes (interleaved rows at any pitch, or planar)
+ *   Images with depth 8 and 3 or 4 channels are fpng files, encoded exactly as fpngb_encode_ragged_device encodes them with the
+ *   same flags (byte-identical), so one call can save a mixed list.  Every other image is written as a PNG that fpng's reader
+ *   does not claim (no fdEC chunk): signature, IHDR (color type 0, 4, 2 or 6, no interlace), one IDAT holding a zlib stream
+ *   (header 78 01, one dynamic Huffman block built for the image, Adler-32), IEND.  Each row takes the PNG filter with the
+ *   smallest sum of min(b, 256 - b) over its filtered bytes (ties to the lower type); runs of equal filtered pixels become
+ *   matches at distance B = chans * depth / 8 bytes; the code is fpng's 2-pass construction.  The file falls back to stored
+ *   blocks (filter 0 on every row) when that is shorter, or with FPNGB_FORCE_UNCOMPRESSED.  FPNGB_ENCODE_SLOWER only affects
+ *   the fpng files.  The exact rules are in DESIGN.md §4.6.
+ *   Output slots: file i goes to d_out + d_out_offsets[i], the exclusive prefix of align_up(fpngb_max_encoded_size(w_i, h_i,
+ *   B_i), 16) with B_i the bytes per pixel (chans for the fpng files); d_out_offsets[n] is the total, d_sizes[i] the file size.
+ *   The bound holds for these files too: their header is 17 bytes shorter than fpng's.  No byte of d_out past the total is written.
+ *   Call-level checks, before anything is enqueued: those of fpngb_encode_ragged_device (FPNGB_ERR_INVALID_ARG,
+ *   FPNGB_ERR_BUFFER_TOO_SMALL, FPNGB_ERR_ALIGNMENT; FPNGB_ERR_ALIGNMENT also for a 16-bit image whose address or strides are
+ *   odd), and FPNGB_ERR_INVALID_ARG for unknown flag bits, a depth other than 8 or 16, chans outside 1..4, and an image whose
+ *   slot bound exceeds 2^31 - 1 bytes.  A rejected call enqueues nothing and writes nothing.
+ *   Stream-ordered, no host synchronisation; descriptors go up from the pinned staging ring as in fpngb_encode_ragged_device.
+ *   Launches: those of fpngb_encode_ragged_device for the fpng images, plus, when the call has other images, three per
+ *   non-empty class (gray8, GA8, gray16, GA16, RGB16, RGBA16: filter choice and histogram, row sizes, pack) and four per-image
+ *   kernels (Huffman build, offsets, Adler-32, CRC).  fpngb_profile_read reports them in slots 0 (filter and histogram),
+ *   1 (Huffman), 2 (row sizes), 3 (offsets), 6 (pack), 7 (Adler-32) and 8 (CRC). */
+FPNGB_API int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                             uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes,
+                                             void* stream);
+
 /* Batch of n equally sized images in HOST memory (ideally pinned: see fpngb_host_alloc) -> n files in host memory,
  * out + i*out_stride, sizes[i].  Internally pipelines H2D copy / kernels / D2H copy over chunks of the batch. */
 FPNGB_API int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
