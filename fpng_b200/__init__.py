@@ -19,5 +19,5 @@ from .api import (  # noqa: F401
     normalize_scale_bias, denormalize_scale_bias, typed_layout,
     FPNGB_DECODE_BAD_CROP, FPNGB_RESIZE_ANTIALIAS, decode_packed_resized_device,
     FPNGB_DECODE_UNSUPPORTED_PNG, FPNGB_RESIZE_ANY_PNG, get_png_info,
-    FPNGB_PNG_ALL_FORMATS, FPNGB_RESIZE_ALL_PNG_FORMATS,
+    FPNGB_PNG_ALL_FORMATS, FPNGB_RESIZE_ALL_PNG_FORMATS, FPNGB_PNG_NATIVE, FPNGB_DTYPE_UINT16, FPNGB_RESIZE_NATIVE,
 )

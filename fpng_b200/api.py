@@ -143,16 +143,17 @@ def fpng_decode_file(filename: str, desired_channels: int):
     return fpng_decode_memory(data, desired_channels)
 
 
-def layout_strides(shape, strides):
+def layout_strides(shape, strides, channels=(3, 4)):
     """Byte strides (image_stride, row_pitch, pixel_stride, chan_stride) of an [n, h, w, chans] uint8 view, in the form the
     *_strided C calls take (include/fpng_b200.h, "Pixel layouts").  Two layouts are supported: interleaved (pixel_stride ==
     chans, chan_stride == 1: HWC rows at any pitch) and planar (pixel_stride == 1, chan_stride >= 1: CHW or HCW planes).  The
     stride of a dimension of size 1 is ignored and replaced by the value of a tightly packed batch (w == 1 is interleaved when
-    chan_stride == 1, planar otherwise).  Raises ValueError for any other layout."""
+    chan_stride == 1, planar otherwise).  Raises ValueError for any other layout.  channels: the channel counts the calling
+    entry point takes (1 .. 4 for the native resized decode)."""
     n, h, w, c = (int(v) for v in shape)
     image, row, pixel, chan = (int(v) for v in strides)
-    if c not in (3, 4):
-        raise ValueError(f"layout_strides: {c} channels (3 or 4 are supported)")
+    if c not in channels:
+        raise ValueError(f"layout_strides: {c} channels ({' or '.join(map(str, channels))} are supported)")
     if min(image, row, pixel, chan) < 0:
         raise ValueError("layout_strides: negative strides are not supported")
     if w == 1:
@@ -169,7 +170,7 @@ def layout_strides(shape, strides):
     return image, row, pixel, chan
 
 
-def _layout(t, shape):
+def _layout(t, shape, channels=(3, 4)):
     """The byte strides (image_stride, row_pitch, pixel_stride, chan_stride) of the C calls for t, an [n, h, w, chans] array of
     the given shape: those of tight rows for a contiguous tensor, else those of a view of that shape in one of the layouts of
     layout_strides.  ValueError for a view of another shape or layout."""
@@ -179,7 +180,7 @@ def _layout(t, shape):
         return h * w * c * es, w * c * es, c * es, es
     if tuple(t.shape) != tuple(shape):
         raise ValueError(f"a non-contiguous view must have shape {tuple(shape)}, got {tuple(t.shape)}")
-    return typed_layout(t.shape, t.stride(), t.element_size())
+    return typed_layout(t.shape, t.stride(), t.element_size(), channels)
 
 
 def _check_arg(t, name, device, dtype, entries=0, row_bytes=None, view=False):
@@ -423,11 +424,11 @@ def _pixel_format(dtype, scale, bias, chans, what="pixel format"):
     return fmt
 
 
-def typed_layout(shape, strides, element_size):
+def typed_layout(shape, strides, element_size, channels=(3, 4)):
     """Byte strides (image_stride, row_pitch, pixel_stride, chan_stride) of an [n, h, w, chans] view whose elements are
     element_size bytes, as the *_typed C calls take them: layout_strides applied to the element strides torch reports, then
     multiplied by the element size.  NCHW float output is torch.empty(n, c, h, w, dtype=...).permute(0, 2, 3, 1)."""
-    return tuple(v * int(element_size) for v in layout_strides(shape, strides))
+    return tuple(v * int(element_size) for v in layout_strides(shape, strides, channels))
 
 
 def normalize_scale_bias(mean, std, max_value=255.0):
@@ -463,6 +464,8 @@ def get_info_ex(data):
 
 FPNGB_DECODE_UNSUPPORTED_PNG = 104   # any_png decodes: a well-formed PNG the GPU decoder does not read (palette, 16-bit, Adam7, tRNS)
 FPNGB_PNG_ALL_FORMATS = 1            # all_formats=True: palette, 1/2/4/16-bit, color-keyed and Adam7 files decode too
+FPNGB_PNG_NATIVE = 4                 # native=True: each file at its own channel count, uint16 output, 1 / 2 channels
+FPNGB_DTYPE_UINT16 = 4               # fpngb_pixel_format.dtype of uint16 output (native calls only)
 
 
 def get_png_info(data, all_formats=False):
@@ -478,9 +481,25 @@ def get_png_info(data, all_formats=False):
     return st, w.value, h.value, c.value, o.value, l.value
 
 
-def _all_formats_check(any_png, all_formats, fn):
+def _all_formats_check(any_png, all_formats, fn, native=False):
     if all_formats and not any_png:
         raise ValueError(f"{fn}: all_formats=True needs any_png=True")
+    if native and not any_png:
+        raise ValueError(f"{fn}: native=True needs any_png=True")
+
+
+def _native_format(dtype, scale, bias, desired_channels, what):
+    """the fmt of a native call: None for uint8, FPNGB_DTYPE_UINT16 for uint16 (no scale or bias: ValueError), else _pixel_format's
+    over the channels the call may write (4 for desired_channels 0)"""
+    import torch
+
+    if dtype == torch.uint16:
+        if scale is not None or bias is not None:
+            raise ValueError(f"{what}: scale and bias apply to float32 / float16 / bfloat16 pixels only; uint16 pixels are taken as they are")
+        fmt = PixelFormat()
+        fmt.dtype = FPNGB_DTYPE_UINT16
+        return fmt
+    return _pixel_format(dtype, scale, bias, desired_channels or 4, what)
 
 
 def pack_files_for_device(files, device=None):
@@ -619,7 +638,7 @@ def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max
                    all_formats=False):
     """The bounds of decode_packed_ragged_device the caller left out, and the exact output size in bytes they give for elements
     of element_size bytes: one device walk (get_info_batch_device) and one read-back of (info, sizes, offsets), which
-    synchronises with the stream."""
+    synchronises with the stream.  desired_channels 0 (native calls) sizes each file at its info row's channel count."""
     import torch
 
     info = get_info_batch_device(data, offsets, sizes, stream, any_png=any_png, all_formats=all_formats)
@@ -634,7 +653,7 @@ def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max
         max_w = int(w[walked].max()) if walked.any() else 1
     if max_h is None:
         max_h = int(h[walked].max()) if walked.any() else 1
-    px = w * h * desired_channels
+    px = w * h * (desired_channels if desired_channels else t[:, 3])
     placed = (walked & (size <= max_file_size) & (ofs % 4 == 0) & (ofs + size <= data.numel()) & (w <= max_w) & (h <= max_h)
               & (px <= 0xFFFFFFFF))
     total = int(((px[placed] * element_size + 15) // 16 * 16).sum())
@@ -642,7 +661,7 @@ def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max
 
 
 def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out=None, max_file_size=None, max_w=None, max_h=None,
-                                stream=None, dtype=None, scale=None, bias=None, any_png=False, all_formats=False):
+                                stream=None, dtype=None, scale=None, bias=None, any_png=False, all_formats=False, native=False):
     """Decode fpng files of ANY shapes and channel counts packed in device memory (the layout of get_info_batch_device; base_bytes
     is data.numel()) in one call, pixels placed back to back.  Returns (out uint8 [out_cap], out_offsets int64 [n + 1],
     info int32 [n, 6], status int32 [n]):
@@ -664,14 +683,27 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     error or FPNG_DECODE_FAILED_INVALID_IDAT for a bad stream; fpng files decode exactly as without it.
     all_formats=True (with any_png=True, else ValueError) also decodes palette, 1/2/4-bit gray, 16-bit, color-keyed (tRNS) and
     Adam7-interlaced files (FPNGB_PNG_ALL_FORMATS; pixel rules in include/fpng_b200.h): sub-byte gray scaled to 0..255, 16-bit
-    samples as their high byte (typed output: s / 257), palette entries with tRNS alpha, a color key as alpha 0."""
+    samples as their high byte (typed output: s / 257), palette entries with tRNS alpha, a color key as alpha 0.
+    native=True (with any_png=True, else ValueError) decodes each file at its own channel count and bit depth (FPNGB_PNG_NATIVE;
+    rules in include/fpng_b200.h): desired_channels may also be 1 (gray, or the luma of color files: Pillow's convert("L")), 2
+    (with alpha) or 0 / None (each file's own channels, info[i, 3]; ragged_views(..., 0) cuts them), and dtype torch.uint16
+    stores 16-bit samples as they are and 8-bit values v as v * 257 (no scale or bias).  Without native those values raise
+    ValueError."""
     import torch
 
-    _all_formats_check(any_png, all_formats, "decode_packed_ragged_device")
-    n = _packed_args(data, offsets, sizes)
-    assert desired_channels in (3, 4), "desired_channels: 3 or 4"
+    _all_formats_check(any_png, all_formats, "decode_packed_ragged_device", native)
     odt = _out_dtype(out, dtype)
-    fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_ragged_device")
+    if native:
+        desired_channels = desired_channels or 0
+        if desired_channels not in (0, 1, 2, 3, 4):
+            raise ValueError(f"decode_packed_ragged_device: desired_channels {desired_channels}: 0 (None), 1, 2, 3 or 4")
+        fmt = _native_format(odt, scale, bias, desired_channels, "decode_packed_ragged_device")
+    else:
+        if desired_channels in (0, 1, 2, None):
+            raise ValueError(f"decode_packed_ragged_device: desired_channels {desired_channels} needs native=True")
+        assert desired_channels in (3, 4), "desired_channels: 3 or 4"
+        fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_ragged_device")
+    n = _packed_args(data, offsets, sizes)
     es = torch.empty((), dtype=odt).element_size()
     if out is None or max_file_size is None or max_w is None or max_h is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
@@ -685,8 +717,9 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     s = _stream(stream, data.device)
     args = (data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
             int(max_h), desired_channels, out.data_ptr(), out.numel() * es, out_offsets.data_ptr(), info.data_ptr())
-    if all_formats:
-        rc = lib().fpngb_decode_packed_png_device_ex(*args, FPNGB_PNG_ALL_FORMATS, None if fmt is None else C.byref(fmt),
+    if all_formats or native:
+        rc = lib().fpngb_decode_packed_png_device_ex(*args, (FPNGB_PNG_ALL_FORMATS if all_formats else 0) |
+                                                     (FPNGB_PNG_NATIVE if native else 0), None if fmt is None else C.byref(fmt),
                                                      status.data_ptr(), s)
     elif any_png:
         rc = lib().fpngb_decode_packed_png_device(*args, None if fmt is None else C.byref(fmt), status.data_ptr(), s)
@@ -700,8 +733,8 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
 
 def ragged_views(out, out_offsets, info, status, desired_channels: int):
     """Per file of a decode_packed_ragged_device result, an [h, w, desired_channels] view into `out` (any dtype: the byte offsets
-    become element offsets), or None when the file's status is not 0.  Reads out_offsets, info and status back to the host, so
-    it waits for the device."""
+    become element offsets), or None when the file's status is not 0.  desired_channels 0 (or None: a native call's) takes each
+    file's info row channel count.  Reads out_offsets, info and status back to the host, so it waits for the device."""
     offs = out_offsets.cpu().numpy()
     inf = info.cpu().numpy()
     st = status.cpu().numpy()
@@ -710,9 +743,9 @@ def ragged_views(out, out_offsets, info, status, desired_channels: int):
         if st[i] != 0:
             views.append(None)
             continue
-        w, h = int(inf[i, 1]), int(inf[i, 2])
+        w, h, c = int(inf[i, 1]), int(inf[i, 2]), int(desired_channels or inf[i, 3])
         o = int(offs[i]) // out.element_size()
-        views.append(out[o:o + h * w * desired_channels].view(h, w, desired_channels))
+        views.append(out[o:o + h * w * c].view(h, w, c))
     return views
 
 
@@ -720,11 +753,12 @@ FPNGB_DECODE_BAD_CROP = 103        # decode_packed_resized_device only: the file
 FPNGB_RESIZE_ANTIALIAS = 1
 FPNGB_RESIZE_ANY_PNG = 4
 FPNGB_RESIZE_ALL_PNG_FORMATS = 8
+FPNGB_RESIZE_NATIVE = 16
 
 
 def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: int, boxes=None, antialias=True, out=None, dtype=None,
                                  scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None,
-                                 any_png=False, all_formats=False):
+                                 any_png=False, all_formats=False, native=False):
     """Decode fpng files of ANY shapes packed in device memory (the layout of decode_packed_ragged_device) into one batch of a fixed
     size = (H, W): file i is cropped to boxes[i] and resized with F.interpolate's bilinear rule (align_corners=False, antialias as
     given) on the GPU, then stored as decode_batch_device stores its pixels (uint8, rounded half to even and clamped, or dtype with
@@ -741,17 +775,25 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     waits for the stream; pixel_cap then becomes the exact size of the decodable files.
     any_png=True decodes general PNGs too, as decode_packed_ragged_device(any_png=True) does (FPNGB_RESIZE_ANY_PNG), and
     all_formats=True (with any_png=True, else ValueError) every PNG format as there (FPNGB_RESIZE_ALL_PNG_FORMATS); the resize
-    reads the uint8 values, so a 16-bit file is resized from its high bytes."""
+    reads the uint8 values, so a 16-bit file is resized from its high bytes.
+    native=True (with any_png=True, else ValueError; FPNGB_RESIZE_NATIVE) resizes every file from its 16-bit domain values (16-bit
+    samples as they are, 8-bit values v as v * 257): desired_channels 1 .. 4 (1 / 2: luma and alpha, as in
+    decode_packed_ragged_device(native=True)), dtype torch.uint16 stores the rounded resampled value, uint8 and the float types
+    the value / 257 as above.  pixel_cap then counts bytes of the uint16 intermediate (align_up(w*h*desired_channels*2, 16) per
+    file)."""
     import torch
 
-    _all_formats_check(any_png, all_formats, "decode_packed_resized_device")
-    if desired_channels not in (3, 4):
-        raise ValueError(f"decode_packed_resized_device: desired_channels {desired_channels}: 3 or 4")
+    _all_formats_check(any_png, all_formats, "decode_packed_resized_device", native)
+    if desired_channels not in ((1, 2, 3, 4) if native else (3, 4)):
+        raise ValueError(f"decode_packed_resized_device: desired_channels {desired_channels}: " + ("1 .. 4" if native else "3 or 4"))
     H, W = (int(v) for v in size)
     if not (1 <= H <= 1 << 24 and 1 <= W <= 1 << 24):
         raise ValueError(f"decode_packed_resized_device: size {tuple(size)}: each side in 1 .. 2^24")
     odt = _out_dtype(out, dtype)
-    fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
+    if native:
+        fmt = _native_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
+    else:
+        fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
     if boxes is not None:
         if not isinstance(boxes, torch.Tensor) or not boxes.is_cuda or boxes.device != data.device:
             raise ValueError(f"boxes: a CUDA tensor on {data.device} is needed")
@@ -765,7 +807,7 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     _check_arg(out, "out", data.device, odt, n * H * W * desired_channels, view=True)
     if max_file_size is None or max_w is None or max_h is None or pixel_cap is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
-                                                             stream, any_png=any_png, all_formats=all_formats)
+                                                             stream, 2 if native else 1, any_png=any_png, all_formats=all_formats)
         if pixel_cap is None:
             pixel_cap = total
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
@@ -774,7 +816,8 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
         data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
         int(max_h), int(pixel_cap), None if boxes is None else boxes.data_ptr(), W, H, desired_channels,
         (FPNGB_RESIZE_ANTIALIAS if antialias else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
-        (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0), None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape),
+        (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0) | (FPNGB_RESIZE_NATIVE if native else 0),
+        None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape, (1, 2, 3, 4) if native else (3, 4)),
         info.data_ptr(), status.data_ptr(), _stream(stream, data.device))
     check(rc, "decode_packed_resized_device")
     return out, info, status

@@ -71,7 +71,9 @@ struct OutStrides {
 // FPNGB_DTYPE_* value).  A separate kernel argument, as OutStrides is, so that no other kernel's parameter block grows; the
 // OutStrides of a typed call are in bytes, with pixel == sizeof(T) for planar output.
 struct PixelAffine { float scale[4], bias[4]; };
-struct TypedOut { uint32_t dtype; PixelAffine aff; };
+// native (FPNGB_PNG_NATIVE): dtype may also be 0 (uint8: the value itself) or FPNGB_DTYPE_UINT16 (v * 257, or a 16-bit sample as it
+// is), desired 1..4 or 0 (each file's own channels), and scale / bias act on the float types only
+struct TypedOut { uint32_t dtype; PixelAffine aff; bool native = false; };
 // Opt-in integrity check of every decode call (fpngb_set_decode_verify).  Two kernels read the file and the delta rows again:
 //   idat_crc_stream_kernel<false, true> (crc_stream_kernel.cu), after decode_prepare_kernel: the CRC-32 of "IDAT" + idat_len data
 //     bytes against the chunk's CRC field; a mismatch sets DecodeState::status to 4 for every file the walk passed, whatever the
@@ -130,7 +132,9 @@ void launch_container_walk(const WalkParams& p, cudaStream_t s);
 // A file whose output, delta rows or records end past out_cap / delta_cap / sub_cap gets FPNGB_DECODE_OUT_OF_SPACE.
 struct PlaceParams {
     FileDesc* files; uint32_t n;
-    uint32_t px_bytes;                      // output bytes per pixel: desired * sizeof(T) (desired for uint8 pixels)
+    uint32_t px_bytes;                      // output bytes per pixel: desired * sizeof(T) (desired for uint8 pixels); 0 in a native
+                                            // call with desired 0: file i's chans * elem
+    uint32_t elem;                          // native calls: bytes per element
     unsigned long long out_cap, delta_cap, sub_cap;
     unsigned long long* out_offsets;        // [n + 1]
 };
@@ -165,12 +169,16 @@ struct PngParams {
     uint8_t* z;                             // gathered zlib streams
     uint8_t* rows;                          // inflated rows: file f at rows + files[f].delta_base (the decode's delta region)
     uint8_t* d_out; uint32_t* d_status;     // pixels as the ragged decode places them (tight HWC rows at d_out + files[f].out_base)
-    uint32_t n, desired, verify;
+    uint32_t n, desired, verify;            // desired 0 (native calls only): each file's own channels, FileDesc::chans
 };
 // container_walk_kernel<true> (png != nullptr only with files != nullptr; flags: png_walk's) and decode_place_kernel<true>, z_cap
 // the gathered bytes
 void launch_container_walk_any(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s);
 void launch_decode_place_any(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s);
+// the same for a native call (FPNGB_PNG_NATIVE): with WalkParams::desired / PlaceParams::px_bytes 0, each file's own channel
+// count (its info row's chans) sizes its output and its FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE check
+void launch_container_walk_native(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s);
+void launch_decode_place_native(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s);
 // gather, inflate and unfilter of the general files (three launches, four with FPNGB_PNG_ALL_FORMATS in flags; grids from n alone),
 // behind launch_decode
 void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags, cudaStream_t s);
@@ -179,7 +187,8 @@ void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags
 // HWC rows (pitch w * desired) at px + px_offsets[f], crops file f to its box and resizes it to out_h x out_w with the bilinear
 // rule of fpngb_decode_packed_resized_device, then stores T(r * scale[c] + bias[c]) (float types) or round_u8(r) (dtype 0).
 // Files whose d_status is not 0 are skipped.  Output strides in bytes: element (f, y, x, c) at d_out + f*image + y*row + x*pixel
-// + c*chan, interleaved (pixel = desired * sizeof(T)) or planar (pixel = sizeof(T)).
+// + c*chan, interleaved (pixel = desired * sizeof(T)) or planar (pixel = sizeof(T)).  A native call (TypedOut::native) reads uint16
+// pixels (pitch w * desired * 2) instead, desired 1 .. 4, and stores the rules of decode_resize_kernels.cu.
 struct ResizeParams {
     const uint8_t* px; const unsigned long long* px_offsets;   // the ragged decode's pixels and their placement
     const FileDesc* files; const int32_t* d_status;

@@ -86,6 +86,16 @@ static int decode_format(bool typed, const fpngb_pixel_format* fmt, uint32_t des
     return FPNGB_OK;
 }
 
+// The output format of a native call (FPNGB_PNG_NATIVE): uint8 (fmt NULL), uint16 (FPNGB_DTYPE_UINT16: scale and bias ignored, as
+// uint8 takes none) or a float fmt checked as the *_typed calls check it, over every channel the call may write (4 for desired 0).
+static int native_format(const fpngb_pixel_format* fmt, uint32_t desired, TypedOut& t, uint32_t& elem)
+{
+    if (fmt && fmt->dtype == FPNGB_DTYPE_UINT16) { t = TypedOut{FPNGB_DTYPE_UINT16, {}, true}; elem = 2; return FPNGB_OK; }
+    const int rc = decode_format(fmt != nullptr, fmt, desired ? desired : 4, t, elem); if (rc) return rc;
+    t.native = true;
+    return FPNGB_OK;
+}
+
 // Enqueue the decode pipeline for n files already resident on the device, file i at d_files + i * file_stride, described by host
 // FileDescs (their base and pre_status are set here).  Caller holds context().mu.
 static int decode_batch_locked(const uint8_t* d_files, size_t file_stride, const FileDesc* h_files, uint32_t n, uint32_t w, uint32_t h,
@@ -215,6 +225,12 @@ static int decode_packed_device_impl(const void* d_base, const uint64_t* d_offse
 //              "2h + 6" Adam7 adds.  So align_up(raw_len, 16) <= 8wh + 2h + 21 <= 8wh + 32h (h >= 1): the bound from out_cap is
 //              out_cap*8/desired + 32 * min(rows, rows_px), and from the shape h * (8w + 32) per file.  Both also bound the 8-bit
 //              general and fpng files (4wh + 16h, and h * (delta_pitch(w, 4) + 16) <= h * (8w + 32)).  Flag off: the bounds above.
+//   native (FPNGB_PNG_NATIVE): file i writes w*h*c_i values, c_i = desired, or its own channel count for desired 0, so c_i >= 1 and
+//              the w*h*c_i of the decoded files sum to at most out_cap.  Every delta need above is a bound per pixel plus one per
+//              row, so it holds with c_i := 1: an fpng file's h * align_up(w*c, 16) <= 4wh + 16h <= 4 (w*h*c_i) + 16h, a general
+//              8-bit file's 4wh + 16h the same, an ext file's 8wh + 32h <= 8 (w*h*c_i) + 32h (the worst ratio: an RGBA16 file decoded
+//              to 1 channel inflates up to 8 bytes per output value), and sum h <= sum w*h*c_i <= out_cap.  So the bounds above
+//              hold with desired := 1; the bound from the shape does not depend on desired.
 // A file whose range still ends past a bound (overlapping files) gets FPNGB_DECODE_OUT_OF_SPACE from decode_place_kernel.
 static unsigned long long sat_u64(unsigned __int128 v) { return v > ~0ull ? ~0ull : (unsigned long long)v; }
 static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired,
@@ -243,7 +259,8 @@ struct ResizeOut {
 // workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes, and the
 // resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
 // general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc); png_flags: png_walk's flags
-// (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel).
+// (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel; FPNGB_PNG_NATIVE takes the native instantiations of the walk, place
+// and unfilter kernels, with desired_chans 0..4 and fmt as native_format reads it).
 static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
@@ -252,18 +269,20 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
 {
     Context& c = context();
     if (!c.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    const bool native = any_png && (png_flags & FPNGB_PNG_NATIVE);
     if (!d_base || !d_offsets || !d_sizes || (!rz && (!d_out || !d_out_offsets)) || !d_status || n == 0 || n > 65535 || !max_file_size ||
-        (desired_chans != 3 && desired_chans != 4) || !max_w || !max_h || max_w > (1u << 24) || max_h > (1u << 24))
+        (native ? desired_chans > 4 || (rz && !desired_chans) : desired_chans != 3 && desired_chans != 4) || !max_w || !max_h ||
+        max_w > (1u << 24) || max_h > (1u << 24))
         return FPNGB_ERR_INVALID_ARG;
     TypedOut t;
     uint32_t elem;
-    int rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
+    int rc = native ? native_format(fmt, desired_chans, t, elem) : decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
     if ((uintptr_t)d_base % 4 || (!rz && (uintptr_t)d_out % 16)) return FPNGB_ERR_ALIGNMENT;
     unsigned long long sub_cap = 0, delta_cap = 0, z_cap = 0;
     // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
     const bool all_formats = any_png && (png_flags & FPNGB_PNG_ALL_FORMATS);
-    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, desired_chans, out_cap / elem, any_png, all_formats, sub_cap, delta_cap,
-                     z_cap);
+    ragged_workspace(n, base_bytes, max_file_size, max_w, max_h, native ? 1u : desired_chans, out_cap / elem, any_png, all_formats, sub_cap,
+                     delta_cap, z_cap);
     if (sub_cap > SIZE_MAX / sizeof(SubInfo) || delta_cap > SIZE_MAX / 2 || (rz && out_cap > SIZE_MAX / 2) || z_cap > SIZE_MAX / 4)
         return FPNGB_ERR_BUFFER_TOO_SMALL;
     const size_t png_desc_bytes = any_png ? align_up((size_t)n * sizeof(PngDesc), 256) : 0;
@@ -284,20 +303,23 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
     wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr;
-    if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags, s);
+    if (native) launch_container_walk_native(wp, (PngDesc*)png, png_flags & FPNGB_PNG_ALL_FORMATS, s);
+    else if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags, s);
     else launch_container_walk(wp, s);
     PlaceParams pp{};
-    pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem;
+    pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem; pp.elem = elem;
     pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
-    if (any_png) launch_decode_place_any(pp, (PngDesc*)png, z_cap, s);
+    if (native) launch_decode_place_native(pp, (PngDesc*)png, z_cap, s);
+    else if (any_png) launch_decode_place_any(pp, (PngDesc*)png, z_cap, s);
     else launch_decode_place(pp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
-    launch_decode(p, OutStrides{0, desired_chans * elem, elem}, n, desired_chans, s, verify, max_file_size, typed ? &t : nullptr);
+    const TypedOut* tp = typed || native ? &t : nullptr;
+    launch_decode(p, OutStrides{0, desired_chans * elem, elem}, n, desired_chans, s, verify, max_file_size, tp);
     if (any_png) {                                  // behind decode_status_kernel: the general files' final statuses
         PngParams q{};
         q.d_files = (const uint8_t*)d_base; q.files = p.files; q.png = (PngDesc*)png; q.z = png + png_desc_bytes; q.rows = p.delta;
         q.d_out = (uint8_t*)d_out; q.d_status = (uint32_t*)d_status; q.n = n; q.desired = desired_chans; q.verify = verify != nullptr;
-        launch_png_decode(q, typed ? &t : nullptr, png_flags, s);
+        launch_png_decode(q, tp, png_flags, s);
     }
     if (rz) {
         ResizeParams rp{};
@@ -576,21 +598,27 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
                                        size_t out_chan_stride, uint32_t* d_info, int32_t* d_status, void* stream)
 {
     if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
+    const bool native = (flags & FPNGB_RESIZE_NATIVE) != 0;
     if (!d_out || n == 0 || n > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
-        (desired_chans != 3 && desired_chans != 4) ||
-        (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS)) ||
-        ((flags & FPNGB_RESIZE_ALL_PNG_FORMATS) && !(flags & FPNGB_RESIZE_ANY_PNG)))
+        (native ? desired_chans < 1 || desired_chans > 4 : desired_chans != 3 && desired_chans != 4) ||
+        (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE)) ||
+        ((flags & (FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE)) && !(flags & FPNGB_RESIZE_ANY_PNG)))
         return FPNGB_ERR_INVALID_ARG;
     ResizeOut rz{};
     rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
     uint32_t elem;
-    int rc = decode_format(fmt != nullptr, fmt, desired_chans, rz.t, elem); if (rc) return rc;
+    int rc = native ? native_format(fmt, desired_chans, rz.t, elem) : decode_format(fmt != nullptr, fmt, desired_chans, rz.t, elem);
+    if (rc) return rc;
     rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, out_h, out_w, desired_chans, elem, true,
                       rz.out);
     if (rc) return rc;
+    // native: the ragged decode holds every file as uint16 values in the 16-bit domain (pixel_cap counts their bytes)
+    static const fpngb_pixel_format u16 = {FPNGB_DTYPE_UINT16, {0, 0, 0, 0}, {0, 0, 0, 0}};
+    const uint32_t png_flags = ((flags & FPNGB_RESIZE_ALL_PNG_FORMATS) ? (uint32_t)FPNGB_PNG_ALL_FORMATS : 0u) |
+                               (native ? (uint32_t)FPNGB_PNG_NATIVE : 0u);
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
-                                     nullptr, d_info, false, nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
-                                     (flags & FPNGB_RESIZE_ALL_PNG_FORMATS) ? (uint32_t)FPNGB_PNG_ALL_FORMATS : 0u);
+                                     nullptr, d_info, false, native ? &u16 : nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
+                                     png_flags);
 }
 
 int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
@@ -598,7 +626,7 @@ int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, con
                                       size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, uint32_t flags,
                                       const fpngb_pixel_format* fmt, int32_t* d_status, void* stream)
 {
-    if (flags & ~(uint32_t)FPNGB_PNG_ALL_FORMATS) return context().ready ? FPNGB_ERR_INVALID_ARG : FPNGB_ERR_NOT_INITIALIZED;
+    if (flags & ~(uint32_t)(FPNGB_PNG_ALL_FORMATS | FPNGB_PNG_NATIVE)) return context().ready ? FPNGB_ERR_INVALID_ARG : FPNGB_ERR_NOT_INITIALIZED;
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
                                      d_out_offsets, d_info, fmt != nullptr, fmt, d_status, stream, nullptr, true, flags);
 }

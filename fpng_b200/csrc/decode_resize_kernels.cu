@@ -7,9 +7,12 @@
 // output row vertically in registers, over the rows of the step its own taps cover.  Weights are computed on the fly from the
 // per-axis rule, so any tap count works, from 1 up to a whole 3840-pixel crop resized to one pixel; no weight table is kept.
 // All output addressing is 64-bit, and stores are the widest the address allows (store_elems).
+// Native calls (FPNGB_RESIZE_NATIVE): the ragged decode holds every file as uint16 values in the 16-bit domain (S = uint16_t), any
+// DST from 1 to 4; the resampled r is stored as cvt.rni.sat.u16(r), round_u8(r / 257) or T((r / 257) * scale + bias).
 #include "decode.cuh"
 #include "typed_store.cuh"
 #include "../../include/fpng_b200.h"
+#include <type_traits>
 
 namespace fpngb {
 
@@ -61,18 +64,39 @@ __device__ __forceinline__ void load_px(const uint8_t* a, float (&v)[DST])
     }
 }
 
-// the stored bits of the resampled value v of channel c: round_u8(v) for uint8, else T(v * scale[c] + bias[c])
-template <typename T>
-__device__ __forceinline__ uint32_t resized_bits(float v, int c, const PixelAffine& pa)
+// uint16 pixels of a native call: 8-byte (DST 4) or 4-byte (DST 2) aligned loads where the pixel size allows
+template <int DST>
+__device__ __forceinline__ void load_px16(const uint8_t* a, float (&v)[DST])
 {
-    if constexpr (sizeof(T) == 1) return typed_bits<T>(v);
-    else return typed_bits<T>(__fadd_rn(__fmul_rn(v, pa.scale[c]), pa.bias[c]));
+    if constexpr (DST == 4) {                                                   // 16-byte file bases, 8-byte pixels
+        const uint2 u = __ldg(reinterpret_cast<const uint2*>(a));
+        v[0] = (float)(u.x & 0xFFFFu); v[1] = (float)(u.x >> 16); v[2] = (float)(u.y & 0xFFFFu); v[3] = (float)(u.y >> 16);
+    } else if constexpr (DST == 2) {
+        const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(a));
+        v[0] = (float)(u & 0xFFFFu); v[1] = (float)(u >> 16);
+    } else {
+#pragma unroll
+        for (int c = 0; c < DST; c++) v[c] = (float)__ldg(reinterpret_cast<const unsigned short*>(a) + c);
+    }
 }
 
-template <int DST, bool PLANAR, typename T>
+// the stored bits of the resampled value v of channel c: round_u8(v) for uint8, else T(v * scale[c] + bias[c]); from a uint16
+// source (native calls): cvt.rni.sat.u16(v) for uint16, else the same rules applied to v / 257
+template <typename T, typename S>
+__device__ __forceinline__ uint32_t resized_bits(float v, int c, const PixelAffine& pa)
+{
+    if constexpr (std::is_same<T, uint16_t>::value) return typed_bits<T>(v);
+    else {
+        if constexpr (sizeof(S) == 2) v = __fdiv_rn(v, 257.0f);
+        if constexpr (sizeof(T) == 1) return typed_bits<T>(v);
+        else return typed_bits<T>(__fadd_rn(__fmul_rn(v, pa.scale[c]), pa.bias[c]));
+    }
+}
+
+template <int DST, bool PLANAR, typename T, typename S = uint8_t>
 __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams p, PixelAffine pa)
 {
-    constexpr int ES = sizeof(T);
+    constexpr int ES = sizeof(T), SS = sizeof(S);
     __shared__ float hbuf[kRsStep][kRsCols][DST];
     const uint32_t f = blockIdx.y;
     if (p.d_status[f] != 0) return;                                             // the same for the whole CTA
@@ -81,7 +105,7 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
     int top = 0, left = 0, bh = (int)fd.h, bw = (int)w;
     if (p.boxes) { const int32_t* b = p.boxes + (size_t)f * 4; top = b[0]; left = b[1]; bh = b[2]; bw = b[3]; }
     const uint8_t* src = p.px + p.px_offsets[f];
-    const size_t pitch = (size_t)w * DST;
+    const size_t pitch = (size_t)w * DST * SS;
     const float sx = __fdiv_rn((float)bw, (float)p.out_w), sy = __fdiv_rn((float)bh, (float)p.out_h);
     const bool aax = p.antialias && sx >= 1.f, aay = p.antialias && sy >= 1.f;
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, slot = threadIdx.x >> 3, grp = threadIdx.x & 7u;
@@ -107,11 +131,12 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
                 float h[DST];
 #pragma unroll
                 for (int c = 0; c < DST; c++) h[c] = 0.f;
-                const uint8_t* s = src + (size_t)(top + row) * pitch + (size_t)(left + hx.lo) * DST;
+                const uint8_t* s = src + (size_t)(top + row) * pitch + (size_t)(left + hx.lo) * DST * SS;
                 for (int j = 0; j < hx.size; j++) {
                     const float wt = tap_weight(hx.lo + j, hx.center, hx.inv);
                     float v[DST];
-                    load_px<DST>(s + (size_t)j * DST, v);
+                    if constexpr (SS == 2) load_px16<DST>(s + (size_t)j * DST * SS, v);
+                    else load_px<DST>(s + (size_t)j * DST, v);
 #pragma unroll
                     for (int c = 0; c < DST; c++) h[c] = fmaf(wt, v[c], h[c]);
                 }
@@ -138,7 +163,7 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
             for (int c = 0; c < DST; c++) {
                 uint32_t e[4];
 #pragma unroll
-                for (int q = 0; q < 4; q++) e[q] = resized_bits<T>(__fmul_rn(acc[q][c], vy.norm), c, pa);
+                for (int q = 0; q < 4; q++) e[q] = resized_bits<T, S>(__fmul_rn(acc[q][c], vy.norm), c, pa);
                 uint8_t* a = o + (size_t)c * p.chan;
                 if (npx == 4) store_elems<T>(a, e);
                 else for (uint32_t q = 0; q < npx; q++) store_elem(a + ES * q, e[q], ES);
@@ -146,7 +171,7 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
         } else {                                                                // 4 * DST * sizeof(T) contiguous bytes
             uint32_t e[4 * DST];
 #pragma unroll
-            for (int k = 0; k < 4 * DST; k++) e[k] = resized_bits<T>(__fmul_rn(acc[k / DST][k % DST], vy.norm), k % DST, pa);
+            for (int k = 0; k < 4 * DST; k++) e[k] = resized_bits<T, S>(__fmul_rn(acc[k / DST][k % DST], vy.norm), k % DST, pa);
             if (npx == 4) store_elems<T>(o, e);
             else {
 #pragma unroll
@@ -166,8 +191,36 @@ static void launch_resize(const ResizeParams& p, const PixelAffine& pa, uint32_t
     else { if (planar) decode_resize_kernel<4, true, T><<<g, kRsThreads, 0, s>>>(p, pa); else decode_resize_kernel<4, false, T><<<g, kRsThreads, 0, s>>>(p, pa); }
 }
 
+// native calls: the uint16 source at DST 1 .. 4
+template <int DST, typename T>
+static void launch_resize16_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cudaStream_t s)
+{
+    if constexpr (DST > 1) {                            // one channel: planar and interleaved address the same elements
+        if (p.pixel == sizeof(T)) { decode_resize_kernel<DST, true, T, uint16_t><<<g, kRsThreads, 0, s>>>(p, pa); return; }
+    }
+    decode_resize_kernel<DST, false, T, uint16_t><<<g, kRsThreads, 0, s>>>(p, pa);
+}
+template <typename T>
+static void launch_resize16(const ResizeParams& p, const PixelAffine& pa, uint32_t n, uint32_t desired, cudaStream_t s)
+{
+    const unsigned long long tiles = (unsigned long long)((p.out_w + kRsCols - 1) / kRsCols) * ((p.out_h + kRsRows - 1) / kRsRows);
+    const dim3 g((uint32_t)(tiles < 65535ull ? tiles : 65535ull), n);
+    if (desired == 1) launch_resize16_dst<1, T>(p, pa, g, s);
+    else if (desired == 2) launch_resize16_dst<2, T>(p, pa, g, s);
+    else if (desired == 3) launch_resize16_dst<3, T>(p, pa, g, s);
+    else launch_resize16_dst<4, T>(p, pa, g, s);
+}
+
 void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t n, uint32_t desired, cudaStream_t s)
 {
+    if (t.native) {
+        if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_resize16<float>(p, t.aff, n, desired, s);
+        else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_resize16<__half>(p, t.aff, n, desired, s);
+        else if (t.dtype == FPNGB_DTYPE_BFLOAT16) launch_resize16<__nv_bfloat16>(p, t.aff, n, desired, s);
+        else if (t.dtype == FPNGB_DTYPE_UINT16) launch_resize16<uint16_t>(p, t.aff, n, desired, s);
+        else launch_resize16<uint8_t>(p, t.aff, n, desired, s);
+        return;
+    }
     if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_resize<float>(p, t.aff, n, desired, s);
     else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_resize<__half>(p, t.aff, n, desired, s);
     else if (t.dtype == FPNGB_DTYPE_BFLOAT16) launch_resize<__nv_bfloat16>(p, t.aff, n, desired, s);

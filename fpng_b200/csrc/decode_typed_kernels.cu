@@ -7,15 +7,36 @@
 #include "unfilter.cuh"
 #include "typed_store.cuh"
 #include "../../include/fpng_b200.h"
+#include <type_traits>
 
 namespace fpngb {
 
-// byte k of the interleaved pixel bytes o[] (k = pixel * DST + channel), mapped to channel c and converted
+// byte k of the interleaved pixel bytes o[] (k = pixel * DST + channel), mapped to channel c and converted; the native calls'
+// uint8 and uint16 output (FPNGB_PNG_NATIVE) store the value v and v * 257, with no scale or bias
 template <typename T, int DST>
 __device__ __forceinline__ uint32_t typed_value(const uint32_t (&o)[DST], int k, int c, const PixelAffine& pa)
 {
-    const float v = __uint2float_rn((o[k >> 2] >> (8 * (k & 3))) & 0xFFu);
-    return typed_bits<T>(__fadd_rn(__fmul_rn(v, pa.scale[c]), pa.bias[c]));
+    const uint32_t b = (o[k >> 2] >> (8 * (k & 3))) & 0xFFu;
+    if constexpr (sizeof(T) == 1) return b;
+    else if constexpr (std::is_same<T, uint16_t>::value) return b * 257u;
+    else return typed_bits<T>(__fadd_rn(__fmul_rn(__uint2float_rn(b), pa.scale[c]), pa.bias[c]));
+}
+
+// DST 1 / 2 (native calls): the 4 pixels of a group as L or (L, A) bytes, L the luma of R, G, B (typed_store.cuh), A 255 for SRC 3
+template <int SRC, int DST>
+__device__ __forceinline__ void luma_row(const uint32_t (&px)[SRC], uint32_t (&o)[DST])
+{
+#pragma unroll
+    for (int i = 0; i < DST; i++) o[i] = 0;
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        const int k = q * SRC;
+        const uint32_t r = (px[k >> 2] >> (8 * (k & 3))) & 0xFFu, g = (px[(k + 1) >> 2] >> (8 * ((k + 1) & 3))) & 0xFFu,
+                       b = (px[(k + 2) >> 2] >> (8 * ((k + 2) & 3))) & 0xFFu;
+        const uint32_t a = SRC == 4 ? (px[(k + 3) >> 2] >> (8 * ((k + 3) & 3))) & 0xFFu : 0xFFu;
+        const uint32_t v = DST == 1 ? luma(r, g, b) : luma(r, g, b) | a << 8;
+        o[(q * DST) >> 2] |= v << (8 * ((q * DST) & 3));
+    }
 }
 
 // OutStrides in bytes: interleaved rows (pixel = DST * sizeof(T)) at any pitch, or planar (pixel = sizeof(T)); row 0: tight rows.
@@ -50,7 +71,12 @@ __global__ void __launch_bounds__(128) unfilter_typed_kernel(DecodeParams p, Out
             const uint32_t y = y0 + j;
             if (y >= h) break;
             uint32_t o[DST];
-            unfilter_row<SRC, DST>(acc, dd[j], summing, o);
+            if constexpr (DST >= 3) unfilter_row<SRC, DST>(acc, dd[j], summing, o);
+            else {
+                uint32_t px[SRC];
+                unfilter_row<SRC, SRC>(acc, dd[j], summing, px);
+                luma_row<SRC, DST>(px, o);
+            }
             uint8_t* orow = out + (size_t)y * out_pitch;
             if (PLANAR) {                                                       // 4 * sizeof(T) contiguous bytes per plane
 #pragma unroll
@@ -61,6 +87,15 @@ __global__ void __launch_bounds__(128) unfilter_typed_kernel(DecodeParams p, Out
                     uint8_t* a = orow + c * cs;
                     if (full) store_elems<T>(a, e);
                     else for (uint32_t q = 0; q < npx; q++) store_elem(a + ES * q, e[q], ES);
+                }
+            } else if (std::is_same<T, uint16_t>::value && full) {             // v * 257 is v in both bytes: 2 * DST words
+                uint32_t wd[2 * DST];
+#pragma unroll
+                for (int i = 0; i < DST; i++) { wd[2 * i] = __byte_perm(o[i], 0, 0x1100); wd[2 * i + 1] = __byte_perm(o[i], 0, 0x3322); }
+                if (((uintptr_t)orow & 3u) == 0u) store_elems<float, 2 * DST>(orow, wd);   // whole words where the address allows
+                else {                                                          // tight rows of odd w * DST: 2-byte aligned
+#pragma unroll
+                    for (int k = 0; k < 4 * DST; k++) store_elem(orow + 2 * k, wd[k >> 1] >> (16 * (k & 1)), 2);
                 }
             } else {                                                            // 4 * DST * sizeof(T) contiguous bytes
                 uint32_t e[4 * DST];
@@ -90,8 +125,34 @@ static void launch_typed(const DecodeParams& p, const OutStrides& os, const Pixe
     }
 }
 
+// native calls (FPNGB_PNG_NATIVE): interleaved tight rows of desired channels, or with desired 0 of the file's own (SRC)
+template <int SRC, typename T>
+static void launch_native_src(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t desired, dim3 g, cudaStream_t s)
+{
+    switch (desired ? desired : (uint32_t)SRC) {
+    case 1: unfilter_typed_kernel<SRC, 1, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
+    case 2: unfilter_typed_kernel<SRC, 2, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
+    case 3: unfilter_typed_kernel<SRC, 3, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
+    default: unfilter_typed_kernel<SRC, 4, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
+    }
+}
+template <typename T>
+static void launch_native(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t desired, dim3 g, cudaStream_t s)
+{
+    if (!p.chans || p.chans == 3) launch_native_src<3, T>(p, os, pa, desired, g, s);
+    if (!p.chans || p.chans == 4) launch_native_src<4, T>(p, os, pa, desired, g, s);
+}
+
 void launch_unfilter_typed(const DecodeParams& p, const OutStrides& os, const TypedOut& t, uint32_t desired, dim3 g, cudaStream_t s)
 {
+    if (t.native) {
+        if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_native<float>(p, os, t.aff, desired, g, s);
+        else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_native<__half>(p, os, t.aff, desired, g, s);
+        else if (t.dtype == FPNGB_DTYPE_BFLOAT16) launch_native<__nv_bfloat16>(p, os, t.aff, desired, g, s);
+        else if (t.dtype == FPNGB_DTYPE_UINT16) launch_native<uint16_t>(p, os, t.aff, desired, g, s);
+        else launch_native<uint8_t>(p, os, t.aff, desired, g, s);
+        return;
+    }
     if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_typed<float>(p, os, t.aff, desired, g, s);
     else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_typed<__half>(p, os, t.aff, desired, g, s);
     else launch_typed<__nv_bfloat16>(p, os, t.aff, desired, g, s);

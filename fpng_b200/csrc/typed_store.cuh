@@ -22,6 +22,15 @@ template <> __device__ __forceinline__ uint32_t typed_bits<float>(float v) { ret
 template <> __device__ __forceinline__ uint32_t typed_bits<__half>(float v) { return __half_as_ushort(__float2half_rn(v)); }
 template <> __device__ __forceinline__ uint32_t typed_bits<__nv_bfloat16>(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
 template <> __device__ __forceinline__ uint32_t typed_bits<uint8_t>(float v) { return round_u8(v); }
+// v rounded to nearest even and clamped to [0, 65535], NaN to 0: uint16 output of the native resized decode (FPNGB_RESIZE_NATIVE)
+template <> __device__ __forceinline__ uint32_t typed_bits<uint16_t>(float v)
+{
+    unsigned short q;
+    asm("cvt.rni.sat.u16.f32 %0, %1;" : "=h"(q) : "f"(v));
+    return q;
+}
+// The luma of 8-bit or 16-bit R, G, B (Pillow's convert("L") for 8-bit values; 32 bits hold it for 16-bit samples)
+__device__ __forceinline__ uint32_t luma(uint32_t r, uint32_t g, uint32_t b) { return (19595u * r + 38470u * g + 7471u * b + 0x8000u) >> 16; }
 
 __device__ __forceinline__ void store_elem(uint8_t* a, uint32_t bits, int size)
 {

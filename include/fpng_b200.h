@@ -541,6 +541,41 @@ FPNGB_API int fpngb_get_png_info(const void* file, uint32_t size, uint32_t* w, u
  *   they run with flags 0. */
 enum { FPNGB_PNG_ALL_FORMATS = 1 };
 enum { FPNGB_RESIZE_ALL_PNG_FORMATS = 8 };
+
+/* ---- native output in the any-PNG ragged decode (opt-in: FPNGB_PNG_NATIVE) -----------------------------------------------------
+ * With flags & FPNGB_PNG_NATIVE, fpngb_decode_packed_png_device_ex decodes each file at its own channel count and bit depth:
+ * desired_chans may be 0 (each file's own channels), 1, 2, 3 or 4, and fmt may also be FPNGB_DTYPE_UINT16.  Bit values 2 and
+ * 0x100 stay unknown; fpngb_get_png_info_*_ex keep rejecting FPNGB_PNG_NATIVE (the walk does not depend on it).
+ * Sample domain: files of depth <= 8 work in 8-bit values v (palette entries, sub-byte gray after the scaling above, tRNS alpha);
+ *   16-bit files in their 16-bit samples s.  Alpha the file lacks is the domain maximum; a color key gives 0 or the maximum.
+ * Storing: uint8 (fmt NULL) stores v, or s >> 8; float stores T(x * scale[c] + bias[c]) with x = v or s / 257 (the rules above);
+ *   uint16 (FPNGB_DTYPE_UINT16; scale and bias ignored, as uint8 takes none) stores v * 257, or s.
+ * Channels: desired 3 / 4 map as above.  desired 1 / 2: gray -> Y; gray+alpha -> Y or (Y, A); RGB, RGBA and palette -> L or (L, A)
+ *   with L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16 in the file's domain (8-bit values for depth <= 8 and palette entries,
+ *   16-bit samples for 16-bit files; 32 bits hold it either way).  For 8-bit files this is Pillow's convert("L") / ("LA").
+ *   fpng files follow the 8-bit RGB / RGBA rule.  desired 0: file i gets c_i = column 3 of its info row (fpng files 3 or 4).
+ * Placement: file i takes align_up(w*h*c_i*elem, 16) bytes, elem 1, 2 or 4; the w*h*desired > 0xFFFFFFFF rule
+ *   (FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE) uses c_i.  Statuses, their order, untouched failed outputs and the workspace rules
+ *   are the call's without the flag.
+ * Call-level checks (a rejected call enqueues nothing and writes nothing): FPNGB_ERR_INVALID_ARG for desired_chans above 4 or a bad
+ *   float fmt; FPNGB_ERR_ALIGNMENT for d_out % 16 as without the flag.  Without FPNGB_PNG_NATIVE every call keeps rejecting dtype
+ *   FPNGB_DTYPE_UINT16 (the *_typed calls included) and desired_chans other than 3 and 4.
+ * Kernels: the launches of the call without the flag, none added; desired 3 / 4 in uint8 and float give that call's bytes.
+ *
+ * fpngb_decode_packed_resized_device with flags & FPNGB_RESIZE_NATIVE (valid only together with FPNGB_RESIZE_ANY_PNG; alone:
+ *   FPNGB_ERR_INVALID_ARG; bits 2 and 8-alone stay rejected): desired_chans 1 .. 4 (0 is rejected: the batch has one shape), fmt
+ *   as above (NULL uint8, FPNGB_DTYPE_UINT16, or a float type).
+ *   * The ragged decode behind the resize holds every file as uint16 values of the desired channels, in the 16-bit domain above
+ *     (8-bit values v as v * 257); pixel_cap counts the bytes of that intermediate, align_up(w*h*desired_chans*2, 16) per file.
+ *   * The resample r runs on those values with the taps and weights above, and stores cvt.rni.sat.u16.f32(r) for uint16,
+ *     round_u8(r / 257) for uint8 and T((r / 257) * scale[c] + bias[c]) for a float fmt, every operation separately rounded.
+ *   * So a 16-bit file is resized from its full samples.  For an 8-bit file r / 257 may differ from the flag-off r in the last
+ *     float bit (the resample runs on 257 times the values), so float output may differ in its last bit from the call without
+ *     the flag; uint8 output may differ by one where r sits within that bit of a rounding tie.
+ *   * Launches, statuses and stream ordering are the call's without the flag. */
+enum { FPNGB_PNG_NATIVE = 4 };
+enum { FPNGB_DTYPE_UINT16 = 4 };
+enum { FPNGB_RESIZE_NATIVE = 16 };
 FPNGB_API int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
                                                 uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans,
                                                 void* d_out, size_t out_cap, uint64_t* d_out_offsets /* n+1 */,
