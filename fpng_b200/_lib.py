@@ -115,6 +115,8 @@ def lib() -> C.CDLL:
                                              C.c_void_p, C.c_void_p, C.c_void_p]
     L.fpngb_encode_png_ragged_device.restype = C.c_int
     L.fpngb_encode_png_ragged_device.argtypes = L.fpngb_encode_ragged_device.argtypes
+    L.fpngb_encode_png_ragged_device_typed.restype = C.c_int
+    L.fpngb_encode_png_ragged_device_typed.argtypes = L.fpngb_encode_ragged_device_typed.argtypes
     L.fpngb_decode_batch_host.restype = C.c_int
     L.fpngb_decode_batch_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, u32p, u32p, u32p, C.c_void_p]
     L.fpngb_train_accumulate_device.restype = C.c_int

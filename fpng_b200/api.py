@@ -321,28 +321,55 @@ def png_slot_offsets(shapes):
     return ofs
 
 
-def encode_png_device(images, flags: int = 0, out=None, stream=None):
-    """Encode device images of 1 to 4 channels, uint8 or uint16, to PNG in one call (fpngb_encode_png_ragged_device).
+def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None, depth=None):
+    """Encode device images of 1 to 4 channels to PNG in one call (fpngb_encode_png_ragged_device, or its _typed twin for float
+    images).
 
-    images: list of CUDA tensors [h, w, c], c from 1 to 4, torch.uint8 (8-bit samples) or torch.uint16 (16-bit samples, written
-    losslessly: depth maps, sensor frames), each contiguous or a view in one of the layouts of layout_strides (HWC rows at any
-    pitch, e.g. a crop, or CHW planes, e.g. x_chw.permute(1, 2, 0)).  uint8 images with 3 or 4 channels become fpng files,
-    byte-identical to encode_ragged_device's with the same flags; the others (masks, mattes, gray+alpha, 16-bit) become PNG files
-    with a per-row filter choice and a Huffman code built per image (include/fpng_b200.h).  Other dtypes raise ValueError.
+    images: list of CUDA tensors [h, w, c], c from 1 to 4, each contiguous or a view in one of the layouts of layout_strides (HWC
+    rows at any pitch, e.g. a crop, or CHW planes, e.g. x_chw.permute(1, 2, 0)).  Either
+      * torch.uint8 (8-bit samples) or torch.uint16 (16-bit samples, written losslessly: depth maps, sensor frames) images, in
+        any mix; depth, scale and bias must then be None; or
+      * images all of one float dtype, float32, float16 or bfloat16, written at `depth` bits per sample (8 or 16: one value for
+        the list or one per image; there is no default, so a depth map is never dropped to 8 bits by accident).  Channel c of
+        element x becomes nan_to_num(x.float() * scale[c] + bias[c], nan=0).round().clamp(0, 2**depth - 1), rounding half to
+        even, converted on the GPU (scale defaults to 1, bias to 0; one value or one per channel up to the list's largest
+        channel count).  Scale and bias are in the output's units: metres to 16-bit millimetres is depth=16, scale=1000.
+        Decoding a 16-bit file natively to float32 with scale k and encoding the result with scale 257 / k gives the file back;
+        float16 and bfloat16 cannot hold every 16-bit sample.
+    The file of an image is byte-identical to the one its quantised uint8 / uint16 image gives: 8-bit images with 3 or 4 channels
+    become fpng files, byte-identical to encode_ragged_device's with the same flags; the others (masks, mattes, gray+alpha,
+    16-bit) become PNG files with a per-row filter choice and a Huffman code built per image (include/fpng_b200.h).  Other
+    dtypes, a mixed float list and the argument combinations above raise ValueError.
     Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]) as encode_ragged_device does, offsets being
-    png_slot_offsets of the shapes -- the (data, offsets, sizes) that decode_packed_ragged_device(any_png=True,
+    png_slot_offsets of the (h, w, c, depth) shapes -- the (data, offsets, sizes) that decode_packed_ragged_device(any_png=True,
     all_formats=True) reads.  Kernels are enqueued on the current torch stream (or `stream`), with no host synchronisation."""
     import torch
 
     n = len(images)
+    dtypes = {t.dtype for t in images}
+    floats = {torch.float32, torch.float16, torch.bfloat16}
+    for dt in dtypes:
+        if dt not in floats and dt not in (torch.uint8, torch.uint16):
+            raise ValueError(f"encode_png_device: torch.uint8, uint16, float32, float16 or bfloat16 images are needed, got {dt}")
+    fmt = None
+    if dtypes & floats:
+        if len(dtypes) > 1:
+            raise ValueError(f"encode_png_device: float images are all one dtype, got {sorted(map(str, dtypes))}")
+        if depth is None:
+            raise ValueError("encode_png_device: float images need depth=8 or depth=16 (one value, or one per image)")
+        depths = [depth] * n if np.ndim(depth) == 0 else list(depth)
+        if len(depths) != n or any(d not in (8, 16) for d in depths):
+            raise ValueError(f"encode_png_device: depth is 8 or 16, one value or one per image ({n}), got {depth}")
+        fmt = _pixel_format(images[0].dtype, scale, bias, max(int(t.shape[-1]) for t in images), "encode_png_device")
+    elif depth is not None or scale is not None or bias is not None:
+        raise ValueError("encode_png_device: depth, scale and bias apply to float images only; uint8 / uint16 are taken as they are")
     ptrs, dims, strides = [], [], []
-    for t in images:
-        if t.dtype not in (torch.uint8, torch.uint16):
-            raise ValueError(f"encode_png_device: torch.uint8 or torch.uint16 images are needed, got {t.dtype}")
+    for i, t in enumerate(images):
         assert t.is_cuda and t.dim() == 3, "images: [h, w, c] CUDA tensors"
         h, w, c = t.shape
         es = t.element_size()
-        ptrs.append(t.data_ptr()); dims.append((w, h, c, 8 * es)); strides.append(tuple(v * es for v in t.stride()))
+        ptrs.append(t.data_ptr()); dims.append((w, h, c, int(depths[i]) if fmt is not None else 8 * es))
+        strides.append(tuple(v * es for v in t.stride()))
     ptrs = np.array(ptrs, dtype=np.uint64)
     dims = np.array(dims, dtype=np.uint32).reshape(n, 4)
     strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
@@ -353,9 +380,12 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None):
     _check_arg(out, "out", device, torch.uint8)
     offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
     sizes = torch.empty((n,), dtype=torch.int32, device=device)
-    rc = lib().fpngb_encode_png_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
-                                              strides.ctypes.data_as(C.c_void_p), flags, out.data_ptr(), out.numel(),
-                                              offsets.data_ptr(), sizes.data_ptr(), _stream(stream, device))
+    args = (n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p), strides.ctypes.data_as(C.c_void_p))
+    rest = (flags, out.data_ptr(), out.numel(), offsets.data_ptr(), sizes.data_ptr(), _stream(stream, device))
+    if fmt is not None:
+        rc = lib().fpngb_encode_png_ragged_device_typed(*args, C.byref(fmt), *rest)
+    else:
+        rc = lib().fpngb_encode_png_ragged_device(*args, *rest)
     check(rc, "encode_png_device")
     return out, offsets, sizes
 

@@ -1,17 +1,20 @@
-// fpng_b200/csrc/encode_typed_kernels.cu -- the conversion pre-pass of the encode calls: strided input -> tight uint8 HWC rows.
+// fpng_b200/csrc/encode_typed_kernels.cu -- the conversion pre-pass of the encode calls: strided input -> tight integer HWC rows.
 //
-// convert_pixels_kernel<T, LAYOUT> reads an [n, h, w, chans] batch of T in an interleaved or planar layout ("Pixel layouts" of
-// include/fpng_b200.h, strides in bytes) and writes tight uint8 rows (pitch w * chans) into a library buffer; the uint8 encode
-// pipeline then runs on that buffer unchanged.  Two uses:
-//  * the *_typed encode calls (T = float, __half, __nv_bfloat16): every element becomes
+// convert_pixels_kernel<T, LAYOUT, PNG> reads an [n, h, w, chans] batch of T in an interleaved or planar layout ("Pixel layouts"
+// of include/fpng_b200.h, strides in bytes) and writes tight rows of OB-byte samples (pitch w * chans * OB) into a library buffer;
+// the integer encode pipeline then runs on that buffer unchanged.  Three uses:
+//  * the *_typed fpng encode calls (T = float, __half, __nv_bfloat16; 3 or 4 channels, OB = 1): every element becomes
 //        q = cvt.rni.sat.u8.f32( __fadd_rn(__fmul_rn((float)x, scale[c]), bias[c]) )
 //    -- two separately rounded fp32 operations, never an FMA, then one round-to-nearest-even conversion that clamps to [0, 255]
 //    and maps NaN to 0 (PTX ISA, cvt: float-to-integer conversions saturate, NaN converts to 0);
+//  * the typed PNG encode call (PNG = true: 1 to 4 channels, OB from ConvDesc::sample_bytes): the same rule, with
+//    cvt.rni.sat.u16.f32 for 16-bit samples, stored as native little-endian uint16 (the PNG row kernels swap the bytes);
 //  * the strided uint8 input of the encoders that read tight rows only (the generic 4-pixel kernels, the single-pass encoder):
 //    T = uint8_t, a plain copy.
 // Each thread converts a group of 4 pixels of one row with the widest loads the address allows (16, 8, then 4 bytes, single
 // elements at row ends).  The CTAs of a launch cover one or more descriptors; a CTA finds its descriptor by a binary search over
-// their CTA prefix, as ragged_locate does.  All input addressing is 64-bit.
+// their CTA prefix, as ragged_locate does.  All input addressing is 64-bit.  The PNG call has its own instantiations, so that the
+// wider run-time switch costs the fpng calls' kernels no registers.
 #include "kernels.cuh"
 #include "typed_store.cuh"
 #include "../../include/fpng_b200.h"
@@ -27,14 +30,16 @@ template <> __device__ __forceinline__ float elem_to_float<float>(uint32_t bits)
 template <> __device__ __forceinline__ float elem_to_float<__half>(uint32_t bits) { return __half2float(__ushort_as_half((unsigned short)bits)); }
 template <> __device__ __forceinline__ float elem_to_float<__nv_bfloat16>(uint32_t bits) { return __uint_as_float(bits << 16); }
 
-// element bits -> the uint8 the encoder reads
-template <typename T>
+// element bits -> the OB-byte sample the encoder reads
+template <typename T, int OB>
 __device__ __forceinline__ uint32_t quantize(uint32_t bits, float scale, float bias)
 {
     if constexpr (sizeof(T) == 1) {
         return bits;
     } else {
-        return round_u8(__fadd_rn(__fmul_rn(elem_to_float<T>(bits), scale), bias));
+        const float y = __fadd_rn(__fmul_rn(elem_to_float<T>(bits), scale), bias);
+        if constexpr (OB == 1) return round_u8(y);
+        else return typed_bits<uint16_t>(y);                               // cvt.rni.sat.u16.f32
     }
 }
 
@@ -117,12 +122,12 @@ __device__ __forceinline__ void store_words(uint8_t* a, const uint32_t (&wd)[NW]
     }
 }
 
-// One group of up to 4 pixels (x0 .. x0 + npx - 1) of one row: src at pixel x0 of the row, dst at byte x0 * CH of the tight row.
-template <typename T, bool PLANAR, int CH>
+// One group of up to 4 pixels (x0 .. x0 + npx - 1) of one row: src at pixel x0 of the row, dst at byte x0 * CH * OB of the tight row.
+template <typename T, bool PLANAR, int CH, int OB>
 __device__ __forceinline__ void convert_group(const uint8_t* src, unsigned long long chan, uint8_t* dst, uint32_t npx, const ConvertParams& p)
 {
     constexpr int ES = sizeof(T);
-    uint32_t q[4 * CH];                                                     // output bytes, interleaved
+    uint32_t q[4 * CH];                                                     // output samples, interleaved
     if (npx == 4) {
         if (PLANAR) {                                                       // 4 * ES contiguous bytes per plane
 #pragma unroll
@@ -130,31 +135,36 @@ __device__ __forceinline__ void convert_group(const uint8_t* src, unsigned long 
                 uint32_t wd[ES];
                 load_words<ES>(src + c * chan, wd);
 #pragma unroll
-                for (int k = 0; k < 4; k++) q[k * CH + c] = quantize<T>(word_elem<ES>(wd, k), p.scale[c], p.bias[c]);
+                for (int k = 0; k < 4; k++) q[k * CH + c] = quantize<T, OB>(word_elem<ES>(wd, k), p.scale[c], p.bias[c]);
             }
         } else {                                                            // 4 * CH * ES contiguous bytes
             uint32_t wd[CH * ES];
             load_words<ES>(src, wd);
 #pragma unroll
-            for (int k = 0; k < 4 * CH; k++) q[k] = quantize<T>(word_elem<ES>(wd, k), p.scale[k % CH], p.bias[k % CH]);
+            for (int k = 0; k < 4 * CH; k++) q[k] = quantize<T, OB>(word_elem<ES>(wd, k), p.scale[k % CH], p.bias[k % CH]);
         }
-        uint32_t ow[CH];
+        uint32_t ow[CH * OB];
 #pragma unroll
-        for (int k = 0; k < CH; k++) ow[k] = q[4 * k] | (q[4 * k + 1] << 8) | (q[4 * k + 2] << 16) | (q[4 * k + 3] << 24);
+        for (int k = 0; k < CH * OB; k++) {
+            if constexpr (OB == 1) ow[k] = q[4 * k] | (q[4 * k + 1] << 8) | (q[4 * k + 2] << 16) | (q[4 * k + 3] << 24);
+            else ow[k] = q[2 * k] | (q[2 * k + 1] << 16);
+        }
         store_words(dst, ow);
     } else {                                                                // row end: element by element
         for (uint32_t x = 0; x < npx; x++) {
 #pragma unroll
             for (int c = 0; c < CH; c++) {
                 const uint8_t* a = PLANAR ? src + (size_t)x * ES + c * chan : src + ((size_t)x * CH + c) * ES;
-                dst[x * CH + c] = (uint8_t)quantize<T>(load_elem<ES>(a), p.scale[c], p.bias[c]);
+                const uint32_t v = quantize<T, OB>(load_elem<ES>(a), p.scale[c], p.bias[c]);
+                if constexpr (OB == 1) dst[x * CH + c] = (uint8_t)v;
+                else reinterpret_cast<uint16_t*>(dst)[x * CH + c] = (uint16_t)v;   // dst is even: even pitch, 16-byte aligned base
             }
         }
     }
 }
 
 // CTA b - d.cta_start of descriptor d: items (image, row, 4-pixel group) in that order, kConvThreads per CTA.
-template <typename T, bool PLANAR, int CH>
+template <typename T, bool PLANAR, int CH, int OB = 1>
 __device__ __forceinline__ void convert_cta(const ConvDesc& d, unsigned long long local, const ConvertParams& p)
 {
     constexpr int ES = sizeof(T);
@@ -164,11 +174,23 @@ __device__ __forceinline__ void convert_cta(const ConvDesc& d, unsigned long lon
     if (item >= (unsigned long long)d.h * groups) return;
     const uint32_t y = (uint32_t)(item / groups), x0 = (uint32_t)(item - (unsigned long long)y * groups) * 4u;
     const uint8_t* src = d.src + img * d.image + (unsigned long long)y * d.row + (unsigned long long)x0 * (PLANAR ? ES : CH * ES);
-    uint8_t* dst = p.dst + d.dst + (img * d.h + y) * ((unsigned long long)d.w * CH) + (unsigned long long)x0 * CH;
-    convert_group<T, PLANAR, CH>(src, d.chan, dst, min(4u, d.w - x0), p);
+    uint8_t* dst = p.dst + d.dst + (img * d.h + y) * ((unsigned long long)d.w * CH * OB) + (unsigned long long)x0 * CH * OB;
+    convert_group<T, PLANAR, CH, OB>(src, d.chan, dst, min(4u, d.w - x0), p);
 }
 
-template <typename T, int LAYOUT>
+// the PNG call's descriptors: 1 to 4 channels, OB = d.sample_bytes; one channel has no planes, so it reads as interleaved rows
+template <typename T, bool PLANAR, int OB>
+__device__ __forceinline__ void convert_cta_png(const ConvDesc& d, unsigned long long local, const ConvertParams& p)
+{
+    switch (d.chans) {
+    case 1: convert_cta<T, false, 1, OB>(d, local, p); break;
+    case 2: convert_cta<T, PLANAR, 2, OB>(d, local, p); break;
+    case 3: convert_cta<T, PLANAR, 3, OB>(d, local, p); break;
+    default: convert_cta<T, PLANAR, 4, OB>(d, local, p); break;
+    }
+}
+
+template <typename T, int LAYOUT, bool PNG>
 __global__ void __launch_bounds__(kConvThreads) convert_pixels_kernel(ConvertParams p)
 {
     for (unsigned long long b = blockIdx.x; b < p.total_ctas; b += gridDim.x) {
@@ -183,7 +205,10 @@ __global__ void __launch_bounds__(kConvThreads) convert_pixels_kernel(ConvertPar
         const ConvDesc d = p.count > 1 ? p.desc[lo] : p.one;             // by value: no local copy of the parameter block
         const unsigned long long local = b - d.cta_start;
         const bool planar = LAYOUT == kConvAny ? d.planar != 0 : LAYOUT == kConvPlanar;
-        if (planar) { if (d.chans == 3) convert_cta<T, true, 3>(d, local, p); else convert_cta<T, true, 4>(d, local, p); }
+        if constexpr (PNG) {
+            if (d.sample_bytes == 2) { if (planar) convert_cta_png<T, true, 2>(d, local, p); else convert_cta_png<T, false, 2>(d, local, p); }
+            else { if (planar) convert_cta_png<T, true, 1>(d, local, p); else convert_cta_png<T, false, 1>(d, local, p); }
+        } else if (planar) { if (d.chans == 3) convert_cta<T, true, 3>(d, local, p); else convert_cta<T, true, 4>(d, local, p); }
         else { if (d.chans == 3) convert_cta<T, false, 3>(d, local, p); else convert_cta<T, false, 4>(d, local, p); }
     }
 }
@@ -193,23 +218,31 @@ uint32_t convert_ctas_per_image(uint32_t w, uint32_t h)
     return (uint32_t)(((unsigned long long)h * ((w + 3u) >> 2) + kConvThreads - 1) / kConvThreads);
 }
 
-template <typename T>
+template <typename T, bool PNG>
 static void launch_t(const ConvertParams& p, int layout, uint32_t grid, cudaStream_t s)
 {
-    if (layout == kConvInterleaved) convert_pixels_kernel<T, kConvInterleaved><<<grid, kConvThreads, 0, s>>>(p);
-    else if (layout == kConvPlanar) convert_pixels_kernel<T, kConvPlanar><<<grid, kConvThreads, 0, s>>>(p);
-    else convert_pixels_kernel<T, kConvAny><<<grid, kConvThreads, 0, s>>>(p);
+    if (layout == kConvInterleaved) convert_pixels_kernel<T, kConvInterleaved, PNG><<<grid, kConvThreads, 0, s>>>(p);
+    else if (layout == kConvPlanar) convert_pixels_kernel<T, kConvPlanar, PNG><<<grid, kConvThreads, 0, s>>>(p);
+    else convert_pixels_kernel<T, kConvAny, PNG><<<grid, kConvThreads, 0, s>>>(p);
 }
 
-void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, cudaStream_t s)
+template <bool PNG>
+static void launch_float(const ConvertParams& p, uint32_t dtype, int layout, uint32_t grid, cudaStream_t s)
+{
+    if (dtype == FPNGB_DTYPE_FLOAT32) launch_t<float, PNG>(p, layout, grid, s);
+    else if (dtype == FPNGB_DTYPE_FLOAT16) launch_t<__half, PNG>(p, layout, grid, s);
+    else launch_t<__nv_bfloat16, PNG>(p, layout, grid, s);
+}
+
+void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, bool png, cudaStream_t s)
 {
     if (!p.total_ctas) return;
     const uint32_t grid = (uint32_t)(p.total_ctas < (1ull << 24) ? p.total_ctas : (1ull << 24));   // grid-stride beyond that
-    if (dtype == FPNGB_DTYPE_FLOAT32) launch_t<float>(p, layout, grid, s);
-    else if (dtype == FPNGB_DTYPE_FLOAT16) launch_t<__half>(p, layout, grid, s);
-    else if (dtype == FPNGB_DTYPE_BFLOAT16) launch_t<__nv_bfloat16>(p, layout, grid, s);
-    else if (layout == kConvPlanar) convert_pixels_kernel<uint8_t, kConvPlanar><<<grid, kConvThreads, 0, s>>>(p);   // uint8 copy
-    else convert_pixels_kernel<uint8_t, kConvInterleaved><<<grid, kConvThreads, 0, s>>>(p);
+    if (dtype == 0) {                                                                                // uint8 copy
+        if (layout == kConvPlanar) convert_pixels_kernel<uint8_t, kConvPlanar, false><<<grid, kConvThreads, 0, s>>>(p);
+        else convert_pixels_kernel<uint8_t, kConvInterleaved, false><<<grid, kConvThreads, 0, s>>>(p);
+    } else if (png) launch_float<true>(p, dtype, layout, grid, s);
+    else launch_float<false>(p, dtype, layout, grid, s);
 }
 
 }  // namespace fpngb

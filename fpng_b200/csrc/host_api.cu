@@ -200,17 +200,20 @@ static void prof_mark(ProfSet* ps, int slot, cudaStream_t s)
     ps->used[slot] = true;
 }
 
-// The conversion descriptor of n images of one shape in byte layout L whose tight uint8 rows go to byte dst of the conversion
-// buffer, converted by the CTAs from cta_start on.
+// The conversion descriptor of n images of one shape in byte layout L whose tight rows of sample_bytes-byte samples go to byte dst
+// of the conversion buffer, converted by the CTAs from cta_start on.
 static ConvDesc conv_desc(const uint8_t* src, const Layout& L, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint64_t dst,
-                          uint64_t cta_start)
+                          uint64_t cta_start, uint32_t sample_bytes = 1)
 {
-    return ConvDesc{src, L.image, L.row, L.chan, dst, cta_start, n, w, h, chans, convert_ctas_per_image(w, h), L.planar ? 1u : 0u};
+    return ConvDesc{src, L.image, L.row, L.chan, dst, cta_start, n, w, h, chans, convert_ctas_per_image(w, h), L.planar ? 1u : 0u,
+                    sample_bytes};
 }
 
 // One launch of the conversion pre-pass over the count descriptors hd (ascending cta_start; for count > 1 also uploaded to d_desc)
-// into tight uint8 rows at dst, the uint8 copy for f.dtype 0.  Profiled in slot kProfConvert of the encode that follows it on the stream.
-static void convert_enqueue(const ConvDesc* hd, uint32_t count, const ConvDesc* d_desc, const PixelFormat& f, uint8_t* dst, cudaStream_t s)
+// into tight rows at dst, the uint8 copy for f.dtype 0; png: the PNG call's instantiations (1 to 4 channels, 8- or 16-bit samples).
+// Profiled in slot kProfConvert of the encode that follows it on the stream.
+static void convert_enqueue(const ConvDesc* hd, uint32_t count, const ConvDesc* d_desc, const PixelFormat& f, uint8_t* dst, cudaStream_t s,
+                            bool png = false)
 {
     ConvertParams cp{};
     cp.one = hd[0]; cp.desc = d_desc; cp.count = count; cp.dst = dst;
@@ -221,7 +224,7 @@ static void convert_enqueue(const ConvDesc* hd, uint32_t count, const ConvDesc* 
     prof_drop_conv();
     ProfSet* ps = g_profile ? prof_alloc() : nullptr;
     if (ps) cudaEventRecord(ps->conv_start, s);
-    launch_convert_pixels(cp, f.dtype, planar == 0 ? kConvInterleaved : planar == count ? kConvPlanar : kConvAny, s);
+    launch_convert_pixels(cp, f.dtype, planar == 0 ? kConvInterleaved : planar == count ? kConvPlanar : kConvAny, png, s);
     count_launch(1);
     if (ps) { prof_mark(ps, kProfConvert, s); g_prof_conv = ps; }
 }
@@ -977,12 +980,24 @@ int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const u
     return encode_ragged_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
 }
 
-int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
-                                   void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+// Body of fpngb_encode_png_ragged_device (typed false, fmt unused) and fpngb_encode_png_ragged_device_typed (fmt required).  A typed
+// call first converts every image in one launch into tight rows of its output depth in c.conv; from there on it is the untyped
+// call on those rows.  The conversion and both routes sit inside one workspace bracket (ws_acquire ... the last ws_release), so a
+// call on another stream cannot overwrite c.conv before this call's kernels have read it.
+static int encode_png_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
+                           const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
+                           uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
     if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
+    PixelFormat f = uint8_format();
+    if (typed) {                                        // scale and bias are in use up to the largest channel count
+        uint32_t max_chans = 0;
+        for (uint32_t i = 0; i < n; i++) max_chans = std::max(max_chans, dims[4 * i + 2]);
+        const int rc = parse_format(fmt, max_chans, f);
+        if (rc) return rc;
+    }
     std::vector<RaggedImage> im(n);
     std::vector<Layout> src(n);
     std::vector<uint32_t> depth(n), fpng_ids, png_ids;
@@ -990,17 +1005,17 @@ int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uin
     for (uint32_t i = 0; i < n; i++) {
         const uint32_t w = dims[4 * i], h = dims[4 * i + 1], chans = dims[4 * i + 2], dep = dims[4 * i + 3];
         if (!pixels[i] || (dep != 8 && dep != 16) || chans < 1 || chans > 4) return FPNGB_ERR_INVALID_ARG;
-        const uint32_t es = dep / 8, bpp = chans * es;
+        const uint32_t es = typed ? f.elem : dep / 8, bpp = chans * dep / 8;   // input element and output pixel bytes
         const bool fpng = dep == 8 && chans >= 3;                        // fpng's files, as fpngb_encode_ragged_device writes them
         if (fpng ? !valid_dims(w, h, chans)
                  : (w < 1 || h < 1 || w > (1u << 24) || h > (1u << 24) || max_encoded_size(w, h, bpp) > 0x7FFFFFFFull))
             return FPNGB_ERR_INVALID_ARG;                                 // one IDAT chunk must hold the stored file
-        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * bpp, pixel = strides ? strides[3 * i + 1] : bpp;
+        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans * es, pixel = strides ? strides[3 * i + 1] : chans * es;
         const uint64_t chan = (strides && chans > 1) ? strides[3 * i + 2] : es;   // a single channel's stride addresses nothing
         Layout& L = src[i];
         const int rc = check_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, chan, 1, h, w, chans, es, false, L);
         if (rc) return rc;
-        if (L.row > 0xFFFFFFFFull) return FPNGB_ERR_INVALID_ARG;          // the kernels take a 32-bit row pitch
+        if (!typed && L.row > 0xFFFFFFFFull) return FPNGB_ERR_INVALID_ARG;  // the integer kernels take a 32-bit row pitch
         im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
         depth[i] = dep;
         (fpng ? fpng_ids : png_ids).push_back(i);
@@ -1014,11 +1029,24 @@ int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uin
     cudaStream_t s = (cudaStream_t)stream;
     uint8_t* out = (uint8_t*)d_out;
 
-    // staging: d_out_offsets (n + 1), then the fpng images' table and work lists, then the PNG images' table and work lists
+    // typed: the conversion buffer holds image i's tight rows (w * chans samples of depth / 8 bytes) at a 16-byte aligned offset
+    // at[i], then the descriptor table at desc_at
+    std::vector<uint64_t> at(typed ? n : 0);
+    uint64_t desc_at = 0;
+    if (typed) {
+        for (uint32_t i = 0; i < n; i++) { at[i] = desc_at; desc_at += align_up((uint64_t)im[i].w * im[i].h * im[i].chans * (depth[i] / 8), 16); }
+        desc_at = align_up(desc_at, 256);
+        const int rc = c.conv.reserve(desc_at + (size_t)n * sizeof(ConvDesc));
+        if (rc) return rc;
+    }
+
+    // staging: d_out_offsets (n + 1), then the fpng images' table and work lists, then the PNG images' table and work lists, then
+    // (typed) the conversion descriptors
     const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
     const size_t fpng_table = align_up(align_up(fpng_ids.size() * sizeof(ImageDesc), 16) + fpng_ids.size() * 5 * 4, 16);
+    const size_t conv_stage = align_up(ofs_bytes + fpng_table + png_table_bytes(png_ids.size()), 16);
     StageSlot* sl = nullptr;
-    int rc = c.stage_slot(ofs_bytes + fpng_table + png_table_bytes(png_ids.size()), &sl);
+    int rc = c.stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
     if (rc) return rc;
     uint8_t* stage = (uint8_t*)sl->buf.p;
     uint64_t* h_ofs = (uint64_t*)stage;
@@ -1026,6 +1054,25 @@ int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uin
     h_ofs[n] = total;
     FPNGB_CUDA_OK(cudaMemcpyAsync(d_out_offsets, h_ofs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
 
+    if (typed) {
+        uint8_t* cb = (uint8_t*)c.conv.p;
+        ConvDesc* hd = (ConvDesc*)(stage + conv_stage);
+        unsigned long long ctas = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            RaggedImage& r = im[i];
+            const uint32_t ob = depth[i] / 8;
+            hd[i] = conv_desc(r.pixels, src[i], 1, r.w, r.h, r.chans, at[i], ctas, ob);
+            ctas += hd[i].ctas_per_image;
+            r.pixels = cb + at[i]; r.row = (uint64_t)r.w * r.chans * ob; r.chan = 0;
+            src[i] = Layout{r.h * r.row, r.row, (uint64_t)r.chans * ob, ob, false};
+        }
+        rc = c.ws_acquire(s);
+        if (rc) return rc;
+        FPNGB_CUDA_OK(cudaMemcpyAsync(cb + desc_at, hd, (size_t)n * sizeof(ConvDesc), cudaMemcpyHostToDevice, s));
+        convert_enqueue(hd, n, (const ConvDesc*)(cb + desc_at), f, cb, s, true);
+    }
+    // a route that fails after the conversion still closes the bracket, so that later calls wait for the conversion
+    auto fail = [&](int code) { prof_drop_conv(); if (typed) c.ws_release(s); cudaEventRecord(sl->ev, s); return code; };
     // the fpng images take fpngb_encode_ragged_device's route: the ragged pipeline, or the uniform one image by image where the
     // 16-pixel kernels do not apply
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
@@ -1036,19 +1083,33 @@ int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uin
         if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
             const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
             rc = encode_batch_locked(c, r.pixels, src[i], uint8_format(), 1, r.w, r.h, r.chans, flags, out + r.slot, slot, d_sizes + i, s);
-            if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+            if (rc) return fail(rc);
         } else ids.push_back(i);
     }
     if (!ids.empty()) {
         rc = encode_ragged_locked(c, im, ids, flags, out, d_sizes, s, stage + ofs_bytes);
-        if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+        if (rc) return fail(rc);
     }
     if (!png_ids.empty()) {
         rc = encode_png_locked(c, im, depth, png_ids, flags, out, d_sizes, s, stage + ofs_bytes + fpng_table, fpng_ids.empty());
-        if (rc) { cudaEventRecord(sl->ev, s); return rc; }
+        if (rc) return fail(rc);
     }
+    prof_drop_conv();
     FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
     return FPNGB_OK;
+}
+
+int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
+                                   void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    return encode_png_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+int fpngb_encode_png_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                         const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap,
+                                         uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    return encode_png_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
 }
 
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)

@@ -188,9 +188,10 @@ void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint
 void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s);
 void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s);
 
-// Conversion pre-pass (encode_typed_kernels.cu): strided input of T -> tight uint8 HWC rows.  One descriptor is an image, or with
-// n > 1 a batch of n images of one shape: element (i, y, x, c) at src + i*image + y*row + x*pixel + c*chan bytes, where pixel is
-// chans * sizeof(T) (interleaved) or sizeof(T) (planar), goes to byte dst + ((i*h + y)*w + x)*chans + c of ConvertParams::dst.
+// Conversion pre-pass (encode_typed_kernels.cu): strided input of T -> tight HWC rows of integer samples.  One descriptor is an
+// image, or with n > 1 a batch of n images of one shape: element (i, y, x, c) at src + i*image + y*row + x*pixel + c*chan bytes,
+// where pixel is chans * sizeof(T) (interleaved) or sizeof(T) (planar), goes to sample (((i*h + y)*w + x)*chans + c) of
+// sample_bytes bytes from byte dst of ConvertParams::dst.  sample_bytes is 1 (uint8) except in the PNG call (2: uint16).
 struct ConvDesc {
     const uint8_t* src;
     unsigned long long image, row, chan;          // byte strides (chan: the plane stride of a planar image)
@@ -199,6 +200,7 @@ struct ConvDesc {
     uint32_t n, w, h, chans;
     uint32_t ctas_per_image;                      // convert_ctas_per_image(w, h)
     uint32_t planar;
+    uint32_t sample_bytes;                        // bytes per output sample: 1, or 2 for 16-bit PNG output (png launches only)
 };
 struct ConvertParams {
     ConvDesc one;                                 // count == 1: the only descriptor, passed by value
@@ -210,8 +212,9 @@ struct ConvertParams {
 };
 enum { kConvInterleaved = 0, kConvPlanar = 1, kConvAny = 2 };   // kConvAny: per descriptor (ConvDesc::planar)
 uint32_t convert_ctas_per_image(uint32_t w, uint32_t h);
-// dtype: an FPNGB_DTYPE_* value, or 0 for the uint8 copy (kConvInterleaved or kConvPlanar only)
-void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, cudaStream_t s);
+// dtype: an FPNGB_DTYPE_* value, or 0 for the uint8 copy (kConvInterleaved or kConvPlanar only).  png: the typed PNG call's
+// instantiations (a float dtype; 1 to 4 channels and sample_bytes 1 or 2 per descriptor), else 3 or 4 channels of uint8 output.
+void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, bool png, cudaStream_t s);
 
 void launch_scan(const ScanParams& p, uint32_t n, uint32_t chans, int mode, bool hist, cudaStream_t s);
 bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans);

@@ -621,6 +621,38 @@ FPNGB_API int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixel
                                                const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap,
                                                uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
 
+/* ---- typed PNG encode input: float32 / float16 / bfloat16 pixels to 8- or 16-bit PNG samples -------------------------------
+ * fpngb_encode_png_ragged_device_typed: the arguments of fpngb_encode_png_ragged_device plus fmt.  Image i has an output depth
+ * D_i (dims[4i + 3]: 8 or 16; the element type is fmt->dtype) and M = 2^D_i - 1.  Channel c of each element x of T becomes the
+ * sample
+ *     f = (float)x                                        exact for all three types
+ *     y = (f * scale[c]) + bias[c]                        two separately rounded fp32 operations, never an FMA
+ *     q = NaN(y) ? 0 : clamp(round_half_to_even(y), 0, M) cvt.rni.sat.u8.f32 / cvt.rni.sat.u16.f32
+ *   For D = 8 this is the rule of the typed encode calls above, bit for bit.  Scale and bias are in the OUTPUT's units: depth in
+ *   metres at D = 16 with scale 1000 writes millimetres.  In torch: torch.nan_to_num(x.float() * s + b, nan=0.0).round()
+ *   .clamp(0, M).to(torch.uint8 or torch.uint16).
+ *   The file written for image i is byte-identical, for every flag, to what fpngb_encode_png_ragged_device writes for the
+ *   quantised uint8 / uint16 image q: D = 8 with 3 or 4 channels gives an fpng file (identical to fpngb_encode_ragged_device_typed's,
+ *   fallbacks included), everything else the PNG format of DESIGN.md §4.6.
+ *   Inverse of the native float decode: a 16-bit sample s decoded to float32 with scale k is x = fl(fl(s / 257) * k); encoding x
+ *   at D = 16 with scale 257 / k gives s back, for every s (checked exhaustively for k = 257, 0.257 and 257 / 65535).  float16
+ *   and bfloat16 cannot hold every 16-bit sample, so a lossless 16-bit round trip needs float32.
+ *     strides  in BYTES of T (or NULL for tight HWC rows of T), the layouts of "Pixel layouts"; all input addressing is 64-bit,
+ *              so the input rows have no 32-bit pitch limit.
+ *   Slots, d_out_offsets, d_sizes, flags and stream ordering: those of fpngb_encode_png_ragged_device (slot i is sized by
+ *   fpngb_max_encoded_size(w, h, chans * D_i / 8)).
+ *   Call-level checks (a rejected call enqueues nothing and writes nothing): those of fpngb_encode_png_ragged_device, with its
+ *   16-bit parity rule replaced by FPNGB_ERR_ALIGNMENT unless every address and stride is a multiple of sizeof(T); and
+ *   FPNGB_ERR_INVALID_ARG for a NULL fmt, a dtype other than float32, float16 or bfloat16 (FPNGB_DTYPE_UINT16 input is the
+ *   untyped call's), or a scale or bias entry in use (index < the call's largest chans) that is not finite.
+ *   How: one conversion launch for the whole call, whatever its mix of depths, channel counts and layouts, writes tight rows of
+ *   each image's samples (native little-endian uint16 for D = 16) into the library-owned buffer of the typed encode calls, which
+ *   needs sum(align16(w * h * chans * D / 8)) bytes; then the untyped call's launches run on those rows.  fpngb_profile_read
+ *   reports the conversion kernel in slot 9. */
+FPNGB_API int fpngb_encode_png_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                                   const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap,
+                                                   uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
+
 /* Pins the calling thread to the CPUs of the NUMA node of the library's GPU (sysfs: the GPU's PCI device -> numa_node ->
  * cpulist), so that pinned buffers allocated afterwards and the thread that issues the H2D/D2H copies are local to the GPU's
  * PCIe root port.  Call once per rank after fpngb_init(), before allocating staging memory.  Returns the node, or -1 if the
