@@ -248,10 +248,50 @@ def encode_batch_device(images, flags: int = 0, out=None, sizes=None, stream=Non
 def ragged_slot_offsets(shapes):
     """The slot offsets of encode_ragged_device for images of the given (h, w, chans) shapes: the exclusive prefix of
     max_encoded_size rounded up to 16 bytes, in index order, with the total as the last of the n + 1 entries."""
-    ofs = np.zeros(len(shapes) + 1, dtype=np.int64)
-    for i, (h, w, c) in enumerate(shapes):
-        ofs[i + 1] = ofs[i] + (max_encoded_size(int(w), int(h), int(c)) + 15) // 16 * 16
-    return ofs
+    return png_slot_offsets([(h, w, c, 8) for (h, w, c) in shapes])
+
+
+def _encode_images(images, depths, fmt, flags, out, stream, png, what):
+    """Encodes images, a list of [h, w, c] CUDA tensors of which image i is written at depths[i] bits per sample, with one call
+    of fpngb_encode_png_ragged_device (png, dims {w, h, c, depth}) or fpngb_encode_ragged_device (dims {w, h, c}), or of its
+    _typed twin when fmt is given.  out defaults to the slot total.  Returns (out, offsets, sizes)."""
+    import torch
+
+    # the per-image work here is the host cost of the call: attribute reads only; the layout rules are checked by the C call
+    # (an unsupported layout raises FpngB200Error "invalid argument")
+    n = len(images)
+    ptrs, dims, strides, elem = [], [], [], []
+    for t, d in zip(images, depths):
+        assert t.is_cuda and t.dim() == 3, "images: [h, w, c] CUDA tensors"
+        h, w, c = t.shape
+        ptrs.append(t.data_ptr()); dims.append((w, h, c, d)); strides.append(t.stride()); elem.append(t.element_size())
+    ptrs = np.array(ptrs, dtype=np.uint64)
+    dims = np.array(dims, dtype=np.uint32).reshape(n, 4)
+    strides = np.array(strides, dtype=np.uint64).reshape(n, 3) * np.array(elem, dtype=np.uint64).reshape(n, 1)    # in bytes
+    device = images[0].device if n else torch.device("cuda")
+    if out is None:
+        slot = {}
+        keys = list(map(tuple, dims.tolist()))
+        for key in keys:
+            if key not in slot:
+                w, h, c, d = key
+                slot[key] = (max_encoded_size(w, h, c * d // 8) + 15) // 16 * 16
+        total = sum(slot[key] for key in keys)
+        out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
+    _check_arg(out, "out", device, torch.uint8)
+    offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
+    sizes = torch.empty((n,), dtype=torch.int32, device=device)
+    if not png:                                                          # fpngb_encode_ragged_device's dims are {w, h, c}
+        dims = np.ascontiguousarray(dims[:, :3])
+    args = (n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p), strides.ctypes.data_as(C.c_void_p))
+    rest = (flags, out.data_ptr(), out.numel(), offsets.data_ptr(), sizes.data_ptr(), _stream(stream, device))
+    name = "fpngb_encode_png_ragged_device" if png else "fpngb_encode_ragged_device"
+    if fmt is not None:
+        rc = getattr(lib(), name + "_typed")(*args, C.byref(fmt), *rest)
+    else:
+        rc = getattr(lib(), name)(*args, *rest)
+    check(rc, what)
+    return out, offsets, sizes
 
 
 def encode_ragged_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None):
@@ -269,46 +309,13 @@ def encode_ragged_device(images, flags: int = 0, out=None, stream=None, scale=No
     synchronisation."""
     import torch
 
-    # the per-image work here is the host cost of the call: attribute reads only; the layout rules are checked by the C call
-    # (an unsupported layout raises FpngB200Error "invalid argument")
     n = len(images)
     dtype = images[0].dtype if n else torch.uint8
     mixed = {t.dtype for t in images} - {dtype}
     if mixed:
         raise ValueError(f"encode_ragged_device: the images are all uint8 or all one float dtype, got {dtype} and {mixed.pop()}")
-    ptrs, dims, strides = [], [], []
-    for t in images:
-        assert t.is_cuda and t.dim() == 3, "images: [h, w, chans] CUDA tensors"
-        h, w, c = t.shape
-        ptrs.append(t.data_ptr()); dims.append((w, h, c)); strides.append(t.stride())
-    ptrs = np.array(ptrs, dtype=np.uint64)
-    dims = np.array(dims, dtype=np.uint32).reshape(n, 3)
-    strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
-    fmt = _pixel_format(dtype, scale, bias, int(dims[:, 2].max()) if n else 3, "encode_ragged_device")
-    if fmt is not None:
-        strides = strides * np.uint64(images[0].element_size())
-    device = images[0].device if n else torch.device("cuda")
-    if out is None:
-        slot = {}
-        for key in map(tuple, dims.tolist()):
-            if key not in slot:
-                slot[key] = (max_encoded_size(*key) + 15) // 16 * 16
-        total = sum(slot[key] for key in map(tuple, dims.tolist()))
-        out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
-    _check_arg(out, "out", device, torch.uint8)
-    offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
-    sizes = torch.empty((n,), dtype=torch.int32, device=device)
-    s = _stream(stream, device)
-    if fmt is not None:
-        rc = lib().fpngb_encode_ragged_device_typed(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
-                                                    strides.ctypes.data_as(C.c_void_p), C.byref(fmt), flags, out.data_ptr(),
-                                                    out.numel(), offsets.data_ptr(), sizes.data_ptr(), s)
-    else:
-        rc = lib().fpngb_encode_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
-                                              strides.ctypes.data_as(C.c_void_p), flags, out.data_ptr(), out.numel(),
-                                              offsets.data_ptr(), sizes.data_ptr(), s)
-    check(rc, "encode_ragged_device")
-    return out, offsets, sizes
+    fmt = _pixel_format(dtype, scale, bias, max((int(t.shape[-1]) for t in images), default=3), "encode_ragged_device")
+    return _encode_images(images, [8] * n, fmt, flags, out, stream, False, "encode_ragged_device")
 
 
 def png_slot_offsets(shapes):
@@ -363,31 +370,8 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None,
         fmt = _pixel_format(images[0].dtype, scale, bias, max(int(t.shape[-1]) for t in images), "encode_png_device")
     elif depth is not None or scale is not None or bias is not None:
         raise ValueError("encode_png_device: depth, scale and bias apply to float images only; uint8 / uint16 are taken as they are")
-    ptrs, dims, strides = [], [], []
-    for i, t in enumerate(images):
-        assert t.is_cuda and t.dim() == 3, "images: [h, w, c] CUDA tensors"
-        h, w, c = t.shape
-        es = t.element_size()
-        ptrs.append(t.data_ptr()); dims.append((w, h, c, int(depths[i]) if fmt is not None else 8 * es))
-        strides.append(tuple(v * es for v in t.stride()))
-    ptrs = np.array(ptrs, dtype=np.uint64)
-    dims = np.array(dims, dtype=np.uint32).reshape(n, 4)
-    strides = np.array(strides, dtype=np.uint64).reshape(n, 3)
-    device = images[0].device if n else torch.device("cuda")
-    if out is None:
-        total = int(png_slot_offsets([(h, w, c, d) for (w, h, c, d) in dims.tolist()])[-1])
-        out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
-    _check_arg(out, "out", device, torch.uint8)
-    offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
-    sizes = torch.empty((n,), dtype=torch.int32, device=device)
-    args = (n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p), strides.ctypes.data_as(C.c_void_p))
-    rest = (flags, out.data_ptr(), out.numel(), offsets.data_ptr(), sizes.data_ptr(), _stream(stream, device))
-    if fmt is not None:
-        rc = lib().fpngb_encode_png_ragged_device_typed(*args, C.byref(fmt), *rest)
-    else:
-        rc = lib().fpngb_encode_png_ragged_device(*args, *rest)
-    check(rc, "encode_png_device")
-    return out, offsets, sizes
+    depths = depths if fmt is not None else [8 * t.element_size() for t in images]
+    return _encode_images(images, depths, fmt, flags, out, stream, True, "encode_png_device")
 
 
 def compact_packed_device(data, offsets, sizes, out=None, stream=None):

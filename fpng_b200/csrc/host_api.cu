@@ -301,6 +301,12 @@ static void make_png_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t chans
     memcpy(hdr + 54, "IDAT", 4);            // bytes 50..53 (IDAT length) are patched per image on the device
 }
 
+static bool force_generic_env()
+{
+    static const bool v = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;
+    return v;
+}
+
 // Enqueue the whole encode pipeline for a device-resident batch.  Caller holds ctx.mu.
 //
 // Two encoders share this entry:
@@ -322,7 +328,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
     // second-generation kernels (16 pixels per lane, coalesced 128-bit loads) whenever every scanline is 16-byte aligned;
     // FPNGB_FORCE_GENERIC=1 keeps the generic kernels (tests compare both)
-    static const bool force_generic = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;
+    const bool force_generic = force_generic_env();
     static const bool env_fused = getenv("FPNGB_FUSED") && atoi(getenv("FPNGB_FUSED")) != 0;
     // RGBA 1-pass under a table where a one-pixel match can lose against four literals: only the generic kernels
     // implement the reference's check (fpng.cpp:1520-1528); it cannot fire with the shipped table
@@ -467,12 +473,6 @@ struct RaggedImage {
     uint32_t w, h, chans;
     uint64_t slot;                                      // offset of its slot in d_out
 };
-
-static bool force_generic_env()
-{
-    static const bool v = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;
-    return v;
-}
 
 // Enqueues the ragged pipeline for images im[k] (k in `ids`), all bound for the 16-pixel kernels.  Caller holds ctx.mu.
 //
@@ -867,130 +867,17 @@ int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_
                                              d_sizes, stream);
 }
 
-// Body of fpngb_encode_ragged_device (typed false, fmt unused) and fpngb_encode_ragged_device_typed (fmt required).
-static int encode_ragged_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
+// Body of the ragged encode calls: fpngb_encode_png_ragged_device and fpngb_encode_ragged_device (typed false, fmt unused) and their
+// _typed twins (fmt required), with dims n x {w, h, chans, depth}.  Images of depth 8 with 3 or 4 channels take fpng's route, the
+// others encode_png_locked.  A typed call first converts every image in one launch into tight rows of its output depth in c.conv;
+// from there on it is the untyped call on those rows.  The conversion and both routes sit inside one workspace bracket
+// (ws_acquire ... the last ws_release), so a call on another stream cannot overwrite c.conv before this call's kernels have read it.
+static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
                               const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
                               uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
-    PixelFormat f = uint8_format();
-    if (typed) {                                        // scale and bias are in use up to the largest channel count
-        uint32_t max_chans = 0;
-        for (uint32_t i = 0; i < n; i++) max_chans = std::max(max_chans, dims[3 * i + 2]);
-        const int rc = parse_format(fmt, max_chans, f);
-        if (rc) return rc;
-    }
-    // every image on its own: the layout rules of the batch call for a batch of one
-    std::vector<RaggedImage> im(n);
-    std::vector<Layout> src(n);
-    uint64_t total = 0;
-    for (uint32_t i = 0; i < n; i++) {
-        const uint32_t w = dims[3 * i], h = dims[3 * i + 1], chans = dims[3 * i + 2];
-        if (!pixels[i] || !valid_dims(w, h, chans)) return FPNGB_ERR_INVALID_ARG;
-        const uint64_t es = f.elem;
-        const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans * es, pixel = strides ? strides[3 * i + 1] : chans * es;
-        const uint64_t chan = strides ? strides[3 * i + 2] : es;
-        Layout& L = src[i];
-        const int rc = check_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, chan, 1, h, w, chans, f.elem, false, L);
-        if (rc) return rc;
-        if (!typed && L.row > 0xFFFFFFFFull) return FPNGB_ERR_INVALID_ARG;  // the uint8 kernels take a 32-bit row pitch
-        im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
-        total += align_up(max_encoded_size(w, h, chans), 16);
-    }
-    if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
-    if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
-    Context& c = g_ctx;
-    std::lock_guard<std::mutex> lk(c.mu);
-    FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    cudaStream_t s = (cudaStream_t)stream;
-    uint8_t* out = (uint8_t*)d_out;
-
-    // staging: d_out_offsets (n + 1), then the descriptor table and work lists, then (typed) the conversion descriptors
-    const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
-    const size_t conv_stage = align_up(ofs_bytes + align_up((size_t)n * sizeof(ImageDesc), 16) + (size_t)n * 5 * 4, 16);
-    StageSlot* sl = nullptr;
-    int rc = c.stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
-    if (rc) return rc;
-    uint8_t* stage = (uint8_t*)sl->buf.p;
-
-    if (typed) {
-        // the conversion buffer: image i's tight uint8 rows at a 16-byte aligned offset, then the descriptor table; one launch
-        // converts every image, and from here on the call is the uint8 call on those rows
-        std::vector<uint64_t> at(n);
-        uint64_t bytes = 0;
-        for (uint32_t i = 0; i < n; i++) { at[i] = bytes; bytes += align_up((uint64_t)im[i].w * im[i].h * im[i].chans, 16); }
-        const uint64_t desc_at = align_up(bytes, 256);
-        rc = c.conv.reserve(desc_at + (size_t)n * sizeof(ConvDesc));
-        if (rc) return rc;
-        uint8_t* cb = (uint8_t*)c.conv.p;
-        ConvDesc* hd = (ConvDesc*)(stage + conv_stage);
-        unsigned long long ctas = 0;
-        for (uint32_t i = 0; i < n; i++) {
-            RaggedImage& r = im[i];
-            hd[i] = conv_desc(r.pixels, src[i], 1, r.w, r.h, r.chans, at[i], ctas);
-            ctas += hd[i].ctas_per_image;
-            r.pixels = cb + at[i]; r.row = (uint64_t)r.w * r.chans; r.chan = 0;
-            src[i] = tight_layout(r.w, r.chans, r.h * r.row);
-        }
-        rc = c.ws_acquire(s);
-        if (rc) return rc;
-        FPNGB_CUDA_OK(cudaMemcpyAsync(cb + desc_at, hd, (size_t)n * sizeof(ConvDesc), cudaMemcpyHostToDevice, s));
-        convert_enqueue(hd, n, (const ConvDesc*)(cb + desc_at), f, cb, s);
-    }
-
-    // images the 16-pixel kernels do not take (RGBA 1-pass under a table whose one-pixel-match rule is live, or FPNGB_FORCE_GENERIC)
-    // go through the uniform pipeline one at a time, into their slots
-    const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
-    const bool lit1_rgba = !two_pass && c.h_static_books[1].lit1_rule;
-    std::vector<uint32_t> ids;
-    ids.reserve(n);
-    for (uint32_t i = 0; i < n; i++) {
-        const RaggedImage& r = im[i];
-        if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
-            const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
-            rc = encode_batch_locked(c, r.pixels, src[i], uint8_format(), 1, r.w, r.h, r.chans, flags, out + r.slot, slot, d_sizes + i, s);
-            if (rc) { prof_drop_conv(); cudaEventRecord(sl->ev, s); return rc; }
-        } else ids.push_back(i);
-    }
-
-    uint64_t* h_ofs = (uint64_t*)stage;
-    for (uint32_t i = 0; i < n; i++) h_ofs[i] = im[i].slot;
-    h_ofs[n] = total;
-    FPNGB_CUDA_OK(cudaMemcpyAsync(d_out_offsets, h_ofs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
-    if (!ids.empty()) {
-        rc = encode_ragged_locked(c, im, ids, flags, out, d_sizes, s, stage + ofs_bytes);
-        if (rc) { cudaEventRecord(sl->ev, s); return rc; }
-    }
-    prof_drop_conv();
-    FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
-    return FPNGB_OK;
-}
-
-int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
-                               void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
-{
-    return encode_ragged_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
-}
-
-int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
-                                     const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
-                                     uint32_t* d_sizes, void* stream)
-{
-    return encode_ragged_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
-}
-
-// Body of fpngb_encode_png_ragged_device (typed false, fmt unused) and fpngb_encode_png_ragged_device_typed (fmt required).  A typed
-// call first converts every image in one launch into tight rows of its output depth in c.conv; from there on it is the untyped
-// call on those rows.  The conversion and both routes sit inside one workspace bracket (ws_acquire ... the last ws_release), so a
-// call on another stream cannot overwrite c.conv before this call's kernels have read it.
-static int encode_png_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
-                           const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
-                           uint32_t* d_sizes, void* stream)
-{
-    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
-    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
     PixelFormat f = uint8_format();
     if (typed) {                                        // scale and bias are in use up to the largest channel count
         uint32_t max_chans = 0;
@@ -1069,12 +956,13 @@ static int encode_png_impl(uint32_t n, const uint64_t* pixels, const uint32_t* d
         rc = c.ws_acquire(s);
         if (rc) return rc;
         FPNGB_CUDA_OK(cudaMemcpyAsync(cb + desc_at, hd, (size_t)n * sizeof(ConvDesc), cudaMemcpyHostToDevice, s));
-        convert_enqueue(hd, n, (const ConvDesc*)(cb + desc_at), f, cb, s, true);
+        // the PNG instantiations only when an image needs them: for 8-bit RGB / RGBA both write the same bytes
+        convert_enqueue(hd, n, (const ConvDesc*)(cb + desc_at), f, cb, s, !png_ids.empty());
     }
     // a route that fails after the conversion still closes the bracket, so that later calls wait for the conversion
     auto fail = [&](int code) { prof_drop_conv(); if (typed) c.ws_release(s); cudaEventRecord(sl->ev, s); return code; };
-    // the fpng images take fpngb_encode_ragged_device's route: the ragged pipeline, or the uniform one image by image where the
-    // 16-pixel kernels do not apply
+    // the fpng images: the ragged pipeline, or the uniform one image by image where the 16-pixel kernels do not take them (RGBA
+    // 1-pass under a table whose one-pixel-match rule is live, or FPNGB_FORCE_GENERIC)
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
     const bool lit1_rgba = !two_pass && c.h_static_books[1].lit1_rule;
     std::vector<uint32_t> ids;
@@ -1102,14 +990,48 @@ static int encode_png_impl(uint32_t n, const uint64_t* pixels, const uint32_t* d
 int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
                                    void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
 {
-    return encode_png_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
+    return encode_images_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
 }
 
 int fpngb_encode_png_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
                                          const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap,
                                          uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
 {
-    return encode_png_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
+    return encode_images_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+// fpngb_encode_ragged_device(_typed): dims n x {w, h, chans} become {w, h, chans, 8} for fpng's 3 and 4 channels and depth 0
+// otherwise, which encode_images_impl rejects at that image, after the same checks of the images before it
+static int encode_ragged_fpng(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
+                              const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
+                              uint32_t* d_sizes, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (n == 0 || n > 65535 || !dims) return FPNGB_ERR_INVALID_ARG;
+    std::vector<uint32_t> dims4(4 * (size_t)n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t chans = dims[3 * i + 2];
+        dims4[4 * i] = dims[3 * i]; dims4[4 * i + 1] = dims[3 * i + 1]; dims4[4 * i + 2] = chans;
+        dims4[4 * i + 3] = chans == 3 || chans == 4 ? 8u : 0u;
+    }
+    return encode_images_impl(n, pixels, dims4.data(), strides, typed, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
+                               void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    return encode_ragged_fpng(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+}
+
+int fpngb_encode_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                     const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
+                                     uint32_t* d_sizes, void* stream)
+{
+    return encode_ragged_fpng(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
 }
 
 int fpngb_encode_host(const void* pixels, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags, void* out, size_t out_cap, size_t* out_size)
@@ -1385,8 +1307,7 @@ int fpngb_train_accumulate_device(const void* d_pixels, size_t image_stride, uin
     sp.pixels = (const uint8_t*)d_pixels; sp.image_stride = image_stride; sp.row_pitch = w * chans; sp.w = w; sp.h = h; sp.books = c.d_static_books; sp.book_stride = 0;
     sp.row_bits = ws.row_bits; sp.row_adler = ws.row_adler; sp.st = ws.st; sp.hist = ws.hist; sp.lane_ofs = ws.lane_ofs; sp.lane_ofs_pitch = ws.lane_ofs_pitch;
     FPNGB_CUDA_OK(cudaMemsetAsync(ws.hist, 0, (size_t)n * 288 * 4, s));
-    static const bool force_generic_t = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;
-    if (!force_generic_t) launch_hist16(sp, n, chans, s);
+    if (!force_generic_env()) launch_hist16(sp, n, chans, s);
     else launch_scan(sp, n, chans, pick_load_mode(d_pixels, image_stride, w, chans), true, s);
     count_launch(1);
     std::vector<uint32_t> hh((size_t)n * 288);

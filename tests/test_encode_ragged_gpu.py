@@ -323,3 +323,52 @@ def test_no_host_synchronisation(gpu, oracle):
     s.synchronize()
     check_oracle(oracle, hosts, files_of(*a), 0, "first")
     check_oracle(oracle, hosts[::-1], files_of(*b), 1, "second")
+
+
+# ---- 10. the uniform pipeline's fallback -----------------------------------------------------------------------------------
+def test_forced_generic_fallback():
+    """FPNGB_FORCE_GENERIC=1 sends every fpng image of the ragged and PNG calls through the uniform pipeline one image at a time,
+    the route of RGBA images under a trained table: uint8, float32 and mixed PNG calls must write the files of the default
+    route (run in subprocesses: the switch is read once)."""
+    import json
+    import os
+    import subprocess
+    import sys
+    code = r"""
+import hashlib, json, os, sys
+sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), 'tests'))
+import numpy as np, torch
+import imagegen, fpng_b200
+fpng_b200.fpng_init()
+def files(out, offsets, sizes):
+    torch.cuda.synchronize()
+    data, ofs, sz = out.cpu().numpy(), offsets.cpu().numpy(), sizes.cpu().numpy().astype(np.int64)
+    return [hashlib.sha256(data[ofs[i]:ofs[i] + sz[i]].tobytes()).hexdigest() for i in range(len(sz))]
+shapes = [(9, 687, 3), (5, 64, 4), (40, 17, 3), (3, 1920, 4), (1, 1, 3), (11, 513, 4)]
+hosts = [imagegen.make('g1', w, h, c, i).reshape(h, w, c) for i, (h, w, c) in enumerate(shapes)]
+u8 = [torch.from_numpy(x).cuda() for x in hosts]
+f32 = [torch.from_numpy(np.ascontiguousarray(x.transpose(2, 0, 1))).cuda().float().div_(255).permute(1, 2, 0) for x in hosts]
+rgba16 = imagegen.make('g1', 300, 7, 4, 9).reshape(7, 300, 4).astype(np.uint16) * 251 + 3
+gray = np.ascontiguousarray(imagegen.make('g1', 70, 6, 3, 7).reshape(6, 70, 3)[..., :1])
+mixed = [torch.from_numpy(gray).cuda(), u8[0],
+         torch.from_numpy(rgba16).cuda(), u8[1]]
+res = {}
+for flags in (0, 1, 2):
+    res[f'ragged {flags}'] = files(*fpng_b200.encode_ragged_device(u8, flags))
+    res[f'ragged float32 {flags}'] = files(*fpng_b200.encode_ragged_device(f32, flags, scale=255.0))
+    res[f'png {flags}'] = files(*fpng_b200.encode_png_device(mixed, flags))
+print(json.dumps({'launches': fpng_b200.launch_count(), 'files': res}))
+"""
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    runs = []
+    for generic in (False, True):
+        env = {k: v for k, v in os.environ.items() if k != "FPNGB_FORCE_GENERIC"}
+        if generic:
+            env["FPNGB_FORCE_GENERIC"] = "1"
+        out = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=600)
+        assert out.returncode == 0, out.stdout + out.stderr
+        runs.append(json.loads(out.stdout.strip().splitlines()[-1]))
+    default, generic = runs
+    assert generic["launches"] > default["launches"], "FPNGB_FORCE_GENERIC=1 did not take the one-image-at-a-time route"
+    for call, want in default["files"].items():
+        assert generic["files"][call] == want, call
