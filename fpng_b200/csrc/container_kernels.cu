@@ -34,8 +34,9 @@ struct DeviceCrc {
 
 // kAny (the any-PNG calls): files container_walk rejects with FPNGB_DECODE_NOT_FPNG are walked again by png_walk (with `flags`); a
 // general file that passes every check of the call gets pre_status kPngPending (kPngPendingExt for the files png_walk marks ext)
-// and, with png != nullptr, its PngDesc (decode.cuh).  kNative (FPNGB_PNG_NATIVE, with kAny): desired 0 checks w * h * chans.
-template <bool kAny, bool kNative = false>
+// and, with png != nullptr, its PngDesc (decode.cuh).  A native call (FPNGB_PNG_NATIVE, with kAny) may pass desired 0: the
+// w * h * desired check then uses the file's own channel count.
+template <bool kAny>
 __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDesc* png, uint32_t flags)
 {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -61,7 +62,7 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDe
         uint32_t pre = bad_arg ? (uint32_t)FPNGB_DECODE_INVALID_ARG : st;
         if (!pre && ragged) {
             if (w > p.w || h > p.h) pre = FPNGB_DECODE_SHAPE_MISMATCH;
-            else if ((unsigned long long)w * h * (kNative && !p.desired ? c : p.desired) > 0xFFFFFFFFull)
+            else if ((unsigned long long)w * h * (kAny && !p.desired ? c : p.desired) > 0xFFFFFFFFull)
                 pre = FPNGB_DECODE_FAILED_DIMENSIONS_TOO_LARGE;                     // fpng.cpp:3103-3105
             else if (p.boxes) {                                                     // the resized call's crop box
                 const int32_t* b = p.boxes + (size_t)i * 4;
@@ -100,17 +101,13 @@ void launch_container_walk_any(const WalkParams& p, PngDesc* png, uint32_t flags
 {
     container_walk_kernel<true><<<(p.n + 127) / 128, 128, 0, s>>>(p, png, flags);
 }
-void launch_container_walk_native(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s)
-{
-    container_walk_kernel<true, true><<<(p.n + 127) / 128, 128, 0, s>>>(p, png, flags);
-}
 
 // One CTA: exclusive scans of the output bytes, delta bytes and records of the accepted files, kPlaceThreads files per round.
 // kAny: general files (pre_status kPngPending or kPngPendingExt) are placed too, with their inflated rows in the delta bytes (an
-// ext file's PngDesc::raw_len), no records, and a fourth scan of their gathered zlib bytes (z_cap).  kNative (with kAny): px_bytes 0
-// gives every file chans * elem output bytes per pixel.
+// ext file's PngDesc::raw_len), no records, and a fourth scan of their gathered zlib bytes (z_cap).  A native call (with kAny) may
+// pass px_bytes 0: every file then takes chans * elem output bytes per pixel.
 constexpr uint32_t kPlaceThreads = 1024;
-template <bool kAny, bool kNative = false>
+template <bool kAny>
 __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams p, PngDesc* png, unsigned long long z_cap)
 {
     constexpr int K = kAny ? 4 : 3;
@@ -127,7 +124,7 @@ __global__ void __launch_bounds__(kPlaceThreads) decode_place_kernel(PlaceParams
 #pragma unroll
         for (int k = 0; k < K; k++) v[k] = 0ull;
         if (placed) {
-            const uint32_t px_bytes = kNative && !p.px_bytes ? fd.chans * p.elem : p.px_bytes;
+            const uint32_t px_bytes = kAny && !p.px_bytes ? fd.chans * p.elem : p.px_bytes;
             v[0] = ((unsigned long long)fd.w * fd.h * px_bytes + 15ull) & ~15ull;
             if (general) {
                 const unsigned long long raw = fd.pre_status == kPngPendingExt ? png[i].raw_len
@@ -187,10 +184,6 @@ void launch_decode_place(const PlaceParams& p, cudaStream_t s)
 void launch_decode_place_any(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s)
 {
     decode_place_kernel<true><<<1, kPlaceThreads, 0, s>>>(p, png, z_cap);
-}
-void launch_decode_place_native(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s)
-{
-    decode_place_kernel<true, true><<<1, kPlaceThreads, 0, s>>>(p, png, z_cap);
 }
 
 }  // namespace fpngb

@@ -71,9 +71,10 @@ struct OutStrides {
 // FPNGB_DTYPE_* value).  A separate kernel argument, as OutStrides is, so that no other kernel's parameter block grows; the
 // OutStrides of a typed call are in bytes, with pixel == sizeof(T) for planar output.
 struct PixelAffine { float scale[4], bias[4]; };
-// native (FPNGB_PNG_NATIVE): dtype may also be 0 (uint8: the value itself) or FPNGB_DTYPE_UINT16 (v * 257, or a 16-bit sample as it
-// is), desired 1..4 or 0 (each file's own channels), and scale / bias act on the float types only
-struct TypedOut { uint32_t dtype; PixelAffine aff; bool native = false; };
+// A native call (FPNGB_PNG_NATIVE) is a runtime case of the same kernels: dtype may also be 0 (uint8: the value itself) or
+// FPNGB_DTYPE_UINT16 (v * 257, or a 16-bit sample as it is), desired 1..4 or 0 (each file's own channels), and scale / bias act on
+// the float types only.
+struct TypedOut { uint32_t dtype; PixelAffine aff; };
 // Opt-in integrity check of every decode call (fpngb_set_decode_verify).  Two kernels read the file and the delta rows again:
 //   idat_crc_stream_kernel<false, true> (crc_stream_kernel.cu), after decode_prepare_kernel: the CRC-32 of "IDAT" + idat_len data
 //     bytes against the chunk's CRC field; a mismatch sets DecodeState::status to 4 for every file the walk passed, whatever the
@@ -172,13 +173,10 @@ struct PngParams {
     uint32_t n, desired, verify;            // desired 0 (native calls only): each file's own channels, FileDesc::chans
 };
 // container_walk_kernel<true> (png != nullptr only with files != nullptr; flags: png_walk's) and decode_place_kernel<true>, z_cap
-// the gathered bytes
+// the gathered bytes.  In a native call (FPNGB_PNG_NATIVE) WalkParams::desired / PlaceParams::px_bytes may be 0: each file's own
+// channel count (its info row's chans) then sizes its output and its FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE check.
 void launch_container_walk_any(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s);
 void launch_decode_place_any(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s);
-// the same for a native call (FPNGB_PNG_NATIVE): with WalkParams::desired / PlaceParams::px_bytes 0, each file's own channel
-// count (its info row's chans) sizes its output and its FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE check
-void launch_container_walk_native(const WalkParams& p, PngDesc* png, uint32_t flags, cudaStream_t s);
-void launch_decode_place_native(const PlaceParams& p, PngDesc* png, unsigned long long z_cap, cudaStream_t s);
 // gather, inflate and unfilter of the general files (three launches, four with FPNGB_PNG_ALL_FORMATS in flags; grids from n alone),
 // behind launch_decode
 void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags, cudaStream_t s);
@@ -187,8 +185,8 @@ void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags
 // HWC rows (pitch w * desired) at px + px_offsets[f], crops file f to its box and resizes it to out_h x out_w with the bilinear
 // rule of fpngb_decode_packed_resized_device, then stores T(r * scale[c] + bias[c]) (float types) or round_u8(r) (dtype 0).
 // Files whose d_status is not 0 are skipped.  Output strides in bytes: element (f, y, x, c) at d_out + f*image + y*row + x*pixel
-// + c*chan, interleaved (pixel = desired * sizeof(T)) or planar (pixel = sizeof(T)).  A native call (TypedOut::native) reads uint16
-// pixels (pitch w * desired * 2) instead, desired 1 .. 4, and stores the rules of decode_resize_kernels.cu.
+// + c*chan, interleaved (pixel = desired * sizeof(T)) or planar (pixel = sizeof(T)).  A native call (src_dtype FPNGB_DTYPE_UINT16)
+// reads uint16 pixels (pitch w * desired * 2) instead, desired 1 .. 4, and stores the rules of decode_resize_kernels.cu.
 struct ResizeParams {
     const uint8_t* px; const unsigned long long* px_offsets;   // the ragged decode's pixels and their placement
     const FileDesc* files; const int32_t* d_status;
@@ -197,7 +195,7 @@ struct ResizeParams {
     unsigned long long image, row, pixel, chan;
     uint32_t out_w, out_h, antialias;
 };
-void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t n, uint32_t desired, cudaStream_t s);
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s);
 // profiling (fpngb_decode_profile_read): the end of the kernel enqueued right behind launch_decode, reported in slot 8
 void decode_profile_mark_resize(cudaStream_t s);
 

@@ -75,24 +75,16 @@ static int decode_shape_check(uint32_t w, uint32_t h, uint32_t chans_in_file, ui
     return FPNGB_OK;
 }
 // The output format of a device decode call as the decode kernels take it: uint8 (typed false, fmt unused) or the *_typed call's
-// fmt.  elem receives the bytes per element.
-static int decode_format(bool typed, const fpngb_pixel_format* fmt, uint32_t desired, TypedOut& t, uint32_t& elem)
+// fmt, checked over every channel the call may write (4 for a native call's desired 0).  A native call (FPNGB_PNG_NATIVE) also takes
+// FPNGB_DTYPE_UINT16, whose scale and bias it ignores, as uint8 takes none.  elem receives the bytes per element.
+static int decode_format(bool typed, const fpngb_pixel_format* fmt, uint32_t desired, bool native, TypedOut& t, uint32_t& elem)
 {
     PixelFormat f = uint8_format();
-    if (typed) { const int rc = parse_format(fmt, desired, f); if (rc) return rc; }
+    if (typed && native && fmt && fmt->dtype == FPNGB_DTYPE_UINT16) { f.dtype = FPNGB_DTYPE_UINT16; f.elem = 2; }
+    else if (typed) { const int rc = parse_format(fmt, desired ? desired : 4, f); if (rc) return rc; }
     t = TypedOut{f.dtype, {}};
     memcpy(t.aff.scale, f.scale, sizeof f.scale); memcpy(t.aff.bias, f.bias, sizeof f.bias);
     elem = f.elem;
-    return FPNGB_OK;
-}
-
-// The output format of a native call (FPNGB_PNG_NATIVE): uint8 (fmt NULL), uint16 (FPNGB_DTYPE_UINT16: scale and bias ignored, as
-// uint8 takes none) or a float fmt checked as the *_typed calls check it, over every channel the call may write (4 for desired 0).
-static int native_format(const fpngb_pixel_format* fmt, uint32_t desired, TypedOut& t, uint32_t& elem)
-{
-    if (fmt && fmt->dtype == FPNGB_DTYPE_UINT16) { t = TypedOut{FPNGB_DTYPE_UINT16, {}, true}; elem = 2; return FPNGB_OK; }
-    const int rc = decode_format(fmt != nullptr, fmt, desired ? desired : 4, t, elem); if (rc) return rc;
-    t.native = true;
     return FPNGB_OK;
 }
 
@@ -156,7 +148,7 @@ static int decode_batch_device_impl(const void* d_files, size_t file_stride, con
     int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
     TypedOut t;
     uint32_t elem;
-    rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
+    rc = decode_format(typed, fmt, desired_chans, false, t, elem); if (rc) return rc;
     Layout out;
     rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, h, w, desired_chans, elem, true, out);
     if (rc) return rc;
@@ -183,7 +175,7 @@ static int decode_packed_device_impl(const void* d_base, const uint64_t* d_offse
     int rc = decode_shape_check(w, h, chans_in_file, desired_chans); if (rc) return rc;
     TypedOut t;
     uint32_t elem;
-    rc = decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
+    rc = decode_format(typed, fmt, desired_chans, false, t, elem); if (rc) return rc;
     Layout out;
     rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, h, w, desired_chans, elem, true, out);
     if (rc) return rc;
@@ -259,8 +251,8 @@ struct ResizeOut {
 // workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes, and the
 // resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
 // general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc); png_flags: png_walk's flags
-// (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel; FPNGB_PNG_NATIVE takes the native instantiations of the walk, place
-// and unfilter kernels, with desired_chans 0..4 and fmt as native_format reads it).
+// (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel; FPNGB_PNG_NATIVE allows desired_chans 0..4 and the formats
+// decode_format takes for a native call, typed exactly when fmt is given).
 static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
@@ -276,7 +268,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         return FPNGB_ERR_INVALID_ARG;
     TypedOut t;
     uint32_t elem;
-    int rc = native ? native_format(fmt, desired_chans, t, elem) : decode_format(typed, fmt, desired_chans, t, elem); if (rc) return rc;
+    int rc = decode_format(typed, fmt, desired_chans, native, t, elem); if (rc) return rc;
     if ((uintptr_t)d_base % 4 || (!rz && (uintptr_t)d_out % 16)) return FPNGB_ERR_ALIGNMENT;
     unsigned long long sub_cap = 0, delta_cap = 0, z_cap = 0;
     // the delta bound holds for out_cap in pixel values (w*h*desired of the decoded files sum to at most out_cap / elem)
@@ -303,14 +295,12 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
     wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr;
-    if (native) launch_container_walk_native(wp, (PngDesc*)png, png_flags & FPNGB_PNG_ALL_FORMATS, s);
-    else if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags, s);
+    if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags & FPNGB_PNG_ALL_FORMATS, s);
     else launch_container_walk(wp, s);
     PlaceParams pp{};
     pp.files = (FileDesc*)p.files; pp.n = n; pp.px_bytes = desired_chans * elem; pp.elem = elem;
     pp.out_cap = out_cap; pp.delta_cap = delta_cap; pp.sub_cap = sub_cap; pp.out_offsets = (unsigned long long*)d_out_offsets;
-    if (native) launch_decode_place_native(pp, (PngDesc*)png, z_cap, s);
-    else if (any_png) launch_decode_place_any(pp, (PngDesc*)png, z_cap, s);
+    if (any_png) launch_decode_place_any(pp, (PngDesc*)png, z_cap, s);
     else launch_decode_place(pp, s);
     p.d_files = (const uint8_t*)d_base; p.d_status = (uint32_t*)d_status; p.d_out = (uint8_t*)d_out;
     const TypedOut* tp = typed || native ? &t : nullptr;
@@ -327,7 +317,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         rp.boxes = rz->boxes; rp.d_out = rz->d_out;
         rp.image = rz->out.image; rp.row = rz->out.row; rp.pixel = rz->out.pixel; rp.chan = rz->out.chan;
         rp.out_w = rz->out_w; rp.out_h = rz->out_h; rp.antialias = rz->flags & FPNGB_RESIZE_ANTIALIAS;
-        launch_decode_resize(rp, rz->t, n, desired_chans, s);
+        launch_decode_resize(rp, rz->t, t.dtype, n, desired_chans, s);
         decode_profile_mark_resize(s);
     }
     count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0) + (all_formats ? 1 : 0));
@@ -607,8 +597,7 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
     ResizeOut rz{};
     rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
     uint32_t elem;
-    int rc = native ? native_format(fmt, desired_chans, rz.t, elem) : decode_format(fmt != nullptr, fmt, desired_chans, rz.t, elem);
-    if (rc) return rc;
+    int rc = decode_format(fmt != nullptr, fmt, desired_chans, native, rz.t, elem); if (rc) return rc;
     rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, out_h, out_w, desired_chans, elem, true,
                       rz.out);
     if (rc) return rc;
@@ -617,7 +606,7 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
     const uint32_t png_flags = ((flags & FPNGB_RESIZE_ALL_PNG_FORMATS) ? (uint32_t)FPNGB_PNG_ALL_FORMATS : 0u) |
                                (native ? (uint32_t)FPNGB_PNG_NATIVE : 0u);
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
-                                     nullptr, d_info, false, native ? &u16 : nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
+                                     nullptr, d_info, native, native ? &u16 : nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
                                      png_flags);
 }
 

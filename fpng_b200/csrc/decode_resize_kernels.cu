@@ -181,50 +181,32 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
     }
 }
 
-template <typename T>
-static void launch_resize(const ResizeParams& p, const PixelAffine& pa, uint32_t n, uint32_t desired, cudaStream_t s)
-{
-    const unsigned long long tiles = (unsigned long long)((p.out_w + kRsCols - 1) / kRsCols) * ((p.out_h + kRsRows - 1) / kRsRows);
-    const dim3 g((uint32_t)(tiles < 65535ull ? tiles : 65535ull), n);
-    const bool planar = p.pixel == sizeof(T);
-    if (desired == 3) { if (planar) decode_resize_kernel<3, true, T><<<g, kRsThreads, 0, s>>>(p, pa); else decode_resize_kernel<3, false, T><<<g, kRsThreads, 0, s>>>(p, pa); }
-    else { if (planar) decode_resize_kernel<4, true, T><<<g, kRsThreads, 0, s>>>(p, pa); else decode_resize_kernel<4, false, T><<<g, kRsThreads, 0, s>>>(p, pa); }
-}
-
-// native calls: the uint16 source at DST 1 .. 4
-template <int DST, typename T>
-static void launch_resize16_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cudaStream_t s)
+template <int DST, typename T, typename S>
+static void launch_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cudaStream_t s)
 {
     if constexpr (DST > 1) {                            // one channel: planar and interleaved address the same elements
-        if (p.pixel == sizeof(T)) { decode_resize_kernel<DST, true, T, uint16_t><<<g, kRsThreads, 0, s>>>(p, pa); return; }
+        if (p.pixel == sizeof(T)) { decode_resize_kernel<DST, true, T, S><<<g, kRsThreads, 0, s>>>(p, pa); return; }
     }
-    decode_resize_kernel<DST, false, T, uint16_t><<<g, kRsThreads, 0, s>>>(p, pa);
+    decode_resize_kernel<DST, false, T, S><<<g, kRsThreads, 0, s>>>(p, pa);
 }
-template <typename T>
-static void launch_resize16(const ResizeParams& p, const PixelAffine& pa, uint32_t n, uint32_t desired, cudaStream_t s)
+
+// src_dtype: the ragged decode's output, FPNGB_DTYPE_UINT16 for a native call (DST 1 .. 4), else 0 (uint8, DST 3 or 4)
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s)
 {
     const unsigned long long tiles = (unsigned long long)((p.out_w + kRsCols - 1) / kRsCols) * ((p.out_h + kRsRows - 1) / kRsRows);
     const dim3 g((uint32_t)(tiles < 65535ull ? tiles : 65535ull), n);
-    if (desired == 1) launch_resize16_dst<1, T>(p, pa, g, s);
-    else if (desired == 2) launch_resize16_dst<2, T>(p, pa, g, s);
-    else if (desired == 3) launch_resize16_dst<3, T>(p, pa, g, s);
-    else launch_resize16_dst<4, T>(p, pa, g, s);
-}
-
-void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t n, uint32_t desired, cudaStream_t s)
-{
-    if (t.native) {
-        if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_resize16<float>(p, t.aff, n, desired, s);
-        else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_resize16<__half>(p, t.aff, n, desired, s);
-        else if (t.dtype == FPNGB_DTYPE_BFLOAT16) launch_resize16<__nv_bfloat16>(p, t.aff, n, desired, s);
-        else if (t.dtype == FPNGB_DTYPE_UINT16) launch_resize16<uint16_t>(p, t.aff, n, desired, s);
-        else launch_resize16<uint8_t>(p, t.aff, n, desired, s);
-        return;
-    }
-    if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_resize<float>(p, t.aff, n, desired, s);
-    else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_resize<__half>(p, t.aff, n, desired, s);
-    else if (t.dtype == FPNGB_DTYPE_BFLOAT16) launch_resize<__nv_bfloat16>(p, t.aff, n, desired, s);
-    else launch_resize<uint8_t>(p, t.aff, n, desired, s);
+    with_out_type(t.dtype, [&](auto v) {
+        using T = decltype(v);
+        if (src_dtype == FPNGB_DTYPE_UINT16) {
+            if (desired == 1) launch_dst<1, T, uint16_t>(p, t.aff, g, s);
+            else if (desired == 2) launch_dst<2, T, uint16_t>(p, t.aff, g, s);
+            else if (desired == 3) launch_dst<3, T, uint16_t>(p, t.aff, g, s);
+            else launch_dst<4, T, uint16_t>(p, t.aff, g, s);
+        } else if constexpr (!std::is_same<T, uint16_t>::value) {
+            if (desired == 3) launch_dst<3, T, uint8_t>(p, t.aff, g, s);
+            else launch_dst<4, T, uint8_t>(p, t.aff, g, s);
+        }
+    });
 }
 
 }  // namespace fpngb

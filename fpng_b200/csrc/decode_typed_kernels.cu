@@ -111,51 +111,33 @@ __global__ void __launch_bounds__(128) unfilter_typed_kernel(DecodeParams p, Out
     }
 }
 
-// one instantiation per source channel count in the call, as for unfilter_kernel
-template <typename T>
-static void launch_typed(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t desired, dim3 g, cudaStream_t s)
+// The planar layout exists for the float types at DST 3 and 4 only (the native calls write tight interleaved rows).
+template <int SRC, int DST, typename T>
+static void launch_one(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, dim3 g, cudaStream_t s)
 {
-    const bool planar = os.pixel == sizeof(T);
-    for (uint32_t src = 3; src <= 4; src++) {
-        if (p.chans && p.chans != src) continue;
-        if (src == 3 && desired == 3) { if (planar) unfilter_typed_kernel<3, 3, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<3, 3, false, T><<<g, 128, 0, s>>>(p, os, pa); }
-        else if (src == 3) { if (planar) unfilter_typed_kernel<3, 4, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<3, 4, false, T><<<g, 128, 0, s>>>(p, os, pa); }
-        else if (desired == 3) { if (planar) unfilter_typed_kernel<4, 3, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<4, 3, false, T><<<g, 128, 0, s>>>(p, os, pa); }
-        else { if (planar) unfilter_typed_kernel<4, 4, true, T><<<g, 128, 0, s>>>(p, os, pa); else unfilter_typed_kernel<4, 4, false, T><<<g, 128, 0, s>>>(p, os, pa); }
+    if constexpr (DST >= 3 && !std::is_integral<T>::value) {
+        if (os.pixel == sizeof(T)) { unfilter_typed_kernel<SRC, DST, true, T><<<g, 128, 0, s>>>(p, os, pa); return; }
     }
+    unfilter_typed_kernel<SRC, DST, false, T><<<g, 128, 0, s>>>(p, os, pa);
 }
-
-// native calls (FPNGB_PNG_NATIVE): interleaved tight rows of desired channels, or with desired 0 of the file's own (SRC)
 template <int SRC, typename T>
-static void launch_native_src(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t desired, dim3 g, cudaStream_t s)
+static void launch_src(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t dst, dim3 g, cudaStream_t s)
 {
-    switch (desired ? desired : (uint32_t)SRC) {
-    case 1: unfilter_typed_kernel<SRC, 1, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
-    case 2: unfilter_typed_kernel<SRC, 2, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
-    case 3: unfilter_typed_kernel<SRC, 3, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
-    default: unfilter_typed_kernel<SRC, 4, false, T><<<g, 128, 0, s>>>(p, os, pa); break;
-    }
-}
-template <typename T>
-static void launch_native(const DecodeParams& p, const OutStrides& os, const PixelAffine& pa, uint32_t desired, dim3 g, cudaStream_t s)
-{
-    if (!p.chans || p.chans == 3) launch_native_src<3, T>(p, os, pa, desired, g, s);
-    if (!p.chans || p.chans == 4) launch_native_src<4, T>(p, os, pa, desired, g, s);
+    if (dst == 1) launch_one<SRC, 1, T>(p, os, pa, g, s);
+    else if (dst == 2) launch_one<SRC, 2, T>(p, os, pa, g, s);
+    else if (dst == 3) launch_one<SRC, 3, T>(p, os, pa, g, s);
+    else launch_one<SRC, 4, T>(p, os, pa, g, s);
 }
 
+// one instantiation per source channel count in the call, as for unfilter_kernel; DST is desired, or for a native call's desired 0
+// the file's own channel count
 void launch_unfilter_typed(const DecodeParams& p, const OutStrides& os, const TypedOut& t, uint32_t desired, dim3 g, cudaStream_t s)
 {
-    if (t.native) {
-        if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_native<float>(p, os, t.aff, desired, g, s);
-        else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_native<__half>(p, os, t.aff, desired, g, s);
-        else if (t.dtype == FPNGB_DTYPE_BFLOAT16) launch_native<__nv_bfloat16>(p, os, t.aff, desired, g, s);
-        else if (t.dtype == FPNGB_DTYPE_UINT16) launch_native<uint16_t>(p, os, t.aff, desired, g, s);
-        else launch_native<uint8_t>(p, os, t.aff, desired, g, s);
-        return;
-    }
-    if (t.dtype == FPNGB_DTYPE_FLOAT32) launch_typed<float>(p, os, t.aff, desired, g, s);
-    else if (t.dtype == FPNGB_DTYPE_FLOAT16) launch_typed<__half>(p, os, t.aff, desired, g, s);
-    else launch_typed<__nv_bfloat16>(p, os, t.aff, desired, g, s);
+    with_out_type(t.dtype, [&](auto v) {
+        using T = decltype(v);
+        if (!p.chans || p.chans == 3) launch_src<3, T>(p, os, t.aff, desired ? desired : 3u, g, s);
+        if (!p.chans || p.chans == 4) launch_src<4, T>(p, os, t.aff, desired ? desired : 4u, g, s);
+    });
 }
 
 }  // namespace fpngb

@@ -32,7 +32,7 @@ __device__ __forceinline__ uint32_t expand_px(uint32_t v, uint32_t bpp)
     return v;
 }
 
-template <typename T, bool kNative = false>
+template <typename T>
 __global__ void __launch_bounds__(32 * kUnfilterWarps) png_unfilter_kernel(PngParams p, PixelAffine pa)
 {
     constexpr uint32_t ES = sizeof(T);
@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(32 * kUnfilterWarps) png_unfilter_kernel(PngPa
     const uint32_t st = p.png[f].status;
     if (lane == 0) p.d_status[f] = st;
     if (st) return;
-    const uint32_t w = fd.w, h = fd.h, bpp = fd.chans, D = kNative && !p.desired ? bpp : p.desired, stride = w * bpp + 1u;
+    const uint32_t w = fd.w, h = fd.h, bpp = fd.chans, D = p.desired ? p.desired : bpp, stride = w * bpp + 1u;
     uint8_t* rows = p.rows + fd.delta_base;
     uint8_t* out = p.d_out + fd.out_base;
     for (uint32_t y0 = 0; y0 < h; y0 += 32) {
@@ -65,26 +65,16 @@ __global__ void __launch_bounds__(32 * kUnfilterWarps) png_unfilter_kernel(PngPa
             if (write_back) store_px(row + 1 + (size_t)x * bpp, raw, bpp);
             const uint32_t o = expand_px(raw, bpp);
             uint8_t* po = orow + (size_t)x * D * ES;
-            if constexpr (kNative) {                                       // D 1 / 2: L or (L, A); gray's luma is Y itself
-                const uint32_t l = D > 2 ? o : luma(o & 0xFFu, o >> 8 & 0xFFu, o >> 16 & 0xFFu) | (o >> 16 & 0xFF00u);
+            if (ES == 1 && D == 4) { *reinterpret_cast<uint32_t*>(po) = o; continue; }   // 16-byte aligned file, 4-byte pixels
+            // D 1 / 2: L or (L, A); gray's luma is Y itself
+            const uint32_t l = D > 2 ? o : luma(o & 0xFFu, o >> 8 & 0xFFu, o >> 16 & 0xFFu) | (o >> 16 & 0xFF00u);
 #pragma unroll
-                for (uint32_t k = 0; k < 4; k++) {
-                    if (k >= D) break;
-                    const uint32_t v = (l >> (8 * k)) & 0xFFu;
-                    if constexpr (ES == 1) po[k] = (uint8_t)v;
-                    else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, v * 257u, ES);
-                    else store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(__uint2float_rn(v), pa.scale[k]), pa.bias[k])), ES);
-                }
-            } else if constexpr (ES == 1) {
-                if (D == 4) *reinterpret_cast<uint32_t*>(po) = o;           // 16-byte aligned file, 4-byte pixels
-                else { po[0] = (uint8_t)o; po[1] = (uint8_t)(o >> 8); po[2] = (uint8_t)(o >> 16); }
-            } else {
-#pragma unroll
-                for (uint32_t k = 0; k < 4; k++) {
-                    if (k >= D) break;
-                    const float v = __uint2float_rn((o >> (8 * k)) & 0xFFu);
-                    store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(v, pa.scale[k]), pa.bias[k])), ES);
-                }
+            for (uint32_t k = 0; k < 4; k++) {
+                if (k >= D) break;
+                const uint32_t v = (l >> (8 * k)) & 0xFFu;
+                if constexpr (ES == 1) po[k] = (uint8_t)v;
+                else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, v * 257u, ES);
+                else store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(__uint2float_rn(v), pa.scale[k]), pa.bias[k])), ES);
             }
         }
         __syncwarp();
@@ -112,41 +102,34 @@ __device__ __forceinline__ float ext_value(uint32_t s, bool wide)
 }
 
 // one output pixel: rg = R | G << 16, ba = B | A << 16 in the 16-bit domain
-template <typename T, bool kNative = false>
+template <typename T>
 __device__ __forceinline__ void store_ext_px(uint8_t* po, uint32_t rg, uint32_t ba, uint32_t D, bool wide, const PixelAffine& pa)
 {
     constexpr uint32_t ES = sizeof(T);
-    if constexpr (kNative) {
-        if (D <= 2) {                       // L or (L, A): L from 16-bit samples, or from the 8-bit values v = s >> 8 (then * 257)
-            const uint32_t r = rg & 0xFFFFu, g = rg >> 16, b = ba & 0xFFFFu;
-            const uint32_t l = wide ? luma(r, g, b) : luma(r >> 8, g >> 8, b >> 8) * 257u;
-            rg = l | (ba & 0xFFFF0000u);    // channel 0 L, channel 1 A
-        }
-#pragma unroll
-        for (uint32_t k = 0; k < 4; k++) {
-            if (k >= D) break;
-            const uint32_t s = D <= 2 ? (rg >> (16 * k)) & 0xFFFFu : ((k < 2 ? rg : ba) >> (16 * (k & 1u))) & 0xFFFFu;
-            if constexpr (ES == 1) po[k] = (uint8_t)(s >> 8);
-            else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, s, ES);
-            else store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(ext_value(s, wide), pa.scale[k]), pa.bias[k])), ES);
-        }
-    } else if constexpr (ES == 1) {
+    if (ES == 1 && D >= 3) {                                                // uint8 at D 3 / 4: the high bytes
         const uint32_t o = (rg >> 8 & 0xFFu) | (rg >> 16 & 0xFF00u) | (ba << 8 & 0xFF0000u) | (ba & 0xFF000000u);
         if (D == 4) *reinterpret_cast<uint32_t*>(po) = o;                   // 16-byte aligned file, 4-byte pixels
         else { po[0] = (uint8_t)o; po[1] = (uint8_t)(o >> 8); po[2] = (uint8_t)(o >> 16); }
-    } else {
+        return;
+    }
+    if (D <= 2) {                           // L or (L, A): L from 16-bit samples, or from the 8-bit values v = s >> 8 (then * 257)
+        const uint32_t r = rg & 0xFFFFu, g = rg >> 16, b = ba & 0xFFFFu;
+        const uint32_t l = wide ? luma(r, g, b) : luma(r >> 8, g >> 8, b >> 8) * 257u;
+        rg = l | (ba & 0xFFFF0000u);        // channel 0 L, channel 1 A
+    }
 #pragma unroll
-        for (uint32_t k = 0; k < 4; k++) {
-            if (k >= D) break;
-            const uint32_t s = ((k < 2 ? rg : ba) >> (16 * (k & 1u))) & 0xFFFFu;
-            store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(ext_value(s, wide), pa.scale[k]), pa.bias[k])), ES);
-        }
+    for (uint32_t k = 0; k < 4; k++) {
+        if (k >= D) break;
+        const uint32_t s = D <= 2 ? (rg >> (16 * k)) & 0xFFFFu : ((k < 2 ? rg : ba) >> (16 * (k & 1u))) & 0xFFFFu;
+        if constexpr (ES == 1) po[k] = (uint8_t)(s >> 8);
+        else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, s, ES);
+        else store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(ext_value(s, wide), pa.scale[k]), pa.bias[k])), ES);
     }
 }
 
 __device__ __forceinline__ uint32_t unit_byte(uint32_t lo, uint32_t hi, uint32_t j) { return ((j < 4 ? lo : hi) >> (8 * (j & 3u))) & 0xFFu; }
 
-template <typename T, bool kNative = false>
+template <typename T>
 __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(PngParams p, PixelAffine pa)
 {
     __shared__ uint32_t s_pal[kExtWarps][256];
@@ -156,7 +139,7 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
     const FileDesc fd = p.files[f];
     if (fd.pre_status != kPngPendingExt) return;
     const PngDesc pd = p.png[f];
-    const uint32_t w = fd.w, h = fd.h, D = kNative && !p.desired ? fd.chans : p.desired, depth = pd.depth, type = pd.type;
+    const uint32_t w = fd.w, h = fd.h, D = p.desired ? p.desired : fd.chans, depth = pd.depth, type = pd.type;
     const uint32_t passes = pd.interlace ? 7u : 1u;
     const uint32_t samples = type == 2 ? 3u : type == 4 ? 2u : type == 6 ? 4u : 1u;
     const uint32_t bits = depth * samples, U = bits < 8 ? 1u : bits / 8;
@@ -250,7 +233,7 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
                             rg = y | y << 16;
                             ba = y | (s == k0 ? 0u : 0xFFFF0000u);
                         }
-                        store_ext_px<T, kNative>(orow + (size_t)(x0 + i * dx) * D * ES, rg, ba, D, false, pa);
+                        store_ext_px<T>(orow + (size_t)(x0 + i * dx) * D * ES, rg, ba, D, false, pa);
                     }
                     continue;
                 }
@@ -273,7 +256,7 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
                     const uint32_t a = type == 6 ? s[3] * mul : (s[0] == k0 && s[1] == k1 && s[2] == k2) ? 0u : 0xFFFFu;
                     rg = s[0] * mul | s[1] * mul << 16; ba = s[2] * mul | a << 16;
                 }
-                store_ext_px<T, kNative>(orow + (size_t)(x0 + (uint32_t)x * dx) * D * ES, rg, ba, D, wide, pa);
+                store_ext_px<T>(orow + (size_t)(x0 + (uint32_t)x * dx) * D * ES, rg, ba, D, wide, pa);
             }
             __syncwarp();
         }
@@ -281,37 +264,15 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
     }
 }
 
-// native calls (FPNGB_PNG_NATIVE): both unfilter kernels for output type T, the ext one with FPNGB_PNG_ALL_FORMATS
-template <typename T>
-static void launch_png_native(const PngParams& p, const PixelAffine& pa, uint32_t flags, cudaStream_t s)
-{
-    png_unfilter_kernel<T, true><<<(p.n + kUnfilterWarps - 1) / kUnfilterWarps, 32 * kUnfilterWarps, 0, s>>>(p, pa);
-    if (flags & FPNGB_PNG_ALL_FORMATS) png_unfilter_ext_kernel<T, true><<<(p.n + kExtWarps - 1) / kExtWarps, 32 * kExtWarps, 0, s>>>(p, pa);
-}
-
 void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags, cudaStream_t s)
 {
     launch_png_inflate(p, s);
-    const dim3 g((p.n + kUnfilterWarps - 1) / kUnfilterWarps), b(32 * kUnfilterWarps);
     const PixelAffine pa = typed ? typed->aff : PixelAffine{};
-    if (typed && typed->native) {
-        if (typed->dtype == FPNGB_DTYPE_FLOAT32) launch_png_native<float>(p, pa, flags, s);
-        else if (typed->dtype == FPNGB_DTYPE_FLOAT16) launch_png_native<__half>(p, pa, flags, s);
-        else if (typed->dtype == FPNGB_DTYPE_BFLOAT16) launch_png_native<__nv_bfloat16>(p, pa, flags, s);
-        else if (typed->dtype == FPNGB_DTYPE_UINT16) launch_png_native<uint16_t>(p, pa, flags, s);
-        else launch_png_native<uint8_t>(p, pa, flags, s);
-        return;
-    }
-    if (!typed) png_unfilter_kernel<uint8_t><<<g, b, 0, s>>>(p, pa);
-    else if (typed->dtype == FPNGB_DTYPE_FLOAT32) png_unfilter_kernel<float><<<g, b, 0, s>>>(p, pa);
-    else if (typed->dtype == FPNGB_DTYPE_FLOAT16) png_unfilter_kernel<__half><<<g, b, 0, s>>>(p, pa);
-    else png_unfilter_kernel<__nv_bfloat16><<<g, b, 0, s>>>(p, pa);
-    if (!(flags & FPNGB_PNG_ALL_FORMATS)) return;
-    const dim3 ge((p.n + kExtWarps - 1) / kExtWarps), be(32 * kExtWarps);
-    if (!typed) png_unfilter_ext_kernel<uint8_t><<<ge, be, 0, s>>>(p, pa);
-    else if (typed->dtype == FPNGB_DTYPE_FLOAT32) png_unfilter_ext_kernel<float><<<ge, be, 0, s>>>(p, pa);
-    else if (typed->dtype == FPNGB_DTYPE_FLOAT16) png_unfilter_ext_kernel<__half><<<ge, be, 0, s>>>(p, pa);
-    else png_unfilter_ext_kernel<__nv_bfloat16><<<ge, be, 0, s>>>(p, pa);
+    with_out_type(typed ? typed->dtype : 0u, [&](auto t) {
+        using T = decltype(t);
+        png_unfilter_kernel<T><<<(p.n + kUnfilterWarps - 1) / kUnfilterWarps, 32 * kUnfilterWarps, 0, s>>>(p, pa);
+        if (flags & FPNGB_PNG_ALL_FORMATS) png_unfilter_ext_kernel<T><<<(p.n + kExtWarps - 1) / kExtWarps, 32 * kExtWarps, 0, s>>>(p, pa);
+    });
 }
 
 }  // namespace fpngb

@@ -1,11 +1,24 @@
 // fpng_b200/csrc/typed_store.cuh -- element conversion and the wide stores of the kernels that write typed pixels
-// (unfilter_typed_kernel, decode_resize_kernel).
+// (unfilter_typed_kernel, png_unfilter_kernel, decode_resize_kernel), and the choice of their element type.
 #pragma once
+#include "../../include/fpng_b200.h"
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
 
 namespace fpngb {
+
+// Calls f with a value of the element type of an output dtype: float, __half, __nv_bfloat16, uint16_t, or uint8_t for dtype 0.  A
+// launcher whose kernel has fewer types guards the others with if constexpr.
+template <typename F>
+inline void with_out_type(uint32_t dtype, F&& f)
+{
+    if (dtype == FPNGB_DTYPE_FLOAT32) f(float{});
+    else if (dtype == FPNGB_DTYPE_FLOAT16) f(__half{});
+    else if (dtype == FPNGB_DTYPE_BFLOAT16) f(__nv_bfloat16{});
+    else if (dtype == FPNGB_DTYPE_UINT16) f(uint16_t{});
+    else f(uint8_t{});
+}
 
 // v rounded to nearest even and clamped to [0, 255], NaN to 0 (PTX ISA, cvt: float-to-integer conversions saturate, NaN
 // converts to 0): the quantiser of the typed encode

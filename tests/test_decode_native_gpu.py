@@ -146,14 +146,14 @@ def test_fpng_files(gpu, oracle):
 
 
 def test_flag_on_keeps_3_and_4_channel_bytes(gpu, oracle):
-    """a mixed fpng, 8-bit general and ext batch: desired 3 / 4 in uint8 and float32 give the flag-off call's bytes"""
+    """a mixed fpng, 8-bit general and ext batch: desired 3 / 4 in uint8 and every float type give the flag-off call's bytes"""
     import torch
     rs = np.random.RandomState(8)
     files = [f for f, _ in fpng_cases(gpu, oracle)[:4]]
     files += [pf.case(rs, 21, 9, ctype, 8, 0, False, seed=ctype)[0] for ctype in (0, 2, 4, 6)]
     files += [pf.case(rs, 13, 12, ctype, depth, il, t, seed=7)[0] for ctype, depth, il, t in ((3, 2, 0, True), (0, 16, 1, True), (6, 16, 0, False))]
     for d in (3, 4):
-        for dtype, kw in (("uint8", {}), ("float32", {"scale": [0.5] * d, "bias": [0.25] * d})):
+        for dtype, kw in [("uint8", {})] + [(t, {"scale": [0.5] * d, "bias": [0.25] * d}) for t in ("float32", "float16", "bfloat16")]:
             _, st_on, _, raw_on = run(gpu, files, d, dtype, **kw)
             _, st_off, _, raw_off = run(gpu, files, d, dtype, native=False, **kw)
             assert (st_on == 0).all() and torch.equal(raw_on, raw_off), (d, dtype)
