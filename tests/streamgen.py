@@ -143,10 +143,11 @@ def filtered_stream(tokens, chans: int, dist: int | None = None) -> bytes | None
 
 
 def dynamic_block(lit_sizes, dist_sizes, tokens, chans: int, rle: str = "rle", hclen: int | None = None, single_cl: bool = False,
-                  dist_sym: int | None = None) -> bytes:
+                  dist_sym: int | None = None, offsets: bool = False):
     """one final dynamic Huffman block (BFINAL = 1, BTYPE = 2) holding `tokens`: ("L", byte), ("M", length), ("E",).
     hclen: code-length code sizes sent (default: as few as the table needs, at least 4; fewer than needed truncates the
-    table).  single_cl: the code-length code has one code word (all sizes must then be one code-length symbol)."""
+    table).  single_cl: the code-length code has one code word (all sizes must then be one code-length symbol).
+    offsets: return (block, [bit offset of each token from the block's first bit]) instead of the block alone."""
     nlit, ndist = len(lit_sizes), len(dist_sizes)
     cl_toks = code_length_tokens(list(lit_sizes) + list(dist_sizes), rle)
     used = sorted({s for s, _, _ in cl_toks})
@@ -171,7 +172,9 @@ def dynamic_block(lit_sizes, dist_sizes, tokens, chans: int, rle: str = "rle", h
         bw.code(cl_codes[s], cl_sizes[s])
         if xb:
             bw.bits(xv, xb)
+    at = []
     for t in tokens:
+        at.append(bw.n)
         if t[0] == "L":
             bw.code(lit_codes[t[1]], lit_sizes[t[1]])
         elif t[0] == "M":
@@ -182,7 +185,7 @@ def dynamic_block(lit_sizes, dist_sizes, tokens, chans: int, rle: str = "rle", h
             bw.code(dist_codes[ds], dist_sizes[ds])                        # distance symbol chans - 1 = distance chans, no extra bits
         else:
             bw.code(lit_codes[EOB], lit_sizes[EOB])
-    return bw.tobytes()
+    return (bw.tobytes(), at) if offsets else bw.tobytes()
 
 
 def _chunk(tag: bytes, body: bytes) -> bytes:
@@ -201,11 +204,13 @@ def zlib_stream(deflate: bytes, data: bytes) -> bytes:
     return b"\x78\x01" + deflate + struct.pack(">I", zlib.adler32(data) & 0xFFFFFFFF)
 
 
-def dynamic_file(w, h, chans, lit_sizes, dist_sizes, tokens, trailing: bytes = b"", **kw):
-    """-> (file, the filtered stream a Deflate decoder produces or None)"""
+def dynamic_file(w, h, chans, lit_sizes, dist_sizes, tokens, trailing: bytes = b"", offsets: bool = False, **kw):
+    """-> (file, the filtered stream a Deflate decoder produces or None); offsets: (file, stream, [bit offset of each token from
+    the zlib stream's first bit])"""
     data = filtered_stream(tokens, chans, kw.get("dist_sym", chans - 1) + 1)
-    blk = dynamic_block(lit_sizes, dist_sizes, tokens, chans, **kw)
-    return png_file(w, h, chans, zlib_stream(blk + trailing, data or b"")), data
+    blk, at = dynamic_block(lit_sizes, dist_sizes, tokens, chans, offsets=True, **kw)
+    f = png_file(w, h, chans, zlib_stream(blk + trailing, data or b""))
+    return (f, data, [16 + a for a in at]) if offsets else (f, data)
 
 
 def stored_file(w, h, chans, data: bytes, block: int):
