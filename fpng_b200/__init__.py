@@ -20,4 +20,5 @@ from .api import (  # noqa: F401
     FPNGB_DECODE_BAD_CROP, FPNGB_RESIZE_ANTIALIAS, decode_packed_resized_device,
     FPNGB_DECODE_UNSUPPORTED_PNG, FPNGB_RESIZE_ANY_PNG, get_png_info,
     FPNGB_PNG_ALL_FORMATS, FPNGB_RESIZE_ALL_PNG_FORMATS, FPNGB_PNG_NATIVE, FPNGB_DTYPE_UINT16, FPNGB_RESIZE_NATIVE,
+    FPNGB_PNG_INDEX, FPNGB_DECODE_NOT_INDEXED, FPNGB_RESIZE_NEAREST, FPNGB_RESIZE_NEAREST_EXACT, FPNGB_RESIZE_INDEX,
 )

@@ -480,6 +480,8 @@ FPNGB_DECODE_UNSUPPORTED_PNG = 104   # any_png decodes: a well-formed PNG the GP
 FPNGB_PNG_ALL_FORMATS = 1            # all_formats=True: palette, 1/2/4/16-bit, color-keyed and Adam7 files decode too
 FPNGB_PNG_NATIVE = 4                 # native=True: each file at its own channel count, uint16 output, 1 / 2 channels
 FPNGB_DTYPE_UINT16 = 4               # fpngb_pixel_format.dtype of uint16 output (native calls only)
+FPNGB_PNG_INDEX = 8                  # indices=True: each pixel's raw sample (palette index, gray sample), uint8 or uint16
+FPNGB_DECODE_NOT_INDEXED = 105       # indices=True: the file has no single sample the output type holds (fpng, color, 16-bit to uint8)
 
 
 def get_png_info(data, all_formats=False):
@@ -500,6 +502,20 @@ def _all_formats_check(any_png, all_formats, fn, native=False):
         raise ValueError(f"{fn}: all_formats=True needs any_png=True")
     if native and not any_png:
         raise ValueError(f"{fn}: native=True needs any_png=True")
+
+
+def _indices_check(indices, any_png, all_formats, native, desired_channels, dtype, fn):
+    """ValueError unless an indices=True call is any_png, all_formats and native, at 1 channel, into uint8 or uint16"""
+    import torch
+
+    if not indices:
+        return
+    if not (any_png and all_formats and native):
+        raise ValueError(f"{fn}: indices=True needs any_png=True, all_formats=True and native=True")
+    if desired_channels != 1:
+        raise ValueError(f"{fn}: indices=True needs desired_channels=1, got {desired_channels}")
+    if dtype not in (torch.uint8, torch.uint16):
+        raise ValueError(f"{fn}: indices=True stores ids as torch.uint8 or torch.uint16, not {dtype}")
 
 
 def _native_format(dtype, scale, bias, desired_channels, what):
@@ -675,7 +691,8 @@ def _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max
 
 
 def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out=None, max_file_size=None, max_w=None, max_h=None,
-                                stream=None, dtype=None, scale=None, bias=None, any_png=False, all_formats=False, native=False):
+                                stream=None, dtype=None, scale=None, bias=None, any_png=False, all_formats=False, native=False,
+                                indices=False):
     """Decode fpng files of ANY shapes and channel counts packed in device memory (the layout of get_info_batch_device; base_bytes
     is data.numel()) in one call, pixels placed back to back.  Returns (out uint8 [out_cap], out_offsets int64 [n + 1],
     info int32 [n, 6], status int32 [n]):
@@ -702,11 +719,17 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
     rules in include/fpng_b200.h): desired_channels may also be 1 (gray, or the luma of color files: Pillow's convert("L")), 2
     (with alpha) or 0 / None (each file's own channels, info[i, 3]; ragged_views(..., 0) cuts them), and dtype torch.uint16
     stores 16-bit samples as they are and 8-bit values v as v * 257 (no scale or bias).  Without native those values raise
-    ValueError."""
+    ValueError.
+    indices=True (FPNGB_PNG_INDEX; needs any_png, all_formats and native, desired_channels=1 and dtype uint8 or uint16, else
+    ValueError) decodes label maps: each pixel's raw sample, with no scaling, palette lookup or alpha.  Palette files give their
+    indices (np.asarray(PIL.Image.open(f)) for PIL mode "P"), gray files of any depth their samples (a 1-bit mask 0 / 1, a 4-bit
+    one 0..15).  fpng files, color files and 16-bit gray into uint8 get FPNGB_DECODE_NOT_INDEXED, take no space and are not
+    decoded."""
     import torch
 
     _all_formats_check(any_png, all_formats, "decode_packed_ragged_device", native)
     odt = _out_dtype(out, dtype)
+    _indices_check(indices, any_png, all_formats, native, desired_channels, odt, "decode_packed_ragged_device")
     if native:
         desired_channels = desired_channels or 0
         if desired_channels not in (0, 1, 2, 3, 4):
@@ -733,7 +756,8 @@ def decode_packed_ragged_device(data, offsets, sizes, desired_channels: int, out
             int(max_h), desired_channels, out.data_ptr(), out.numel() * es, out_offsets.data_ptr(), info.data_ptr())
     if all_formats or native:
         rc = lib().fpngb_decode_packed_png_device_ex(*args, (FPNGB_PNG_ALL_FORMATS if all_formats else 0) |
-                                                     (FPNGB_PNG_NATIVE if native else 0), None if fmt is None else C.byref(fmt),
+                                                     (FPNGB_PNG_NATIVE if native else 0) | (FPNGB_PNG_INDEX if indices else 0),
+                                                     None if fmt is None else C.byref(fmt),
                                                      status.data_ptr(), s)
     elif any_png:
         rc = lib().fpngb_decode_packed_png_device(*args, None if fmt is None else C.byref(fmt), status.data_ptr(), s)
@@ -768,11 +792,15 @@ FPNGB_RESIZE_ANTIALIAS = 1
 FPNGB_RESIZE_ANY_PNG = 4
 FPNGB_RESIZE_ALL_PNG_FORMATS = 8
 FPNGB_RESIZE_NATIVE = 16
+FPNGB_RESIZE_NEAREST = 32            # interpolation="nearest": F.interpolate(mode="nearest")
+FPNGB_RESIZE_NEAREST_EXACT = 64      # interpolation="nearest-exact": F.interpolate(mode="nearest-exact")
+FPNGB_RESIZE_INDEX = 128             # indices=True in the resized call
+_INTERPOLATION = {"bilinear": 0, "nearest": FPNGB_RESIZE_NEAREST, "nearest-exact": FPNGB_RESIZE_NEAREST_EXACT}
 
 
 def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: int, boxes=None, antialias=True, out=None, dtype=None,
                                  scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None,
-                                 any_png=False, all_formats=False, native=False):
+                                 any_png=False, all_formats=False, native=False, interpolation="bilinear", indices=False):
     """Decode fpng files of ANY shapes packed in device memory (the layout of decode_packed_ragged_device) into one batch of a fixed
     size = (H, W): file i is cropped to boxes[i] and resized with F.interpolate's bilinear rule (align_corners=False, antialias as
     given) on the GPU, then stored as decode_batch_device stores its pixels (uint8, rounded half to even and clamped, or dtype with
@@ -794,16 +822,26 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     samples as they are, 8-bit values v as v * 257): desired_channels 1 .. 4 (1 / 2: luma and alpha, as in
     decode_packed_ragged_device(native=True)), dtype torch.uint16 stores the rounded resampled value, uint8 and the float types
     the value / 257 as above.  pixel_cap then counts bytes of the uint16 intermediate (align_up(w*h*desired_channels*2, 16) per
-    file)."""
+    file).
+    interpolation="nearest" / "nearest-exact" (FPNGB_RESIZE_NEAREST / _EXACT) resizes by nearest neighbour with F.interpolate's
+    rule of that mode instead: each element is, bit for bit, the element decode_packed_ragged_device with the same arguments stores
+    at the source pixel, so at identity size the result is the ragged decode cropped to the box.  antialias applies to bilinear only.
+    indices=True (FPNGB_RESIZE_INDEX) takes decode_packed_ragged_device's indices rule and needs a nearest mode as well; pixel_cap
+    then counts align_up(w*h*element_size, 16) bytes per file."""
     import torch
 
     _all_formats_check(any_png, all_formats, "decode_packed_resized_device", native)
+    if interpolation not in _INTERPOLATION:
+        raise ValueError(f"decode_packed_resized_device: interpolation {interpolation!r}: 'bilinear', 'nearest' or 'nearest-exact'")
+    if indices and interpolation == "bilinear":
+        raise ValueError("decode_packed_resized_device: indices=True needs interpolation 'nearest' or 'nearest-exact'")
     if desired_channels not in ((1, 2, 3, 4) if native else (3, 4)):
         raise ValueError(f"decode_packed_resized_device: desired_channels {desired_channels}: " + ("1 .. 4" if native else "3 or 4"))
     H, W = (int(v) for v in size)
     if not (1 <= H <= 1 << 24 and 1 <= W <= 1 << 24):
         raise ValueError(f"decode_packed_resized_device: size {tuple(size)}: each side in 1 .. 2^24")
     odt = _out_dtype(out, dtype)
+    _indices_check(indices, any_png, all_formats, native, desired_channels, odt, "decode_packed_resized_device")
     if native:
         fmt = _native_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
     else:
@@ -821,7 +859,8 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     _check_arg(out, "out", data.device, odt, n * H * W * desired_channels, view=True)
     if max_file_size is None or max_w is None or max_h is None or pixel_cap is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
-                                                             stream, 2 if native else 1, any_png=any_png, all_formats=all_formats)
+                                                             stream, odt.itemsize if indices else 2 if native else 1, any_png=any_png,
+                                                             all_formats=all_formats)
         if pixel_cap is None:
             pixel_cap = total
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
@@ -829,8 +868,9 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     rc = lib().fpngb_decode_packed_resized_device(
         data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
         int(max_h), int(pixel_cap), None if boxes is None else boxes.data_ptr(), W, H, desired_channels,
-        (FPNGB_RESIZE_ANTIALIAS if antialias else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
-        (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0) | (FPNGB_RESIZE_NATIVE if native else 0),
+        (FPNGB_RESIZE_ANTIALIAS if antialias and interpolation == "bilinear" else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
+        (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0) | (FPNGB_RESIZE_NATIVE if native else 0) |
+        _INTERPOLATION[interpolation] | (FPNGB_RESIZE_INDEX if indices else 0),
         None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape, (1, 2, 3, 4) if native else (3, 4)),
         info.data_ptr(), status.data_ptr(), _stream(stream, data.device))
     check(rc, "decode_packed_resized_device")

@@ -35,7 +35,8 @@ struct DeviceCrc {
 // kAny (the any-PNG calls): files container_walk rejects with FPNGB_DECODE_NOT_FPNG are walked again by png_walk (with `flags`); a
 // general file that passes every check of the call gets pre_status kPngPending (kPngPendingExt for the files png_walk marks ext)
 // and, with png != nullptr, its PngDesc (decode.cuh).  A native call (FPNGB_PNG_NATIVE, with kAny) may pass desired 0: the
-// w * h * desired check then uses the file's own channel count.
+// w * h * desired check then uses the file's own channel count.  An index call (WalkParams::index, with FPNGB_PNG_ALL_FORMATS in
+// flags, so fm describes every general file) gives FPNGB_DECODE_NOT_INDEXED right after the walk.
 template <bool kAny>
 __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDesc* png, uint32_t flags)
 {
@@ -60,6 +61,9 @@ __global__ void __launch_bounds__(128) container_walk_kernel(WalkParams p, PngDe
     if (p.files) {
         // argument checks first, then the walk's code, then the call's shape
         uint32_t pre = bad_arg ? (uint32_t)FPNGB_DECODE_INVALID_ARG : st;
+        // an index call stores one raw sample per pixel: palette indices, and gray samples of every depth but 16 into uint8
+        if (kAny && !pre && p.index && !(general && (fm.type == 3 || (fm.type == 0 && (fm.depth < 16 || p.index == 2)))))
+            pre = FPNGB_DECODE_NOT_INDEXED;
         if (!pre && ragged) {
             if (w > p.w || h > p.h) pre = FPNGB_DECODE_SHAPE_MISMATCH;
             else if ((unsigned long long)w * h * (kAny && !p.desired ? c : p.desired) > 0xFFFFFFFFull)

@@ -111,7 +111,8 @@ bool decode_set_pre_roll(uint32_t bits);    // DecodeParams::pre_roll of later c
 // offset % 4, and for the ragged call offset + size > base_bytes), the walk's code, then the shape check:
 //   uniform call (chans != 0): FPNGB_DECODE_SHAPE_MISMATCH when a valid file is not w x h x chans; the workspace bases are
 //     i * (h * delta_pitch(w, chans)), i * out_stride and i * subs_for(max_file_size);
-//   ragged call (chans == 0): the walk runs only when the argument checks pass; FPNGB_DECODE_SHAPE_MISMATCH when the file is
+//   ragged call (chans == 0): the walk runs only when the argument checks pass; with index != 0 FPNGB_DECODE_NOT_INDEXED for a
+//     file that has no single sample an element of index bytes holds (include/fpng_b200.h); FPNGB_DECODE_SHAPE_MISMATCH when the file is
 //     wider than w or taller than h, FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE when w * h * desired > 0xFFFFFFFF, then, for the
 //     resized call (boxes != nullptr), FPNGB_DECODE_BAD_CROP when the file's box is empty or not inside the image; the bases are
 //     set by decode_place_kernel.
@@ -124,6 +125,7 @@ struct WalkParams {
     unsigned long long base_bytes;          // ragged call: length of the buffer behind base
     unsigned long long out_stride;          // uniform call: output bytes per file
     const int32_t* boxes;                   // resized call: [n][4] {top, left, height, width}, or nullptr (whole images)
+    uint32_t index;                         // index call (FPNGB_PNG_INDEX): bytes per output element, 1 or 2; else 0
 };
 void launch_container_walk(const WalkParams& p, cudaStream_t s);
 
@@ -171,6 +173,7 @@ struct PngParams {
     uint8_t* rows;                          // inflated rows: file f at rows + files[f].delta_base (the decode's delta region)
     uint8_t* d_out; uint32_t* d_status;     // pixels as the ragged decode places them (tight HWC rows at d_out + files[f].out_base)
     uint32_t n, desired, verify;            // desired 0 (native calls only): each file's own channels, FileDesc::chans
+    uint32_t index;                         // FPNGB_PNG_INDEX: each pixel's raw sample (desired 1, uint8 or uint16 output)
 };
 // container_walk_kernel<true> (png != nullptr only with files != nullptr; flags: png_walk's) and decode_place_kernel<true>, z_cap
 // the gathered bytes.  In a native call (FPNGB_PNG_NATIVE) WalkParams::desired / PlaceParams::px_bytes may be 0: each file's own
@@ -194,9 +197,10 @@ struct ResizeParams {
     uint8_t* d_out;
     unsigned long long image, row, pixel, chan;
     uint32_t out_w, out_h, antialias;
+    uint32_t nearest;                       // 0 bilinear, 1 FPNGB_RESIZE_NEAREST, 2 FPNGB_RESIZE_NEAREST_EXACT (decode_nearest_kernel)
 };
 void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s);
-// profiling (fpngb_decode_profile_read): the end of the kernel enqueued right behind launch_decode, reported in slot 8
-void decode_profile_mark_resize(cudaStream_t s);
+// profiling (fpngb_decode_profile_read): the start (done false) and end (done true) of the resize kernel, reported in slot 8
+void decode_profile_mark_resize(cudaStream_t s, bool done);
 
 }  // namespace fpngb

@@ -252,7 +252,8 @@ struct ResizeOut {
 // resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
 // general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc); png_flags: png_walk's flags
 // (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel; FPNGB_PNG_NATIVE allows desired_chans 0..4 and the formats
-// decode_format takes for a native call, typed exactly when fmt is given).
+// decode_format takes for a native call, typed exactly when fmt is given; FPNGB_PNG_INDEX, with both, the raw samples of desired 1
+// into uint8 or uint16).
 static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                      uint32_t max_file_size, uint32_t max_w, uint32_t max_h, uint32_t desired_chans, void* d_out,
                                      size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, bool typed, const fpngb_pixel_format* fmt,
@@ -265,6 +266,10 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     if (!d_base || !d_offsets || !d_sizes || (!rz && (!d_out || !d_out_offsets)) || !d_status || n == 0 || n > 65535 || !max_file_size ||
         (native ? desired_chans > 4 || (rz && !desired_chans) : desired_chans != 3 && desired_chans != 4) || !max_w || !max_h ||
         max_w > (1u << 24) || max_h > (1u << 24))
+        return FPNGB_ERR_INVALID_ARG;
+    const bool index = any_png && (png_flags & FPNGB_PNG_INDEX);
+    if (index && ((png_flags & (FPNGB_PNG_ALL_FORMATS | FPNGB_PNG_NATIVE)) != (FPNGB_PNG_ALL_FORMATS | FPNGB_PNG_NATIVE) ||
+                  desired_chans != 1 || (typed && (!fmt || fmt->dtype != FPNGB_DTYPE_UINT16))))
         return FPNGB_ERR_INVALID_ARG;
     TypedOut t;
     uint32_t elem;
@@ -294,7 +299,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
-    wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr;
+    wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr; wp.index = index ? elem : 0u;
     if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags & FPNGB_PNG_ALL_FORMATS, s);
     else launch_container_walk(wp, s);
     PlaceParams pp{};
@@ -309,6 +314,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         PngParams q{};
         q.d_files = (const uint8_t*)d_base; q.files = p.files; q.png = (PngDesc*)png; q.z = png + png_desc_bytes; q.rows = p.delta;
         q.d_out = (uint8_t*)d_out; q.d_status = (uint32_t*)d_status; q.n = n; q.desired = desired_chans; q.verify = verify != nullptr;
+        q.index = index;
         launch_png_decode(q, tp, png_flags, s);
     }
     if (rz) {
@@ -317,8 +323,10 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         rp.boxes = rz->boxes; rp.d_out = rz->d_out;
         rp.image = rz->out.image; rp.row = rz->out.row; rp.pixel = rz->out.pixel; rp.chan = rz->out.chan;
         rp.out_w = rz->out_w; rp.out_h = rz->out_h; rp.antialias = rz->flags & FPNGB_RESIZE_ANTIALIAS;
+        rp.nearest = (rz->flags & FPNGB_RESIZE_NEAREST) ? 1u : (rz->flags & FPNGB_RESIZE_NEAREST_EXACT) ? 2u : 0u;
+        decode_profile_mark_resize(s, false);
         launch_decode_resize(rp, rz->t, t.dtype, n, desired_chans, s);
-        decode_profile_mark_resize(s);
+        decode_profile_mark_resize(s, true);
     }
     count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0) + (all_formats ? 1 : 0));
     FPNGB_CUDA_OK(cudaGetLastError());
@@ -588,11 +596,16 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
                                        size_t out_chan_stride, uint32_t* d_info, int32_t* d_status, void* stream)
 {
     if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
-    const bool native = (flags & FPNGB_RESIZE_NATIVE) != 0;
+    const bool native = (flags & FPNGB_RESIZE_NATIVE) != 0, index = (flags & FPNGB_RESIZE_INDEX) != 0;
+    const uint32_t nearest = flags & (FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT);
+    const uint32_t index_needs = FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE;
     if (!d_out || n == 0 || n > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
         (native ? desired_chans < 1 || desired_chans > 4 : desired_chans != 3 && desired_chans != 4) ||
-        (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE)) ||
-        ((flags & (FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE)) && !(flags & FPNGB_RESIZE_ANY_PNG)))
+        (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE |
+                             FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT | FPNGB_RESIZE_INDEX)) ||
+        ((flags & (FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE)) && !(flags & FPNGB_RESIZE_ANY_PNG)) ||
+        nearest == (FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT) || (nearest && (flags & FPNGB_RESIZE_ANTIALIAS)) ||
+        (index && ((flags & index_needs) != index_needs || !nearest || desired_chans != 1 || (fmt && fmt->dtype != FPNGB_DTYPE_UINT16))))
         return FPNGB_ERR_INVALID_ARG;
     ResizeOut rz{};
     rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
@@ -601,12 +614,14 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
     rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, out_h, out_w, desired_chans, elem, true,
                       rz.out);
     if (rc) return rc;
-    // native: the ragged decode holds every file as uint16 values in the 16-bit domain (pixel_cap counts their bytes)
+    // native: the ragged decode holds every file as uint16 values in the 16-bit domain (pixel_cap counts their bytes); index: as
+    // raw samples of the output's element type
     static const fpngb_pixel_format u16 = {FPNGB_DTYPE_UINT16, {0, 0, 0, 0}, {0, 0, 0, 0}};
     const uint32_t png_flags = ((flags & FPNGB_RESIZE_ALL_PNG_FORMATS) ? (uint32_t)FPNGB_PNG_ALL_FORMATS : 0u) |
-                               (native ? (uint32_t)FPNGB_PNG_NATIVE : 0u);
+                               (native ? (uint32_t)FPNGB_PNG_NATIVE : 0u) | (index ? (uint32_t)FPNGB_PNG_INDEX : 0u);
+    const fpngb_pixel_format* mid = index ? fmt : native ? &u16 : nullptr;
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
-                                     nullptr, d_info, native, native ? &u16 : nullptr, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
+                                     nullptr, d_info, mid != nullptr, mid, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
                                      png_flags);
 }
 
@@ -615,7 +630,8 @@ int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, con
                                       size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_info, uint32_t flags,
                                       const fpngb_pixel_format* fmt, int32_t* d_status, void* stream)
 {
-    if (flags & ~(uint32_t)(FPNGB_PNG_ALL_FORMATS | FPNGB_PNG_NATIVE)) return context().ready ? FPNGB_ERR_INVALID_ARG : FPNGB_ERR_NOT_INITIALIZED;
+    if (flags & ~(uint32_t)(FPNGB_PNG_ALL_FORMATS | FPNGB_PNG_NATIVE | FPNGB_PNG_INDEX))
+        return context().ready ? FPNGB_ERR_INVALID_ARG : FPNGB_ERR_NOT_INITIALIZED;
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, d_out, out_cap,
                                      d_out_offsets, d_info, fmt != nullptr, fmt, d_status, stream, nullptr, true, flags);
 }

@@ -1440,21 +1440,21 @@ __global__ void decode_status_kernel(DecodeParams p, uint32_t n)
 // call while profiling is on; fpngb_decode_profile_read() returns the device times of prepare, scan, link, write, stored,
 // unfilter (ms), and for a verified call also the IDAT CRC (slot 6) and Adler-32 (slot 7) kernels.  Events 0..6 bound the six
 // slots; a verified call also records event 7 after the CRC kernel (scan then starts there) and event 8 after the Adler kernel
-// (unfilter then starts there).  The resized call records event 9 after its resize kernel, which starts at event 6: slot 8, with
-// slots 6 and 7 0 when the call is not verified.
+// (unfilter then starts there).  The resized call records event 10 right before its resize kernel (behind the any-PNG kernels
+// when it has them) and event 9 after it: slot 8, with slots 6 and 7 0 when the call is not verified.
 static bool g_dec_profile = false;
-static cudaEvent_t g_dec_ev[10];
+static cudaEvent_t g_dec_ev[11];
 static bool g_dec_ev_ready = false, g_dec_ev_valid = false, g_dec_ev_verify = false, g_dec_ev_resize = false;
 void decode_profile_enable(bool on)
 {
     g_dec_profile = on;
-    if (on && !g_dec_ev_ready) { for (int i = 0; i < 10; i++) cudaEventCreate(&g_dec_ev[i]); g_dec_ev_ready = true; }
+    if (on && !g_dec_ev_ready) { for (int i = 0; i < 11; i++) cudaEventCreate(&g_dec_ev[i]); g_dec_ev_ready = true; }
 }
 int decode_profile_read(float* ms, int n)
 {
     if (!g_dec_ev_valid) return 0;
     cudaEventSynchronize(g_dec_ev[g_dec_ev_resize ? 9 : 6]);
-    int from[9] = {0, 1, 2, 3, 4, 5, 1, 5, 6}, to[9] = {1, 2, 3, 4, 5, 6, 7, 8, 9};
+    int from[9] = {0, 1, 2, 3, 4, 5, 1, 5, 10}, to[9] = {1, 2, 3, 4, 5, 6, 7, 8, 9};
     if (g_dec_ev_verify) { from[1] = 7; from[5] = 8; }
     const int slots = g_dec_ev_resize ? 9 : g_dec_ev_verify ? 8 : 6;
     for (int i = 0; i < n && i < slots; i++) {
@@ -1464,10 +1464,10 @@ int decode_profile_read(float* ms, int n)
     return 1;
 }
 #define DEC_MARK(i) do { if (g_dec_profile && g_dec_ev_ready) cudaEventRecord(g_dec_ev[i], s); } while (0)
-void decode_profile_mark_resize(cudaStream_t s)
+void decode_profile_mark_resize(cudaStream_t s, bool done)
 {
-    DEC_MARK(9);
-    if (g_dec_profile && g_dec_ev_ready) g_dec_ev_resize = true;
+    DEC_MARK(done ? 9 : 10);
+    if (done && g_dec_profile && g_dec_ev_ready) g_dec_ev_resize = true;
 }
 
 // FPNGB_DEC_STAGED=1 / fpngb_debug_decode_staged(1) put decode_write_staged_kernel in front of decode_write_kernel.  Off by default:

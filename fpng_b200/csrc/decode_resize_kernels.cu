@@ -9,6 +9,11 @@
 // All output addressing is 64-bit, and stores are the widest the address allows (store_elems).
 // Native calls (FPNGB_RESIZE_NATIVE): the ragged decode holds every file as uint16 values in the 16-bit domain (S = uint16_t), any
 // DST from 1 to 4; the resampled r is stored as cvt.rni.sat.u16(r), round_u8(r / 257) or T((r / 257) * scale + bias).
+//
+// decode_nearest_kernel takes decode_resize_kernel's place for FPNGB_RESIZE_NEAREST / FPNGB_RESIZE_NEAREST_EXACT.  It is a pure
+// gather: each thread owns 4 consecutive output pixels of one row (the store group of the bilinear kernel), computes their source
+// row and columns from the per-axis rule on the fly, and stores the source element converted to the ragged decode's element of the
+// same call.  Threads of a warp own neighbouring groups of a row, so the stores are coalesced; the kernel is bound by them.
 #include "decode.cuh"
 #include "typed_store.cuh"
 #include "../../include/fpng_b200.h"
@@ -181,6 +186,132 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
     }
 }
 
+// source index of output index i along one axis of a crop of length in, scale = in / out: torch's nearest_neighbor_compute_source_index
+// and nearest_neighbor_exact_compute_source_index (ATen/native/cuda/UpSample.cuh), each operation a separately rounded fp32 one
+__device__ __forceinline__ int nearest_src(uint32_t i, float scale, int in, bool exact)
+{
+    const float x = exact ? __fadd_rn((float)i, 0.5f) : (float)i;
+    return min((int)floorf(__fmul_rn(x, scale)), in - 1);
+}
+
+// DST elements of S at a (a pixel of the ragged decode's tight rows: 16-byte file bases, so aligned to DST * sizeof(S) where that is
+// a power of two), as the widest load that alignment allows
+template <int DST, typename S>
+__device__ __forceinline__ void gather_px(const uint8_t* a, uint32_t (&v)[DST])
+{
+    constexpr int B = DST * (int)sizeof(S);
+    if constexpr (B == 8) {
+        const uint2 u = __ldg(reinterpret_cast<const uint2*>(a));
+        v[0] = u.x & 0xFFFFu; v[1] = u.x >> 16; v[2] = u.y & 0xFFFFu; v[3] = u.y >> 16;
+    } else if constexpr (B == 4 || B == 2) {
+        const uint32_t u = B == 4 ? __ldg(reinterpret_cast<const unsigned int*>(a)) : __ldg(reinterpret_cast<const unsigned short*>(a));
+        constexpr int SB = 8 * (int)sizeof(S);
+#pragma unroll
+        for (int c = 0; c < DST; c++) v[c] = (u >> (SB * c)) & ((1u << SB) - 1u);
+    } else {
+#pragma unroll
+        for (int c = 0; c < DST; c++) v[c] = sizeof(S) == 2 ? __ldg(reinterpret_cast<const unsigned short*>(a) + c) : __ldg(a + c);
+    }
+}
+
+// the stored bits of source element u of channel c: the element the ragged decode of the same call stores.  From a uint16 source
+// (native calls: the 16-bit domain; index calls into uint16: the raw sample) u for uint16, u >> 8 for uint8, T(__fdiv_rn(u, 257) *
+// scale + bias) for the float types; from a uint8 source u for uint8, T(u * scale + bias) for the float types.
+template <typename T, typename S>
+__device__ __forceinline__ uint32_t nearest_bits(uint32_t u, int c, const PixelAffine& pa)
+{
+    if constexpr (std::is_same<T, S>::value) return u;
+    else if constexpr (std::is_same<T, uint8_t>::value) return u >> 8;
+    else {
+        const float x = sizeof(S) == 2 ? __fdiv_rn(__uint2float_rn(u), 257.0f) : __uint2float_rn(u);
+        return typed_bits<T>(__fadd_rn(__fmul_rn(x, pa.scale[c]), pa.bias[c]));
+    }
+}
+
+template <int DST, bool PLANAR, typename T, typename S>
+__global__ void __launch_bounds__(kRsThreads) decode_nearest_kernel(ResizeParams p, PixelAffine pa)
+{
+    constexpr int ES = sizeof(T), SS = sizeof(S);
+    const uint32_t f = blockIdx.y;
+    if (p.d_status[f] != 0) return;                                             // the same for the whole CTA
+    const FileDesc& fd = p.files[f];
+    int top = 0, left = 0, bh = (int)fd.h, bw = (int)fd.w;
+    if (p.boxes) { const int32_t* b = p.boxes + (size_t)f * 4; top = b[0]; left = b[1]; bh = b[2]; bw = b[3]; }
+    const uint8_t* src = p.px + p.px_offsets[f] + ((size_t)top * fd.w + left) * DST * SS;
+    const size_t pitch = (size_t)fd.w * DST * SS;
+    const float sx = __fdiv_rn((float)bw, (float)p.out_w), sy = __fdiv_rn((float)bh, (float)p.out_h);
+    const bool exact = p.nearest == 2;
+    // groups of 4 output pixels: gx per row; each thread steps through them by the grid's thread count, carried as (row, group)
+    const uint32_t gx = (p.out_w + 3) / 4;
+    const unsigned long long groups = (unsigned long long)gx * p.out_h, step = (unsigned long long)gridDim.x * blockDim.x;
+    const unsigned long long g0 = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g0 >= groups) return;
+    uint32_t oy = (uint32_t)(g0 / gx), xq = (uint32_t)(g0 % gx);
+    const uint32_t dy = (uint32_t)(step / gx), dq = (uint32_t)(step % gx);
+    for (unsigned long long g = g0; g < groups; g += step) {
+        const uint32_t xg = 4 * xq, npx = min(4u, p.out_w - xg);
+        const uint8_t* srow = src + (size_t)nearest_src(oy, sy, bh, exact) * pitch;
+        uint32_t v[4][DST];
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+            const int x = (uint32_t)q < npx ? nearest_src(xg + q, sx, bw, exact) : 0;
+            gather_px<DST, S>(srow + (size_t)x * DST * SS, v[q]);
+        }
+        uint8_t* o = p.d_out + (size_t)f * p.image + (size_t)oy * p.row + (size_t)xg * p.pixel;
+        if (PLANAR) {                                                           // 4 * sizeof(T) contiguous bytes per plane
+#pragma unroll
+            for (int c = 0; c < DST; c++) {
+                uint32_t e[4];
+#pragma unroll
+                for (int q = 0; q < 4; q++) e[q] = nearest_bits<T, S>(v[q][c], c, pa);
+                uint8_t* a = o + (size_t)c * p.chan;
+                if (npx == 4) store_elems<T>(a, e);
+                else for (uint32_t q = 0; q < npx; q++) store_elem(a + ES * q, e[q], ES);
+            }
+        } else {                                                                // 4 * DST * sizeof(T) contiguous bytes
+            uint32_t e[4 * DST];
+#pragma unroll
+            for (int k = 0; k < 4 * DST; k++) e[k] = nearest_bits<T, S>(v[k / DST][k % DST], k % DST, pa);
+            if (npx == 4) store_elems<T>(o, e);
+            else {
+#pragma unroll
+                for (int k = 0; k < 4 * DST; k++) if ((uint32_t)k < npx * DST) store_elem(o + ES * k, e[k], ES);
+            }
+        }
+        oy += dy; xq += dq;
+        if (xq >= gx) { xq -= gx; oy++; }
+    }
+}
+
+template <int DST, typename T, typename S>
+static void launch_nearest_dst(const ResizeParams& p, const PixelAffine& pa, uint32_t n, cudaStream_t s)
+{
+    const unsigned long long groups = (unsigned long long)((p.out_w + 3) / 4) * p.out_h, ctas = (groups + kRsThreads - 1) / kRsThreads;
+    const dim3 g((uint32_t)(ctas < 65535ull ? ctas : 65535ull), n);
+    if constexpr (DST > 1) {                            // one channel: planar and interleaved address the same elements
+        if (p.pixel == sizeof(T)) { decode_nearest_kernel<DST, true, T, S><<<g, kRsThreads, 0, s>>>(p, pa); return; }
+    }
+    decode_nearest_kernel<DST, false, T, S><<<g, kRsThreads, 0, s>>>(p, pa);
+}
+
+// the nearest resize: S uint16 for native calls and uint16 index calls (DST 1 .. 4), else uint8 (DST 3 / 4, or 1 for a uint8 index call)
+static void launch_decode_nearest(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s)
+{
+    with_out_type(t.dtype, [&](auto v) {
+        using T = decltype(v);
+        if (src_dtype == FPNGB_DTYPE_UINT16) {
+            if (desired == 1) launch_nearest_dst<1, T, uint16_t>(p, t.aff, n, s);
+            else if (desired == 2) launch_nearest_dst<2, T, uint16_t>(p, t.aff, n, s);
+            else if (desired == 3) launch_nearest_dst<3, T, uint16_t>(p, t.aff, n, s);
+            else launch_nearest_dst<4, T, uint16_t>(p, t.aff, n, s);
+        } else if constexpr (!std::is_same<T, uint16_t>::value) {
+            if (desired == 1) { if constexpr (std::is_same<T, uint8_t>::value) launch_nearest_dst<1, T, uint8_t>(p, t.aff, n, s); }
+            else if (desired == 3) launch_nearest_dst<3, T, uint8_t>(p, t.aff, n, s);
+            else launch_nearest_dst<4, T, uint8_t>(p, t.aff, n, s);
+        }
+    });
+}
+
 template <int DST, typename T, typename S>
 static void launch_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cudaStream_t s)
 {
@@ -193,6 +324,7 @@ static void launch_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cud
 // src_dtype: the ragged decode's output, FPNGB_DTYPE_UINT16 for a native call (DST 1 .. 4), else 0 (uint8, DST 3 or 4)
 void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s)
 {
+    if (p.nearest) { launch_decode_nearest(p, t, src_dtype, n, desired, s); return; }
     const unsigned long long tiles = (unsigned long long)((p.out_w + kRsCols - 1) / kRsCols) * ((p.out_h + kRsRows - 1) / kRsRows);
     const dim3 g((uint32_t)(tiles < 65535ull ? tiles : 65535ull), n);
     with_out_type(t.dtype, [&](auto v) {

@@ -73,7 +73,7 @@ __global__ void __launch_bounds__(32 * kUnfilterWarps) png_unfilter_kernel(PngPa
                 if (k >= D) break;
                 const uint32_t v = (l >> (8 * k)) & 0xFFu;
                 if constexpr (ES == 1) po[k] = (uint8_t)v;
-                else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, v * 257u, ES);
+                else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, p.index ? v : v * 257u, ES);
                 else store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(__uint2float_rn(v), pa.scale[k]), pa.bias[k])), ES);
             }
         }
@@ -91,7 +91,8 @@ __global__ void __launch_bounds__(32 * kUnfilterWarps) png_unfilter_kernel(PngPa
 // the pass width ignored), each placed at its image position (x0 + i dx, y0 + j dy).  Pixels are carried as four 16-bit channels:
 // 16-bit samples as they are, 8-bit values v (palette entries and scaled gray included) as v * 257, an alpha the file does not
 // have and a color key's 0 / 255 as 0 / 0xFFFF.  uint8 output stores the high bytes; typed output converts v = s / 257 for 16-bit
-// files (the header's rule) and v = s >> 8 otherwise.
+// files (the header's rule) and v = s >> 8 otherwise.  An index call (PngParams::index) stages no palette and stores each pixel's
+// raw sample (palette index, gray sample of any depth) as it is, through store_index.
 // The launch bound's 4 CTAs per SM allow up to 128 registers: without it ptxas kept this kernel at 64 and spilled.
 constexpr uint32_t kExtWarps = 4;
 
@@ -125,6 +126,13 @@ __device__ __forceinline__ void store_ext_px(uint8_t* po, uint32_t rg, uint32_t 
         else if constexpr (std::is_same<T, uint16_t>::value) store_elem(po + k * ES, s, ES);
         else store_elem(po + k * ES, typed_bits<T>(__fadd_rn(__fmul_rn(ext_value(s, wide), pa.scale[k]), pa.bias[k])), ES);
     }
+}
+
+// the raw sample s of an index call: uint8 or uint16 output, desired 1 (the walk gave every file s does not fit FPNGB_DECODE_NOT_INDEXED)
+template <typename T>
+__device__ __forceinline__ void store_index(uint8_t* po, uint32_t s)
+{
+    if constexpr (sizeof(T) == 1 || std::is_same<T, uint16_t>::value) store_elem(po, s, sizeof(T));
 }
 
 __device__ __forceinline__ uint32_t unit_byte(uint32_t lo, uint32_t hi, uint32_t j) { return ((j < 4 ? lo : hi) >> (8 * (j & 3u))) & 0xFFu; }
@@ -164,7 +172,7 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
     if (st) return;
     const uint8_t* file = p.d_files + fd.base;
     uint32_t* pal = s_pal[warp];
-    if (type == 3) {
+    if (type == 3 && !p.index) {
         for (uint32_t i = lane; i < 256; i += 32) {
             uint32_t e = 0xFF000000u;
             if (i < pd.plte_n) {
@@ -223,6 +231,7 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
                         const uint32_t i = (uint32_t)x * sub_per + j;
                         if (i >= pw) break;
                         const uint32_t s = rlo >> (8 - depth * (j + 1)) & sub_mask;
+                        if (p.index) { store_index<T>(orow + (size_t)(x0 + i * dx) * ES, s); continue; }
                         uint32_t rg, ba;
                         if (type == 3) {
                             const uint32_t e = pal[s];
@@ -242,6 +251,7 @@ __global__ void __launch_bounds__(32 * kExtWarps, 4) png_unfilter_ext_kernel(Png
 #pragma unroll
                 for (uint32_t m = 0; m < 4; m++)
                     s[m] = wide ? unit_byte(rlo, rhi, 2 * m) << 8 | unit_byte(rlo, rhi, 2 * m + 1) : unit_byte(rlo, rhi, m);
+                if (p.index) { store_index<T>(orow + (size_t)(x0 + (uint32_t)x * dx) * ES, s[0]); continue; }
                 uint32_t rg, ba;
                 const uint32_t mul = wide ? 1u : 257u;
                 if (type == 3) {

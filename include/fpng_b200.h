@@ -581,12 +581,56 @@ FPNGB_API int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_
                                                 void* d_out, size_t out_cap, uint64_t* d_out_offsets /* n+1 */,
                                                 uint32_t* d_info /* n*6 or NULL */, uint32_t flags,
                                                 const fpngb_pixel_format* fmt /* NULL = uint8 */, int32_t* d_status, void* stream);
+
 FPNGB_API int fpngb_get_png_info_batch_device_ex(const void* d_base, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
                                                  uint32_t flags, uint32_t* d_info, void* stream);
 FPNGB_API int fpngb_get_png_info_ex(const void* file, uint32_t size, uint32_t flags, uint32_t* w, uint32_t* h, uint32_t* chans,
                                     uint32_t* idat_ofs, uint32_t* idat_len);
 /* test hook: png_raw_len, the inflated size above, of a w x h file of bits_per_pixel bits (1..64) and interlace method 0 / 1 */
 FPNGB_API uint64_t fpngb_debug_png_raw_len(uint32_t w, uint32_t h, uint32_t bits_per_pixel, uint32_t interlace);
+
+/* ---- label maps: raw sample output (opt-in: FPNGB_PNG_INDEX, FPNGB_RESIZE_INDEX) and nearest-neighbour resize ------------------
+ * A label map stores class or instance ids, not colours: a palette file's indices (PASCAL VOC, PIL mode "P"), 1-bit masks (PIL
+ * mode "1"), 8- or 16-bit gray id maps (Cityscapes *_instanceIds.png).  With flags & FPNGB_PNG_INDEX, fpngb_decode_packed_png_device_ex
+ * stores each file's one raw sample per pixel:
+ *   * valid only together with FPNGB_PNG_ALL_FORMATS | FPNGB_PNG_NATIVE, desired_chans 1 and fmt NULL (uint8) or
+ *     FPNGB_DTYPE_UINT16; anything else (a float fmt included: ids are not scaled) gives FPNGB_ERR_INVALID_ARG.  Bits 2 and 0x100
+ *     stay unknown; fpngb_get_png_info_*_ex keep rejecting FPNGB_PNG_INDEX (the walk does not depend on it; info rows unchanged).
+ *   * Pixel rule: the sample as stored, with no scaling, no palette lookup and no alpha.  Color type 3: the palette index (an index
+ *     at or past the entry count is stored as it is; tRNS ignored).  Color type 0, any depth: the gray sample s (1-bit: 0 / 1,
+ *     4-bit: 0..15; a color key ignored).  Adam7 pixels land at their image positions.  For palette files and 8-bit gray this is
+ *     np.asarray(PIL.Image.open(f)); for mode "1" that array as uint8; for 2- and 4-bit gray PIL scales the samples, this rule
+ *     does not.
+ *   * FPNGB_DECODE_NOT_INDEXED (per file) for a file with no single sample the output type holds: fpng files, color types 2, 4
+ *     and 6, and a 16-bit gray file decoded to uint8 (it is not truncated).  It comes right after a successful walk, before the
+ *     shape, size, crop and space checks; such a file takes no output space, is not decoded, and its output bytes are left
+ *     untouched.  Its info row is written as usual.
+ *   * Placement: file i takes align_up(w*h*elem, 16) bytes, elem 1 or 2.  Launches: those of the ALL_FORMATS | NATIVE call, none
+ *     added (8-bit gray files without tRNS or Adam7 keep the 8-bit unfilter kernel, the others take the ext files' one).
+ *
+ * fpngb_decode_packed_resized_device with flags & FPNGB_RESIZE_NEAREST or FPNGB_RESIZE_NEAREST_EXACT resizes by nearest neighbour
+ * instead of bilinearly: torch's F.interpolate(mode="nearest") / ("nearest-exact"), torchvision's InterpolationMode.NEAREST /
+ * NEAREST_EXACT.  Either flag goes with every other flag combination except FPNGB_RESIZE_ANTIALIAS; both together, or either one
+ * with FPNGB_RESIZE_ANTIALIAS, give FPNGB_ERR_INVALID_ARG (torch has no antialiased nearest).  Bit 2, and 8 without 4, stay rejected.
+ *   * Rule per axis, crop length `in`, output length `out`, output index i, all fp32 and separately rounded (torch's CUDA kernel,
+ *     ATen/native/cuda/UpSample.cuh):
+ *         scale = (float)in / (float)out
+ *         nearest:        src = min((int)floorf((float)i * scale), in - 1)
+ *         nearest-exact:  src = min((int)floorf(((float)i + 0.5f) * scale), in - 1)
+ *   * Stored value: element (y, x, c) of file i's slice is, bit for bit, what the ragged decode with the same flags, dtype, scale
+ *     and bias stores at source pixel (top + src_y, left + src_x).  A native call gathers from the uint16 intermediate u and stores
+ *     u >> 8 for uint8, u for uint16 and T(__fdiv_rn(u, 257) * scale[c] + bias[c]) for a float fmt, the native ragged element;
+ *     other calls store the uint8 value or its typed conversion.  At identity size nearest is the ragged decode cropped to the
+ *     box.  So native uint8 output of a 16-bit file is s >> 8 here, not the bilinear path's round_u8(s / 257).
+ *   * FPNGB_RESIZE_INDEX: the FPNGB_PNG_INDEX rule above in the resized call.  It needs FPNGB_RESIZE_ANY_PNG |
+ *     FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE, a nearest flag, desired_chans 1 and fmt NULL or FPNGB_DTYPE_UINT16; anything
+ *     else gives FPNGB_ERR_INVALID_ARG (bilinear on ids is refused).  The intermediate has the output's element type, and pixel_cap
+ *     counts align_up(w*h*elem, 16) per file.  FPNGB_DECODE_NOT_INDEXED as above; FPNGB_DECODE_BAD_CROP comes after it.
+ *   * Launches are those of the call without the flag: decode_nearest_kernel takes decode_resize_kernel's place, and
+ *     fpngb_decode_profile_read reports it in slot 8. */
+enum { FPNGB_PNG_INDEX = 8 };
+enum { FPNGB_DECODE_NOT_INDEXED = 105 };   /* index decode: the file has no single sample the output type holds */
+enum { FPNGB_RESIZE_NEAREST = 32, FPNGB_RESIZE_NEAREST_EXACT = 64, FPNGB_RESIZE_INDEX = 128 };
 
 /* ---- typed encode input: float32 / float16 / bfloat16 pixels with a per-channel scale and bias, rounded to 8 bits ------------
  * The *_typed encode calls take the input as elements x of T (fmt->dtype: float32, float16 or bfloat16) and encode, for channel c,
