@@ -42,7 +42,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(objdir, exist_ok=True)
     headers = glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) + glob.glob(os.path.join(PKG, "..", "include", "*.h"))
     hdr_time = max(os.path.getmtime(h) for h in headers)
-    cflags = [f for f in NVCC_FLAGS if f != "-shared"] + os.environ.get("FPNGB_NVCC_DEFS", "").split()   # e.g. "-DFPNGB_LIT64=1" for A/B builds
+    cflags = [f for f in NVCC_FLAGS if f != "-shared"] + os.environ.get("FPNGB_NVCC_DEFS", "").split()   # e.g. "-DFPNGB_FUSED_TICKET=1" for A/B builds
 
     def compile_one(src):
         obj = os.path.join(objdir, os.path.basename(src) + ".o")

@@ -162,12 +162,6 @@ def lib() -> C.CDLL:
     L.fpngb_debug_use_fused.argtypes = [C.c_int]
     L.fpngb_debug_crc_overlap.restype = None
     L.fpngb_debug_crc_overlap.argtypes = [C.c_int]
-    L.fpngb_debug_crc_stream.restype = None
-    L.fpngb_debug_crc_stream.argtypes = [C.c_int]
-    L.fpngb_debug_inline_crc.restype = None
-    L.fpngb_debug_inline_crc.argtypes = [C.c_int]
-    L.fpngb_debug_decode_staged.restype = None
-    L.fpngb_debug_decode_staged.argtypes = [C.c_int]
     L.fpngb_debug_decode_repairs.restype = C.c_ulonglong
     L.fpngb_debug_decode_repairs.argtypes = [C.c_int]
     L.fpngb_debug_decode_preroll.restype = C.c_int

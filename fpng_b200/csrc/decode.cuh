@@ -102,7 +102,6 @@ void launch_idat_crc_verify(const VerifyParams& p, uint32_t n, size_t max_file_b
 void decode_profile_enable(bool on);
 int decode_profile_read(float* ms, int n);
 unsigned long long decode_link_repairs(bool reset);
-void decode_set_staged(bool on);            // write pass through the shared-memory staged kernel (default) or decode_write_kernel alone
 bool decode_set_pre_roll(uint32_t bits);    // DecodeParams::pre_roll of later calls; false (unchanged) above kPreRoll
 
 // container_walk_kernel (container_kernels.cu): one thread per file of a packed buffer (d_base + offsets[i], sizes[i] bytes).

@@ -512,7 +512,6 @@ FPNGB_API int fpngb_get_decode_verify(void) { return g_decode_verify.load(); }
 FPNGB_API int fpngb_decode_profile_enable(int on) { decode_profile_enable(on != 0); return 0; }
 FPNGB_API int fpngb_decode_profile_read(float* ms, int n) { return decode_profile_read(ms, n); }
 // test hook: number of subsequences the link pass had to decode again since the last reset (synchronises the device)
-FPNGB_API void fpngb_debug_decode_staged(int on) { decode_set_staged(on != 0); }   // tests / A/B: 0 = decode_write_kernel alone
 FPNGB_API unsigned long long fpngb_debug_decode_repairs(int reset) { cudaDeviceSynchronize(); return decode_link_repairs(reset != 0); }
 // test hook: speculative lead-in (bits) of the scan kernel for later decode calls, default 256; 0 makes nearly every guessed subsequence
 // start wrong, so the link pass has to repair it.  Pixels and statuses never depend on it.  FPNGB_ERR_INVALID_ARG (unchanged) above 256.

@@ -930,7 +930,7 @@ __global__ void __launch_bounds__(kDecThreads) decode_write_kernel(DecodeParams 
     const unsigned long long g = sp.g0 + (unsigned long long)blockIdx.x * kDecThreads + tid;
     SubInfo in; in.nlit = 0; in.n_out = 0;
     if (g <= sp.g1) in = p.subs[fd.sub_base + (g - sp.g0)];
-    // decode_write_staged_kernel ran first and cleared the live flag of everything it wrote (all of it, for literal-dominated files)
+    // a CTA whose subsequences the link pass left dead or empty stages nothing
     if (!__syncthreads_or(in.nlit && in.n_out)) return;
     stage_fast_table(s_fast, p.fast + (size_t)f * kFastWords);
     stage_window(sm, s_win, sp.g0 + (unsigned long long)blockIdx.x * kDecThreads);
@@ -947,273 +947,6 @@ __global__ void __launch_bounds__(kDecThreads) decode_write_kernel(DecodeParams 
         else decode_write_range<3>(sm, s_fast, lutg, in.start, (uint32_t)(hi_abs - in.start), dl, pitch, bpl, h, in.exit /*out_pos*/, in.lits /*tail*/, &err);
     }
     if (err) stp->status = 1;
-}
-
-// ------------------------------------------------------------------------------------------------
-// D2c' decode_write_staged_kernel: the write pass for literal-dominated streams (photographic content; runs first, the kernel above
-// takes what it leaves).  ncu of the kernel above: ~100 warp instructions per loop iteration for ~2.2 bytes per lane -- every lane
-// is somewhere else in its scanline, so the warp executes the union of the byte sink's paths (word complete / queue / 128-bit
-// store / scanline end) in almost every iteration, and every lane's stores go to a cache line of their own.  Here the CTA's output
-// (a contiguous range of the filtered stream, filter bytes included) is assembled in shared memory first:
-//   * the loop body is straight-line: table look-up, append the 1-3 literal bytes to a 64-bit accumulator, and when a 32-bit word is
-//     complete OR it into the staging buffer (predicated red.shared.or; the words two neighbouring subsequences share need no
-//     special case because the buffer starts zeroed).  No scanline bookkeeping: a match computes its column from its stream position
-//     when it needs it (fpng.cpp:2289-2388 checks), the filter bytes are checked by the copy below (fpng.cpp:2253-2262);
-//   * afterwards the CTA copies the staged bytes to the delta rows (filter bytes dropped, scanlines at their pitch) with realigning
-//     128-bit stores: coalesced, one transaction per 16 bytes instead of one per lane and word.
-// A CTA whose subsequences produce more than kWsStageBytes (RLE-dominated content) leaves them to decode_write_kernel; the ones
-// written here get their live flag (SubInfo::nlit) cleared.  Statuses and pixels are identical either way (same tokens, same checks).
-// ------------------------------------------------------------------------------------------------
-constexpr int kWsThreads = 224;                        // subsequences per CTA (2 CTAs per SM with the 64 KiB staging buffer)
-constexpr uint32_t kWsStageBytes = 64u * 1024u;
-constexpr uint32_t kWsWinWords = kWinLead + kWsThreads * (kSubBits / 32) + kWinTail;
-constexpr uint32_t kWsWinSmemWords = (kWsWinWords + kWsWinWords / 32 + 1 + 3) / 4 * 4;
-constexpr uint32_t kWsStageWords = kWsStageBytes / 4 + 8;                         // slack: the realigning copy reads one word past the data
-constexpr size_t kWsSmem = (size_t)(kFastWords + kWsWinSmemWords + kWsStageWords) * 4;
-
-__device__ __forceinline__ void stage_window_n(Stream& st, uint32_t* s_win, unsigned long long first_sub, uint32_t nwords)
-{
-    const unsigned long long w0 = first_sub * (kSubBits / 32);
-    const uint32_t base = (uint32_t)(w0 >= kWinLead ? w0 - kWinLead : 0ull);
-    for (uint32_t i = threadIdx.x; i < nwords; i += blockDim.x) {                 // same layout as stage_window()
-        const uint32_t* src = st.words + min(base + i, st.max_widx);
-        cp_async4(s_win + i + (i >> 5), src);
-        if ((i & 31u) == 0u && i) cp_async4(s_win + i + (i >> 5) - 1u, src);
-    }
-    st.swin = s_win; st.sw_base = base; st.sw_count = nwords;
-}
-
-// A value the compiler must keep in its register: shared-window addresses are otherwise re-derived (S2R SR_CgaCtaId + LEA) inside the
-// decode loop, on its critical path.
-__device__ __forceinline__ uint32_t pin_u32(uint32_t v) { uint32_t r; asm volatile("mov.b32 %0, %1;\n" : "=r"(r) : "r"(v)); return r; }
-__device__ __forceinline__ uint32_t lds32(uint32_t saddr) { uint32_t v; asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(v) : "r"(saddr)); return v; }
-// win_peek() on the window's shared-window address
-__device__ __forceinline__ uint32_t win_peek_s(uint32_t win_s, uint32_t q)
-{
-    const uint32_t si = q >> 5, a = win_s + ((si + (si >> 5)) << 2);
-    return __funnelshift_r(lds32(a), lds32(a + 4u), q);
-}
-
-// Byte sink of the staged write pass: `lo`/`hi` hold the pending bytes (sh / 8 < 4 of them, + up to 4 new ones) of the word at shared
-// address `saddr`; sh = 8 * pending bytes.
-struct StageSink {
-    uint32_t lo, hi, sh, saddr, send;
-    __device__ __forceinline__ void begin(uint32_t stage_s, uint32_t byte_ofs, uint32_t stage_end_s)
-    {
-        lo = 0u; hi = 0u; sh = 8u * (byte_ofs & 3u); saddr = stage_s + (byte_ofs & ~3u); send = stage_end_s;
-    }
-    // append the bits8 / 8 (1..4) low bytes of v (higher bytes zero)
-    __device__ __forceinline__ void put(uint32_t v, uint32_t bits8)
-    {
-        lo |= v << sh;
-        hi |= __funnelshift_l(v, 0u, sh);                                  // the bytes that spill into the next word (0 when sh == 0)
-        sh += bits8;
-        // word complete: plain store (this thread wrote the word's last byte, so it is the only one that ever stores it; bytes of the
-        // word that belong to a neighbouring subsequence are zero here and are OR-ed in after the CTA barrier, see tail());
-        // never beyond the buffer, whatever the stream holds
-        asm volatile("{\n.reg .pred p;\nsetp.ge.u32 p, %1, 32;\nsetp.lt.and.u32 p, %0, %3, p;\n@p st.shared.u32 [%0], %2;\n}\n"
-                     :: "r"(saddr), "r"(sh), "r"(lo), "r"(send) : "memory");
-        const bool adv = sh >= 32u;
-        saddr += adv ? 4u : 0u;
-        lo = adv ? hi : lo;
-        hi = adv ? 0u : hi;
-        sh &= 31u;
-    }
-    // the last, incomplete word: OR-ed into the buffer AFTER every thread of the CTA has finished its stores (shared atomics in the
-    // loop itself made the LSU the bottleneck: measured 3.0 ms vs 2.4 ms for the per-thread sink on C2)
-    __device__ __forceinline__ void tail() const
-    {
-        if (lo && saddr < send) asm volatile("red.shared.or.b32 [%0], %1;\n" :: "r"(saddr), "r"(lo) : "memory");
-    }
-    __device__ __forceinline__ uint32_t pos(uint32_t stage_s) const { return saddr - stage_s + (sh >> 3); }   // byte offset of the next byte
-};
-
-// General step of the staged write loop: one token the way decode_write_range takes it (trimming at the end of the subsequence, matches,
-// slow-table tokens, end of block).  Returns true when the subsequence is finished.
-template <int CHANS>
-__device__ __forceinline__ bool stage_general_step(StageSink& sk, const uint32_t* __restrict__ win, uint32_t O, const uint32_t* __restrict__ s_fast, uint32_t sizes_s,
-                                                const uint32_t* __restrict__ lutg, uint32_t hi, uint32_t stage_s, uint32_t byte_ofs, uint32_t col0, uint32_t bpl,
-                                                uint32_t& rel, uint32_t& lits, uint32_t* err)
-{
-    if (rel >= hi) return true;
-    FastTok t;
-    uint32_t run;
-    if (fast_tok(win, s_fast, sizes_s, O + rel, rel, hi, t)) {
-        rel += t.L;
-        if (t.cnt) {
-            lits = __funnelshift_r(lits, t.payload, 8u * t.cnt);
-            sk.put(t.payload, 8u * t.cnt);
-            return false;
-        }
-        run = t.payload;
-    } else {
-        uint32_t sym;
-        const uint32_t l = slow_tok(lutg, t.w, sym, run);
-        if (!l) return true;                                                 // invalid code: the link pass already flagged it
-        if (sym == 256u) return true;
-        rel += l;
-        if (sym < 256u) { lits = (lits >> 8) | (sym << 24); sk.put(sym, 8u); return false; }
-    }
-    // RLE match (fpng.cpp:2289-2388): inside a scanline, pixel aligned, not across its end; replicates the previous delta pixel
-    const uint32_t c = (col0 + (sk.pos(stage_s) - byte_ofs)) % (bpl + 1u);
-    const uint32_t dcol = c - 1u;
-    if (c == 0u || dcol < (uint32_t)CHANS || (dcol % CHANS) != 0u || (run % CHANS) != 0u || dcol + run > bpl) { *err = 1; return true; }
-    const uint32_t px = CHANS == 4 ? lits : (lits >> 8);                      // last CHANS literals, oldest in the low byte
-    for (uint32_t i = 0; i < run; i += CHANS) sk.put(px, 8u * CHANS);
-    return false;
-}
-
-// One subsequence into the staging buffer.  `col0`: column of its first output byte in the filtered stream (0 = filter byte).
-// The loop is software-pipelined around its only true dependency (token length -> next bit position -> next window read -> next table
-// entry): the window read of the NEXT token is issued as soon as this token's length is known, before its bytes go to the sink; the
-// common case (1-3 literals, more than 12 bits away from the end of the subsequence, so no trimming can apply) is one straight-line
-// block behind one branch.  Everything else takes the general step, which is the loop of decode_write_range.
-template <int CHANS>
-__device__ __forceinline__ void decode_stage_range(uint32_t mask, StageSink& sk, const uint32_t* __restrict__ win, uint32_t O, const uint32_t* __restrict__ s_fast, const uint32_t* __restrict__ lutg,
-                                                   uint32_t hi, uint32_t stage_s, uint32_t stage_end_s, uint32_t byte_ofs, uint32_t col0, uint32_t bpl,
-                                                   uint32_t tail, uint32_t* err)
-{
-    sk.begin(stage_s, byte_ofs, stage_end_s);
-    uint32_t rel = 0, lits = tail;
-    const uint32_t sizes_s = (uint32_t)__cvta_generic_to_shared(s_fast + 4096);
-    const uint32_t fast_s = pin_u32((uint32_t)__cvta_generic_to_shared(s_fast)), win_s = pin_u32((uint32_t)__cvta_generic_to_shared(win));
-    uint32_t w = win_peek_s(win_s, O);
-    // The warp votes once per iteration, which makes every iteration a convergence point: left to itself the compiler peels the
-    // literal block into an inner loop, and a lane that needs the general step (a match, ~1 in 450 tokens of photographic content) then
-    // waits until EVERY other lane of the warp needs one too -- ncu of the first version: 20 of 32 lanes active in the literal block.
-    // The end of the subsequence (a multi-literal entry cut down to its first literal within 12 bits of the end, same rule as
-    // fast_tok) is handled inside the literal block with predicated instructions, so the general step stays rare.
-    while (true) {
-        const bool more = rel < hi;
-        if (!__any_sync(mask, more)) break;
-        if (more) {
-            const uint32_t e = lds32(fast_s + ((w & 4095u) << 2));
-            uint32_t L = e & 15u, c8 = (e >> 1) & 0x18u, P = e >> 8;        // c8 = 8 * literal count
-            if (L != 0u && c8 != 0u) {
-                if (c8 >= 16u && rel + 12u > hi) {
-                    P &= 0xFFu; c8 = 8u;
-                    asm volatile("ld.shared.u8 %0, [%1+16384];\n" : "=r"(L) : "r"(fast_s + P));   // code size of the first literal
-                }
-                rel += L;
-                w = win_peek_s(win_s, O + rel);
-                lits = __funnelshift_r(lits, P, c8);
-                sk.put(P, c8);
-            } else {
-                if (stage_general_step<CHANS>(sk, win, O, s_fast, sizes_s, lutg, hi, stage_s, byte_ofs, col0, bpl, rel, lits, err)) rel = hi;
-                w = win_peek_s(win_s, O + rel);
-            }
-        }
-    }
-}
-
-__global__ void __launch_bounds__(kWsThreads) decode_write_staged_kernel(DecodeParams p)
-{
-    extern __shared__ __align__(16) uint32_t dec_smem[];
-    uint32_t* s_fast = dec_smem;                            // [kFastWords]
-    uint32_t* s_win = dec_smem + kFastWords;                // [kWsWinSmemWords]
-    uint32_t* s_stage = s_win + kWsWinSmemWords;            // [kWsStageWords]
-    __shared__ unsigned long long s_lo, s_hi, s_wlo[kWsThreads / 32], s_whi[kWsThreads / 32];
-    __shared__ uint32_t s_err;
-    const uint32_t f = blockIdx.y, tid = threadIdx.x;
-    DecodeState* stp = p.state + f;
-    if (stp->status || stp->stored) return;
-    const FileDesc fd = p.files[f];
-    Stream sm = open_stream(p.d_files + fd.base, fd);
-    const FileSpan sp = file_span(*stp, sm, fd);
-    const unsigned long long first_sub = sp.g0 + (unsigned long long)blockIdx.x * kWsThreads;
-    if (first_sub > sp.g1) return;
-    const unsigned long long g = first_sub + tid;
-    SubInfo* sub = p.subs + fd.sub_base + (g - sp.g0);
-    SubInfo in; in.nlit = 0; in.n_out = 0; in.start = 0; in.exit = 0; in.lits = 0;
-    if (g <= sp.g1) in = *sub;
-    const unsigned long long hi_abs = (g + 1) * kSubBits;
-    const bool live = in.nlit && in.n_out && in.start < hi_abs;
-    // the CTA's output range in the filtered stream: warp reductions, then one thread combines the warps
-    {
-        unsigned long long vlo = live ? in.exit : ~0ull, vhi = live ? in.exit + in.n_out : 0ull;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const unsigned long long a = __shfl_xor_sync(kFullMask, vlo, o), b = __shfl_xor_sync(kFullMask, vhi, o);
-            vlo = a < vlo ? a : vlo; vhi = b > vhi ? b : vhi;
-        }
-        if ((tid & 31u) == 0u) { s_wlo[tid >> 5] = vlo; s_whi[tid >> 5] = vhi; }
-        if (tid == 0) s_err = 0u;
-        __syncthreads();
-        if (tid == 0) {
-            for (uint32_t k = 1; k < kWsThreads / 32; k++) { vlo = s_wlo[k] < vlo ? s_wlo[k] : vlo; vhi = s_whi[k] > vhi ? s_whi[k] : vhi; }
-            s_lo = vlo; s_hi = vhi;
-        }
-        __syncthreads();
-    }
-    const unsigned long long lo = s_lo, hi = s_hi;
-    if (lo >= hi) return;                                                        // nothing to write
-    const unsigned long long bw = lo & ~15ull;                                   // stream offset of staging byte 0
-    if (hi - bw > (unsigned long long)kWsStageBytes) return;                     // too much output to stage: decode_write_kernel
-    stage_fast_table(s_fast, p.fast + (size_t)f * kFastWords);
-    stage_window_n(sm, s_win, first_sub, kWsWinWords);
-    // only the range's last (possibly incomplete) word and the slack the realigning copy reads beyond it need zeroing: every other
-    // word is stored whole by the thread that completes it
-    if (tid < 8u) s_stage[(uint32_t)((hi - bw) >> 2) + tid] = 0u;
-    stage_wait();
-
-    const uint32_t chans = fd.chans, bpl = fd.w * chans, pitch = fd.pitch, rb = bpl + 1u;
-    StageSink sk; sk.lo = 0u; sk.saddr = 0u; sk.send = 0u;
-    const uint32_t live_mask = __ballot_sync(kFullMask, live);                   // the lanes that decode (they vote together inside)
-    if (live) {
-        const uint32_t* lutg = p.luts + (size_t)f * 4096;
-        const uint32_t stage_s = (uint32_t)__cvta_generic_to_shared(s_stage);
-        const uint32_t O = (uint32_t)(in.start - 32ull * sm.sw_base);
-        const uint32_t col0 = (uint32_t)(in.exit % rb);
-        uint32_t err = 0;
-        if (chans == 4) decode_stage_range<4>(live_mask, sk, s_win, O, s_fast, lutg, (uint32_t)(hi_abs - in.start), stage_s, stage_s + kWsStageBytes, (uint32_t)(in.exit - bw), col0, bpl, in.lits, &err);
-        else decode_stage_range<3>(live_mask, sk, s_win, O, s_fast, lutg, (uint32_t)(hi_abs - in.start), stage_s, stage_s + kWsStageBytes, (uint32_t)(in.exit - bw), col0, bpl, in.lits, &err);
-        if (err) s_err = 1u;
-        sub->nlit = 0u;                                                          // written (or failed): nothing left for decode_write_kernel
-    }
-    __syncthreads();
-    sk.tail();
-    __syncthreads();
-
-    // ---- staged stream bytes [lo, hi) -> delta rows
-    const uint8_t* sb = reinterpret_cast<const uint8_t*>(s_stage);
-    uint8_t* dl = p.delta + fd.delta_base;
-    const unsigned long long y0 = lo / rb, y1 = (hi - 1ull) / rb;                // scanlines the range touches (link pass: hi <= rb * h)
-    uint32_t bad = 0;
-    for (unsigned long long y = y0 + tid; y <= y1; y += kWsThreads) {            // filter bytes: 0 on the first scanline, 2 (Up) below (fpng.cpp:2253-2262)
-        const unsigned long long s = y * rb;
-        if (s >= lo && s < hi && sb[(uint32_t)(s - bw)] != (y ? 2u : 0u)) bad = 1u;
-    }
-    if (rb < 256u) {
-        // narrow images: one thread per stream byte
-        for (unsigned long long s = lo + tid; s < hi; s += kWsThreads) {
-            const unsigned long long y = s / rb; const uint32_t c = (uint32_t)(s - y * rb);
-            if (c) dl[(size_t)y * pitch + (c - 1u)] = sb[(uint32_t)(s - bw)];
-        }
-    } else {
-        for (unsigned long long y = y0; y <= y1; y++) {                          // warp-uniform: a scanline per round
-            const unsigned long long rs = y * rb + 1ull;                         // stream offset of the scanline's first data byte
-            const unsigned long long a = rs > lo ? rs : lo, b = rs + bpl < hi ? rs + bpl : hi;
-            if (a >= b) continue;
-            const uint32_t d_lo = (uint32_t)(a - rs), d_hi = (uint32_t)(b - rs); // data columns [d_lo, d_hi) of this scanline are staged here
-            uint8_t* drow = dl + (size_t)y * pitch;
-            const uint32_t src0 = (uint32_t)(rs - bw);                           // staging byte offset of column 0 (may lie before the buffer: only
-                                                                                 // columns >= d_lo are read); unsigned wrap-around is fine below
-            for (uint32_t c = (d_lo >> 4) + tid; 16u * c < d_hi; c += kWsThreads) {
-                const uint32_t c0 = 16u * c, c1 = min(c0 + 16u, bpl);
-                if (c0 >= d_lo && c1 <= d_hi && c1 - c0 == 16u) {
-                    const uint32_t o = src0 + c0, k = o >> 2, sh = 8u * (o & 3u);
-                    const uint32_t w0 = s_stage[k], w1 = s_stage[k + 1], w2 = s_stage[k + 2], w3 = s_stage[k + 3], w4 = s_stage[k + 4];
-                    *reinterpret_cast<uint4*>(drow + c0) = make_uint4(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh),
-                                                                      __funnelshift_r(w2, w3, sh), __funnelshift_r(w3, w4, sh));
-                } else {
-                    for (uint32_t x = max(c0, d_lo); x < min(c1, d_hi); x++) drow[x] = sb[src0 + x];
-                }
-            }
-        }
-    }
-    if (bad) s_err = 1u;
-    __syncthreads();
-    if (tid == 0 && s_err) stp->status = 1;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1470,14 +1203,6 @@ void decode_profile_mark_resize(cudaStream_t s, bool done)
     if (done && g_dec_profile && g_dec_ev_ready) g_dec_ev_resize = true;
 }
 
-// FPNGB_DEC_STAGED=1 / fpngb_debug_decode_staged(1) put decode_write_staged_kernel in front of decode_write_kernel.  Off by default:
-// measured slower than decode_write_kernel alone.  The staging buffer limits an SM to 2 CTAs = 448 decode
-// chains (the per-thread sink runs 1024), and the chain token length -> next window read -> next table entry is latency bound at that
-// occupancy (ncu: issue active 54 %, 63 instructions per iteration against ~100 of the per-thread sink, both converged); byte-exact,
-// covered by tests/test_decode_gpu.py::test_decode_write_paths_agree.
-static bool g_dec_staged = getenv("FPNGB_DEC_STAGED") && atoi(getenv("FPNGB_DEC_STAGED")) != 0;
-void decode_set_staged(bool on) { g_dec_staged = on; }
-
 // Speculative lead-in of decode_scan_kernel (fpngb_debug_decode_preroll).  The link pass makes the result independent of it; tests set
 // it below the default to force wrong guesses.  At most kPreRoll: the scan kernel's stream window starts kWinLead words before its
 // first subsequence.
@@ -1513,11 +1238,6 @@ void launch_decode(const DecodeParams& params, const OutStrides& os, uint32_t n,
     DEC_MARK(2);
     decode_link_kernel<<<n, kLinkThreads, 0, s>>>(p);
     DEC_MARK(3);
-    if (g_dec_staged) {
-        FPNGB_SET_SMEM(decode_write_staged_kernel, kWsSmem);
-        dim3 gws((p.max_subs + kWsThreads - 1) / kWsThreads, n);
-        decode_write_staged_kernel<<<gws, kWsThreads, kWsSmem, s>>>(p);
-    }
     decode_write_kernel<<<gsub, kDecThreads, kDecSmem, s>>>(p);
     DEC_MARK(4);
     dim3 gs((p.max_h + 7) / 8, n);

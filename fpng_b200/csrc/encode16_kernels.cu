@@ -74,15 +74,10 @@ __device__ __forceinline__ uint32_t ragged_image16(P& p, uint32_t& cta)
 // ------------------------------------------------------------------------------------------------
 // K1 (v2): per-row bit count + Adler partials (+ per-lane bit offsets inside the row for the pack kernel)
 // ------------------------------------------------------------------------------------------------
-// FPNGB_SCAN_MINB (A/B build): minimum CTAs per SM the scan kernel is compiled for (5 caps the RGB kernel at 48 registers: 40 instead of
-// 32 warps per SM).  Measured slower than the default: the kernel is ALU-pipe bound, not latency bound.
-#ifdef FPNGB_SCAN_MINB
-#define FPNGB_SCAN_BOUNDS __launch_bounds__(32 * kScan16Rows, FPNGB_SCAN_MINB)
-#else
-#define FPNGB_SCAN_BOUNDS __launch_bounds__(32 * kScan16Rows)
-#endif
+// No minimum CTAs per SM: a bound of 5 (48 registers for RGB, 40 instead of 32 warps per SM) measured slower, since the kernel is
+// ALU-pipe bound, not latency bound.
 template <int CHANS, int LOAD, bool RAGGED = false>
-__global__ void FPNGB_SCAN_BOUNDS row_scan16_kernel(std::conditional_t<RAGGED, RaggedParams<ScanParams>, ScanParams> p)
+__global__ void __launch_bounds__(32 * kScan16Rows) row_scan16_kernel(std::conditional_t<RAGGED, RaggedParams<ScanParams>, ScanParams> p)
 {
     using WK = typename Loader16<CHANS, LOAD>::type;
     constexpr uint32_t M = max_match_pixels(CHANS);

@@ -121,15 +121,11 @@ struct LaneStager {
     __device__ __forceinline__ uint32_t finish() { sts32(dst, cur); return P; }
 };
 
-// FPNGB_LIT64: literal table entries as (code, size) register pairs fetched with one 64-bit shared load, instead of one
-// packed 32-bit word whose fields have to be shifted / masked apart (2 ALU instructions less per literal)
-#ifndef FPNGB_LIT64
-#define FPNGB_LIT64 1
-#endif
 #ifndef FPNGB_FUSED_TICKET
 #define FPNGB_FUSED_TICKET 0
 #endif
-#if FPNGB_LIT64
+// fput_word*: literal table entries as (code, size) register pairs fetched with one 64-bit shared load, instead of one packed
+// 32-bit word whose fields have to be shifted / masked apart (2 ALU instructions less per literal)
 __device__ __forceinline__ uint2 lds64c(uint32_t saddr) { uint2 v; asm("ld.shared.v2.u32 {%0, %1}, [%2];\n" : "=r"(v.x), "=r"(v.y) : "r"(saddr)); return v; }
 template <int POS>
 __device__ __forceinline__ uint32_t flit_off8(uint32_t w, uint32_t nb)
@@ -138,7 +134,6 @@ __device__ __forceinline__ uint32_t flit_off8(uint32_t w, uint32_t nb)
     return (x & 0x7F8u) | nb;
 }
 __device__ __forceinline__ void fput_pair2(LaneStager& bs, uint2 a, uint2 b) { bs.put(a.x | (b.x << a.y), a.y + b.y); }
-#endif
 
 __device__ __forceinline__ void fput_pair(LaneStager& bs, uint32_t a, uint32_t b)
 {
@@ -158,37 +153,23 @@ __device__ __forceinline__ uint32_t flit_off(uint32_t w, uint32_t nb)
 }
 __device__ __forceinline__ void fput_word(LaneStager& bs, uint32_t lit_s, uint32_t w, uint32_t nb)
 {
-#if FPNGB_LIT64
     const uint32_t nb8 = nb << 1;                                            // null half of the 8-byte table
     const uint32_t l64 = lit_s - 4096u;                                       // the 8-byte table sits directly below the 4-byte one
     const uint2 e0 = lds64c(l64 + flit_off8<0>(w, nb8)), e1 = lds64c(l64 + flit_off8<1>(w, nb8));
     const uint2 e2 = lds64c(l64 + flit_off8<2>(w, nb8)), e3 = lds64c(l64 + flit_off8<3>(w, nb8));
     fput_pair2(bs, e0, e1);
     fput_pair2(bs, e2, e3);
-#else
-    const uint32_t e0 = lds32c(lit_s + flit_off<0>(w, nb)), e1 = lds32c(lit_s + flit_off<1>(w, nb));
-    const uint32_t e2 = lds32c(lit_s + flit_off<2>(w, nb)), e3 = lds32c(lit_s + flit_off<3>(w, nb));
-    fput_pair(bs, e0, e1);
-    fput_pair(bs, e2, e3);
-#endif
 }
 // the 4 literal codes of a word whose bytes belong to two pixels: bytes [0, SPLIT) carry null flag nbA, bytes [SPLIT, 4) nbB
 // (0 or 0x400: the all-zero half of the table switches a pixel's literals off without a branch)
 template <int SPLIT>
 __device__ __forceinline__ void fput_word_2nb(LaneStager& bs, uint32_t lit_s, uint32_t w, uint32_t nbA, uint32_t nbB)
 {
-#if FPNGB_LIT64
     const uint32_t l64 = lit_s - 4096u, a8 = nbA << 1, b8 = nbB << 1;
     const uint2 e0 = lds64c(l64 + flit_off8<0>(w, SPLIT > 0 ? a8 : b8)), e1 = lds64c(l64 + flit_off8<1>(w, SPLIT > 1 ? a8 : b8));
     const uint2 e2 = lds64c(l64 + flit_off8<2>(w, SPLIT > 2 ? a8 : b8)), e3 = lds64c(l64 + flit_off8<3>(w, SPLIT > 3 ? a8 : b8));
     fput_pair2(bs, e0, e1);
     fput_pair2(bs, e2, e3);
-#else
-    const uint32_t e0 = lds32c(lit_s + flit_off<0>(w, SPLIT > 0 ? nbA : nbB)), e1 = lds32c(lit_s + flit_off<1>(w, SPLIT > 1 ? nbA : nbB));
-    const uint32_t e2 = lds32c(lit_s + flit_off<2>(w, SPLIT > 2 ? nbA : nbB)), e3 = lds32c(lit_s + flit_off<3>(w, SPLIT > 3 ? nbA : nbB));
-    fput_pair(bs, e0, e1);
-    fput_pair(bs, e2, e3);
-#endif
 }
 
 template <int CHANS>
@@ -221,7 +202,6 @@ struct FusedParams {
     uint32_t rows_per_group, steps_per_row, groups_per_image, n_images;
     uint8_t* out; size_t out_stride;
     uint32_t merge_first_unit;
-    uint32_t inline_crc;
 };
 
 template <int CHANS, bool DIRECT>
@@ -238,12 +218,8 @@ __global__ void __launch_bounds__(32 * kFusedWarps, CHANS == 3 ? 4 : 3) encode_f
     const uint32_t nwarps = blockDim.x >> 5;
     uint32_t* s_stage = reinterpret_cast<uint32_t*>(dyn_smem + kFusedWarps * kUnitBytes);
     const uint32_t stage_words = kFusedWarps * kUnitWords + 2;
-#if FPNGB_LIT64
     uint32_t* s_lit64 = s_stage + stage_words;      // [512][2]: (code, size) pairs + the all-zero null half, directly below s_lit
     uint32_t* s_lit = s_lit64 + 1024;
-#else
-    uint32_t* s_lit = s_stage + stage_words;
-#endif
     uint32_t* s_match = s_lit + 512;
     uint32_t* s_small = s_match + 88;               // 48 words
     // s_small: [0..7] has_lit, [8..15] trail, [16..23] npix, [24..31] unit bits, [32] ticket, [33] pred tail, [34] sh, [35] status
@@ -268,13 +244,11 @@ __global__ void __launch_bounds__(32 * kFusedWarps, CHANS == 3 ? 4 : 3) encode_f
     for (uint32_t i = tid; i < 256; i += blockDim.x) {
         const uint32_t e = book->lit[i];
         s_lit[i] = e; s_lit[256 + i] = 0u;
-#if FPNGB_LIT64
         s_lit64[2 * i] = e & 0xFFFFu; s_lit64[2 * i + 1] = e >> 16; s_lit64[512 + 2 * i] = 0u; s_lit64[512 + 2 * i + 1] = 0u;
-#endif
     }
     if (tid < 88) s_match[tid] = book->match[tid];
     uint32_t* s_crc = reinterpret_cast<uint32_t*>(s_u64 + 18);                // [4][256] slice tables of the 128-byte advance
-    if (p.inline_crc) for (uint32_t i = tid; i < 1024; i += blockDim.x) s_crc[i] = (&g_f128b[0][0])[i];
+    for (uint32_t i = tid; i < 1024; i += blockDim.x) s_crc[i] = (&g_f128b[0][0])[i];
 
     const uint32_t w = p.w, bpl = w * CHANS, S = p.steps_per_row;
     const uint32_t r_in_group = warp / S, step = warp - r_in_group * S;
@@ -567,11 +541,11 @@ __global__ void __launch_bounds__(32 * kFusedWarps, CHANS == 3 ? 4 : 3) encode_f
             s_small[33] = pred;
             if (!nfull) st_volatile_u64(&desc[g].tail, kTailReady | tailw | pred);
         }
-        if (p.inline_crc && lane == 0 && nwarps > 1) s_small[36] = 0u;
+        if (lane == 0 && nwarps > 1) s_small[36] = 0u;
     }
     // ---- CRC-32 partial of the group's bit string (staging words, group-relative: independent of the file position); warp 0
     // is busy with the look-back unless it is the only warp
-    if (p.inline_crc && (warp != 0 || nwarps == 1)) {
+    if (warp != 0 || nwarps == 1) {
         const uint32_t cw = nwarps > 1 ? nwarps - 1u : 1u, first = nwarps > 1 ? warp - 1u : 0u;
         uint32_t acc = 0;
         // this warp takes the chunks first, first + cw, ... counted from the END of the string
@@ -603,7 +577,7 @@ __global__ void __launch_bounds__(32 * kFusedWarps, CHANS == 3 ? 4 : 3) encode_f
     const uint32_t span = sh + group_bits, nfull = span >> 5;                // words whose bit 31 this group covers
     (void)span;
     if (s_small[35]) { if (tid == 0) p.st[img].status = 2u; return; }
-    if (p.inline_crc && tid == 0) {
+    if (tid == 0) {
         uint32_t r = 0;
         for (uint32_t u = 0; u < nwarps; u++) r ^= s_small[36 + u];
         desc[g].crc = (unsigned long long)r | ((unsigned long long)NWc << 32);
@@ -767,7 +741,7 @@ void launch_fused_crc(const void* desc_mem, uint32_t n, uint32_t w, uint32_t h, 
 // ------------------------------------------------------------------------------------------------------------------
 template <int CHANS, bool DIRECT> constexpr size_t fused_smem()
 {
-    return (size_t)kFusedWarps * fused_unit_bytes<CHANS, DIRECT>() + ((size_t)kFusedWarps * fused_unit_words<CHANS>() + 2 + 512 + 88 + 48 + (FPNGB_LIT64 ? 1024 : 0)) * 4 + 18 * 8 + 1024 * 4 + 16;
+    return (size_t)kFusedWarps * fused_unit_bytes<CHANS, DIRECT>() + ((size_t)kFusedWarps * fused_unit_words<CHANS>() + 2 + 512 + 88 + 48 + 1024) * 4 + 18 * 8 + 1024 * 4 + 16;
 }
 
 bool fused_eligible(const void* base, size_t image_stride, uint32_t w, uint32_t h, uint32_t chans, uint32_t n)
@@ -790,7 +764,7 @@ size_t fused_desc_bytes(uint32_t n, uint32_t w, uint32_t h)
 int launch_encode_fused(const uint8_t* pixels, size_t image_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags,
                         const CodeBook* books, uint32_t book_stride, uint2* row_adler, ImageState* st, void* desc_mem,
                         uint8_t* out, size_t out_stride, uint32_t* sizes, const uint8_t* png_header, uint32_t merge_first_unit, cudaStream_t s,
-                        cudaEvent_t mid_event, bool inline_crc)
+                        cudaEvent_t mid_event)
 {
     const uint32_t S = (w + kStep16 - 1) / kStep16, R = kFusedWarps / S, G = (h + R - 1) / R;
     const size_t dbytes = (size_t)n * G * sizeof(GroupDesc);
@@ -800,7 +774,7 @@ int launch_encode_fused(const uint8_t* pixels, size_t image_stride, uint32_t n, 
     p.pixels = pixels; p.image_stride = image_stride; p.w = w; p.h = h; p.books = books; p.book_stride = book_stride;
     p.row_adler = row_adler; p.st = st; p.desc = (GroupDesc*)desc_mem; p.ticket = (uint32_t*)((uint8_t*)desc_mem + dbytes);
     p.rows_per_group = R; p.steps_per_row = S; p.groups_per_image = G; p.n_images = n; p.out = out; p.out_stride = out_stride;
-    p.merge_first_unit = merge_first_unit; p.inline_crc = inline_crc ? 1u : 0u;
+    p.merge_first_unit = merge_first_unit;
     const uint32_t threads = 32u * R * S;
     const unsigned long long groups = (unsigned long long)n * G;
     const bool direct = !walk16_eligible(pixels, image_stride, w * chans, w, chans);

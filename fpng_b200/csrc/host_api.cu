@@ -26,9 +26,7 @@ namespace fpngb {
 static std::atomic<uint64_t> g_launches{0};
 
 static bool g_pack_crc = true;                  // fpngb_debug_pack_crc(): the 16-pixel pack kernel computes scanline CRCs (no CRC pass over the file)
-static bool g_inline_crc = true;                // fpngb_debug_inline_crc(): the single-pass encoder computes the IDAT CRC from in-kernel partials
-static bool g_crc_stream = true;                // fpngb_debug_crc_stream(0): first-generation (tile-staging) IDAT CRC kernel
-static int g_fused_mode = -1;                   // fpngb_debug_use_fused(): 1 single-pass encoder, 0 two-kernel encoder, -1 environment (FPNGB_FUSED)
+static bool g_fused = false;                    // fpngb_debug_use_fused(1): the single-pass encoder instead of the two-kernel encoder
 static bool g_crc_overlap = false;              // fpngb_debug_crc_overlap(1): chunked batches with the CRC kernel on a side stream (off by default: measured slower than the serial order)
 void count_launch(uint64_t n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
@@ -314,7 +312,7 @@ static bool force_generic_env()
 //    batches are cut into chunks and the CRC kernel of chunk k runs on a side stream underneath the scan and pack kernels of
 //    chunk k + 1 -- measured slower than the serial order (the kernels slow each other down more than the overlap gains),
 //    so it is off by default;
-//  * the single-pass encoder (encode_fused.cu), selected with FPNGB_FUSED=1 / fpngb_debug_use_fused(1): reads the pixels once
+//  * the single-pass encoder (encode_fused.cu), selected with fpngb_debug_use_fused(1): reads the pixels once
 //    and writes the file once, byte-identical output, measured slower than the two-kernel path because it is bound by
 //    instruction issue, not by HBM.
 //
@@ -329,15 +327,13 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
     // second-generation kernels (16 pixels per lane, coalesced 128-bit loads) whenever every scanline is 16-byte aligned;
     // FPNGB_FORCE_GENERIC=1 keeps the generic kernels (tests compare both)
     const bool force_generic = force_generic_env();
-    static const bool env_fused = getenv("FPNGB_FUSED") && atoi(getenv("FPNGB_FUSED")) != 0;
     // RGBA 1-pass under a table where a one-pixel match can lose against four literals: only the generic kernels
     // implement the reference's check (fpng.cpp:1520-1528); it cannot fire with the shipped table
     const uint32_t lit1_rule = (!two_pass && chans == 4 && c.h_static_books[1].lit1_rule) ? 1u : 0u;
     // the 16-pixel kernels take any scanline alignment (staged-tile loader for 16-byte aligned scanlines, direct realigning
     // loads otherwise); the generic 4-pixel kernels remain for the trained-table rule and for A/B tests
     const bool v2 = !force_generic && !lit1_rule;
-    const bool want_fused = g_fused_mode == 1 || (g_fused_mode < 0 && env_fused);
-    const bool fused = want_fused && !force_generic && !lit1_rule && !(flags & FPNGB_FORCE_UNCOMPRESSED) &&
+    const bool fused = g_fused && !force_generic && !lit1_rule && !(flags & FPNGB_FORCE_UNCOMPRESSED) &&
                        fused_eligible(src, L.image, w, h, chans, n);
     const bool convert = f.dtype != 0 || ((!v2 || fused) && (L.planar || L.row != (uint64_t)w * chans));
     const size_t image_bytes = (size_t)w * h * chans;
@@ -406,7 +402,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
         if (fused) {
             cudaEvent_t mid = ps ? ps->ev[kProfFused + 1] : nullptr;
             rc = launch_encode_fused(px, image_stride, cnt, w, h, chans, flags, books, book_stride, sp.row_adler, sp.st, ws.fused_desc,
-                                     out, out_stride, d_sizes + i0, png_header, merge_first_unit, s, mid, g_inline_crc);
+                                     out, out_stride, d_sizes + i0, png_header, merge_first_unit, s, mid);
             if (rc) return rc;
             if (ps) ps->used[kProfFused] = true;
             prof_mark(ps, kProfFinish, s);
@@ -433,7 +429,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
 
         CrcParams cp{};
         cp.out = out; cp.out_stride = out_stride; cp.st = sp.st;
-        cp.max_tiles = crc_ctas_for(max_encoded_size(w, h, chans)); cp.msg_start = kPngHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu;
+        cp.msg_start = kPngHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu;
         cudaStream_t cs = s;
         if (nchunks > 1) {                                                    // this chunk's CRC goes to the side stream
             FPNGB_CUDA_OK(cudaEventRecord(c.side_ev[k], s));
@@ -441,7 +437,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
             cs = c.side;
             if (ps) { cudaEventRecord(ps->crc_start, cs); ps->crc_side = true; }
         }
-        if (fused && g_inline_crc) {
+        if (fused) {
             launch_fused_crc(ws.fused_desc, cnt, w, h, books, book_stride, sp.st, out, out_stride, cs);   // combine the in-kernel partials
             cp.stored_only = 1u;                                              // the file-reading CRC kernel is only needed for stored-block images
             count_launch(1);
@@ -452,7 +448,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
             cp.stored_only = 1u;
             count_launch(1);
         }
-        if (g_crc_stream) launch_crc_stream(cp, cnt, max_encoded_size(w, h, chans), cs); else launch_crc(cp, cnt, cs);
+        launch_crc_stream(cp, cnt, max_encoded_size(w, h, chans), cs);
         prof_mark(ps, kProfCrc, cs);
         count_launch(2);
     }
@@ -794,12 +790,10 @@ size_t fpngb_max_encoded_size(uint32_t w, uint32_t h, uint32_t chans) { return m
 // test hook: scanlines per warp of the 16-pixel scan/pack kernels (0 = automatic); not part of the reference surface
 FPNGB_API void fpngb_debug_rows_per_warp(uint32_t v) { set_rows_per_warp16(v); }
 
-// test hook: 1 = use the two-kernel (scan + pack) encoder even where the single-pass encoder applies; not part of the reference surface
-FPNGB_API void fpngb_debug_disable_fused(int off) { g_fused_mode = off ? 0 : 1; }
-FPNGB_API void fpngb_debug_use_fused(int mode) { g_fused_mode = mode; }
+// test hook: 1 = the single-pass encoder where it applies; any other value (the tests restore the default with -1) = the two-kernel
+// encoder; not part of the reference surface
+FPNGB_API void fpngb_debug_use_fused(int mode) { g_fused = mode == 1; }
 FPNGB_API void fpngb_debug_crc_overlap(int on) { g_crc_overlap = on != 0; }
-FPNGB_API void fpngb_debug_crc_stream(int on) { g_crc_stream = on != 0; }
-FPNGB_API void fpngb_debug_inline_crc(int on) { g_inline_crc = on != 0; }
 // test hook: 0 = the two-kernel encoder leaves the IDAT CRC to the file-reading CRC kernel instead of computing it in the pack kernel
 FPNGB_API void fpngb_debug_pack_crc(int on) { g_pack_crc = on != 0; }
 

@@ -161,7 +161,7 @@ size_t fused_desc_bytes(uint32_t n, uint32_t w, uint32_t h);
 int launch_encode_fused(const uint8_t* pixels, size_t image_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags,
                         const CodeBook* books, uint32_t book_stride, uint2* row_adler, ImageState* st, void* desc_mem,
                         uint8_t* out, size_t out_stride, uint32_t* sizes, const uint8_t* png_header, uint32_t merge_first_unit, cudaStream_t s,
-                        cudaEvent_t mid_event, bool inline_crc);
+                        cudaEvent_t mid_event);
 void launch_fused_crc(const void* desc_mem, uint32_t n, uint32_t w, uint32_t h, const CodeBook* books, uint32_t book_stride, const ImageState* st,
                       uint8_t* out, size_t out_stride, cudaStream_t s);
 int fused_tables_init();

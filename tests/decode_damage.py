@@ -1,10 +1,10 @@
 """Seeded damaged fpng streams for the fpng decode (decode_prepare_kernel, decode_scan_kernel, decode_link_kernel,
-decode_write_kernel, decode_write_staged_kernel, decode_stored_kernel), placed at the boundaries where those kernels split a
-stream between them.
+decode_write_kernel, decode_stored_kernel), placed at the boundaries where those kernels split a stream between them.
 
 The kernels cut a file's stream into subsequences of SUB_BITS bits, counted from the 4-byte aligned file byte
-(idat_ofs + 8) & ~3 ("aligned bits" below).  A scan or write CTA covers DEC_THREADS subsequences (32 KiB), a staged write CTA
-WS_THREADS (28 KiB), and the link kernel walks chunks of LINK_THREADS subsequences (128 KiB) with a carry between them.  Every
+(idat_ofs + 8) & ~3 ("aligned bits" below).  A scan or write CTA covers DEC_THREADS subsequences (32 KiB), and the link kernel
+walks chunks of LINK_THREADS subsequences (128 KiB) with a carry between them.  The WS_THREADS boundary (28 KiB) is where the CTAs
+of an earlier, shared-memory staged write kernel met; the cases placed there are kept as a boundary that falls inside a CTA.  Every
 case names the construct it reaches: its family and, where it was placed, the boundary and the aligned bit of the damage.
 tests/test_decode_damage_cpu.py checks that each placed case lands where it claims and that the oracle equals the reference on
 every case; tests/test_decode_damage_gpu.py compares every decode entry point with the reference.
@@ -31,11 +31,12 @@ import streamgen
 
 SUB_BITS = 1024                 # decode.cuh kSubBits
 DEC_THREADS = 256               # decode.cuh kDecThreads: subsequences per scan / write CTA
-WS_THREADS = 224                # decode_kernels.cu kWsThreads: subsequences per staged write CTA
+WS_THREADS = 224                # subsequences per CTA of the removed staged write kernel
 LINK_THREADS = 1024             # decode.cuh kLinkThreads: subsequences per link chunk
 PRE_ROLL = 256                  # decode.cuh kPreRoll: default speculative lead-in of the scan
 
-# named boundaries, in aligned bits: the first two subsequence boundaries, one staged and one scan CTA, one and two link chunks
+# named boundaries, in aligned bits: the first two subsequence boundaries, WS_THREADS subsequences, one scan CTA, one and two
+# link chunks
 BOUNDS = {"sub1": SUB_BITS, "sub2": 2 * SUB_BITS, "ws_cta": WS_THREADS * SUB_BITS, "cta": DEC_THREADS * SUB_BITS,
           "link": LINK_THREADS * SUB_BITS, "link2": 2 * LINK_THREADS * SUB_BITS}
 NEAR_BYTES = 8                  # random damage "near" a boundary: within +-8 bytes

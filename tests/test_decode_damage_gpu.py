@@ -1,7 +1,7 @@
 """GPU tests of the fpng decode on damaged streams (tests/decode_damage.py): every decode entry point gives the reference's status
 for every case, and its pixels where the status is 0, with damage at the subsequence, CTA and link-chunk boundaries where the
 decode kernels hand a stream from one to the next.  The same large-file set runs with every speculative start wrong (pre-roll 0)
-and through both write kernels, and with the integrity check on.  A disagreement is accepted only when a token trace of the file
+and with the integrity check on.  A disagreement is accepted only when a token trace of the file
 (tests/deflatetrace.py) shows one of the documented deviations of INTEGRATION.md section 7; the test prints how many."""
 import hashlib
 from collections import Counter
@@ -232,8 +232,8 @@ def test_device_entry_points(gpu, damage):
 
 
 def test_speculation_and_write_paths(gpu, damage):
-    """the large-file, stored and placed cases with the scan's pre-roll at 256 and 0 (every speculative start wrong on a damaged
-    stream) and the write pass through decode_write_kernel alone and behind decode_write_staged_kernel"""
+    """the large-file, stored and placed cases through the write and stored-block kernels with the scan's pre-roll at 256 and 0
+    (every speculative start wrong on a damaged stream)"""
     from fpng_b200._lib import lib
     L = lib()
     cases, bases, want = damage
@@ -242,18 +242,15 @@ def test_speculation_and_write_paths(gpu, damage):
     try:
         for pre in (256, 0):
             assert L.fpngb_debug_decode_preroll(pre) == 0
-            for staged in (0, 1):
-                L.fpngb_debug_decode_staged(staged)
-                L.fpngb_debug_decode_repairs(1)
-                for d in (3, 4):
-                    res = gpu.decode_files([cases[i].file for i in sel], d)
-                    for i, r in zip(sel, res):
-                        t.check(gpu, cases[i], d, r[0], r[1], want[(i, d)], f"pre{pre}_staged{staged}")
-                print(f"pre-roll {pre}, staged {staged}: {L.fpngb_debug_decode_repairs(0)} repaired subsequences")
+            L.fpngb_debug_decode_repairs(1)
+            for d in (3, 4):
+                res = gpu.decode_files([cases[i].file for i in sel], d)
+                for i, r in zip(sel, res):
+                    t.check(gpu, cases[i], d, r[0], r[1], want[(i, d)], f"pre{pre}")
+            print(f"pre-roll {pre}: {L.fpngb_debug_decode_repairs(0)} repaired subsequences")
     finally:
         L.fpngb_debug_decode_preroll(dd.PRE_ROLL)
-        L.fpngb_debug_decode_staged(0)
-    print(f"{len(sel)} cases x 4 settings; accepted deviations:", dict(t.accepted) or 0)
+    print(f"{len(sel)} cases x 2 settings; accepted deviations:", dict(t.accepted) or 0)
 
 
 def test_verify_switch(gpu, damage, reference):

@@ -47,8 +47,7 @@ def L(gpu):
     from test_decoder_model_cpu import K_PRE_ROLL
     L = lib()
     yield L
-    L.fpngb_debug_decode_preroll(K_PRE_ROLL)                                 # the defaults
-    L.fpngb_debug_decode_staged(0)
+    L.fpngb_debug_decode_preroll(K_PRE_ROLL)                                 # the default
 
 
 # ---- 1. walk parity ------------------------------------------------------------------------------------------------------
@@ -277,18 +276,16 @@ def test_strided_offsets_equal_decode_batch_device(gpu, L, oracle):
         m = len(files)
         offsets = torch.arange(m, dtype=torch.int64, device="cuda") * stride
         dsizes = torch.from_numpy(sizes.view(np.int32).copy()).cuda()
-        for mode in (0, 1):
-            L.fpngb_debug_decode_staged(mode)
-            for d in (3, 4):
-                a_px, a_st = gpu.decode_batch_device(t, sizes, ofs, lens, w, h, c, d)
-                b_px = torch.full((m, h, w, d), 0x5A, dtype=torch.uint8, device="cuda")
-                _, b_st = gpu.decode_packed_device(t.reshape(-1), offsets, dsizes, w, h, c, d, out=b_px)
-                torch.cuda.synchronize()
-                a_st, b_st = a_st.cpu().numpy(), b_st.cpu().numpy()
-                assert np.array_equal(a_st, b_st), (w, h, c, mode, d, a_st, b_st)
-                assert set(a_st.tolist()) <= {0, 1} and (a_st == 0).sum() >= n
-                ok = torch.from_numpy(a_st == 0).cuda()
-                assert torch.equal(a_px[ok], b_px[ok]), (w, h, c, mode, d)
+        for d in (3, 4):
+            a_px, a_st = gpu.decode_batch_device(t, sizes, ofs, lens, w, h, c, d)
+            b_px = torch.full((m, h, w, d), 0x5A, dtype=torch.uint8, device="cuda")
+            _, b_st = gpu.decode_packed_device(t.reshape(-1), offsets, dsizes, w, h, c, d, out=b_px)
+            torch.cuda.synchronize()
+            a_st, b_st = a_st.cpu().numpy(), b_st.cpu().numpy()
+            assert np.array_equal(a_st, b_st), (w, h, c, d, a_st, b_st)
+            assert set(a_st.tolist()) <= {0, 1} and (a_st == 0).sum() >= n
+            ok = torch.from_numpy(a_st == 0).cuda()
+            assert torch.equal(a_px[ok], b_px[ok]), (w, h, c, d)
 
 
 # ---- 4. shape and argument statuses in one call --------------------------------------------------------------------------

@@ -129,12 +129,9 @@ def test_decode_batch_host(gpu, oracle):
                 assert np.array_equal(out[i], epx), i
 
 
-def test_decode_write_paths_agree(gpu, oracle):
-    """The write pass has two kernels: the shared-memory staged one (literal-dominated CTAs) and the per-thread sink (everything the
-    staged kernel leaves: more than 64 KiB of output per CTA).  Both alone and together must give the oracle's pixels and statuses,
-    on clean and on corrupted streams; the large cases cross many scanlines / CTAs and mix matches into literal runs."""
-    from fpng_b200._lib import lib
-    L = lib()
+def test_decode_write_pass_matches_oracle(gpu, oracle):
+    """The write pass (decode_write_kernel, one thread per subsequence) must give the oracle's pixels and statuses, on clean and on
+    corrupted streams; the large cases cross many scanlines / CTAs and mix matches into literal runs."""
     rs = np.random.RandomState(3)
     cases = []
     for (kind, w, h, c, flags) in (("g1", 700, 200, 3, 0), ("g1", 512, 160, 4, 0), ("mut", 1000, 120, 3, 1), ("runs", 640, 200, 4, 0),
@@ -146,14 +143,9 @@ def test_decode_write_paths_agree(gpu, oracle):
             bad = bytearray(png); pos = int(rs.randint(60, len(bad))); bad[pos] ^= 1 << int(rs.randint(0, 8))
             cases.append((bytes(bad), c))
     expect = [(oracle.decode(png, 3), oracle.decode(png, 4)) for png, c in cases]
-    try:
-        for mode in (0, 1):
-            L.fpngb_debug_decode_staged(mode)
-            for (png, c), (e3, e4) in zip(cases, expect):
-                for d, e in ((3, e3), (4, e4)):
-                    st, px, *_ = gpu.fpng_decode_memory(png, d)
-                    assert st == e[0], (mode, len(png), d, st, e[0])
-                    if st == 0:
-                        assert np.array_equal(px, e[1]), (mode, len(png), d)
-    finally:
-        L.fpngb_debug_decode_staged(0)                          # the default
+    for (png, c), (e3, e4) in zip(cases, expect):
+        for d, e in ((3, e3), (4, e4)):
+            st, px, *_ = gpu.fpng_decode_memory(png, d)
+            assert st == e[0], (len(png), d, st, e[0])
+            if st == 0:
+                assert np.array_equal(px, e[1]), (len(png), d)

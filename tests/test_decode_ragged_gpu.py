@@ -147,7 +147,7 @@ def test_reference_written_files(gpu, oracle):
         assert (st == 0).all()
 
 
-# ---- 2. the same bytes as the uniform call, both write kernels, repairs ----------------------------------------------------
+# ---- 2. the same bytes as the uniform call, repairs ------------------------------------------------------------------------
 @pytest.mark.parametrize("pre_roll", [256, 0])
 def test_same_bytes_as_uniform_call(gpu, L, oracle, pre_roll):  # noqa: F811
     import torch
@@ -168,26 +168,24 @@ def test_same_bytes_as_uniform_call(gpu, L, oracle, pre_roll):  # noqa: F811
         groups.setdefault(inf[1:4], []).append(i)
     bounds = bounds_of(gpu, files)
     assert L.fpngb_debug_decode_preroll(pre_roll) == 0
-    for mode in (0, 1):
-        L.fpngb_debug_decode_staged(mode)
-        for d in (3, 4):
-            L.fpngb_debug_decode_repairs(1)
-            out, oo, info, st = gpu.decode_packed_ragged_device(data, offsets, sizes, d, max_file_size=bounds[0], max_w=bounds[1],
-                                                                max_h=bounds[2])
-            torch.cuda.synchronize()
-            assert int(L.fpngb_debug_decode_repairs(1)) == want_repairs, (mode, d)
-            views = gpu.ragged_views(out, oo, info, st, d)
-            st = st.cpu().numpy()
-            for (w, h, c), idx in groups.items():
-                sub = offsets[idx]
-                px, ust = gpu.decode_packed_device(data, sub, sizes[idx], w, h, c, d, max_file_size=bounds[0])
-                ust = ust.cpu().numpy()
-                assert np.array_equal(ust, st[idx]), ((w, h, c), mode, d)
-                for k, i in enumerate(idx):
-                    if ust[k] == 0:
-                        assert torch.equal(views[i], px[k]), ((w, h, c), mode, d, i)
-                    else:
-                        assert views[i] is None
+    for d in (3, 4):
+        L.fpngb_debug_decode_repairs(1)
+        out, oo, info, st = gpu.decode_packed_ragged_device(data, offsets, sizes, d, max_file_size=bounds[0], max_w=bounds[1],
+                                                            max_h=bounds[2])
+        torch.cuda.synchronize()
+        assert int(L.fpngb_debug_decode_repairs(1)) == want_repairs, d
+        views = gpu.ragged_views(out, oo, info, st, d)
+        st = st.cpu().numpy()
+        for (w, h, c), idx in groups.items():
+            sub = offsets[idx]
+            px, ust = gpu.decode_packed_device(data, sub, sizes[idx], w, h, c, d, max_file_size=bounds[0])
+            ust = ust.cpu().numpy()
+            assert np.array_equal(ust, st[idx]), ((w, h, c), d)
+            for k, i in enumerate(idx):
+                if ust[k] == 0:
+                    assert torch.equal(views[i], px[k]), ((w, h, c), d, i)
+                else:
+                    assert views[i] is None
 
 
 # ---- 3. statuses and guards ------------------------------------------------------------------------------------------------

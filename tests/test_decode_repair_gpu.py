@@ -20,8 +20,7 @@ def L(gpu):
     from fpng_b200._lib import lib
     L = lib()
     yield L
-    L.fpngb_debug_decode_preroll(K_PRE_ROLL)                                 # the defaults
-    L.fpngb_debug_decode_staged(0)
+    L.fpngb_debug_decode_preroll(K_PRE_ROLL)                                 # the default
 
 
 def decode_counted(gpu, L, png, desired):
@@ -31,20 +30,18 @@ def decode_counted(gpu, L, png, desired):
     return st, px, int(L.fpngb_debug_decode_repairs(1))
 
 
-def check_file(gpu, L, oracle, png, pre_roll=K_PRE_ROLL, modes=(0,), desired=(3, 4), want=None):
-    """decodes `png` with every write kernel mode and desired channel count: statuses / pixels against the oracle, repairs
-    against the model (`want`: already known); returns the repair count"""
+def check_file(gpu, L, oracle, png, pre_roll=K_PRE_ROLL, desired=(3, 4), want=None):
+    """decodes `png` at every desired channel count: statuses / pixels against the oracle, repairs against the model (`want`:
+    already known); returns the repair count"""
     if want is None:
         want = model_repairs(png, pre_roll)
     for d in desired:
         est, epx, *_ = oracle.decode(png, d)
-        for mode in modes:
-            L.fpngb_debug_decode_staged(mode)
-            st, px, rep = decode_counted(gpu, L, png, d)
-            assert st == est, (len(png), pre_roll, mode, d, st, est)
-            if st == 0:
-                assert np.array_equal(px, epx), (len(png), pre_roll, mode, d)
-            assert rep == want, (len(png), pre_roll, mode, d, rep, want)
+        st, px, rep = decode_counted(gpu, L, png, d)
+        assert st == est, (len(png), pre_roll, d, st, est)
+        if st == 0:
+            assert np.array_equal(px, epx), (len(png), pre_roll, d)
+        assert rep == want, (len(png), pre_roll, d, rep, want)
     return want
 
 
@@ -65,11 +62,11 @@ def test_slow_synchronising_files(gpu, L, oracle, kind, w, h, chans, flags):
         assert ok and len(iters) >= 2                                       # several 1024-subsequence chunks
         if flags == 1 and kind in ("u128", "u64"):
             assert repairs > (m.g1 - m.g0) // 2 and max(iters) >= 3, (repairs, iters)
-        check_file(gpu, L, oracle, f, modes=(0, 1), want=repairs)
+        check_file(gpu, L, oracle, f, want=repairs)
         np.testing.assert_array_equal(gpu.fpng_decode_memory(f, chans)[1], img.reshape(-1))
         # a corrupted copy: a bit flip after the header
         bad = bytearray(f); pos = int(rs.randint(60 + (12 + pad if pad else 0), len(bad))); bad[pos] ^= 1 << int(rs.randint(0, 8))
-        check_file(gpu, L, oracle, bytes(bad), modes=(0, 1))
+        check_file(gpu, L, oracle, bytes(bad))
 
 
 def test_batch_mixes_slow_and_ordinary_files(gpu, L, oracle):
@@ -126,9 +123,9 @@ def test_forced_wrong_guesses(gpu, L, oracle, pre_roll):
             check_file(gpu, L, oracle, bytes(bad), pre_roll, desired=(c,))
     for (kind, w, h, c, flags) in (("g1", 700, 200, 3, 0), ("mut", 1000, 120, 3, 1), ("runs", 640, 200, 4, 0), ("g1", 3, 3000, 4, 0)):
         png = oracle.encode(imagegen.make(kind, w, h, c, 5), w, h, c, flags)
-        total += check_file(gpu, L, oracle, png, pre_roll, modes=(0, 1))
+        total += check_file(gpu, L, oracle, png, pre_roll)
         bad = bytearray(png); pos = int(rs.randint(60, len(bad))); bad[pos] ^= 1 << int(rs.randint(0, 8))
-        check_file(gpu, L, oracle, bytes(bad), pre_roll, modes=(0, 1))
+        check_file(gpu, L, oracle, bytes(bad), pre_roll)
     assert total > 1000                                                    # the guesses really were wrong
 
 
@@ -143,13 +140,11 @@ def test_hand_built_streams(gpu, L, oracle, pre_roll):
         want = model_repairs(f, pre_roll)
         for d in (3, 4):
             est, epx, *_ = oracle.decode(f, d)
-            for mode in (0, 1):
-                L.fpngb_debug_decode_staged(mode)
-                st, px, rep = decode_counted(gpu, L, f, d)
-                if deviation:
-                    assert est == 0 and st == gpu.FPNG_DECODE_NOT_FPNG, (name, d, mode, st)
-                else:
-                    assert st == est, (name, pre_roll, d, mode, st, est)
-                    if st == 0:
-                        assert np.array_equal(px, epx), (name, pre_roll, d, mode)
-                assert rep == want, (name, pre_roll, d, mode, rep, want)
+            st, px, rep = decode_counted(gpu, L, f, d)
+            if deviation:
+                assert est == 0 and st == gpu.FPNG_DECODE_NOT_FPNG, (name, d, st)
+            else:
+                assert st == est, (name, pre_roll, d, st, est)
+                if st == 0:
+                    assert np.array_equal(px, epx), (name, pre_roll, d)
+            assert rep == want, (name, pre_roll, d, rep, want)

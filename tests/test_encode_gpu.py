@@ -263,16 +263,15 @@ def test_random_dimension_fuzz_like_reference_E(gpu, oracle):
                 assert st == 0
 
 
-@pytest.mark.parametrize("mode", ["fused+inline_crc", "fused", "two_kernel", "two_kernel_chunked", "two_kernel_file_crc", "two_kernel_file_crc_chunked"])
+@pytest.mark.parametrize("mode", ["fused", "two_kernel", "two_kernel_chunked", "two_kernel_file_crc", "two_kernel_file_crc_chunked"])
 def test_encoder_generations_agree_with_oracle(gpu, oracle, mode):
-    """The single-pass encoder (encode_fused.cu: decoupled look-back, lane-local bit strings, in-kernel CRC partials), the same
-    with the file-reading CRC kernel, and the two-kernel scan + pack encoder (default: scanline CRCs from the pack kernel; with the
-    file-reading CRC kernel; each also cut into chunks with the CRC work on a side stream) must all write the reference's bytes."""
+    """The single-pass encoder (encode_fused.cu: decoupled look-back, lane-local bit strings, in-kernel CRC partials) and the
+    two-kernel scan + pack encoder (default: scanline CRCs from the pack kernel; with the file-reading CRC kernel; each also cut
+    into chunks with the CRC work on a side stream) must all write the reference's bytes."""
     import torch
     from fpng_b200._lib import lib
     L = lib()
-    L.fpngb_debug_inline_crc(1 if mode == "fused+inline_crc" else 0)
-    L.fpngb_debug_use_fused(1 if mode.startswith("fused") else 0)
+    L.fpngb_debug_use_fused(1 if mode == "fused" else 0)
     L.fpngb_debug_crc_overlap(1 if mode.endswith("_chunked") else 0)
     L.fpngb_debug_pack_crc(0 if "file_crc" in mode else 1)
     try:
@@ -294,7 +293,6 @@ def test_encoder_generations_agree_with_oracle(gpu, oracle, mode):
                         for i in range(nimg):
                             assert oh[i, : sz[i]].tobytes() == oracle.encode(imgs[i], w, h, c, flags), (mode, kind, w, h, c, flags, i)
     finally:
-        L.fpngb_debug_inline_crc(1)
         L.fpngb_debug_use_fused(-1)
         L.fpngb_debug_crc_overlap(0)
         L.fpngb_debug_pack_crc(1)
