@@ -10,18 +10,7 @@
 
 namespace fpngb {
 
-struct CrcByteTable { uint32_t t[256]; };
-static constexpr CrcByteTable make_crc_byte_table()
-{
-    CrcByteTable r{};
-    for (uint32_t n = 0; n < 256; n++) {
-        uint32_t c = n;
-        for (int k = 0; k < 8; k++) c = (c & 1u) ? (kCrcPoly ^ (c >> 1)) : (c >> 1);
-        r.t[n] = c;
-    }
-    return r;
-}
-__constant__ CrcByteTable c_walk_crc = make_crc_byte_table();
+__constant__ CrcByteTable c_walk_crc = crc_byte_table();
 
 struct DeviceCrc {
     __device__ uint32_t operator()(const uint8_t* p, size_t n) const

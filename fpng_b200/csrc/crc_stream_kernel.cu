@@ -1,9 +1,8 @@
-// fpng_b200/csrc/crc_stream_kernel.cu -- second-generation IDAT CRC-32 kernel of the encoder (fpng.cpp:1797-1800 computes
-// fpng_crc32 over "IDAT" + zlib stream with PCLMULQDQ folding, fpng.cpp:255-281; NVIDIA GPUs have no carry-less multiply).
+// fpng_b200/csrc/crc_stream_kernel.cu -- CRC-32 of a byte stream on the device: the IDAT CRC of the encoders (fpng.cpp:1797-1800
+// computes fpng_crc32 over "IDAT" + zlib stream with PCLMULQDQ folding, fpng.cpp:255-281; NVIDIA GPUs have no carry-less
+// multiply), the decoder's IDAT check and fpngb_crc32 on host buffers of at least 4 KiB (host_api.cu).
 //
-// The first kernel (idat_crc_kernel, checksum_kernels.cu) stages 32 KiB tiles in shared memory, gives every thread a
-// 128-byte chunk and combines 256 chunk CRCs with an 8-level multiply tree per tile: 7.8 thread-instructions per byte, two
-// block barriers per tile, 0.27 of the HBM peak.  This kernel never stages the data and has no barrier in its main loop:
+// idat_crc_stream_kernel never stages the data and has no barrier in its main loop:
 //   * a warp owns 8 KiB of the file; its lanes read consecutive 32-bit words straight from global memory (one coalesced
 //     128-byte request per step, 8 independent requests in flight) and each lane runs a Horner recurrence whose step advances
 //     the CRC register over 128 bytes (four 256-entry slice tables of that advance in shared memory);
@@ -13,7 +12,8 @@
 //     CTA of an image appends the (at most 3) bytes after the last whole word, applies init/xorout and stores the CRC.
 // The message may start at any byte: the first word's bytes in front of it are masked to zero, which a zero-initialised CRC
 // register does not see.  The decoder's opt-in integrity check runs the same kernel over the files it reads (VERIFY).
-// About 3.3 thread-instructions per byte (4 table look-ups + 8 address instructions + 3 XORs per word).
+// About 3.3 thread-instructions per byte (4 table look-ups + 8 address instructions + 3 XORs per word): it replaced a kernel
+// that staged 32 KiB tiles in shared memory and combined 128-byte chunk CRCs with a multiply tree, at 7.8 per byte.
 #include "kernels.cuh"
 #include "crc_math.cuh"
 #include "decode.cuh"
@@ -35,27 +35,18 @@ __device__ uint32_t g2_xpow8[4][256];             // x^(8 * d * 256^k): powers o
 
 int crc_stream_tables_init()
 {
-    static uint32_t t[4][256], f[4][256], lane[32][8][16], wm[kCs2Warps][8][16], xp[64];
-    for (uint32_t n = 0; n < 256; n++) {
-        uint32_t c = n;
-        for (int k = 0; k < 8; k++) c = (c & 1) ? (kCrcPoly ^ (c >> 1)) : (c >> 1);
-        t[0][n] = c;
-    }
-    for (uint32_t n = 0; n < 256; n++) for (int k = 1; k < 4; k++) t[k][n] = (t[k - 1][n] >> 8) ^ t[0][t[k - 1][n] & 0xFF];
-    xp[0] = 0x40000000u;
-    for (int k = 1; k < 64; k++) xp[k] = gf2_mulmod(xp[k - 1], xp[k - 1]);
-    auto xpow = [&](unsigned long long e) { uint32_t r = kCrcOne; for (int k = 0; e; k++, e >>= 1) if (e & 1ull) r = gf2_mulmod(r, xp[k]); return r; };
-    const uint32_t adv = xpow(8ull * 124ull);        // the slice-by-4 word update advances 4 bytes; 124 more
-    for (int k = 0; k < 4; k++) for (uint32_t n = 0; n < 256; n++) f[k][n] = gf2_mulmod(t[3 - k][n], adv);
-    for (uint32_t l = 0; l < 32; l++) { const uint32_t c = xpow(32ull * (32 - l)); for (int j = 0; j < 8; j++) for (uint32_t n = 0; n < 16; n++) lane[l][j][n] = gf2_mulmod(n << (4 * j), c); }
-    for (uint32_t m = 0; m < kCs2Warps; m++) { const uint32_t c = xpow(32ull * kCs2WarpWords * m); for (int j = 0; j < 8; j++) for (uint32_t n = 0; n < 16; n++) wm[m][j][n] = gf2_mulmod(n << (4 * j), c); }
+    static uint32_t f[4][256], lane[32][8][16], wm[kCs2Warps][8][16], xp[64], p8[4][256];
+    static constexpr CrcByteTable t = crc_byte_table();
+    crc_advance_tables(f, 128);
+    for (uint32_t l = 0; l < 32; l++) crc_mul_table(lane[l], xpow(32ull * (32 - l)));
+    for (uint32_t m = 0; m < kCs2Warps; m++) crc_mul_table(wm[m], xpow(32ull * kCs2WarpWords * m));
+    crc_xpow2_table(xp);
+    for (int k = 0; k < 4; k++) for (unsigned long long d = 0; d < 256; d++) p8[k][d] = xpow(8ull * (d << (8 * k)));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g2_f128b, f, sizeof f));
-    FPNGB_CUDA_OK(cudaMemcpyToSymbol(g2_byte, t[0], sizeof t[0]));
+    FPNGB_CUDA_OK(cudaMemcpyToSymbol(g2_byte, t.t, sizeof t.t));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g2_lane_mul, lane, sizeof lane));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g2_warp_mul, wm, sizeof wm));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(c2_xpow2, xp, sizeof xp));
-    static uint32_t p8[4][256];
-    for (int k = 0; k < 4; k++) for (unsigned long long d = 0; d < 256; d++) p8[k][d] = xpow(8ull * (d << (8 * k)));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g2_xpow8, p8, sizeof p8));
     return 0;
 }
@@ -67,14 +58,6 @@ int crc_stream_table_ptrs(const uint32_t** f128b, const uint32_t** lane_mul)
     FPNGB_CUDA_OK(cudaGetSymbolAddress(&b, g2_lane_mul));
     *f128b = (const uint32_t*)a; *lane_mul = (const uint32_t*)b;
     return 0;
-}
-
-__device__ __forceinline__ uint32_t mul_nib(const uint32_t (*t)[16], uint32_t a)
-{
-    uint32_t r = __ldg(&t[0][a & 15u]);
-#pragma unroll
-    for (int j = 1; j < 8; j++) r ^= __ldg(&t[j][(a >> (4 * j)) & 15u]);
-    return r;
 }
 
 // grid (max CTAs per image, n images); only images with st.stored == want_stored (or all when want_stored < 0) are processed.
@@ -158,7 +141,7 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStre
                 else c = x;
             }
         }
-        c = mul_nib(g2_lane_mul[lane], c);
+        c = mul_nibbles(g2_lane_mul[lane], c);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) c ^= __shfl_xor_sync(0xFFFFFFFFu, c, o);
@@ -209,12 +192,6 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStre
 // the initial value and the final XOR (both linear as well) and stores the CRC.
 // ------------------------------------------------------------------------------------------------------------------
 constexpr uint32_t kRowCrcThreads = 256, kRowCrcSplit = 8;
-
-__device__ __forceinline__ uint32_t crc_bits(uint32_t reg, uint32_t v, uint32_t nbits)
-{
-    for (uint32_t i = 0; i < nbits; i++) { reg = (reg >> 1) ^ (((reg ^ (v >> i)) & 1u) ? kCrcPoly : 0u); }
-    return reg;
-}
 
 // x^e from byte-digit tables: x^e = x^(e & 7) * prod_k g2_xpow8[k][digit k of e >> 3]  (e < 2^35: every file this library writes)
 __device__ __forceinline__ uint32_t xpow_tab(unsigned long long e)

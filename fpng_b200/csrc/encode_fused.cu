@@ -42,31 +42,13 @@ __device__ uint32_t g_lane_mul[32][8][16];        // nibble tables: multiply by 
 __device__ uint32_t g_chunk_mul[32][8][16];       // nibble tables: multiply by x^(32 * kCrcChunkWords * m)
 __constant__ uint32_t c_fx_pow2[64];              // x^(2^k)
 
-__device__ __forceinline__ uint32_t mul_nibbles(const uint32_t (*t)[16], uint32_t a)
-{
-    uint32_t r = __ldg(&t[0][a & 15u]);
-#pragma unroll
-    for (int j = 1; j < 8; j++) r ^= __ldg(&t[j][(a >> (4 * j)) & 15u]);
-    return r;
-}
-
 int fused_tables_init()
 {
-    static uint32_t t[4][256], f[4][256], lane[32][8][16], chunk[32][8][16], xp[64];
-    for (uint32_t n = 0; n < 256; n++) {
-        uint32_t c = n;
-        for (int k = 0; k < 8; k++) c = (c & 1) ? (kCrcPoly ^ (c >> 1)) : (c >> 1);
-        t[0][n] = c;
-    }
-    for (uint32_t n = 0; n < 256; n++) for (int k = 1; k < 4; k++) t[k][n] = (t[k - 1][n] >> 8) ^ t[0][t[k - 1][n] & 0xFF];
-    xp[0] = 0x40000000u;
-    for (int k = 1; k < 64; k++) xp[k] = gf2_mulmod(xp[k - 1], xp[k - 1]);
-    auto xpow = [&](unsigned long long e) { uint32_t r = kCrcOne; for (int k = 0; e; k++, e >>= 1) if (e & 1ull) r = gf2_mulmod(r, xp[k]); return r; };
-    // the word update "reg = T3[b0] ^ T2[b1] ^ T1[b2] ^ T0[b3]" advances (reg ^ word) over 4 bytes; 124 more bytes = x^(8*124)
-    const uint32_t adv = xpow(8ull * 124ull);
-    for (int k = 0; k < 4; k++) for (uint32_t n = 0; n < 256; n++) f[k][n] = gf2_mulmod(t[3 - k][n], adv);
-    for (uint32_t l = 0; l < 32; l++) { const uint32_t c = xpow(32ull * (32 - l)); for (int j = 0; j < 8; j++) for (uint32_t n = 0; n < 16; n++) lane[l][j][n] = gf2_mulmod(n << (4 * j), c); }
-    for (uint32_t m = 0; m < 32; m++) { const uint32_t c = xpow(32ull * kCrcChunkWords * m); for (int j = 0; j < 8; j++) for (uint32_t n = 0; n < 16; n++) chunk[m][j][n] = gf2_mulmod(n << (4 * j), c); }
+    static uint32_t f[4][256], lane[32][8][16], chunk[32][8][16], xp[64];
+    crc_advance_tables(f, 128);
+    for (uint32_t l = 0; l < 32; l++) crc_mul_table(lane[l], xpow(32ull * (32 - l)));
+    for (uint32_t m = 0; m < 32; m++) crc_mul_table(chunk[m], xpow(32ull * kCrcChunkWords * m));
+    crc_xpow2_table(xp);
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g_f128b, f, sizeof f));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g_lane_mul, lane, sizeof lane));
     FPNGB_CUDA_OK(cudaMemcpyToSymbol(g_chunk_mul, chunk, sizeof chunk));
@@ -682,14 +664,12 @@ struct FusedCrcParams {
     uint8_t* out; size_t out_stride;
 };
 
-__device__ __forceinline__ uint32_t crc_bit_step(uint32_t reg, uint32_t bit) { return (reg >> 1) ^ (((reg ^ bit) & 1u) ? kCrcPoly : 0u); }
-
 __global__ void __launch_bounds__(256) fused_crc_kernel(FusedCrcParams p)
 {
     __shared__ uint32_t s_part[8];
     const uint32_t img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const ImageState st = p.st[img];
-    if (st.stored || st.status) return;                                      // stored-block images: idat_crc_kernel reads the file
+    if (st.stored || st.status) return;                                      // stored-block images: idat_crc_stream_kernel reads the file
     const CodeBook* book = p.books + (size_t)img * p.book_stride;
     const GroupDesc* desc = p.desc + (size_t)img * p.groups_per_image;
     const unsigned long long E = (unsigned long long)(kPngHeaderSize + st.zsize) * 8ull;

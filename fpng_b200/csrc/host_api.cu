@@ -7,6 +7,7 @@
 // device every entry point fails with FPNGB_ERR_NO_DEVICE.
 #include "../../include/fpng_b200.h"
 #include "kernels.cuh"
+#include "crc_math.cuh"
 #include "layout.h"
 #include "row_walk.cuh"
 #include "static_tables.h"
@@ -429,7 +430,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
 
         CrcParams cp{};
         cp.out = out; cp.out_stride = out_stride; cp.st = sp.st;
-        cp.msg_start = kPngHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu;
+        cp.msg_start = kPngHeaderSize - 4;
         cudaStream_t cs = s;
         if (nchunks > 1) {                                                    // this chunk's CRC goes to the side stream
             FPNGB_CUDA_OK(cudaEventRecord(c.side_ev[k], s));
@@ -599,7 +600,7 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
     RowCrcParams rp{row_crc, row_ofs, row_bits, nullptr, 0, st, d_out, 0, 0, d_desc};
     launch_row_crc_combine_ragged(rp, m, max_split, s);
     RaggedParams<CrcParams> cp{};
-    cp.out = d_out; cp.st = st; cp.msg_start = kPngHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu; cp.stored_only = 1u;
+    cp.out = d_out; cp.st = st; cp.msg_start = kPngHeaderSize - 4; cp.stored_only = 1u;
     cp.ragged = RaggedWork{d_desc, d_lists + 3 * (size_t)m, d_lists + 4 * (size_t)m, m};
     launch_crc_stream_ragged(cp, (uint32_t)crc_ctas, s);
     count_launch(2);
@@ -732,7 +733,7 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
     launch_adler_finalize_png(ap, m, s);
     prof_mark(ps, kProfAdler, s);
     RaggedParams<CrcParams> cp{};
-    cp.out = d_out; cp.st = p.st; cp.msg_start = kPngEncHeaderSize - 4; cp.init_xor = 0xFFFFFFFFu; cp.stored_only = 0u;
+    cp.out = d_out; cp.st = p.st; cp.msg_start = kPngEncHeaderSize - 4; cp.stored_only = 0u;
     cp.ragged = RaggedWork{d_desc, d_lists + 2 * (size_t)m, d_lists + 3 * (size_t)m, m};
     launch_crc_stream_png(cp, (uint32_t)crc_ctas, s);
     prof_mark(ps, kProfCrc, s);
@@ -766,9 +767,7 @@ int fpngb_init(int device)
     if (!build_static_book(c.h_static_books[1], kStaticHdrRGBA, sizeof kStaticHdrRGBA, kStaticHdrRGBATail, kStaticHdrRGBATailBits, 4)) return FPNGB_ERR_INTERNAL;
     FPNGB_CUDA_OK(cudaMalloc(&c.d_static_books, 2 * sizeof(CodeBook)));
     FPNGB_CUDA_OK(cudaMemcpy(c.d_static_books, c.h_static_books, 2 * sizeof(CodeBook), cudaMemcpyHostToDevice));
-    int rc = checksum_tables_init();
-    if (rc) return rc;
-    rc = fused_tables_init();
+    int rc = fused_tables_init();
     if (rc) return rc;
     rc = crc_stream_tables_init();
     if (rc) return rc;
@@ -1183,21 +1182,23 @@ int fpngb_crc32_ex(const void* data, size_t size, uint32_t prev, uint32_t* out)
     Context& c = g_ctx;
     std::lock_guard<std::mutex> lk(c.mu);
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
-    const size_t padded = align_up(size + 16, 16);
+    // the buffer stands where "IDAT" + zlib stream stands in a file, bytes [54, 54 + size): the stream CRC kernel's message
+    const size_t msg = kPngHeaderSize - 4, padded = align_up(msg + size + 4, 16);
     int rc = c.dev_in.reserve(padded + 256); if (rc) return rc;
-    ImageState hst{}; hst.zsize = (uint32_t)size - kPngHeaderSize;       // kernel computes L = 58 + zsize = size
+    ImageState hst{}; hst.zsize = (uint32_t)size - 4;                   // kernel computes L = 58 + zsize = 54 + size
     ImageState* dst = (ImageState*)((uint8_t*)c.dev_in.p + padded);
-    FPNGB_CUDA_OK(cudaMemcpyAsync(c.dev_in.p, data, size, cudaMemcpyHostToDevice, c.stream));
+    FPNGB_CUDA_OK(cudaMemcpyAsync((uint8_t*)c.dev_in.p + msg, data, size, cudaMemcpyHostToDevice, c.stream));
     FPNGB_CUDA_OK(cudaMemcpyAsync(dst, &hst, sizeof hst, cudaMemcpyHostToDevice, c.stream));
     CrcParams cp{};
-    cp.out = (uint8_t*)c.dev_in.p; cp.out_stride = 0; cp.st = dst; cp.max_tiles = crc_ctas_for(size); cp.msg_start = 0; cp.init_xor = ~prev;
-    launch_crc(cp, 1, c.stream);
+    cp.out = (uint8_t*)c.dev_in.p; cp.st = dst;
+    launch_crc_stream(cp, 1, msg + size + 4, c.stream);
     count_launch(1);
     FPNGB_CUDA_OK(cudaGetLastError());
     uint8_t be[4] = {0, 0, 0, 0};
-    FPNGB_CUDA_OK(cudaMemcpyAsync(be, (uint8_t*)c.dev_in.p + size, 4, cudaMemcpyDeviceToHost, c.stream));
+    FPNGB_CUDA_OK(cudaMemcpyAsync(be, (uint8_t*)c.dev_in.p + msg + size, 4, cudaMemcpyDeviceToHost, c.stream));
     FPNGB_CUDA_OK(cudaStreamSynchronize(c.stream));
-    *out = ((uint32_t)be[0] << 24) | ((uint32_t)be[1] << 16) | ((uint32_t)be[2] << 8) | be[3];
+    // the kernel starts from a fresh CRC; by linearity crc(prev, M) = crc(0, M) ^ prev * x^(8 |M|)
+    *out = (((uint32_t)be[0] << 24) | ((uint32_t)be[1] << 16) | ((uint32_t)be[2] << 8) | be[3]) ^ gf2_mulmod(prev, xpow(8ull * size));
     return FPNGB_OK;
 }
 

@@ -26,25 +26,13 @@ namespace fpngb {
 
 // ---- gather -------------------------------------------------------------------------------------------------------------------
 struct PngCrcTables { uint32_t byte[256]; uint32_t x8pow[32]; };   // byte table; x^(8 * 2^k) in the reflected form of crc_math.cuh
-static constexpr uint32_t cx_mulmod(uint32_t a, uint32_t b)
-{
-    uint32_t p = 0;
-    for (int i = 0; i < 32; i++) {
-        if (a & (0x80000000u >> i)) p ^= b;
-        b = (b >> 1) ^ ((b & 1u) ? kCrcPoly : 0u);
-    }
-    return p;
-}
 static constexpr PngCrcTables make_png_crc_tables()
 {
     PngCrcTables r{};
-    for (uint32_t n = 0; n < 256; n++) {
-        uint32_t c = n;
-        for (int k = 0; k < 8; k++) c = (c & 1u) ? (kCrcPoly ^ (c >> 1)) : (c >> 1);
-        r.byte[n] = c;
-    }
+    const CrcByteTable b = crc_byte_table();
+    for (uint32_t n = 0; n < 256; n++) r.byte[n] = b.t[n];
     r.x8pow[0] = kCrcOne >> 8;                                               // x^8
-    for (int k = 1; k < 32; k++) r.x8pow[k] = cx_mulmod(r.x8pow[k - 1], r.x8pow[k - 1]);
+    for (int k = 1; k < 32; k++) r.x8pow[k] = gf2_mulmod(r.x8pow[k - 1], r.x8pow[k - 1]);
     return r;
 }
 __constant__ PngCrcTables c_png_crc = make_png_crc_tables();

@@ -111,9 +111,7 @@ struct AdlerParams {
 struct CrcParams {
     uint8_t* out; size_t out_stride;
     ImageState* st;
-    uint32_t max_tiles;                           // grid.x; CTAs beyond an image's length exit immediately
     uint32_t msg_start;                           // first byte of the CRC'd region (54 = "IDAT" for a PNG file)
-    uint32_t init_xor;                            // initial register value (0xFFFFFFFF for a fresh CRC)
     uint32_t stored_only;                         // only images that fell back to stored blocks (the single-pass encoder computed the others' CRC inline)
 };
 
@@ -225,15 +223,12 @@ void set_rows_per_warp16(uint32_t v);          // 0 = automatic (5 scanlines per
 void launch_offsets(const OffsetsParams& p, uint32_t n, cudaStream_t s);
 void launch_pack(const PackParams& p, uint32_t n, uint32_t chans, int mode, cudaStream_t s);
 void launch_adler_finalize(const AdlerParams& p, uint32_t n, cudaStream_t s);
-void launch_crc(const CrcParams& p, uint32_t n, cudaStream_t s);
 void launch_huffman_build(const HuffParams& p, uint32_t n, cudaStream_t s);
-uint32_t crc_ctas_for(size_t max_file_bytes);
 uint32_t adler_chunk_bytes();
 void launch_adler_buffer(const uint8_t* d_buf, size_t n, uint2* d_partials, cudaStream_t s);
 // src_offsets: file f at files + src_offsets[f] (multiples of 16), or nullptr: at files + f * stride
 void launch_compact(const uint8_t* files, size_t stride, const uint32_t* sizes, uint32_t n, uint8_t* dst, size_t dst_cap,
                     unsigned long long* offsets, cudaStream_t s, const unsigned long long* src_offsets = nullptr);
-int  checksum_tables_init();                      // uploads CRC slice tables / x^(2^k) powers (idempotent)
 
 // host helpers shared by host_api.cu and the tests
 uint32_t host_crc32(const void* data, size_t n, uint32_t prev);

@@ -99,7 +99,7 @@ def test_scanline_crcs_combine_to_the_idat_crc(oracle, kind, w, h, chans):
 def test_mulmod_and_powers():
     assert mulmod(ONE, 0x12345678) == 0x12345678 and mulmod(0x40000000, ONE) == 0x40000000
     assert mulmod(xpow(5), xpow(27)) == xpow(32) == POLY                         # x^32 mod P = P's low terms
-    assert mulmod(xpow(1000), 0xDB710641) == xpow(999)                           # kCrcXInv = x^-1
+    assert mulmod(xpow(1000), 0xDB710641) == xpow(999)                           # x^-1 mod P
     # advancing a finished CRC over n zero bytes = multiplying its raw form by x^(8n)
     data = bytes(range(200))
     for n in (1, 7, 64):

@@ -172,6 +172,19 @@ def test_checksum_utilities(gpu, oracle):
         assert gpu.fpng_adler32(d, 0x00030002) == oracle.adler32(d, 0x00030002), n
     assert gpu.fpng_crc32(b"123456789") == 0xCBF43926
     assert gpu.fpng_adler32(b"Wikipedia") == 0x11E60398
+    # fpng_crc32 from 4 KiB on runs idat_crc_stream_kernel over the buffer placed at device byte 54 (where "IDAT" sits in a
+    # file): floor((54 + n) / 4) - 13 whole words and (54 + n) % 4 tail bytes, k whole 64 KiB CTAs for n in [65536k - 2, 65536k + 1]
+    base = rs.randint(0, 256, size=(1 << 17) + 64, dtype=np.uint8)
+    sizes = [4095, 4096, 4097, 200_000, 200_001, 200_002, 200_003] + [65536 * k + d for k in (1, 2) for d in range(-5, 6)]
+    for n in sizes:
+        for ofs in (0, 1, 2, 3):                                             # host buffers at every byte alignment
+            d = base[ofs:ofs + n]
+            for prev in (0, 0x12345678, 0xFFFFFFFF):
+                assert gpu.fpng_crc32(d, prev) == oracle.crc32(d, prev), (n, ofs, prev)
+    # chaining, with the cut on both sides of the 4 KiB switch between the host and the device routine
+    d = base[:70_001]
+    for cut in (4095, 4096, 4097, d.size - 4097, d.size - 4096, d.size - 4095):
+        assert gpu.fpng_crc32(d[cut:], gpu.fpng_crc32(d[:cut])) == oracle.crc32(d), cut
 
 
 def test_generic_kernels_still_match(oracle):
