@@ -1,6 +1,6 @@
-// fpng_b200/csrc/encode16_kernels.cu -- second-generation scan (K1) and pack (K3) kernels on the 16-pixels-per-lane
-// walker (row_walk16.cuh).  Same outputs, bit for bit, as the generic kernels in encode_kernels.cu; used whenever every
-// scanline is 16-byte aligned (all BASELINE.json shapes).  Reference lines: see encode_kernels.cu.
+// fpng_b200/csrc/encode16_kernels.cu -- scan (K1) and pack (K3) kernels of the two-kernel encoder on the 16-pixels-per-lane
+// walker (row_walk16.cuh), for every shape, alignment and layout.  K2 and the Adler-32 finalize are in encode_kernels.cu.
+// LIT1: the RGBA 1-pass instantiations under a table whose "one-pixel match vs four literals" rule can fire (fpng.cpp:1520-1528).
 #include "row_walk16.cuh"
 #include "kernels.cuh"
 
@@ -55,6 +55,27 @@ __device__ __forceinline__ uint32_t literal_bits16(const uint8_t* s_lit, uint32_
     return b;
 }
 
+// RGBA pixel k - 1 of a lane (its words are its pixels), `left` (the pixel left of the lane) for k == 0
+template <int N>
+__device__ __forceinline__ uint32_t pixel_before16(const uint32_t (&px)[N], uint32_t left, uint32_t k)
+{
+    uint32_t v = left;
+#pragma unroll
+    for (int q = 0; q < N; q++) v = k == (uint32_t)q + 1u ? px[q] : v;
+    return v;
+}
+
+// bits of a pending run of r pixels flushed before lane pixel k.  LIT1: a one-pixel match costs min(match, the four literals of
+// the pixel it covers); the literals are taken iff the match costs more (fpng.cpp:1520-1528)
+template <bool LIT1>
+__device__ __forceinline__ uint32_t run_bits16(const uint8_t* s_lit, const uint8_t* s_match, uint32_t r, const uint32_t (&px)[16], uint32_t left,
+                                               uint32_t k)
+{
+    const uint32_t b = s_match[r];
+    if (!LIT1 || r != 1u) return b;
+    return min(b, literal_bits16<4>(s_lit, pixel_before16(px, left, k)));
+}
+
 // Ragged launches (RAGGED = true): CTA blockIdx.x is CTA `cta` of one image (ragged_locate); the image's descriptor replaces the
 // call-wide pixels, strides, shape and books, and the row / lane tables, image state and output are rebased to it, so that the
 // kernel bodies run as for image 0 of a uniform batch.  The uniform instantiations compile without any of this.  Returns the
@@ -76,9 +97,10 @@ __device__ __forceinline__ uint32_t ragged_image16(P& p, uint32_t& cta)
 // ------------------------------------------------------------------------------------------------
 // No minimum CTAs per SM: a bound of 5 (48 registers for RGB, 40 instead of 32 warps per SM) measured slower, since the kernel is
 // ALU-pipe bound, not latency bound.
-template <int CHANS, int LOAD, bool RAGGED = false>
+template <int CHANS, int LOAD, bool RAGGED = false, bool LIT1 = false>
 __global__ void __launch_bounds__(32 * kScan16Rows) row_scan16_kernel(std::conditional_t<RAGGED, RaggedParams<ScanParams>, ScanParams> p)
 {
+    static_assert(!LIT1 || CHANS == 4, "the one-pixel-match rule is RGBA only");
     using WK = typename Loader16<CHANS, LOAD>::type;
     constexpr uint32_t M = max_match_pixels(CHANS);
     extern __shared__ __align__(16) uint8_t dyn_smem[];
@@ -119,6 +141,11 @@ __global__ void __launch_bounds__(32 * kScan16Rows) row_scan16_kernel(std::condi
         if (step + 1 < nsteps) wk.prefetch(cur, prev, step + 1, bpl, lane, tiles);         // lands while this step is processed
         WK::pixels(dw, px);
         const uint32_t p0 = step * kStep16 + lane * kPix16;
+        uint32_t left = 0;                       // LIT1: the pixel left of the lane's first, which a run entering the lane covers
+        if constexpr (LIT1) {
+            left = __shfl_up_sync(kFullMask, px[15], 1);
+            if (lane == 0) left = carry.prev_px;
+        }
         const Lane16 t = classify16<CHANS>(px, p0, w, carry, lane);
 
         uint32_t bits = 0;
@@ -154,14 +181,14 @@ __global__ void __launch_bounds__(32 * kScan16Rows) row_scan16_kernel(std::condi
                     if (r >= M) { bits += s_match[M]; r -= M; }
                     if (pos >= nvp) break;
                 }
-                if (r) { bits += s_match[r]; r = 0; }                                     // a literal follows: flush the remainder
+                if (r) { bits += run_bits16<LIT1>(s_lit, s_match, r, px, left, pos); r = 0; }   // a literal follows: flush the remainder
                 const uint32_t mz = t.eqm >> pos;
                 const uint32_t zeros = mz ? (uint32_t)__ffs((int)mz) - 1u : 32u;
                 pos += zeros;
             }
         }
         if (t.last) {
-            if (r) bits += s_match[r];
+            if (r) bits += run_bits16<LIT1>(s_lit, s_match, r, px, left, nvp);
             // capacity rule (SURVEY Q5): size of the scanline's last flush unit
             const uint32_t k = nvp - 1u;
             if (t.litm & (1u << k)) {
@@ -170,6 +197,7 @@ __global__ void __launch_bounds__(32 * kScan16Rows) row_scan16_kernel(std::condi
                 for (int q = 1; q < 16; q++) lastpx = (k == (uint32_t)q) ? px[q] : lastpx;
                 last_unit = literal_bits16<CHANS>(s_lit, lastpx) + ((w == 1 && p.merge_first_unit) ? s_lit[filt] : 0u);
             } else last_unit = r ? s_match[r] : s_match[M];
+            if constexpr (LIT1) if (r == 1u && !(t.litm & (1u << k))) last_unit = run_bits16<true>(s_lit, s_match, r, px, left, nvp);
             if (y == p.h - 1) p.st[img].last_unit_bits = last_unit;
         }
         // bit offset of this lane's first token inside the row (the pack kernel starts writing there)
@@ -370,12 +398,28 @@ __device__ __forceinline__ uint32_t run_before16(uint32_t eqm, uint32_t r_in, ui
     return kk - 1u - (31u - (uint32_t)__clz((int)t));
 }
 
+// a pending run of r > 0 pixels whose last pixel is `covered`.  LIT1: a one-pixel match is written as that pixel's four literals
+// when the match costs more bits (fpng.cpp:1520-1528; the scan kernel counted the same choice)
+template <bool LIT1>
+__device__ __forceinline__ void put_run16(BitStager16& bs, uint32_t s_lit_saddr, uint32_t s_match_saddr, uint32_t r, uint32_t covered)
+{
+    if (LIT1 && r == 1u) {
+        const uint32_t c0 = lds_u32(s_lit_saddr + lit_off16<0>(covered)), c1 = lds_u32(s_lit_saddr + lit_off16<1>(covered));
+        const uint32_t c2 = lds_u32(s_lit_saddr + lit_off16<2>(covered)), c3 = lds_u32(s_lit_saddr + lit_off16<3>(covered));
+        const uint32_t m = lds_u32(s_match_saddr + 4u);
+        if ((m >> 24) > (c0 >> 16) + (c1 >> 16) + (c2 >> 16) + (c3 >> 16)) { put_pair16(bs, c0, c1); put_pair16(bs, c2, c3); return; }
+    }
+    put_match16(bs, s_match_saddr, r);
+}
+
 // a token event at pixel kk: the run reaches M at this (match) pixel, or a pending run is flushed before this literal
-template <uint32_t M>
-__device__ __forceinline__ void put_event16(BitStager16& bs, uint32_t s_match_saddr, uint32_t eqm, uint32_t r_in, uint32_t kk)
+// (LIT1: `covered` is pixel kk - 1, see put_run16)
+template <uint32_t M, bool LIT1 = false>
+__device__ __forceinline__ void put_event16(BitStager16& bs, uint32_t s_match_saddr, uint32_t eqm, uint32_t r_in, uint32_t kk,
+                                            uint32_t s_lit_saddr = 0u, uint32_t covered = 0u)
 {
     const uint32_t len = ((eqm >> kk) & 1u) ? M : run_before16<M>(eqm, r_in, kk);
-    if (len) put_match16(bs, s_match_saddr, len);
+    if (len) put_run16<LIT1>(bs, s_lit_saddr, s_match_saddr, len, covered);
 }
 
 // the literal codes of word J (0 .. kHalfWords-1) of a mixed half: one 64-bit (code, size) load per byte, each byte's entry taken
@@ -383,9 +427,10 @@ __device__ __forceinline__ void put_event16(BitStager16& bs, uint32_t s_match_sa
 // for RGB that byte can sit inside the word, and only then (rare: a run ends or reaches M in this word) the word is put code by
 // code with the match token in between.
 __device__ __forceinline__ uint32_t null_ofs8(uint32_t nl, int k) { return (nl << (11 - k)) & 0x800u; }   // bit k of nl -> 0x800 (k <= 7)
-template <int CHANS, int J, uint32_t M>
+// LIT1 (RGBA, one pixel per word): prev is the pixel before the word's
+template <int CHANS, int J, uint32_t M, bool LIT1>
 __device__ __forceinline__ void put_mixed_word16(BitStager16& bs, uint32_t lit_s, uint32_t match_s, uint32_t w, uint32_t nl, uint32_t ev8,
-                                                 uint32_t eqm, uint32_t r_in, uint32_t kbase)
+                                                 uint32_t eqm, uint32_t r_in, uint32_t kbase, uint32_t prev)
 {
     constexpr int kFirst = 4 * J / CHANS;                              // pixel of byte 0
     constexpr int kIn = (4 * J + 3) / CHANS;                           // pixel of byte 3: starts inside the word iff kIn != kFirst (RGB)
@@ -395,7 +440,7 @@ __device__ __forceinline__ void put_mixed_word16(BitStager16& bs, uint32_t lit_s
     const uint2 f1 = lds_u64(l64 + lit_off16x8<1>(w, null_ofs8(nl, (4 * J + 1) / CHANS)));
     const uint2 f2 = lds_u64(l64 + lit_off16x8<2>(w, null_ofs8(nl, (4 * J + 2) / CHANS)));
     const uint2 f3 = lds_u64(l64 + lit_off16x8<3>(w, null_ofs8(nl, kIn)));
-    if (CHANS * kFirst == 4 * J && (ev8 & (1u << kFirst))) put_event16<M>(bs, match_s, eqm, r_in, kbase + kFirst);
+    if (CHANS * kFirst == 4 * J && (ev8 & (1u << kFirst))) put_event16<M, LIT1>(bs, match_s, eqm, r_in, kbase + kFirst, lit_s, prev);
     if (kIn != kFirst && (ev8 & (1u << kIn))) {
         const uint2 f[4] = {f0, f1, f2, f3};
 #pragma unroll
@@ -408,13 +453,14 @@ __device__ __forceinline__ void put_mixed_word16(BitStager16& bs, uint32_t lit_s
     bs.put(f0.x | (f1.x << f0.y), f0.y + f1.y);
     bs.put(f2.x | (f3.x << f2.y), f2.y + f3.y);
 }
-// words J.. of a mixed half (hw: its 2 * CHANS filtered words; nl: bit k set when pixel k is not a literal)
-template <int CHANS, uint32_t M, int J = 0>
+// words J.. of a mixed half (hw: its 2 * CHANS filtered words; nl: bit k set when pixel k is not a literal; before: LIT1, the pixel
+// before the half)
+template <int CHANS, uint32_t M, bool LIT1, int J = 0>
 __device__ __forceinline__ void put_mixed_half16(BitStager16& bs, uint32_t lit_s, uint32_t match_s, const uint32_t (&hw)[2 * CHANS], uint32_t nl,
-                                                 uint32_t ev8, uint32_t eqm, uint32_t r_in, uint32_t kbase)
+                                                 uint32_t ev8, uint32_t eqm, uint32_t r_in, uint32_t kbase, uint32_t before)
 {
-    put_mixed_word16<CHANS, J, M>(bs, lit_s, match_s, hw[J], nl, ev8, eqm, r_in, kbase);
-    if constexpr (J + 1 < 2 * CHANS) put_mixed_half16<CHANS, M, J + 1>(bs, lit_s, match_s, hw, nl, ev8, eqm, r_in, kbase);
+    put_mixed_word16<CHANS, J, M, LIT1>(bs, lit_s, match_s, hw[J], nl, ev8, eqm, r_in, kbase, J ? hw[J ? J - 1 : 0] : before);
+    if constexpr (J + 1 < 2 * CHANS) put_mixed_half16<CHANS, M, LIT1, J + 1>(bs, lit_s, match_s, hw, nl, ev8, eqm, r_in, kbase, before);
 }
 
 // one Horner step of the in-kernel CRC: the register (XOR-ed with the lane's previous word) advanced over 128 bytes, then the next
@@ -427,10 +473,11 @@ __device__ __forceinline__ uint32_t crc_step16(uint32_t crc_s, uint32_t cx, uint
     return v ^ lds_u32(crc_s + b0 * 4u) ^ lds_u32(crc_s + 1024u + b1 * 4u) ^ lds_u32(crc_s + 2048u + b2 * 4u) ^ lds_u32(crc_s + 3072u + b3 * 4u);
 }
 
-template <int CHANS, int LOAD, bool RAGGED = false>
+template <int CHANS, int LOAD, bool RAGGED = false, bool LIT1 = false>
 __global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(std::conditional_t<RAGGED, RaggedParams<PackParams>, PackParams> p,
                                                                        uint32_t rows_per_warp)
 {
+    static_assert(!LIT1 || CHANS == 4, "the one-pixel-match rule is RGBA only");
     using WK = typename Loader16<CHANS, LOAD>::type;
     uint32_t img = blockIdx.y, cta = blockIdx.x;
     if constexpr (RAGGED) {
@@ -497,6 +544,8 @@ __global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(s
     uint32_t g31 = 0, row_total = 0;
     uint32_t flushed_bits = 0;                   // row bits (incl. the G & 31 lead-in) already flushed to global, multiple of 32
     uint32_t leftover = 0;                       // bits of the partially filled word carried from the previous step (lane 0 seeds with it)
+    // LIT1: lane 31's last pixel of the previous step.  Not reset at a scanline's start: no run enters its first lane, so it is unread there
+    uint32_t prev_px = 0;
 
     WK wk; wk.init(lane, tiles); set_planes(wk, p.chan_stride);
     uint32_t dummyA = 0; unsigned long long dummyB = 0;
@@ -550,6 +599,11 @@ __global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(s
             uint32_t hw[kHalfWords];
 #pragma unroll
             for (int j = 0; j < kHalfWords; j++) hw[j] = h ? dw[kHalfWords + j] : dw[j];
+            uint32_t before = 0;                 // LIT1: the pixel before the half, which a run entering it covers
+            if constexpr (LIT1) {
+                const uint32_t up = __shfl_up_sync(kFullMask, dw[15], 1);
+                before = h ? dw[kHalfWords - 1] : (lane ? up : prev_px);
+            }
             if (__all_sync(kFullMask, lit8 == 0xFFu && ev8 == 0u)) {
                 // (1) all 256 pixels are literals, no run pending (noisy rows): the filtered bytes in order, two codes per put
 #pragma unroll
@@ -560,7 +614,7 @@ __global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(s
             } else if (__reduce_add_sync(kFullMask, (uint32_t)__popc(lit8)) >= 16u) {
                 // (3) mixed: the all-literal emission word by word, each byte switched off through the table's null half when
                 //     its pixel is not a literal; the rare run tokens are inserted by a per-word event check
-                put_mixed_half16<CHANS, M>(bs, lit_s, match_s, hw, ~lit8, ev8, eqm, r_in, 8u * h);
+                put_mixed_half16<CHANS, M, LIT1>(bs, lit_s, match_s, hw, ~lit8, ev8, eqm, r_in, 8u * h, before);
             } else {
                 // (4) sparse literals (RLE-dominated rows): per-pixel token walk, 4 pixels at a time
                 uint32_t r = run_before16<M>(eqm, r_in, 8u * h);
@@ -578,13 +632,14 @@ __global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(s
                         q[3] = w2 >> 8;
                     }
                     const uint32_t e4 = eqm >> (8u * h + 4u * g), base = 8u * h + 4u * g;
+                    const uint32_t pb = g ? hw[3] : before;                                   // LIT1: the pixel before q[0]
 #pragma unroll
                     for (int j = 0; j < 4; j++) {
                         if (base + j < nvp) {
                             if (e4 & (1u << j)) {
                                 if (++r == M) { put_match16(bs, match_s, M); r = 0; }
                             } else {
-                                if (r) { put_match16(bs, match_s, r); r = 0; }
+                                if (r) { put_run16<LIT1>(bs, lit_s, match_s, r, j ? q[j ? j - 1 : 0] : pb); r = 0; }
                                 put_literal16<CHANS>(bs, lit_s, q[j]);
                             }
                         }
@@ -592,9 +647,10 @@ __global__ void __launch_bounds__(32 * pack16_warps(CHANS)) pack_rows16_kernel(s
                 }
             }
         }
+        if constexpr (LIT1) prev_px = __shfl_sync(kFullMask, dw[15], 31);
         if (info >> 28) {                                                // this lane holds the scanline's last pixel: flush the trailing run
             const uint32_t r = run_before16<M>(eqm, r_in, nvp);
-            if (r) put_match16(bs, match_s, r);
+            if (r) put_run16<LIT1>(bs, lit_s, match_s, r, pixel_before16(dw, 0u, nvp));   // nvp >= 1
         }
         // row bits after this step (the next step's first offset was loaded a whole emission ago)
         const uint32_t step_end = more ? __shfl_sync(kFullMask, mine.x, 0) : row_total;
@@ -685,13 +741,21 @@ template <int CHANS, int LOAD> constexpr size_t hist16_smem() { return kScan16Ro
             else FPNGB_LAUNCH16_ONE(3, kLoad16Staged, R, kernel, smemfn, grid, threads, __VA_ARGS__); \
         } \
     } while (0)
+// the RGBA scan and pack kernels with the one-pixel-match rule (ScanParams / PackParams::lit1_rule)
+#define FPNGB_TARGS(...) __VA_ARGS__
+#define FPNGB_LAUNCH16_LIT1(kernel, R, smemfn, grid, threads, ...) do { \
+        if (load == kLoad16Planar) FPNGB_LAUNCH16_ONE(4, kLoad16Planar, FPNGB_TARGS(R, true), kernel, smemfn, grid, threads, __VA_ARGS__); \
+        else if (load == kLoad16Direct) FPNGB_LAUNCH16_ONE(4, kLoad16Direct, FPNGB_TARGS(R, true), kernel, smemfn, grid, threads, __VA_ARGS__); \
+        else FPNGB_LAUNCH16_ONE(4, kLoad16Staged, FPNGB_TARGS(R, true), kernel, smemfn, grid, threads, __VA_ARGS__); \
+    } while (0)
 
 void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
 {
     // one scanline per warp: the multi-scanline sequence that pays off in the pack kernel measured neutral (RGB) to 4 % slower (RGBA) here
     const int load = load16_mode(p, chans);
     dim3 grid((p.h + kScan16Rows - 1) / kScan16Rows, n);
-    FPNGB_LAUNCH16(row_scan16_kernel, false, scan16_smem, grid, 32 * kScan16Rows, p);
+    if (chans == 4 && p.lit1_rule) FPNGB_LAUNCH16_LIT1(row_scan16_kernel, false, scan16_smem, grid, 32 * kScan16Rows, p);
+    else FPNGB_LAUNCH16(row_scan16_kernel, false, scan16_smem, grid, 32 * kScan16Rows, p);
 }
 
 void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s)
@@ -706,7 +770,8 @@ void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t
     const int load = load16_mode(p, chans);
     const uint32_t rpw = rows_per_warp16(n, p.h), rows_per_cta = pack16_warps(chans) * rpw;
     dim3 grid((p.h + rows_per_cta - 1) / rows_per_cta, n);
-    FPNGB_LAUNCH16(pack_rows16_kernel, false, pack16_smem, grid, 32 * pack16_warps(chans), p, rpw);
+    if (chans == 4 && p.lit1_rule) FPNGB_LAUNCH16_LIT1(pack_rows16_kernel, false, pack16_smem, grid, 32 * pack16_warps(chans), p, rpw);
+    else FPNGB_LAUNCH16(pack_rows16_kernel, false, pack16_smem, grid, 32 * pack16_warps(chans), p, rpw);
 }
 
 // Ragged launches: one per (chans, loader) class, over the class's CTAs (the host sums them per image: ceil(h / rows per CTA)).
@@ -720,7 +785,8 @@ uint32_t pack16_rows_per_cta(uint32_t rows_per_warp, uint32_t chans) { return pa
 
 void launch_scan16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s)
 {
-    FPNGB_LAUNCH16(row_scan16_kernel, true, scan16_smem, ctas, 32 * kScan16Rows, p);
+    if (chans == 4 && p.lit1_rule) FPNGB_LAUNCH16_LIT1(row_scan16_kernel, true, scan16_smem, ctas, 32 * kScan16Rows, p);
+    else FPNGB_LAUNCH16(row_scan16_kernel, true, scan16_smem, ctas, 32 * kScan16Rows, p);
 }
 
 void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint32_t chans, int load, cudaStream_t s)
@@ -730,7 +796,8 @@ void launch_hist16_ragged(const RaggedParams<ScanParams>& p, uint32_t ctas, uint
 
 void launch_pack16_ragged(const RaggedParams<PackParams>& p, uint32_t ctas, uint32_t chans, int load, uint32_t rows_per_warp, cudaStream_t s)
 {
-    FPNGB_LAUNCH16(pack_rows16_kernel, true, pack16_smem, ctas, 32 * pack16_warps(chans), p, rows_per_warp);
+    if (chans == 4 && p.lit1_rule) FPNGB_LAUNCH16_LIT1(pack_rows16_kernel, true, pack16_smem, ctas, 32 * pack16_warps(chans), p, rows_per_warp);
+    else FPNGB_LAUNCH16(pack_rows16_kernel, true, pack16_smem, ctas, 32 * pack16_warps(chans), p, rows_per_warp);
 }
 
 }  // namespace fpngb

@@ -9,7 +9,7 @@
 //    and maps NaN to 0 (PTX ISA, cvt: float-to-integer conversions saturate, NaN converts to 0);
 //  * the typed PNG encode call (PNG = true: 1 to 4 channels, OB from ConvDesc::sample_bytes): the same rule, with
 //    cvt.rni.sat.u16.f32 for 16-bit samples, stored as native little-endian uint16 (the PNG row kernels swap the bytes);
-//  * the strided uint8 input of the encoders that read tight rows only (the generic 4-pixel kernels, the single-pass encoder):
+//  * the strided uint8 input of the single-pass encoder, which reads tight rows only:
 //    T = uint8_t, a plain copy.
 // Each thread converts a group of 4 pixels of one row with the widest loads the address allows (16, 8, then 4 bytes, single
 // elements at row ends).  The CTAs of a launch cover one or more descriptors; a CTA finds its descriptor by a binary search over

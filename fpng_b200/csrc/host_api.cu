@@ -261,18 +261,6 @@ static int carve_workspace(Context& c, uint32_t n, uint32_t h, uint32_t width, b
     return 0;
 }
 
-static int pick_load_mode(const void* base, size_t image_stride, uint32_t w, uint32_t chans)
-{
-    const uintptr_t a = (uintptr_t)base;
-    if (chans == 4) {
-        if (a % 16 == 0 && image_stride % 16 == 0 && w % 4 == 0) return kLoadVec16;
-        if (a % 4 == 0 && image_stride % 4 == 0) return kLoadWords;
-        return kLoadBytes;
-    }
-    if (a % 4 == 0 && image_stride % 4 == 0 && w % 4 == 0) return kLoadWords;
-    return kLoadBytes;
-}
-
 static bool valid_dims(uint32_t w, uint32_t h, uint32_t chans)
 {
     // fpng.cpp:1670-1680; additionally the filtered stream must be addressable with 32 bits like the reference's
@@ -300,12 +288,6 @@ static void make_png_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t chans
     memcpy(hdr + 54, "IDAT", 4);            // bytes 50..53 (IDAT length) are patched per image on the device
 }
 
-static bool force_generic_env()
-{
-    static const bool v = getenv("FPNGB_FORCE_GENERIC") && atoi(getenv("FPNGB_FORCE_GENERIC")) != 0;
-    return v;
-}
-
 // Enqueue the whole encode pipeline for a device-resident batch.  Caller holds ctx.mu.
 //
 // Two encoders share this entry:
@@ -317,26 +299,19 @@ static bool force_generic_env()
 //    and writes the file once, byte-identical output, measured slower than the two-kernel path because it is bound by
 //    instruction issue, not by HBM.
 //
-// The input is n images of format f at src in byte layout L (layout.h; a uint8 row pitch fits in 32 bits).  The 16-pixel scan and
-// pack kernels read every uint8 layout in place.  The conversion pre-pass (convert_pixels_kernel) first writes tight uint8 rows into
-// c.conv for a float input, and for a uint8 input that is not tight interleaved but bound for the generic kernels or the single-pass
-// encoder, which read tight interleaved rows only.  Rows already in c.conv are tight uint8, so they are never converted again.
+// The input is n images of format f at src in byte layout L (layout.h; a uint8 row pitch fits in 32 bits).  The scan and pack
+// kernels read every uint8 layout in place.  The conversion pre-pass (convert_pixels_kernel) first writes tight uint8 rows into
+// c.conv for a float input, and for a uint8 input that is not tight interleaved but bound for the single-pass encoder, which reads
+// tight interleaved rows only.  Rows already in c.conv are tight uint8, so they are never converted again.
 static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, const PixelFormat& f, uint32_t n, uint32_t w, uint32_t h,
                                uint32_t chans, uint32_t flags, uint8_t* d_out, size_t out_stride, uint32_t* d_sizes, cudaStream_t s)
 {
     const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
-    // second-generation kernels (16 pixels per lane, coalesced 128-bit loads) whenever every scanline is 16-byte aligned;
-    // FPNGB_FORCE_GENERIC=1 keeps the generic kernels (tests compare both)
-    const bool force_generic = force_generic_env();
-    // RGBA 1-pass under a table where a one-pixel match can lose against four literals: only the generic kernels
-    // implement the reference's check (fpng.cpp:1520-1528); it cannot fire with the shipped table
+    // RGBA 1-pass under a table where a one-pixel match can lose against four literals (fpng.cpp:1520-1528; never with the shipped
+    // table): the scan and pack kernels' LIT1 instantiations; the single-pass encoder does not implement the rule
     const uint32_t lit1_rule = (!two_pass && chans == 4 && c.h_static_books[1].lit1_rule) ? 1u : 0u;
-    // the 16-pixel kernels take any scanline alignment (staged-tile loader for 16-byte aligned scanlines, direct realigning
-    // loads otherwise); the generic 4-pixel kernels remain for the trained-table rule and for A/B tests
-    const bool v2 = !force_generic && !lit1_rule;
-    const bool fused = g_fused && !force_generic && !lit1_rule && !(flags & FPNGB_FORCE_UNCOMPRESSED) &&
-                       fused_eligible(src, L.image, w, h, chans, n);
-    const bool convert = f.dtype != 0 || ((!v2 || fused) && (L.planar || L.row != (uint64_t)w * chans));
+    const bool fused = g_fused && !lit1_rule && !(flags & FPNGB_FORCE_UNCOMPRESSED) && fused_eligible(src, L.image, w, h, chans, n);
+    const bool convert = f.dtype != 0 || (fused && (L.planar || L.row != (uint64_t)w * chans));
     const size_t image_bytes = (size_t)w * h * chans;
     Workspace ws;
     int rc = carve_workspace(c, n, h, w, two_pass, ws, fused);
@@ -347,7 +322,6 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
     const uint8_t* d_pixels = convert ? (const uint8_t*)c.conv.p : src;
     const size_t image_stride = convert ? image_bytes : L.image, chan_stride = convert || !L.planar ? 0 : L.chan;
     const uint32_t row_pitch = convert ? w * chans : (uint32_t)L.row;
-    const int mode = pick_load_mode(d_pixels, image_stride, w, chans);
     const CodeBook* books0 = two_pass ? ws.books : c.d_static_books + (chans == 4 ? 1 : 0);
     const uint32_t book_stride = two_pass ? 1u : 0u;
     const uint32_t merge_first_unit = (!two_pass && chans == 3) ? 1u : 0u;
@@ -385,7 +359,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
         ProfSet* ps = prof_begin(s);
         if (two_pass) {
             FPNGB_CUDA_OK(cudaMemsetAsync(sp.hist, 0, (size_t)cnt * 288 * 4, s));
-            if (v2) launch_hist16(sp, cnt, chans, s); else launch_scan(sp, cnt, chans, mode, true, s);
+            launch_hist16(sp, cnt, chans, s);
             prof_mark(ps, kProfHist, s);
             HuffParams hp{sp.hist, ws.books + i0, chans, 0u};
             launch_huffman_build(hp, cnt, s);
@@ -398,7 +372,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
         pp.row_adler = sp.row_adler; pp.st = sp.st; pp.out = out; pp.out_stride = out_stride;
         pp.lit1_rule = lit1_rule;
         // the 16-pixel pack kernel computes each scanline's CRC while its code words are staged; the file is not read back
-        const bool pack_crc = v2 && !fused && g_pack_crc;
+        const bool pack_crc = !fused && g_pack_crc;
         if (pack_crc) { pp.row_crc = ws.row_crc + r0; pp.crc_f128b = c.crc_f128b; pp.crc_lane_mul = c.crc_lane_mul; }
         if (fused) {
             cudaEvent_t mid = ps ? ps->ev[kProfFused + 1] : nullptr;
@@ -412,7 +386,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
             prof_mark(ps, kProfPack, s);
             count_launch(3);
         } else {
-            if (v2) launch_scan16(sp, cnt, chans, s); else launch_scan(sp, cnt, chans, mode, false, s);
+            launch_scan16(sp, cnt, chans, s);
             prof_mark(ps, kProfScan, s);
             OffsetsParams op{};
             op.row_bits = sp.row_bits; op.row_ofs = ws.row_ofs + r0; op.books = books; op.book_stride = book_stride; op.st = sp.st;
@@ -420,7 +394,7 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
             memcpy(op.png_header, png_header, kPngHeaderSize);
             launch_offsets(op, cnt, s);
             prof_mark(ps, kProfOffsets, s);
-            if (v2) launch_pack16(pp, cnt, chans, s); else launch_pack(pp, cnt, chans, mode, s);
+            launch_pack16(pp, cnt, chans, s);
             prof_mark(ps, kProfPack, s);
             count_launch(3);
         }
@@ -553,9 +527,11 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
     if (g_profile) g_prof_call++;
     ProfSet* ps = prof_begin(s);
 
+    // RGBA 1-pass under a table whose one-pixel-match rule can fire: the launchers take the RGBA classes' LIT1 kernels
+    const uint32_t lit1_rule = (!two_pass && c.h_static_books[1].lit1_rule) ? 1u : 0u;
     RaggedParams<ScanParams> sp{};
     sp.row_bits = row_bits; sp.row_adler = row_adler; sp.st = st; sp.hist = hist; sp.lane_ofs = lane_ofs;
-    sp.merge_first_unit = 0u;
+    sp.merge_first_unit = 0u; sp.lit1_rule = lit1_rule;
     if (two_pass) {
         FPNGB_CUDA_OK(cudaMemsetAsync(hist, 0, (size_t)m * 288 * 4, s));
         for (int k = 0; k < kClasses; k++) {
@@ -585,7 +561,7 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
     prof_mark(ps, kProfOffsets, s);
     RaggedParams<PackParams> pp{};
     pp.row_ofs = row_ofs; pp.row_bits = row_bits; pp.lane_ofs = lane_ofs; pp.row_adler = row_adler; pp.st = st; pp.out = d_out;
-    pp.row_crc = row_crc; pp.crc_f128b = c.crc_f128b; pp.crc_lane_mul = c.crc_lane_mul;
+    pp.row_crc = row_crc; pp.crc_f128b = c.crc_f128b; pp.crc_lane_mul = c.crc_lane_mul; pp.lit1_rule = lit1_rule;
     for (int k = 0; k < kClasses; k++) {
         if (!cls_count[k]) continue;
         pp.ragged = work(k, 2);
@@ -944,7 +920,6 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
             hd[i] = conv_desc(r.pixels, src[i], 1, r.w, r.h, r.chans, at[i], ctas, ob);
             ctas += hd[i].ctas_per_image;
             r.pixels = cb + at[i]; r.row = (uint64_t)r.w * r.chans * ob; r.chan = 0;
-            src[i] = Layout{r.h * r.row, r.row, (uint64_t)r.chans * ob, ob, false};
         }
         rc = c.ws_acquire(s);
         if (rc) return rc;
@@ -954,21 +929,8 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
     }
     // a route that fails after the conversion still closes the bracket, so that later calls wait for the conversion
     auto fail = [&](int code) { prof_drop_conv(); if (typed) c.ws_release(s); cudaEventRecord(sl->ev, s); return code; };
-    // the fpng images: the ragged pipeline, or the uniform one image by image where the 16-pixel kernels do not take them (RGBA
-    // 1-pass under a table whose one-pixel-match rule is live, or FPNGB_FORCE_GENERIC)
-    const bool two_pass = (flags & FPNGB_ENCODE_SLOWER) && !(flags & FPNGB_FORCE_UNCOMPRESSED);
-    const bool lit1_rgba = !two_pass && c.h_static_books[1].lit1_rule;
-    std::vector<uint32_t> ids;
-    for (uint32_t i : fpng_ids) {
-        const RaggedImage& r = im[i];
-        if (force_generic_env() || (lit1_rgba && r.chans == 4)) {
-            const size_t slot = align_up(max_encoded_size(r.w, r.h, r.chans), 16);
-            rc = encode_batch_locked(c, r.pixels, src[i], uint8_format(), 1, r.w, r.h, r.chans, flags, out + r.slot, slot, d_sizes + i, s);
-            if (rc) return fail(rc);
-        } else ids.push_back(i);
-    }
-    if (!ids.empty()) {
-        rc = encode_ragged_locked(c, im, ids, flags, out, d_sizes, s, stage + ofs_bytes);
+    if (!fpng_ids.empty()) {
+        rc = encode_ragged_locked(c, im, fpng_ids, flags, out, d_sizes, s, stage + ofs_bytes);
         if (rc) return fail(rc);
     }
     if (!png_ids.empty()) {
@@ -1132,7 +1094,7 @@ int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
 
 // Per-kernel device times (ms) averaged over the encode calls since the last read; slots in ProfSlot order:
 // hist, huffman, scan, offsets, fused, finish, pack, adler, crc, conversion pre-pass (slot 9: the *_typed calls, and the uint8 copy of a
-// strided batch bound for the generic or single-pass encoder).  A caller asking for 9 slots gets the first nine.  Returns the number
+// strided batch bound for the single-pass encoder).  A caller asking for 9 slots gets the first nine.  Returns the number
 // of calls averaged.
 FPNGB_API int fpngb_profile_enable(int on)
 {
@@ -1302,8 +1264,7 @@ int fpngb_train_accumulate_device(const void* d_pixels, size_t image_stride, uin
     sp.pixels = (const uint8_t*)d_pixels; sp.image_stride = image_stride; sp.row_pitch = w * chans; sp.w = w; sp.h = h; sp.books = c.d_static_books; sp.book_stride = 0;
     sp.row_bits = ws.row_bits; sp.row_adler = ws.row_adler; sp.st = ws.st; sp.hist = ws.hist; sp.lane_ofs = ws.lane_ofs; sp.lane_ofs_pitch = ws.lane_ofs_pitch;
     FPNGB_CUDA_OK(cudaMemsetAsync(ws.hist, 0, (size_t)n * 288 * 4, s));
-    if (!force_generic_env()) launch_hist16(sp, n, chans, s);
-    else launch_scan(sp, n, chans, pick_load_mode(d_pixels, image_stride, w, chans), true, s);
+    launch_hist16(sp, n, chans, s);
     count_launch(1);
     std::vector<uint32_t> hh((size_t)n * 288);
     FPNGB_CUDA_OK(cudaMemcpyAsync(hh.data(), ws.hist, hh.size() * 4, cudaMemcpyDeviceToHost, s));

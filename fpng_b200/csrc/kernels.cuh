@@ -5,11 +5,7 @@
 
 namespace fpngb {
 
-constexpr int kRowsPerBlock = 8;                  // one warp per scanline, 8 scanlines per CTA
-constexpr int kScanThreads = 32 * kRowsPerBlock;
-constexpr int kPackThreads = 32 * kRowsPerBlock;
 constexpr int kOffsetsThreads = 256;
-constexpr int kStageWords = 272;                  // >= (31 + 12 + 128 * 66) / 32 + 1 words per 128-pixel step
 
 // One image of a ragged encode call (fpngb_encode_ragged_device): its pixels and shape, where its scanlines sit in the row tables
 // and lane records, its code book, its output slot and its container header (the IHDR differs per image).
@@ -49,7 +45,7 @@ __device__ __forceinline__ uint32_t ragged_locate(const RaggedWork& rw, uint32_t
 
 struct ScanParams {
     const uint8_t* pixels; size_t image_stride;   // n images
-    uint32_t row_pitch;                           // bytes between scanlines (the generic 4-pixel kernels assume w * chans)
+    uint32_t row_pitch;                           // bytes between scanlines
     size_t chan_stride;                           // 0: interleaved pixels; else planar, channel c of pixel x at row + x + c * chan_stride
     uint32_t w, h;
     const CodeBook* books; uint32_t book_stride;  // 0: one shared (1-pass) book, 1: per-image books (2-pass)
@@ -58,8 +54,9 @@ struct ScanParams {
     ImageState* st;                               // [n]
     uint32_t* hist;                               // [n*288] (histogram mode)
     uint32_t merge_first_unit;                    // RGB 1-pass: filter literal and pixel 0 share a flush unit (fpng.cpp:1187-1203)
-    uint2* lane_ofs; uint32_t lane_ofs_pitch;     // v2 kernels: [n*h][pitch] per 16-pixel group: .x bit offset inside its row, .y lane_info16()
-    uint32_t lit1_rule;                           // RGBA 1-pass with a table under which fpng.cpp:1520-1528 can fire (generic kernels only)
+    uint2* lane_ofs; uint32_t lane_ofs_pitch;     // [n*h][pitch] per 16-pixel group: .x bit offset inside its row, .y lane_info16()
+    uint32_t lit1_rule;                           // 1-pass with an RGBA table under which fpng.cpp:1520-1528 can fire: the launchers
+                                                  // take the RGBA kernels' LIT1 instantiations (call-wide: one static RGBA table)
 };
 
 struct OffsetsParams {
@@ -78,7 +75,7 @@ struct PackParams {
     uint32_t w, h;
     const CodeBook* books; uint32_t book_stride;
     const unsigned long long* row_ofs;
-    const uint32_t* row_bits;                     // v2 kernels: total token bits per row
+    const uint32_t* row_bits;                     // total token bits per row
     const uint2* lane_ofs; uint32_t lane_ofs_pitch;
     uint2* row_adler;                             // rewritten for stored images (raw bytes, filter 0)
     const ImageState* st;
@@ -214,14 +211,12 @@ uint32_t convert_ctas_per_image(uint32_t w, uint32_t h);
 // instantiations (a float dtype; 1 to 4 channels and sample_bytes 1 or 2 per descriptor), else 3 or 4 channels of uint8 output.
 void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, bool png, cudaStream_t s);
 
-void launch_scan(const ScanParams& p, uint32_t n, uint32_t chans, int mode, bool hist, cudaStream_t s);
 bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans);
 void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);
 void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);
 void launch_pack16(const PackParams& p, uint32_t n, uint32_t chans, cudaStream_t s);
 void set_rows_per_warp16(uint32_t v);          // 0 = automatic (5 scanlines per warp on large batches, 1 otherwise)
 void launch_offsets(const OffsetsParams& p, uint32_t n, cudaStream_t s);
-void launch_pack(const PackParams& p, uint32_t n, uint32_t chans, int mode, cudaStream_t s);
 void launch_adler_finalize(const AdlerParams& p, uint32_t n, cudaStream_t s);
 void launch_huffman_build(const HuffParams& p, uint32_t n, cudaStream_t s);
 uint32_t adler_chunk_bytes();

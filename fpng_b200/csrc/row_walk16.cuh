@@ -1,16 +1,18 @@
-// fpng_b200/csrc/row_walk16.cuh -- second-generation scanline walker: 16 consecutive pixels per lane, 512 per warp step.
+// fpng_b200/csrc/row_walk16.cuh -- the encoder's scanline walker: 16 consecutive pixels per lane, 512 per warp step.
 //
-// Same tokenisation as row_walk.cuh (reference: fpng.cpp:1182-1243 / 1468-1558, SURVEY.md Appendix B) with the
-// per-step warp-wide work (neighbour shuffle, ballot, run phase) amortised over 4x more pixels and with fully coalesced
-// 128-bit global loads:
+// The tokenisation of the reference's greedy scalar coder (fpng.cpp:1182-1243 RGB, 1468-1558 RGBA; 2-pass: 1021-1084,
+// 1299-1363) restated data-parallel (SURVEY.md Appendix B): a run of pixels equal to their left neighbour is cut into match
+// tokens of M = 85 (RGB) / 63 (RGBA) pixels from the run start, and each token is attributed to the pixel where it ENDS (full
+// token) or to the literal that follows it / the end of the row (remainder token), which preserves the serial token order.
+// Per warp step:
 //   1. one elected lane issues a TMA bulk copy (cp.async.bulk + mbarrier) of the step's 512 cur and prev pixels into the
 //      warp's shared-memory tile, one step ahead of the computation;
 //   2. each lane reads its own 16 consecutive pixels with 128-bit shared loads, subtracts the previous scanline (PNG
 //      filter 2 "Up", fpng.cpp:1605-1652) and accumulates the Adler-32 partial sums;
 //   3. equality with the left pixel gives a 16-bit mask per lane; the run phase entering the lane is one ballot + one
 //      shuffle; the lane then walks its pixels.
-// Requires every scanline to start 16-byte aligned and bpl % 16 == 0 (RGBA: w % 4 == 0, RGB: w % 16 == 0); other
-// shapes use the generic kernels of row_walk.cuh.
+// The staged loaders require every scanline to start 16-byte aligned and bpl % 16 == 0 (RGBA: w % 4 == 0, RGB: w % 16 == 0);
+// the direct and planar loaders below take any other shape.
 #pragma once
 #include "row_walk.cuh"
 

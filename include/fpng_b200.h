@@ -88,8 +88,7 @@ FPNGB_API int fpngb_encode_batch_device(const void* d_pixels, size_t image_strid
 /* fpngb_encode_batch_device with the input in any layout of "Pixel layouts" above: d_pixels and the four strides describe
  * the [n, h, w, chans] batch; everything else as fpngb_encode_batch_device, with the same output bytes as for a tightly packed
  * copy.  The scan and pack kernels read interleaved rows at any pitch and planar images in place; where the batch would
- * go to the generic kernels (a trained RGBA table whose one-pixel-match rule can fire, FPNGB_FORCE_GENERIC) or to the opt-in
- * single-pass encoder, it is first copied into the library's workspace by one extra kernel. */
+ * go to the opt-in single-pass encoder, it is first copied into the library's workspace by one extra kernel. */
 FPNGB_API int fpngb_encode_batch_device_strided(const void* d_pixels, size_t image_stride, size_t row_pitch, size_t pixel_stride,
                                                 size_t chan_stride, uint32_t n, uint32_t w, uint32_t h, uint32_t chans, uint32_t flags,
                                                 void* d_out, size_t out_stride, uint32_t* d_sizes, void* stream);
@@ -114,10 +113,8 @@ FPNGB_API int fpngb_encode_batch_device_strided(const void* d_pixels, size_t ima
  *   Launches: per non-empty (chans, loader) class -- 3 or 4 channels times staged / direct / planar loader -- one scan and one
  *   pack kernel, plus one hist kernel with FPNG_ENCODE_SLOWER; then four per-image kernels (offsets, Adler-32, scanline-CRC
  *   combine, stored-block CRC), plus the Huffman build with FPNG_ENCODE_SLOWER.  fpngb_profile_read reports the call in its
- *   usual slots.
- *   Fallbacks: RGBA images in 1-pass mode under an installed table whose one-pixel-match rule can fire (never the shipped
- *   table), and every image under FPNGB_FORCE_GENERIC, are encoded by the uniform pipeline one image at a time into their
- *   slots: correct, but one uniform call's launches per image.  The opt-in single-pass encoder is not used by this call. */
+ *   usual slots.  Every image takes this route, also under an installed table whose one-pixel-match rule can fire.  The opt-in
+ *   single-pass encoder is not used by this call. */
 FPNGB_API int fpngb_encode_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,
                                          void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
 

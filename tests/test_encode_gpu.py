@@ -187,33 +187,33 @@ def test_checksum_utilities(gpu, oracle):
         assert gpu.fpng_crc32(d[cut:], gpu.fpng_crc32(d[:cut])) == oracle.crc32(d), cut
 
 
-def test_generic_kernels_still_match(oracle):
-    """The second-generation kernels are the default for 16-byte aligned scanlines; FPNGB_FORCE_GENERIC=1 selects the
-    generic kernels for the same shapes.  Both must produce the reference bytes (run in a subprocess: the switch is read once)."""
-    import os
-    import subprocess
-    import sys
-    code = r"""
-import sys, os
-sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), 'tests'))
-import imagegen, fpng_b200
-from oracle.pyoracle import Oracle
-o = Oracle(); fpng_b200.fpng_init()
-bad = 0
-for kind in ('g1', 'g0', 'runs', 'g2'):
-    for (w, h) in ((16, 2), (512, 9), (1024, 5), (1920, 3), (4096, 2)):
-        for c in (3, 4):
-            img = imagegen.make(kind, w, h, c, 3)
-            for flags in (0, 1):
-                ok, png = fpng_b200.fpng_encode_image_to_memory(img, w, h, c, flags)
-                bad += (not ok) or png != o.encode(img, w, h, c, flags)
-print('bad', bad)
-sys.exit(1 if bad else 0)
-"""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, FPNGB_FORCE_GENERIC="1")
-    out = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stdout + out.stderr
+def test_trained_rgba_table_parity(gpu, oracle):
+    """Under the RGBA fixture table of tests/golden/trained_tables.json, whose one-pixel-match rule fires, RGBA 1-pass runs the
+    scan and pack kernels' LIT1 instantiations: every image must equal the oracle running the same table (RGB and 2-pass keep
+    their usual kernels), with one and with five scanlines per pack warp."""
+    from fpng_b200 import _lib
+    from test_trained_tables_cpu import load_tables
+    t = load_tables()["4"]
+    sizes = np.array(t["sizes"], np.uint8)
+    pal = [int(v) for v in np.argsort(sizes[:256], kind="stable")[:4]]
+    prefix = bytes.fromhex(t["prefix"])
+    assert oracle.set_static_table(4, prefix, t["bit_buf"], t["bit_buf_size"])
+    try:
+        gpu.set_static_table(4, prefix, t["bit_buf"], t["bit_buf_size"])
+        for rpw in (1, 5):
+            _lib.lib().fpngb_debug_rows_per_warp(rpw)
+            for (w, h) in ((16, 2), (512, 9), (1024, 5), (1920, 3), (4096, 2)):
+                for c in (3, 4):
+                    imgs = [(kind, imagegen.make(kind, w, h, c, 3)) for kind in ("g1", "g0", "runs", "g2")]
+                    imgs.append(("short_runs", imagegen.short_runs(w, h, c, 5, pal)))
+                    for kind, img in imgs:
+                        for flags in (0, 1):
+                            ok, png = gpu.fpng_encode_image_to_memory(img, w, h, c, flags)
+                            assert ok and png == oracle.encode(img, w, h, c, flags), (rpw, kind, w, h, c, flags)
+    finally:
+        _lib.lib().fpngb_debug_rows_per_warp(0)
+        gpu.set_static_table(4)
+        oracle.set_static_table(4)
 
 
 def test_concurrent_host_threads_and_streams(gpu, oracle):

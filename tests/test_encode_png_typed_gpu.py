@@ -168,8 +168,9 @@ def test_mixed_call(gpu, png_oracle, flags):
             assert got[k] == png_oracle.png_encode(host(q), flags), k
 
 
-def test_fpng_fallback_route(gpu, oracle):
-    """RGBA 1-pass under a table whose one-pixel-match rule is live goes through the uniform pipeline, as in the untyped call"""
+def test_trained_table_typed_call(gpu, oracle):
+    """RGBA 1-pass under a table whose one-pixel-match rule is live: the typed call writes the untyped call's files with one
+    launch more, its conversion kernel; both stay in the ragged pipeline"""
     import torch
     t = load_tables()["4"]
     prefix = bytes.fromhex(t["prefix"])

@@ -190,8 +190,8 @@ def test_slots_and_guard(gpu, oracle):
 
 # ---- 5. trained tables -----------------------------------------------------------------------------------------------------
 def test_trained_tables(gpu, oracle):
-    """RGB images run the ragged kernels under the trained table, RGBA images (one-pixel-match rule live) the per-image
-    fallback; both equal the oracle running the same tables"""
+    """RGB and RGBA images run the ragged kernels under the trained tables (for RGBA the one-pixel-match rule's instantiations)
+    and equal the oracle running the same tables"""
     import torch
     tables = load_tables()
     try:
@@ -325,50 +325,42 @@ def test_no_host_synchronisation(gpu, oracle):
     check_oracle(oracle, hosts[::-1], files_of(*b), 1, "second")
 
 
-# ---- 10. the uniform pipeline's fallback -----------------------------------------------------------------------------------
-def test_forced_generic_fallback():
-    """FPNGB_FORCE_GENERIC=1 sends every fpng image of the ragged and PNG calls through the uniform pipeline one image at a time,
-    the route of RGBA images under a trained table: uint8, float32 and mixed PNG calls must write the files of the default
-    route (run in subprocesses: the switch is read once)."""
-    import json
-    import os
-    import subprocess
-    import sys
-    code = r"""
-import hashlib, json, os, sys
-sys.path.insert(0, os.getcwd()); sys.path.insert(0, os.path.join(os.getcwd(), 'tests'))
-import numpy as np, torch
-import imagegen, fpng_b200
-fpng_b200.fpng_init()
-def files(out, offsets, sizes):
-    torch.cuda.synchronize()
-    data, ofs, sz = out.cpu().numpy(), offsets.cpu().numpy(), sizes.cpu().numpy().astype(np.int64)
-    return [hashlib.sha256(data[ofs[i]:ofs[i] + sz[i]].tobytes()).hexdigest() for i in range(len(sz))]
-shapes = [(9, 687, 3), (5, 64, 4), (40, 17, 3), (3, 1920, 4), (1, 1, 3), (11, 513, 4)]
-hosts = [imagegen.make('g1', w, h, c, i).reshape(h, w, c) for i, (h, w, c) in enumerate(shapes)]
-u8 = [torch.from_numpy(x).cuda() for x in hosts]
-f32 = [torch.from_numpy(np.ascontiguousarray(x.transpose(2, 0, 1))).cuda().float().div_(255).permute(1, 2, 0) for x in hosts]
-rgba16 = imagegen.make('g1', 300, 7, 4, 9).reshape(7, 300, 4).astype(np.uint16) * 251 + 3
-gray = np.ascontiguousarray(imagegen.make('g1', 70, 6, 3, 7).reshape(6, 70, 3)[..., :1])
-mixed = [torch.from_numpy(gray).cuda(), u8[0],
-         torch.from_numpy(rgba16).cuda(), u8[1]]
-res = {}
-for flags in (0, 1, 2):
-    res[f'ragged {flags}'] = files(*fpng_b200.encode_ragged_device(u8, flags))
-    res[f'ragged float32 {flags}'] = files(*fpng_b200.encode_ragged_device(f32, flags, scale=255.0))
-    res[f'png {flags}'] = files(*fpng_b200.encode_png_device(mixed, flags))
-print(json.dumps({'launches': fpng_b200.launch_count(), 'files': res}))
-"""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    runs = []
-    for generic in (False, True):
-        env = {k: v for k, v in os.environ.items() if k != "FPNGB_FORCE_GENERIC"}
-        if generic:
-            env["FPNGB_FORCE_GENERIC"] = "1"
-        out = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=600)
-        assert out.returncode == 0, out.stdout + out.stderr
-        runs.append(json.loads(out.stdout.strip().splitlines()[-1]))
-    default, generic = runs
-    assert generic["launches"] > default["launches"], "FPNGB_FORCE_GENERIC=1 did not take the one-image-at-a-time route"
-    for call, want in default["files"].items():
-        assert generic["files"][call] == want, call
+# ---- 10. trained tables on every RGBA loader -------------------------------------------------------------------------------
+def test_trained_tables_mixed_layouts(gpu, oracle):
+    """Under both trained tables (the RGBA one's one-pixel-match rule fires) a ragged call over RGB images and interleaved,
+    cropped (direct loader) and planar RGBA views, of uint8 and of float32, writes the oracle's files with as many launches as
+    the same call under the shipped tables: no image leaves the ragged pipeline."""
+    import torch
+    tables = load_tables()
+    sizes = np.array(tables["4"]["sizes"], np.uint8)
+    pal = [int(v) for v in np.argsort(sizes[:256], kind="stable")[:4]]
+    rgba = [imagegen.short_runs(w, h, 4, 20 + i, pal) for i, (h, w) in enumerate([(24, 61), (9, 513), (5, 1030), (1, 16)])]
+    hosts, u8, f32 = [], [], []
+    for x in rgba + host_images([(9, 687, 3), (40, 17, 3)], "runs", 30):
+        h, w, c = x.shape
+        for layout in (("interleaved", "cropped", "planar") if c == 4 else ("interleaved",)):
+            hosts.append(x)
+            for dst, t in ((u8, torch.from_numpy(np.ascontiguousarray(x)).cuda()),
+                           (f32, torch.from_numpy(np.ascontiguousarray(x)).cuda().float().div_(255))):
+                if layout == "cropped":
+                    canvas = torch.zeros((h, w + 3, c), dtype=t.dtype, device="cuda"); canvas[:, 3:] = t; t = canvas[:, 3:]
+                elif layout == "planar":
+                    t = t.permute(2, 0, 1).contiguous().permute(1, 2, 0)
+                dst.append(t)
+    calls = {f"{name} {flags}": (lambda imgs=imgs, flags=flags, kw=kw: gpu.encode_ragged_device(imgs, flags, **kw))
+             for name, imgs, kw in (("uint8", u8, {}), ("float32", f32, {"scale": 255.0})) for flags in (0, 1)}
+    shipped = {name: launches(gpu, fn)[0] for name, fn in calls.items()}
+    try:
+        for chans in (3, 4):
+            t = tables[str(chans)]
+            prefix = bytes.fromhex(t["prefix"])
+            assert oracle.set_static_table(chans, prefix, t["bit_buf"], t["bit_buf_size"])
+            gpu.set_static_table(chans, prefix, t["bit_buf"], t["bit_buf_size"])
+        for name, fn in calls.items():
+            k, r = launches(gpu, fn)
+            check_oracle(oracle, hosts, files_of(*r), int(name[-1]), name)
+            assert k == shipped[name], (name, k, shipped[name])
+    finally:
+        for chans in (3, 4):
+            gpu.set_static_table(chans)
+            oracle.set_static_table(chans)

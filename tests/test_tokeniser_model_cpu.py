@@ -9,11 +9,19 @@ ends (full match), or to the literal / row end that follows it (remainder).  Per
   eqm  -- 16-bit mask "pixel k equals its left neighbour",
   r_in -- the unfinished run entering the lane (from the nearest lower lane holding a literal: one ballot + one shuffle),
 and derive from them (a) the literal pixels, (b) the "events": a pending run flushed before a literal, or the run
-reaching M at a match pixel (at most one per lane since M > 16)."""
+reaching M at a match pixel (at most one per lane since M > 16).
+
+RGBA 1-pass under a table whose "one-pixel match vs four literals" rule can fire (fpng.cpp:1520-1528; the kernels' LIT1
+instantiations) a flushed match of exactly one pixel is written as the four literals of the pixel it covers when the match
+costs more bits.  The serial coder knows that pixel as the last literal; a lane knows it as its own pixel k - 1, or at lane
+pixel 0 as the lane to the left's pixel 15 (one shuffle), or for lane 0 as lane 31's pixel 15 of the previous step."""
+import json
+import os
 import numpy as np
 import pytest
 
 import imagegen
+from common import HERE
 
 LEN_BASE = [3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258]
 LEN_XBITS = [0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2, 2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0]
@@ -39,7 +47,22 @@ def filtered_pixels(img, y):
     return (0 if y == 0 else 2), [int(v) for v in px]
 
 
-def serial_tokens(filt, px, M):
+def lit1_takes_literals(sizes, p):
+    """The one-pixel-match rule (fpng.cpp:1520-1528): a one-pixel match covering the RGBA pixel p is written as p's four
+    literals iff the match (length code + extra bits + the 1-bit distance) costs more bits than they do."""
+    sym, xb = len_symbol(4)
+    return int(sizes[sym]) + xb + 1 > sum(int(sizes[(p >> (8 * c)) & 255]) for c in range(4))
+
+
+def flush(out, n, covered, lit1):
+    """Appends the token of a pending run of n pixels whose last pixel is `covered` (lit1: the RGBA table's code sizes)."""
+    if n == 1 and lit1 is not None and lit1_takes_literals(lit1, covered):
+        out.append(("L", covered))
+    elif n:
+        out.append(("M", n))
+
+
+def serial_tokens(filt, px, M, lit1=None):
     out = [("F", filt)]
     prev, run = None, 0
     for x, p in enumerate(px):
@@ -48,11 +71,9 @@ def serial_tokens(filt, px, M):
             if run == M:
                 out.append(("M", M)); run = 0
         else:
-            if run:
-                out.append(("M", run)); run = 0
+            flush(out, run, prev, lit1); run = 0
             out.append(("L", p)); prev = p
-    if run:
-        out.append(("M", run))
+    flush(out, run, prev, lit1)
     return out
 
 
@@ -65,8 +86,9 @@ def run_before(eqm, r_in, kk, M):
     return kk - 1 - (t.bit_length() - 1)
 
 
-def parallel_tokens(filt, px, M):
-    """Tokens of one scanline as 32 lanes x 16 pixels per warp step produce them, lanes concatenated in order."""
+def parallel_tokens(filt, px, M, lit1=None, sites=None):
+    """Tokens of one scanline as 32 lanes x 16 pixels per warp step produce them, lanes concatenated in order.  lit1: the RGBA
+    table's code sizes, applying the one-pixel-match rule; sites (a Counter) counts where the rule took the literals."""
     w = len(px)
     out = [("F", filt)]
     carry_prev, carry_run = 0, 0
@@ -75,6 +97,7 @@ def parallel_tokens(filt, px, M):
         for lane in range(32):
             p0 = s0 + lane * 16
             nvp = min(16, w - p0) if p0 < w else 0
+            lpx = [px[p0 + k] if k < nvp else 0 for k in range(16)]   # the lane's filtered pixels, zero beyond the row
             eqm = 0
             for k in range(nvp):
                 x = p0 + k
@@ -84,7 +107,7 @@ def parallel_tokens(filt, px, M):
             valid = (1 << nvp) - 1
             litm = valid & ~eqm
             trail = (nvp - 1 - (litm.bit_length() - 1)) if litm else nvp
-            lanes.append(dict(p0=p0, nvp=nvp, eqm=eqm, litm=litm, trail=trail))
+            lanes.append(dict(p0=p0, nvp=nvp, eqm=eqm, litm=litm, trail=trail, px=lpx))
         # run phase entering each lane: the nearest lower lane with a literal decides (ballot + shuffle in classify16)
         for lane, t in enumerate(lanes):
             src = max((l for l in range(lane) if lanes[l]["litm"]), default=None)
@@ -92,23 +115,26 @@ def parallel_tokens(filt, px, M):
             t["run"] = run % M
         last = lanes[31]
         carry_run = last["trail"] if last["litm"] else (last["run"] + last["nvp"]) % M
-        # per-lane emission from (eqm, r_in) alone: literals + events
-        for t in lanes:
-            eqm, litm, nvp, r_in = t["eqm"], t["litm"], t["nvp"], t["run"]
+        # per-lane emission from (eqm, r_in) alone: literals + events; under the rule also the pixel left of the lane
+        for lane, t in enumerate(lanes):
+            eqm, litm, nvp, r_in, lpx = t["eqm"], t["litm"], t["nvp"], t["run"], t["px"]
+            left = lanes[lane - 1]["px"][15] if lane else carry_prev
             lead = ((~eqm) & -(~eqm)).bit_length() - 1            # leading match pixels (ffs(~eqm) - 1)
             kM = M - 1 - r_in
             evm = (litm & ((eqm << 1) | (1 if r_in else 0))) | ((1 << kM) if kM < lead else 0)
-            for k in range(nvp):
-                if evm >> k & 1:
-                    n = M if eqm >> k & 1 else run_before(eqm, r_in, k, M)
-                    if n:
-                        out.append(("M", n))
-                if litm >> k & 1:
-                    out.append(("L", px[t["p0"] + k]))
-            if nvp and t["p0"] + nvp == w:                         # the lane holding the scanline's last pixel
-                n = run_before(eqm, r_in, nvp, M)
-                if n:
-                    out.append(("M", n))
+            for k in range(nvp + 1):
+                tail = k == nvp
+                if tail and not (nvp and t["p0"] + nvp == w):     # the lane holding the scanline's last pixel flushes its run
+                    break
+                if tail or evm >> k & 1:
+                    n = M if not tail and eqm >> k & 1 else run_before(eqm, r_in, k, M)
+                    covered = lpx[k - 1] if k else left
+                    if sites is not None and n == 1 and lit1 is not None and lit1_takes_literals(lit1, covered):
+                        sites["row end" if tail else "mid-lane" if k else "lane 0, previous step" if lane == 0 else "lane pixel 0"] += 1
+                    flush(out, n, covered, lit1)
+                if not tail and litm >> k & 1:
+                    out.append(("L", lpx[k]))
+        carry_prev = last["px"][15]
     return out
 
 
@@ -149,3 +175,50 @@ def test_run_boundaries_at_max_match():
             for lead_in in (0, 1, 15, 16, 17, 500):
                 px = list(range(1, lead_in + 1)) + [777] * run_len + [5, 5, 6]
                 assert parallel_tokens(2, px, M) == serial_tokens(2, px, M), (chans, run_len, lead_in)
+
+
+def test_one_pixel_match_rule_under_trained_rgba_table(oracle):
+    """RGBA 1-pass under the fixture table of tests/golden/trained_tables.json, whose one-pixel-match rule fires: the lane-parallel
+    tokens equal the serial ones and their bits equal the oracle's per-row counts, at widths on both sides of the 16-pixel lane
+    and the 512-pixel step, with the rule taking the literals at every kind of site the kernels handle."""
+    from collections import Counter
+    with open(os.path.join(HERE, "golden", "trained_tables.json")) as f:
+        t = json.load(f)["tables"]["4"]
+    assert oracle.set_static_table(4, bytes.fromhex(t["prefix"]), t["bit_buf"], t["bit_buf_size"])
+    try:
+        sizes, _, _ = oracle.static_table(4)
+        order = np.argsort(sizes[:256], kind="stable")
+        cheap = [int(v) for v in order[:5]]
+        pals = (cheap[:2], cheap + [int(order[40]), int(order[200])])   # the rule fires mostly / rarely
+        images = [(name, img) for name, _, _, img in imagegen.trained_table_images(4, sizes)]
+        for i, w in enumerate((15, 16, 17, 31, 33, 511, 512, 513, 527, 1023, 1024, 1025, 1553)):
+            for j, pal in enumerate(pals):
+                images.append((f"short_runs w={w} palette {j}", imagegen.short_runs(w, 24, 4, 300 + i, pal)))
+            images.append((f"runs w={w}", imagegen.make("runs", w, 4, 4, 300 + i)))
+        sites = Counter()
+        for name, img in images:
+            h, w, _ = img.shape
+            _, row_bits, stored = oracle.encode(img, w, h, 4, 0, want_rows=True)
+            assert not stored, name
+            for y in range(h):
+                filt, px = filtered_pixels(img, y)
+                ser = serial_tokens(filt, px, 63, sizes)
+                assert parallel_tokens(filt, px, 63, sizes, sites) == ser, (name, y)
+                assert token_bits(ser, sizes, 4) == int(row_bits[y]), (name, y)
+        for site in ("mid-lane", "lane pixel 0", "lane 0, previous step", "row end"):
+            assert sites[site] > 0, (site, sites)
+    finally:
+        oracle.set_static_table(4)
+
+
+def test_one_pixel_remainder_of_max_match_under_rule(oracle):
+    """A run of M + 1 pixels ends in a one-pixel match: the rule applies to it, wherever the run sits in lanes and steps."""
+    with open(os.path.join(HERE, "golden", "trained_tables.json")) as f:
+        sizes = np.array(json.load(f)["tables"]["4"]["sizes"], np.uint8)
+    cheap = int(np.argmin(sizes[:256]))
+    assert lit1_takes_literals(sizes, cheap * 0x01010101)
+    for lead_in in (0, 1, 15, 16, 17, 448, 449, 500):
+        for tail in ([5, 5, 6], [], [cheap * 0x01010101 + 1]):
+            px = list(range(1, lead_in + 1)) + [cheap * 0x01010101] * 65 + tail
+            ser = serial_tokens(2, px, 63, sizes)
+            assert ser.count(("L", cheap * 0x01010101)) == 2 and parallel_tokens(2, px, 63, sizes) == ser, (lead_in, tail)
