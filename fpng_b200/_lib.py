@@ -17,6 +17,11 @@ class PixelFormat(C.Structure):
     _fields_ = [("dtype", C.c_uint32), ("scale", C.c_float * 4), ("bias", C.c_float * 4)]
 
 
+class LabelPalette(C.Structure):
+    """fpngb_label_palette: entries x chans (3 or 4) colour bytes in host memory; entries 0 is a gray label map"""
+    _fields_ = [("colors", C.c_void_p), ("entries", C.c_uint32), ("chans", C.c_uint32)]
+
+
 def lib() -> C.CDLL:
     global _lib
     if _lib is not None:
@@ -115,6 +120,11 @@ def lib() -> C.CDLL:
                                              C.c_void_p, C.c_void_p, C.c_void_p]
     L.fpngb_encode_png_ragged_device.restype = C.c_int
     L.fpngb_encode_png_ragged_device.argtypes = L.fpngb_encode_ragged_device.argtypes
+    L.fpngb_max_label_encoded_size.restype = C.c_size_t
+    L.fpngb_max_label_encoded_size.argtypes = [C.c_uint32] * 3 + [C.POINTER(LabelPalette)]
+    L.fpngb_encode_label_ragged_device.restype = C.c_int
+    L.fpngb_encode_label_ragged_device.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                   C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
     L.fpngb_encode_png_ragged_device_typed.restype = C.c_int
     L.fpngb_encode_png_ragged_device_typed.argtypes = L.fpngb_encode_ragged_device_typed.argtypes
     L.fpngb_decode_batch_host.restype = C.c_int

@@ -12,7 +12,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import FpngB200Error, PixelFormat, check, lib
+from ._lib import FpngB200Error, LabelPalette, PixelFormat, check, lib
 
 FPNG_ENCODE_SLOWER = 1          # src/fpng.h:38
 FPNG_FORCE_UNCOMPRESSED = 2     # src/fpng.h:41
@@ -372,6 +372,130 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None,
         raise ValueError("encode_png_device: depth, scale and bias apply to float images only; uint8 / uint16 are taken as they are")
     depths = depths if fmt is not None else [8 * t.element_size() for t in images]
     return _encode_images(images, depths, fmt, flags, out, stream, True, "encode_png_device")
+
+
+def _label_palettes(palette, n):
+    """The per-image palettes of encode_labels_device as uint8 [K, 3 | 4] numpy arrays (None: gray), ValueError otherwise."""
+    if palette is None:
+        return [None] * n
+    if isinstance(palette, (list, tuple)):
+        if len(palette) != n:
+            raise ValueError(f"encode_labels_device: palette is one array or a list of {n} (one per image), got {len(palette)}")
+        pals = list(palette)
+    else:
+        pals = [palette] * n
+    out = []
+    for p in pals:
+        if p is None:
+            out.append(None)
+            continue
+        if hasattr(p, "detach"):
+            p = p.detach().cpu().numpy()
+        a = np.asarray(p)
+        if a.dtype != np.uint8 or a.ndim != 2 or a.shape[1] not in (3, 4) or not 1 <= a.shape[0] <= 256:
+            raise ValueError(f"encode_labels_device: a palette is a uint8 array of shape [K, 3 or 4] with 1 <= K <= 256, got "
+                             f"{a.dtype} {a.shape}")
+        out.append(np.ascontiguousarray(a))
+    return out
+
+
+def _palette_struct(a):
+    return LabelPalette(None, 0, 0) if a is None else LabelPalette(a.ctypes.data, a.shape[0], a.shape[1])
+
+
+def _pil_depth(k):
+    """PIL's bit depth for a palette of k entries"""
+    return 1 if k <= 2 else 2 if k <= 4 else 4 if k <= 16 else 8
+
+
+def max_label_encoded_size(w: int, h: int, depth: int, palette=None) -> int:
+    """fpngb_max_label_encoded_size: the slot bound of a w x h label map at `depth` bits with an optional [K, 3 | 4] palette"""
+    pal = _label_palettes(palette, 1)[0]
+    return lib().fpngb_max_label_encoded_size(w, h, depth, C.byref(_palette_struct(pal)))
+
+
+def label_slot_offsets(shapes, palettes=None):
+    """The slot offsets of encode_labels_device for label maps of the given (h, w, depth) shapes, with palettes None (all gray)
+    or one [K, 3 | 4] array (or None) per map: the exclusive prefix of max_label_encoded_size rounded up to 16 bytes, with the
+    total as the last of the n + 1 entries."""
+    pals = palettes if palettes is not None else [None] * len(shapes)
+    ofs = np.zeros(len(shapes) + 1, dtype=np.int64)
+    for i, ((h, w, depth), pal) in enumerate(zip(shapes, pals)):
+        ofs[i + 1] = ofs[i] + (max_label_encoded_size(int(w), int(h), int(depth), pal) + 15) // 16 * 16
+    return ofs
+
+
+def encode_labels_device(images, palette=None, depth=None, flags: int = 0, out=None, stream=None):
+    """Encode label maps (class ids, masks) on the GPU to palette or gray PNGs in one call (fpngb_encode_label_ragged_device).
+
+    images: list of CUDA tensors [h, w] or [h, w, 1], torch.uint8 or torch.int64 ids (the output of logits.argmax(1)[i] goes in
+    as it is), contiguous or a view whose ids are contiguous within a row, at any row pitch (a crop, an expand of one row).
+    palette: None (gray files), one uint8 array [K, 3 | 4] (RGB or RGBA, K <= 256) for every image, or a list with one such
+    array or None per image.  depth: bits per id, one
+    value or one per image; for a palette image it defaults to PIL's rule (K <= 2: 1, <= 4: 2, <= 16: 4, else 8); a gray image
+    needs it (1, 2, 4, 8 or 16, 16 only from int64), so that a mask is never truncated by accident.  flags: 0 or
+    FPNG_FORCE_UNCOMPRESSED.  An image holding an id outside [0, 2^depth) (gray) or [0, K) (palette) gets size 0; the others are
+    unaffected.  Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]) as encode_png_device does, offsets being
+    label_slot_offsets -- the (data, offsets, sizes) decode_packed_ragged_device(any_png=True, all_formats=True) reads, with
+    indices=True giving the ids back.  Kernels are enqueued on the current torch stream (or `stream`), with no host
+    synchronisation.  Other dtypes, shapes and argument values raise ValueError."""
+    import torch
+
+    n = len(images)
+    if n == 0:
+        raise ValueError("encode_labels_device: at least one image is needed")
+    pals = _label_palettes(palette, n)
+    depths = [depth] * n if depth is None or np.ndim(depth) == 0 else list(depth)
+    if len(depths) != n:
+        raise ValueError(f"encode_labels_device: depth is one value or one per image ({n}), got {depth}")
+    ptrs, dims, strides = [], [], []
+    for i, t in enumerate(images):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError("encode_labels_device: images are CUDA tensors")
+        if t.dtype not in (torch.uint8, torch.int64):
+            raise ValueError(f"encode_labels_device: torch.uint8 or torch.int64 ids are needed, got {t.dtype}")
+        if not (t.dim() == 2 or (t.dim() == 3 and t.shape[2] == 1)):
+            raise ValueError(f"encode_labels_device: images are [h, w] or [h, w, 1], got {tuple(t.shape)}")
+        h, w = int(t.shape[0]), int(t.shape[1])
+        d, pal = depths[i], pals[i]
+        if d is None:
+            if pal is None:
+                raise ValueError("encode_labels_device: gray label maps need depth (1, 2, 4, 8 or 16)")
+            d = _pil_depth(pal.shape[0])
+        d = int(d)
+        if pal is None and d not in (1, 2, 4, 8, 16):
+            raise ValueError(f"encode_labels_device: gray depth is 1, 2, 4, 8 or 16, got {d}")
+        if pal is not None and (d not in (1, 2, 4, 8) or pal.shape[0] > 1 << d):
+            raise ValueError(f"encode_labels_device: a palette of {pal.shape[0]} entries needs depth 1, 2, 4 or 8 with K <= 2^depth, "
+                             f"got {d}")
+        if t.dtype == torch.uint8 and d > 8:
+            raise ValueError("encode_labels_device: depth 16 needs int64 ids")
+        es = t.element_size()
+        ptrs.append(t.data_ptr()); dims.append((w, h, d, es)); strides.append((t.stride(0) * es, t.stride(1) * es))
+        depths[i] = d
+    device = images[0].device
+    if any(t.device != device for t in images):
+        raise ValueError("encode_labels_device: the images are on one device")
+    if flags & ~FPNG_FORCE_UNCOMPRESSED:
+        raise ValueError("encode_labels_device: flags is 0 or FPNG_FORCE_UNCOMPRESSED")
+    if min(s for st in strides for s in st) < 0:
+        raise ValueError("encode_labels_device: negative strides are not supported")
+    structs = (LabelPalette * n)(*[_palette_struct(p) for p in pals])
+    if out is None:
+        total = int(label_slot_offsets([(dm[1], dm[0], dm[2]) for dm in dims], pals)[-1])
+        out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
+    _check_arg(out, "out", device, torch.uint8)
+    offsets = torch.empty((n + 1,), dtype=torch.int64, device=device)
+    sizes = torch.empty((n,), dtype=torch.int32, device=device)
+    ptrs = np.array(ptrs, dtype=np.uint64)
+    dims = np.array(dims, dtype=np.uint32).reshape(n, 4)
+    strides = np.array(strides, dtype=np.uint64).reshape(n, 2)
+    rc = lib().fpngb_encode_label_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
+                                                strides.ctypes.data_as(C.c_void_p), C.cast(structs, C.c_void_p), flags,
+                                                out.data_ptr(), out.numel(), offsets.data_ptr(), sizes.data_ptr(),
+                                                _stream(stream, device))
+    check(rc, "encode_labels_device")
+    return out, offsets, sizes
 
 
 def compact_packed_device(data, offsets, sizes, out=None, stream=None):

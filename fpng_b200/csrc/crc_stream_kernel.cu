@@ -71,7 +71,8 @@ static_assert(offsetof(ImageState, tiles_done) == offsetof(ImageState, crc_acc) 
 template <bool RAGGED = false, bool VERIFY = false>
 using CrcStreamParams = std::conditional_t<VERIFY, VerifyParams, std::conditional_t<RAGGED, RaggedParams<CrcParams>, CrcParams>>;
 
-// MSG_AT: the message starts at byte p.msg_start of the file (the 41-byte header of png_encode_kernels.cu: 37) instead of byte 54
+// MSG_AT (RAGGED only): the message starts at byte ImageDesc::hdr_len - 4 of the file (the files of png_encode_kernels.cu, whose
+// header is 41 bytes, or more with a label map's PLTE and tRNS) instead of byte 54
 template <bool RAGGED = false, bool VERIFY = false, bool MSG_AT = false>
 __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStreamParams<RAGGED, VERIFY> p)
 {
@@ -82,7 +83,7 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStre
     uint32_t img = blockIdx.y, bx = blockIdx.x;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     // the message is bytes [m0, L) of the 4-byte aligned buffer file_base()
-    uint32_t m0, L;
+    uint32_t m0 = kPngHeaderSize - 4u, L;                                   // the message starts at byte 54 ("IDAT")
     [[maybe_unused]] ImageState* st = nullptr;
     auto file_base = [&]() -> const uint8_t* {                               // recomputed where needed rather than kept live
         if constexpr (VERIFY) return p.d_files + p.files[img].base;
@@ -96,11 +97,11 @@ __global__ void __launch_bounds__(32 * kCs2Warps) idat_crc_stream_kernel(CrcStre
         if constexpr (RAGGED) {
             const uint32_t i = ragged_locate(p.ragged, blockIdx.x, bx);
             p.st += i; p.out += p.ragged.desc[i].out_ofs;
+            if constexpr (MSG_AT) m0 = p.ragged.desc[i].hdr_len - 4u;
             img = 0;
         }
         st = p.st + img;
         if (p.stored_only && !st->stored) return;
-        m0 = MSG_AT ? p.msg_start : kPngHeaderSize - 4u;                     // the message starts at byte 54 ("IDAT")
         L = m0 + 4u + st->zsize;                                             // end of the message (file offset)
     }
     const uint32_t w0 = m0 >> 2;                                             // first word; its bytes before m0 are masked off

@@ -126,16 +126,18 @@ __global__ void __launch_bounds__(kOffsetsThreads) row_offsets_kernel(OffsetsPar
 // ------------------------------------------------------------------------------------------------
 // K3b: Adler-32 combine.  State after row r: a' = a + S1_r, b' = b + n*a + S2_r  (mod 65521), start (1, 0).
 // ------------------------------------------------------------------------------------------------
-// ZLIB_AT: the file offset of the zlib stream (kPngEncHeaderSize for the files of png_encode_kernels.cu)
-template <bool RAGGED = false, uint32_t ZLIB_AT = kPngHeaderSize>
+// HDR_LEN (RAGGED only): the zlib stream starts at the image's ImageDesc::hdr_len (the files of png_encode_kernels.cu) instead of
+// byte 58
+template <bool RAGGED = false, bool HDR_LEN = false>
 __global__ void __launch_bounds__(kOffsetsThreads) adler_finalize_kernel(AdlerParams p)
 {
     __shared__ unsigned long long s_red[3][kOffsetsThreads / 32];
-    uint32_t img = blockIdx.x;
+    uint32_t img = blockIdx.x, zlib_at = kPngHeaderSize;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if constexpr (RAGGED) {                      // image blockIdx.x of p.desc (see row_offsets_kernel)
         const ImageDesc& d = p.desc[img];
         p.row_adler += d.row_base; p.st += img; p.out += d.out_ofs; p.w = d.w; p.h = d.h; p.chans = d.chans;
+        if constexpr (HDR_LEN) zlib_at = d.hdr_len;
         img = 0;
     }
     const uint32_t h = p.h;
@@ -158,7 +160,7 @@ __global__ void __launch_bounds__(kOffsetsThreads) adler_finalize_kernel(AdlerPa
         const unsigned long long b = (S2 % kAdlerMod + n * before) % kAdlerMod;
         const uint32_t adler = (uint32_t)((b << 16) | a);
         const ImageState st = p.st[img];
-        store_be32(p.out + (size_t)img * p.out_stride + ZLIB_AT + st.zsize - 4u, adler);
+        store_be32(p.out + (size_t)img * p.out_stride + zlib_at + st.zsize - 4u, adler);
         p.st[img].adler = adler;
     }
 }
@@ -183,7 +185,7 @@ void launch_adler_finalize_ragged(const AdlerParams& p, uint32_t n, cudaStream_t
 
 void launch_adler_finalize_png(const AdlerParams& p, uint32_t n, cudaStream_t s)
 {
-    adler_finalize_kernel<true, kPngEncHeaderSize><<<n, kOffsetsThreads, 0, s>>>(p);
+    adler_finalize_kernel<true, true><<<n, kOffsetsThreads, 0, s>>>(p);
 }
 
 void launch_adler_finalize(const AdlerParams& p, uint32_t n, cudaStream_t s)

@@ -404,7 +404,6 @@ static int encode_batch_locked(Context& c, const uint8_t* src, const Layout& L, 
 
         CrcParams cp{};
         cp.out = out; cp.out_stride = out_stride; cp.st = sp.st;
-        cp.msg_start = kPngHeaderSize - 4;
         cudaStream_t cs = s;
         if (nchunks > 1) {                                                    // this chunk's CRC goes to the side stream
             FPNGB_CUDA_OK(cudaEventRecord(c.side_ev[k], s));
@@ -576,7 +575,7 @@ static int encode_ragged_locked(Context& c, const std::vector<RaggedImage>& im, 
     RowCrcParams rp{row_crc, row_ofs, row_bits, nullptr, 0, st, d_out, 0, 0, d_desc};
     launch_row_crc_combine_ragged(rp, m, max_split, s);
     RaggedParams<CrcParams> cp{};
-    cp.out = d_out; cp.st = st; cp.msg_start = kPngHeaderSize - 4; cp.stored_only = 1u;
+    cp.out = d_out; cp.st = st; cp.stored_only = 1u;
     cp.ragged = RaggedWork{d_desc, d_lists + 3 * (size_t)m, d_lists + 4 * (size_t)m, m};
     launch_crc_stream_ragged(cp, (uint32_t)crc_ctas, s);
     count_launch(2);
@@ -613,14 +612,17 @@ static int png_class(uint32_t bpp, uint32_t depth)
     return -1;
 }
 
-// bytes of the descriptor table and work lists encode_png_locked stages for m images
-static size_t png_table_bytes(size_t m) { return align_up(m * sizeof(ImageDesc), 16) + m * 4 * 4; }
+// bytes of the descriptor table, work lists and container headers (hdr_bytes in all) encode_png_locked stages for m images
+static size_t png_table_bytes(size_t m, size_t hdr_bytes) { return align_up(m * sizeof(ImageDesc), 16) + m * 4 * 4 + hdr_bytes; }
 
 // Enqueues the PNG pipeline for images im[k] (k in `ids`, depth[k] bits per sample) into their slots.  Caller holds ctx.mu.
 // Launches: per non-empty (bytes per pixel, depth) class a filter/histogram, a row-size and a pack kernel, then four per-image
 // kernels: Huffman build, offsets, Adler-32, stream CRC.  own_call: no fpng pipeline ran in this call (a new profile call).
+// hdrs: the container header of image k is (*hdrs)[k] (a label map's, with PLTE / tRNS), or the 41-byte make_png_enc_header
+// one when hdrs is null; d_bad: the label pre-pass's per-image flags (size 0 for a flagged image), or null.
 static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, const std::vector<uint32_t>& depth, const std::vector<uint32_t>& ids,
-                             uint32_t flags, uint8_t* d_out, uint32_t* d_sizes, cudaStream_t s, uint8_t* stage, bool own_call)
+                             uint32_t flags, uint8_t* d_out, uint32_t* d_sizes, cudaStream_t s, uint8_t* stage, bool own_call,
+                             const std::vector<std::vector<uint8_t>>* hdrs = nullptr, const uint32_t* d_bad = nullptr)
 {
     const uint32_t m = (uint32_t)ids.size();
     const uint32_t rpc = png_rows_per_cta();
@@ -633,7 +635,9 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
         cls[j] = png_class(r.chans * depth[ids[j]] / 8, depth[ids[j]]);
         cls_count[cls[j]]++;
     }
-    const size_t table = png_table_bytes(m);
+    size_t hdr_bytes = 0;
+    for (uint32_t k : ids) hdr_bytes += hdrs ? (*hdrs)[k].size() : kPngEncHeaderSize;
+    const size_t table = png_table_bytes(m, hdr_bytes);
     size_t o = 0;
     const size_t o_bits = o; o = align_up(o + rows * 4, 256);
     const size_t o_ofs = o; o = align_up(o + rows * 8, 256);
@@ -653,12 +657,16 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
     p.row_filter = b + o_filt; p.st = (ImageState*)(b + o_st); p.hist = (uint32_t*)(b + o_hist);
     CodeBook* books = (CodeBook*)(b + o_books);
     const ImageDesc* d_desc = (const ImageDesc*)(b + o_table);
-    p.out = d_out; p.sizes = d_sizes; p.flags = flags; p.desc = d_desc;
+    const size_t lists_at = align_up((size_t)m * sizeof(ImageDesc), 16), hdr_at = lists_at + (size_t)m * 4 * 4;
+    p.out = d_out; p.sizes = d_sizes; p.flags = flags; p.desc = d_desc; p.headers = (const uint8_t*)d_desc + hdr_at; p.bad = d_bad;
 
-    // the table in staging: ImageDesc[m] | row-kernel img[] and CTA prefix[] per class, in class order | crc img[], crc prefix[]
+    // the table in staging: ImageDesc[m] | row-kernel img[] and CTA prefix[] per class, in class order | crc img[], crc prefix[] |
+    // the container headers
     ImageDesc* desc = (ImageDesc*)stage;
-    uint32_t* lists = (uint32_t*)(stage + align_up((size_t)m * sizeof(ImageDesc), 16));
+    uint32_t* lists = (uint32_t*)(stage + lists_at);
     uint32_t* l_img = lists; uint32_t* l_cta = lists + m; uint32_t* l_crc_img = lists + 2 * m; uint32_t* l_crc = lists + 3 * m;
+    uint8_t* headers = stage + hdr_at;
+    uint32_t hdr_fill = 0;
     uint32_t cls_first[kPngClasses], fill[kPngClasses];
     for (int k = 0, acc = 0; k < kPngClasses; k++) { cls_first[k] = fill[k] = acc; acc += cls_count[k]; }
     uint64_t cls_ctas[kPngClasses] = {0}, crc_ctas = 0;
@@ -670,17 +678,27 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
         memset(&d, 0, sizeof d);
         d.pixels = r.pixels; d.chan_stride = r.chan; d.row_base = row_base; d.out_ofs = r.slot; d.book = books + j;
         d.row_pitch = (uint32_t)r.row; d.w = r.w; d.h = r.h; d.chans = bpp; d.index = ids[j];
-        make_png_enc_header(d.png_header, r.w, r.h, r.chans, depth[ids[j]]);
+        d.hdr_at = hdr_fill;
+        if (hdrs) {
+            const std::vector<uint8_t>& hv = (*hdrs)[ids[j]];
+            memcpy(headers + hdr_fill, hv.data(), hv.size());
+            d.hdr_len = (uint32_t)hv.size();
+        } else {
+            make_png_enc_header(headers + hdr_fill, r.w, r.h, r.chans, depth[ids[j]]);
+            d.hdr_len = kPngEncHeaderSize;
+        }
+        hdr_fill += d.hdr_len;
         row_base += r.h;
         const int k = cls[j];
         const uint32_t q = fill[k]++;
         l_img[q] = j; l_cta[q] = (uint32_t)cls_ctas[k]; cls_ctas[k] += (r.h + rpc - 1) / rpc;
-        l_crc_img[j] = j; l_crc[j] = (uint32_t)crc_ctas; crc_ctas += crc_stream_ctas_for(max_encoded_size(r.w, r.h, bpp));
+        l_crc_img[j] = j; l_crc[j] = (uint32_t)crc_ctas;
+        crc_ctas += crc_stream_ctas_for(max_encoded_size(r.w, r.h, bpp) + (d.hdr_len - kPngEncHeaderSize));
     }
     for (int k = 0; k < kPngClasses; k++) if (cls_ctas[k] > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
     if (crc_ctas > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
     FPNGB_CUDA_OK(cudaMemcpyAsync((void*)d_desc, stage, table, cudaMemcpyHostToDevice, s));
-    const uint32_t* d_lists = (const uint32_t*)((const uint8_t*)d_desc + align_up((size_t)m * sizeof(ImageDesc), 16));
+    const uint32_t* d_lists = (const uint32_t*)((const uint8_t*)d_desc + lists_at);
     if (g_profile && own_call) g_prof_call++;
     ProfSet* ps = prof_begin(s);
     uint64_t launches = 0;
@@ -709,7 +727,7 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
     launch_adler_finalize_png(ap, m, s);
     prof_mark(ps, kProfAdler, s);
     RaggedParams<CrcParams> cp{};
-    cp.out = d_out; cp.st = p.st; cp.msg_start = kPngEncHeaderSize - 4; cp.stored_only = 0u;
+    cp.out = d_out; cp.st = p.st; cp.stored_only = 0u;
     cp.ragged = RaggedWork{d_desc, d_lists + 2 * (size_t)m, d_lists + 3 * (size_t)m, m};
     launch_crc_stream_png(cp, (uint32_t)crc_ctas, s);
     prof_mark(ps, kProfCrc, s);
@@ -900,7 +918,7 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
     // (typed) the conversion descriptors
     const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
     const size_t fpng_table = align_up(align_up(fpng_ids.size() * sizeof(ImageDesc), 16) + fpng_ids.size() * 5 * 4, 16);
-    const size_t conv_stage = align_up(ofs_bytes + fpng_table + png_table_bytes(png_ids.size()), 16);
+    const size_t conv_stage = align_up(ofs_bytes + fpng_table + png_table_bytes(png_ids.size(), png_ids.size() * kPngEncHeaderSize), 16);
     StageSlot* sl = nullptr;
     int rc = c.stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
     if (rc) return rc;
@@ -940,6 +958,158 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
     prof_drop_conv();
     FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
     return FPNGB_OK;
+}
+
+// ---- label maps (fpngb_encode_label_ragged_device) -------------------------------------------------------------------------
+// tRNS length of a palette: 1 + the last entry whose alpha is not 255, 0 for an RGB palette or one that is opaque throughout
+static uint32_t label_trns_len(const fpngb_label_palette* pal)
+{
+    uint32_t t = 0;
+    if (pal && pal->entries && pal->chans == 4)
+        for (uint32_t e = 0; e < pal->entries; e++) if (pal->colors[4 * e + 3] != 255) t = e + 1;
+    return t;
+}
+
+// PLTE and tRNS chunk bytes of a palette (0 for a gray map)
+static size_t label_chunk_bytes(const fpngb_label_palette* pal)
+{
+    if (!pal || !pal->entries) return 0;
+    const uint32_t t = label_trns_len(pal);
+    return 12 + 3 * (size_t)pal->entries + (t ? 12 + (size_t)t : 0);
+}
+
+// the rows the pre-pass writes: a gray8 image ceil(w * depth / 8) bytes wide, or for depth 16 a gray16 image w wide
+static uint32_t label_packed_width(uint32_t w, uint32_t depth) { return depth == 16 ? w : (uint32_t)(((uint64_t)w * depth + 7) / 8); }
+
+static size_t label_bound(uint32_t w, uint32_t h, uint32_t depth, const fpngb_label_palette* pal)
+{
+    return max_encoded_size(label_packed_width(w, depth), h, depth == 16 ? 2 : 1) + label_chunk_bytes(pal);
+}
+
+static void put_chunk(std::vector<uint8_t>& v, const char* type, const uint8_t* data, size_t len)
+{
+    const size_t at = v.size();
+    v.resize(at + 12 + len);
+    uint8_t* q = v.data() + at;
+    for (int i = 0; i < 4; i++) q[i] = (uint8_t)(len >> (24 - 8 * i));
+    memcpy(q + 4, type, 4);
+    if (len) memcpy(q + 8, data, len);
+    const uint32_t c = host_crc32(q + 4, 4 + len, 0);
+    for (int i = 0; i < 4; i++) q[8 + len + i] = (uint8_t)(c >> (24 - 8 * i));
+}
+
+// signature, IHDR (depth, color type 0 or 3), PLTE and tRNS of a palette, the IDAT length (patched on the device) and type
+static std::vector<uint8_t> make_label_header(uint32_t w, uint32_t h, uint32_t depth, const fpngb_label_palette* pal)
+{
+    uint8_t base[kPngEncHeaderSize];
+    make_png_enc_header(base, w, h, 1, depth);
+    std::vector<uint8_t> v(base, base + 8);
+    const bool palette = pal && pal->entries;
+    uint8_t ihdr[13];
+    memcpy(ihdr, base + 16, 13);
+    ihdr[9] = palette ? 3 : 0;
+    put_chunk(v, "IHDR", ihdr, 13);
+    if (palette) {
+        std::vector<uint8_t> rgb(3 * (size_t)pal->entries), alpha;
+        for (uint32_t e = 0; e < pal->entries; e++) for (int k = 0; k < 3; k++) rgb[3 * e + k] = pal->colors[pal->chans * e + k];
+        put_chunk(v, "PLTE", rgb.data(), rgb.size());
+        const uint32_t t = label_trns_len(pal);
+        for (uint32_t e = 0; e < t; e++) alpha.push_back(pal->colors[4 * e + 3]);
+        if (t) put_chunk(v, "tRNS", alpha.data(), t);
+    }
+    v.insert(v.end(), base + 33, base + kPngEncHeaderSize);
+    return v;
+}
+
+size_t fpngb_max_label_encoded_size(uint32_t w, uint32_t h, uint32_t depth, const fpngb_label_palette* pal)
+{
+    return label_bound(w, h, depth, pal);
+}
+
+// The label-map encode: call-level checks; the slots; then, in one workspace bracket, the pre-pass (label_pack_kernel) into tight
+// packed rows in c.conv and encode_png_locked on those rows with each image's own header and the pre-pass's range flags.
+int fpngb_encode_label_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                     const fpngb_label_palette* palettes, uint32_t flags, void* d_out, size_t out_cap,
+                                     uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
+{
+    if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
+    if (flags & ~(uint32_t)FPNGB_FORCE_UNCOMPRESSED) return FPNGB_ERR_INVALID_ARG;
+    if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
+    std::vector<RaggedImage> im(n);
+    std::vector<uint32_t> depth(n), ids(n);
+    std::vector<std::vector<uint8_t>> hdrs(n);
+    std::vector<LabelDesc> ld(n);
+    uint64_t total = 0, conv_bytes = 0, ctas = 0;
+    size_t hdr_bytes = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t w = dims[4 * i], h = dims[4 * i + 1], dep = dims[4 * i + 2], elem = dims[4 * i + 3];
+        const fpngb_label_palette* pal = palettes ? &palettes[i] : nullptr;
+        const uint32_t K = pal ? pal->entries : 0;
+        if (!pixels[i] || w < 1 || h < 1 || w > (1u << 24) || h > (1u << 24)) return FPNGB_ERR_INVALID_ARG;
+        if ((elem != 1 && elem != 8) || (dep != 1 && dep != 2 && dep != 4 && dep != 8 && dep != 16) || (elem == 1 && dep > 8))
+            return FPNGB_ERR_INVALID_ARG;
+        if (K && (dep == 16 || !pal->colors || (pal->chans != 3 && pal->chans != 4) || K > std::min(256u, 1u << dep)))
+            return FPNGB_ERR_INVALID_ARG;
+        const uint64_t row = strides ? strides[2 * i] : (uint64_t)w * elem, pixel = strides ? strides[2 * i + 1] : elem;
+        Layout L;
+        const int rc = check_layout((const void*)(uintptr_t)pixels[i], 0, row, pixel, elem, 1, h, w, 1, elem, false, L);
+        if (rc) return rc;
+        const size_t bound = label_bound(w, h, dep, pal);
+        if (bound > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;             // one IDAT chunk must hold the stored file
+        const uint32_t words = dep == 16 ? (w + 1) / 2 : (uint32_t)(((uint64_t)w * dep + 31) / 32);
+        ld[i] = LabelDesc{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.pixel, conv_bytes, ctas, w, h, dep,
+                          K ? K : (dep == 16 ? 65536u : 1u << dep), words, i, elem, 0u};
+        ctas += label_pack_ctas(words, h);
+        conv_bytes += align_up((uint64_t)words * 4 * h, 16);
+        im[i] = RaggedImage{nullptr, (uint64_t)words * 4, 0, label_packed_width(w, dep), h, 1, total};
+        depth[i] = dep == 16 ? 16 : 8;
+        ids[i] = i;
+        hdrs[i] = make_label_header(w, h, dep, pal);
+        hdr_bytes += hdrs[i].size();
+        total += align_up(bound, 16);
+    }
+    if (ctas > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
+    if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
+    if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
+    Context& c = g_ctx;
+    std::lock_guard<std::mutex> lk(c.mu);
+    FPNGB_CUDA_OK(cudaSetDevice(c.device));
+    cudaStream_t s = (cudaStream_t)stream;
+
+    // conversion buffer: the packed rows, then the pre-pass descriptors, then the per-image range flags
+    const uint64_t desc_at = align_up(conv_bytes, 256), bad_at = align_up(desc_at + (uint64_t)n * sizeof(LabelDesc), 256);
+    int rc = c.conv.reserve(bad_at + (size_t)n * 4);
+    if (rc) return rc;
+    uint8_t* cb = (uint8_t*)c.conv.p;
+    // staging: d_out_offsets (n + 1), the PNG table, the pre-pass descriptors
+    const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
+    const size_t ld_stage = align_up(ofs_bytes + png_table_bytes(n, hdr_bytes), 16);
+    StageSlot* sl = nullptr;
+    rc = c.stage_slot(ld_stage + (size_t)n * sizeof(LabelDesc), &sl);
+    if (rc) return rc;
+    uint8_t* stage = (uint8_t*)sl->buf.p;
+    uint64_t* h_ofs = (uint64_t*)stage;
+    for (uint32_t i = 0; i < n; i++) { h_ofs[i] = im[i].slot; im[i].pixels = cb + ld[i].dst; }
+    h_ofs[n] = total;
+    memcpy(stage + ld_stage, ld.data(), (size_t)n * sizeof(LabelDesc));
+    FPNGB_CUDA_OK(cudaMemcpyAsync(d_out_offsets, h_ofs, (size_t)(n + 1) * 8, cudaMemcpyHostToDevice, s));
+    rc = c.ws_acquire(s);
+    if (rc) return rc;
+    FPNGB_CUDA_OK(cudaMemcpyAsync(cb + desc_at, stage + ld_stage, (size_t)n * sizeof(LabelDesc), cudaMemcpyHostToDevice, s));
+    uint32_t* d_bad = (uint32_t*)(cb + bad_at);
+    FPNGB_CUDA_OK(cudaMemsetAsync(d_bad, 0, (size_t)n * 4, s));
+    LabelPackParams lp{(const LabelDesc*)(cb + desc_at), n, cb, d_bad};
+    prof_drop_conv();
+    ProfSet* ps = g_profile ? prof_alloc() : nullptr;                      // slot kProfConvert of the encode that follows
+    if (ps) cudaEventRecord(ps->conv_start, s);
+    launch_label_pack(lp, ctas, s);
+    count_launch(1);
+    if (ps) { prof_mark(ps, kProfConvert, s); g_prof_conv = ps; }
+    rc = encode_png_locked(c, im, depth, ids, flags, (uint8_t*)d_out, d_sizes, s, stage + ofs_bytes, true, &hdrs, d_bad);
+    prof_drop_conv();
+    if (rc) c.ws_release(s);                                                // later calls still wait for the pre-pass
+    FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
+    return rc;
 }
 
 int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, uint32_t flags,

@@ -20,7 +20,9 @@ struct ImageDesc {
     uint32_t lane_pitch;                          // lane records per scanline: 32 * ceil(w / 512)
     uint32_t index;                               // the image's index in the call (its d_sizes entry)
     uint8_t png_header[kPngHeaderSize];
-    uint8_t pad_[6];
+    uint8_t pad_[2];
+    uint32_t hdr_len;                             // PNG call: container header bytes L (41, or 41 + PLTE / tRNS for a label map),
+    uint32_t hdr_at;                              // staged at PngEncParams::headers + hdr_at; the zlib stream starts at file byte L
 };
 
 // The images one ragged launch covers: CTA b works on image img[j] for the j with cta_start[j] <= b < cta_start[j + 1] (every
@@ -108,7 +110,6 @@ struct AdlerParams {
 struct CrcParams {
     uint8_t* out; size_t out_stride;
     ImageState* st;
-    uint32_t msg_start;                           // first byte of the CRC'd region (54 = "IDAT" for a PNG file)
     uint32_t stored_only;                         // only images that fell back to stored blocks (the single-pass encoder computed the others' CRC inline)
 };
 
@@ -125,9 +126,10 @@ struct HuffParams {
     const ImageDesc* desc;                        // ragged kernel: the channel count of image blockIdx.x
 };
 
-// fpngb_encode_png_ragged_device (png_encode_kernels.cu): the images are ImageDesc entries whose chans is B, the bytes per pixel,
-// whose png_header holds the 41-byte container header (the sample depth at byte 24), and whose chan_stride is the plane stride of
-// a planar image (0: interleaved).  One block of parameters for every kernel of the pipeline.
+// fpngb_encode_png_ragged_device and fpngb_encode_label_ragged_device (png_encode_kernels.cu): the images are ImageDesc entries
+// whose chans is B, the bytes per pixel, whose hdr_len / hdr_at locate the container header in `headers` (signature, IHDR, a label
+// map's PLTE and tRNS, the IDAT length and type), and whose chan_stride is the plane stride of a planar image (0: interleaved).
+// One block of parameters for every kernel of the pipeline.
 struct PngEncParams {
     ImageState* st;                               // [m]
     uint32_t* hist;                               // [m * 288]
@@ -137,6 +139,8 @@ struct PngEncParams {
     uint2* row_adler;                             // [rows] (S1, S2) of the scanline as written
     uint8_t* out; uint32_t* sizes; uint32_t flags;
     const ImageDesc* desc;                        // the images (offsets kernel: image blockIdx.x)
+    const uint8_t* headers;                       // the images' container headers (ImageDesc::hdr_at, hdr_len)
+    const uint32_t* bad;                          // [call images] nonzero: a label map with an out-of-range id, size 0 (nullptr: none)
     RaggedWork ragged;                            // the images and CTA map of a row-kernel launch
 };
 uint32_t png_rows_per_cta();
@@ -168,7 +172,7 @@ int crc_stream_table_ptrs(const uint32_t** f128b, const uint32_t** lane_mul);
 uint32_t crc_stream_ctas_for(size_t max_file_bytes);     // CTAs of the stream CRC kernel for a file of at most that many bytes
 uint32_t row_crc_split_for(uint32_t h);                   // CTAs of the scanline-CRC combine for an image of h scanlines
 void launch_crc_stream_ragged(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s);
-void launch_crc_stream_png(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s);   // message from p.msg_start
+void launch_crc_stream_png(const RaggedParams<CrcParams>& p, uint32_t total_ctas, cudaStream_t s);   // message from ImageDesc::hdr_len - 4
 void launch_row_crc_combine_ragged(const RowCrcParams& p, uint32_t n, uint32_t max_split, cudaStream_t s);
 void launch_offsets_ragged(const OffsetsParams& p, uint32_t n, cudaStream_t s);
 void launch_adler_finalize_ragged(const AdlerParams& p, uint32_t n, cudaStream_t s);
@@ -210,6 +214,29 @@ uint32_t convert_ctas_per_image(uint32_t w, uint32_t h);
 // dtype: an FPNGB_DTYPE_* value, or 0 for the uint8 copy (kConvInterleaved or kConvPlanar only).  png: the typed PNG call's
 // instantiations (a float dtype; 1 to 4 channels and sample_bytes 1 or 2 per descriptor), else 3 or 4 channels of uint8 output.
 void launch_convert_pixels(const ConvertParams& p, uint32_t dtype, int layout, bool png, cudaStream_t s);
+
+// Label-map pre-pass (label_pack_kernels.cu): image i's w x h ids (uint8 or int64, `elem` bytes each) at src + y*row + x*pixel bytes are
+// range-checked against limit (2^depth for gray, the palette size K for a palette) and packed into rows of `pitch` bytes (a
+// multiple of 4) at dst: depth < 16 MSB-first, ceil(w*depth/8) bytes per row, the unused low bits zero; depth 16 native little-endian
+// uint16.  An id out of range sets bad[index].  One launch over every image of the call; descriptors ascend in cta_start.
+struct LabelDesc {
+    const uint8_t* src;
+    unsigned long long row, pixel;                // byte strides of the ids
+    unsigned long long dst;                       // byte offset of the packed rows in LabelPackParams::dst
+    unsigned long long cta_start;                 // first CTA of the image in the launch
+    uint32_t w, h, depth, limit;
+    uint32_t words;                               // 32-bit output words per row: ceil(w * depth / 32)
+    uint32_t index;                               // the image's index in the call (its bad flag)
+    uint32_t elem;                                // bytes per id: 1 (uint8) or 8 (int64)
+    uint32_t pad_;
+};
+struct LabelPackParams {
+    const LabelDesc* desc; uint32_t count;
+    uint8_t* dst;
+    uint32_t* bad;
+};
+uint32_t label_pack_ctas(uint32_t words, uint32_t h);
+void launch_label_pack(const LabelPackParams& p, unsigned long long total_ctas, cudaStream_t s);
 
 bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans);
 void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);

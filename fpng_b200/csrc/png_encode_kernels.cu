@@ -8,7 +8,8 @@
 //   png_row_kernel<B, ES, kPngBits>  per row: the row's code bits under the image's book
 //   png_offsets_kernel               per image: exclusive scan of the row bits, compressed-vs-stored decision, container, IEND
 //   png_row_kernel<B, ES, kPngPack>  per row: the codes at the row's bit offset (or the raw row of a stored file), row Adler
-//   adler_finalize_kernel / idat_crc_stream_kernel (the fpng kernels at the 41-byte header of these files)
+//   adler_finalize_kernel / idat_crc_stream_kernel (the fpng kernels at each file's header length L: 41 bytes, or more for a label
+//                                    map's PLTE and tRNS)
 //
 // A row is one warp's: lanes take consecutive pixels, 32 per step.  Runs of equal filtered pixels are found with a ballot of the
 // pixels that differ from their left neighbour, carried across steps; every token is written by the lane of the pixel it ends on
@@ -188,7 +189,7 @@ __global__ void __launch_bounds__(32 * kPngRows) png_row_kernel(PngEncParams p)
                 const unsigned long long x = i / B, j = i - x * B, c = j / ES;
                 return __ldg(row + x * ps + c * cs + (ES == 2 ? 1u - (uint32_t)(j & 1u) : 0u));
             };
-            store_row_raw(at, file + kPngEncHeaderSize, y, bpl, lane, &p.row_adler[r]);
+            store_row_raw(at, file + d.hdr_len, y, bpl, lane, &p.row_adler[r]);
             return;
         }
 
@@ -306,16 +307,17 @@ __device__ __forceinline__ void store_be32_png(uint8_t* q, uint32_t v)
 }
 
 // Image blockIdx.x of p.desc: row bit offsets, the compressed-vs-stored decision (stored iff FPNGB_FORCE_UNCOMPRESSED or the
-// compressed zlib stream would be longer), the 41-byte container header with the IDAT length, the zlib and block headers, the
-// stored block headers or the end-of-block code, the IEND chunk and the file size.  Zeroes the words neighbouring rows share.
+// compressed zlib stream would be longer), the L-byte container header (L = hdr_len) with the IDAT length at L - 8, the zlib and
+// block headers, the stored block headers or the end-of-block code, the IEND chunk and the file size (0 for a label map with an
+// out-of-range id: the file is written in its slot all the same, and read by nothing).  Zeroes the words neighbouring rows share.
 __global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncParams p)
 {
     __shared__ unsigned long long s_warp[kOffsetsThreads / 32];
     const uint32_t img = blockIdx.x, tid = threadIdx.x;
     const ImageDesc& d = p.desc[img];
     const CodeBook* book = d.book;
-    const uint32_t h = d.h, hdr_bits = book->hdr_bits;
-    const unsigned long long base = 8ull * kPngEncHeaderSize + hdr_bits;
+    const uint32_t h = d.h, hdr_bits = book->hdr_bits, L = d.hdr_len;
+    const unsigned long long base = 8ull * L + hdr_bits;
     const uint32_t* row_bits = p.row_bits + d.row_base;
     unsigned long long* row_ofs = p.row_ofs + d.row_base;
     uint8_t* file = p.out + d.out_ofs;
@@ -344,17 +346,18 @@ __global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncPara
     }
     __syncthreads();
     const uint32_t hbytes = compressed ? (hdr_bits + 7u) >> 3 : 2u;
-    const uint32_t hend = compressed ? 4u * ((uint32_t)(base >> 5) + 1u) : kPngEncHeaderSize + 2u;
+    const uint32_t hend = compressed ? 4u * ((uint32_t)(base >> 5) + 1u) : L + 2u;
+    const uint8_t* hdr = p.headers + d.hdr_at;
     for (uint32_t i = tid; i < hend; i += blockDim.x) {
         uint8_t v = 0;
-        if (i < kPngEncHeaderSize) v = d.png_header[i];
-        else if (i - kPngEncHeaderSize < hbytes) v = compressed ? book->hdr[i - kPngEncHeaderSize] : (i == kPngEncHeaderSize ? 0x78 : 0x01);
-        if (i >= 33 && i < 37) v = (uint8_t)(zsize >> (8 * (36 - i)));
+        if (i < L) v = hdr[i];
+        else if (i - L < hbytes) v = compressed ? book->hdr[i - L] : (i == L ? 0x78 : 0x01);
+        if (i >= L - 8u && i < L - 4u) v = (uint8_t)(zsize >> (8 * (L - 5u - i)));
         file[i] = v;
     }
     if (!compressed) {
         for (unsigned long long j = tid; j < nblk; j += blockDim.x) {
-            uint8_t* b = file + kPngEncHeaderSize + 2ull + j * 65540ull;
+            uint8_t* b = file + L + 2ull + j * 65540ull;
             const unsigned long long remaining = raw - j * 65535ull;
             const uint32_t len = remaining < 65535ull ? (uint32_t)remaining : 65535u;
             b[0] = (j + 1 == nblk) ? 1 : 0;
@@ -371,7 +374,7 @@ __global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncPara
             for (int i = 0; i < 3; i++) { const uint8_t b = (uint8_t)(v >> (8 * i)); if (b) q[i] |= b; }
         }
         static const uint8_t iend[12] = { 0, 0, 0, 0, 'I', 'E', 'N', 'D', 0xAE, 0x42, 0x60, 0x82 };
-        uint8_t* t = file + kPngEncHeaderSize + zsize;
+        uint8_t* t = file + L + zsize;
         store_be32_png(t, 0u);
         for (int i = 0; i < 12; i++) t[4 + i] = iend[i];
         st->zsize = zsize;
@@ -379,7 +382,7 @@ __global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncPara
         st->crc_acc = 0u;
         st->tiles_done = 0u;
         st->status = 0u;
-        p.sizes[d.index] = kPngEncHeaderSize + zsize + kPngTrailerSize;
+        p.sizes[d.index] = (p.bad && p.bad[d.index]) ? 0u : L + zsize + kPngTrailerSize;
     }
 }
 

@@ -149,6 +149,42 @@ FPNGB_API int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels,
                                              uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes,
                                              void* stream);
 
+/* fpngb_encode_label_ragged_device: encodes n label maps (segmentation class ids, masks) in device memory to palette or gray PNGs
+ *   in one call, into the packed layout of fpngb_encode_ragged_device.  Image i is a w x h map of ids v, one of two kinds:
+ *     gray     (color type 0) at depth d in {1, 2, 4, 8, 16}; valid ids are 0 <= v < 2^d;
+ *     palette  (color type 3) at depth d in {1, 2, 4, 8} with K entries, 1 <= K <= min(256, 2^d); valid ids are 0 <= v < K.
+ *     pixels   HOST array of n device addresses
+ *     dims     HOST array of n x {w, h, depth, elem}: elem 1 (uint8 ids, depth <= 8) or 8 (int64 ids, e.g. argmax output)
+ *     strides  HOST array of n x {row_pitch, pixel_stride} in bytes, or NULL for tight rows (w * elem, elem): the layouts of
+ *              "Pixel layouts" above with one channel (any row pitch, stride-0 rows included; 64-bit addressing)
+ *     palettes HOST array of n fpngb_label_palette, or NULL: all gray.  entries = 0 means gray; otherwise colors holds entries x
+ *              chans bytes in host memory, chans 3 (RGB) or 4 (RGBA).
+ *   The file: signature, IHDR (w, h, d, color type, 0, 0, no interlace); for a palette PLTE (K x RGB), then tRNS holding the
+ *   alphas of entries 0 .. t-1, t = 1 + the last entry whose alpha is not 255 (no tRNS for an RGB or fully opaque palette); one
+ *   IDAT; IEND.  Row bytes: for d < 16 ceil(w*d/8) bytes per row, ids packed MSB-first, the unused low bits of the last byte zero;
+ *   for d = 16 big-endian samples.  These rows are encoded exactly as fpngb_encode_png_ragged_device encodes a gray8 image
+ *   ceil(w*d/8) pixels wide (a gray16 image for d = 16): filter choice, matches at distance 1 (2), fpng's 2-pass code, the stored
+ *   fallback and FPNGB_FORCE_UNCOMPRESSED.  So gray d = 8 from uint8 ids and gray d = 16 from int64 ids give the files
+ *   fpngb_encode_png_ragged_device writes for the same uint8 / uint16 image, byte for byte.  DESIGN.md §4.6 "Label maps".
+ *   Range check: an image with an id out of range (a negative int64 included) gets d_sizes[i] = 0; nothing outside its slot is
+ *   written and every other image of the call is as without it.  The decoders take a size of 0 as FPNGB_DECODE_INVALID_ARG.
+ *   Output slots: the exclusive prefix of align_up(fpngb_max_label_encoded_size(w_i, h_i, d_i, palette_i), 16) in d_out_offsets
+ *   (n + 1 entries, the last the total); d_sizes[i] the file size.  No byte of d_out past the total is written.
+ *   Call-level checks, before anything is enqueued: FPNGB_ERR_INVALID_ARG for flags other than 0 / FPNGB_FORCE_UNCOMPRESSED,
+ *   n outside 1..65535, a NULL pointer, w or h outside 1..2^24, a bad depth, elem, palette size or chans, a palette at depth 16,
+ *   an unsupported layout or a slot bound above 2^31 - 1; FPNGB_ERR_BUFFER_TOO_SMALL when out_cap is below the total;
+ *   FPNGB_ERR_ALIGNMENT unless d_out % 16 == 0 and each image's address and strides are multiples of elem.  A rejected call
+ *   enqueues nothing and writes nothing.  Stream-ordered, no host synchronisation.
+ *   Launches: one pre-pass over every image (label_pack_kernel: reads each id once, checks it and writes the packed rows;
+ *   fpngb_profile_read slot 9), then the PNG pipeline of fpngb_encode_png_ragged_device on the packed rows. */
+typedef struct { const uint8_t* colors; uint32_t entries; uint32_t chans; } fpngb_label_palette;
+/* the slot bound: the bound of the packed rows (fpngb_max_encoded_size(ceil(w*d/8), h, 1), or (w, h, 2) for d = 16) plus the
+ * PLTE and tRNS chunk bytes of pal (NULL or entries = 0: gray) */
+FPNGB_API size_t fpngb_max_label_encoded_size(uint32_t w, uint32_t h, uint32_t depth, const fpngb_label_palette* pal);
+FPNGB_API int fpngb_encode_label_ragged_device(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
+                                               const fpngb_label_palette* palettes, uint32_t flags, void* d_out, size_t out_cap,
+                                               uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
+
 /* Batch of n equally sized images in HOST memory (ideally pinned: see fpngb_host_alloc) -> n files in host memory,
  * out + i*out_stride, sizes[i].  Internally pipelines H2D copy / kernels / D2H copy over chunks of the batch. */
 FPNGB_API int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
