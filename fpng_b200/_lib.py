@@ -104,6 +104,10 @@ def lib() -> C.CDLL:
     L.fpngb_decode_packed_resized_device.restype = C.c_int
     L.fpngb_decode_packed_resized_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p] + [C.c_uint32] * 4 + \
         [C.c_size_t, C.c_void_p] + [C.c_uint32] * 4 + [C.POINTER(PixelFormat), C.c_void_p] + [C.c_size_t] * 4 + [C.c_void_p] * 3
+    L.fpngb_decode_packed_views_device.restype = C.c_int
+    L.fpngb_decode_packed_views_device.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p] + [C.c_uint32] * 4 + \
+        [C.c_size_t, C.c_void_p] + [C.c_uint32] * 5 + [C.POINTER(PixelFormat), C.POINTER(C.c_uint32), C.c_void_p] + [C.c_size_t] * 4 + \
+        [C.c_void_p] * 4
     L.fpngb_encode_batch_device_typed.restype = C.c_int
     L.fpngb_encode_batch_device_typed.argtypes = [C.c_void_p] + [C.c_size_t] * 4 + [C.c_uint32] * 4 + [C.POINTER(PixelFormat), C.c_uint32,
                                                                                                    C.c_void_p, C.c_size_t, C.c_void_p,

@@ -919,6 +919,9 @@ FPNGB_RESIZE_NATIVE = 16
 FPNGB_RESIZE_NEAREST = 32            # interpolation="nearest": F.interpolate(mode="nearest")
 FPNGB_RESIZE_NEAREST_EXACT = 64      # interpolation="nearest-exact": F.interpolate(mode="nearest-exact")
 FPNGB_RESIZE_INDEX = 128             # indices=True in the resized call
+FPNGB_VIEW_HFLIP = 1                 # decode_packed_views_device: view row flag, flip after the resize (torch.flip(dims=[-1]))
+FPNGB_VIEW_VFLIP = 2                 # the same for rows
+FPNGB_DECODE_BAD_VIEW = 106          # decode_packed_views_device only: a view row names no file, or has a bad size, offset or flag
 _INTERPOLATION = {"bilinear": 0, "nearest": FPNGB_RESIZE_NEAREST, "nearest-exact": FPNGB_RESIZE_NEAREST_EXACT}
 
 
@@ -952,35 +955,79 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     at the source pixel, so at identity size the result is the ragged decode cropped to the box.  antialias applies to bilinear only.
     indices=True (FPNGB_RESIZE_INDEX) takes decode_packed_ragged_device's indices rule and needs a nearest mode as well; pixel_cap
     then counts align_up(w*h*element_size, 16) bytes per file."""
+    out, info, status, _ = _resized_call("decode_packed_resized_device", data, offsets, sizes, size, desired_channels, boxes, None, None,
+                                         antialias, out, dtype, scale, bias, max_file_size, max_w, max_h, pixel_cap, stream, any_png,
+                                         all_formats, native, interpolation, indices)
+    return out, info, status
+
+
+def decode_packed_views_device(data, offsets, sizes, views, size, desired_channels: int, fill=None, antialias=True, out=None, dtype=None,
+                               scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None,
+                               any_png=False, all_formats=False, native=False, interpolation="bilinear", indices=False):
+    """Decode the packed files of decode_packed_resized_device once and write any number of output images from them: a "view" here
+    is one output image (not one of ragged_views' per-file tensors), a crop of a file resized to its own size, optionally flipped,
+    and placed on a fixed canvas size = (H, W) holding a fill value elsewhere (fpngb_decode_packed_views_device in
+    include/fpng_b200.h).  Returns (out [m, H, W, desired_channels], info int32 [n, 6], status int32 [n], view_status int32 [m]).
+      * views: a contiguous int32 CUDA tensor [m, 10], 1 <= m <= 65535; row v = (file, top, left, height, width, resize_h,
+        resize_w, offset_y, offset_x, flags), flags FPNGB_VIEW_HFLIP | FPNGB_VIEW_VFLIP.  View v is, bit for bit, what
+        decode_packed_resized_device stores for that file with that box at size (resize_h, resize_w), then torch.flip for the
+        flags, pasted at (offset_y, offset_x) (negative offsets and offsets past the canvas clip) onto a canvas of the fill.  A
+        file may have any number of views, or none; resize_crop_views and letterbox_views build common tables, and flips or
+        several views per file are plain torch ops on the table (views[:, 9] |= mask, torch.cat);
+      * fill: None (zeros), one value or one per channel: a source value of the call, stored as the call stores one (uint8 as it
+        is, float fill * scale + bias, native a 16-bit value, indices the raw id, e.g. 255 for "ignore"); 0..255, or 0..65535 in
+        native calls and indices=True into uint16;
+      * status[i] is decode_packed_ragged_device's code for file i (no box is checked per file); view_status[v] is
+        FPNGB_DECODE_BAD_VIEW for a file outside 0..n-1, else the file's status, else FPNGB_DECODE_BAD_CROP for a box that is
+        empty or not inside the image, else FPNGB_DECODE_BAD_VIEW for a resize size outside 1..2^24, an offset beyond +-2^24 or
+        an unknown flag, else 0.  The output image of a view whose status is not 0 is left untouched;
+      * out: any non-overlapping [m, H, W, C] view in the layouts of layout_strides (NCHW included).
+    Every other argument is decode_packed_resized_device's, with the same rules: interpolation, antialias, indices, native,
+    any_png, all_formats, dtype, scale and bias; pixel_cap and the bounds as there (all given: stream-ordered, no host
+    synchronisation)."""
+    return _resized_call("decode_packed_views_device", data, offsets, sizes, size, desired_channels, None, views, fill, antialias, out,
+                         dtype, scale, bias, max_file_size, max_w, max_h, pixel_cap, stream, any_png, all_formats, native,
+                         interpolation, indices)
+
+
+def _resized_call(fn, data, offsets, sizes, size, desired_channels, boxes, views, fill, antialias, out, dtype, scale, bias,
+                  max_file_size, max_w, max_h, pixel_cap, stream, any_png, all_formats, native, interpolation, indices):
+    """The argument checks and the library call of decode_packed_resized_device (views None) and decode_packed_views_device"""
     import torch
 
-    _all_formats_check(any_png, all_formats, "decode_packed_resized_device", native)
+    _all_formats_check(any_png, all_formats, fn, native)
     if interpolation not in _INTERPOLATION:
-        raise ValueError(f"decode_packed_resized_device: interpolation {interpolation!r}: 'bilinear', 'nearest' or 'nearest-exact'")
+        raise ValueError(f"{fn}: interpolation {interpolation!r}: 'bilinear', 'nearest' or 'nearest-exact'")
     if indices and interpolation == "bilinear":
-        raise ValueError("decode_packed_resized_device: indices=True needs interpolation 'nearest' or 'nearest-exact'")
+        raise ValueError(f"{fn}: indices=True needs interpolation 'nearest' or 'nearest-exact'")
     if desired_channels not in ((1, 2, 3, 4) if native else (3, 4)):
-        raise ValueError(f"decode_packed_resized_device: desired_channels {desired_channels}: " + ("1 .. 4" if native else "3 or 4"))
+        raise ValueError(f"{fn}: desired_channels {desired_channels}: " + ("1 .. 4" if native else "3 or 4"))
     H, W = (int(v) for v in size)
     if not (1 <= H <= 1 << 24 and 1 <= W <= 1 << 24):
-        raise ValueError(f"decode_packed_resized_device: size {tuple(size)}: each side in 1 .. 2^24")
+        raise ValueError(f"{fn}: size {tuple(size)}: each side in 1 .. 2^24")
     odt = _out_dtype(out, dtype)
-    _indices_check(indices, any_png, all_formats, native, desired_channels, odt, "decode_packed_resized_device")
+    _indices_check(indices, any_png, all_formats, native, desired_channels, odt, fn)
     if native:
-        fmt = _native_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
+        fmt = _native_format(odt, scale, bias, desired_channels, fn)
     else:
-        fmt = _pixel_format(odt, scale, bias, desired_channels, "decode_packed_resized_device")
+        fmt = _pixel_format(odt, scale, bias, desired_channels, fn)
     if boxes is not None:
         if not isinstance(boxes, torch.Tensor) or not boxes.is_cuda or boxes.device != data.device:
             raise ValueError(f"boxes: a CUDA tensor on {data.device} is needed")
         n = sizes.shape[0]
         if boxes.dtype != torch.int32 or tuple(boxes.shape) != (n, 4) or not boxes.is_contiguous():
             raise ValueError(f"boxes: dtype {boxes.dtype}, shape {tuple(boxes.shape)}: a contiguous int32 [{n}, 4] tensor is needed")
+    fill_arg = None
+    if views is not None or fn == "decode_packed_views_device":
+        fill_arg = _view_args(fn, views, fill, desired_channels, native and (not indices or odt == torch.uint16))
+        if not views.is_cuda or data is None or views.device != data.device:
+            raise ValueError(f"{fn}: views: a CUDA tensor on the device of data is needed")
     n = _packed_args(data, offsets, sizes)
-    shape = (n, H, W, desired_channels)
+    m = n if views is None else int(views.shape[0])
+    shape = (m, H, W, desired_channels)
     if out is None:
         out = torch.empty(shape, dtype=odt, device=data.device)
-    _check_arg(out, "out", data.device, odt, n * H * W * desired_channels, view=True)
+    _check_arg(out, "out", data.device, odt, m * H * W * desired_channels, view=True)
     if max_file_size is None or max_w is None or max_h is None or pixel_cap is None:
         max_file_size, max_w, max_h, total = _ragged_bounds(data, offsets, sizes, n, desired_channels, max_file_size, max_w, max_h,
                                                              stream, odt.itemsize if indices else 2 if native else 1, any_png=any_png,
@@ -989,16 +1036,110 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
             pixel_cap = total
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
     status = torch.empty((n,), dtype=torch.int32, device=data.device)
-    rc = lib().fpngb_decode_packed_resized_device(
-        data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
-        int(max_h), int(pixel_cap), None if boxes is None else boxes.data_ptr(), W, H, desired_channels,
-        (FPNGB_RESIZE_ANTIALIAS if antialias and interpolation == "bilinear" else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
-        (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0) | (FPNGB_RESIZE_NATIVE if native else 0) |
-        _INTERPOLATION[interpolation] | (FPNGB_RESIZE_INDEX if indices else 0),
-        None if fmt is None else C.byref(fmt), out.data_ptr(), *_layout(out, shape, (1, 2, 3, 4) if native else (3, 4)),
-        info.data_ptr(), status.data_ptr(), _stream(stream, data.device))
-    check(rc, "decode_packed_resized_device")
-    return out, info, status
+    flags = ((FPNGB_RESIZE_ANTIALIAS if antialias and interpolation == "bilinear" else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
+             (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0) | (FPNGB_RESIZE_NATIVE if native else 0) |
+             _INTERPOLATION[interpolation] | (FPNGB_RESIZE_INDEX if indices else 0))
+    head = (data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),
+            int(max_h), int(pixel_cap))
+    tail = (out.data_ptr(), *_layout(out, shape, (1, 2, 3, 4) if native else (3, 4)), info.data_ptr(), status.data_ptr())
+    fmt_arg = None if fmt is None else C.byref(fmt)
+    if views is None:
+        rc = lib().fpngb_decode_packed_resized_device(*head, None if boxes is None else boxes.data_ptr(), W, H, desired_channels, flags,
+                                                      fmt_arg, *tail, _stream(stream, data.device))
+        view_status = None
+    else:
+        view_status = torch.empty((m,), dtype=torch.int32, device=data.device)
+        rc = lib().fpngb_decode_packed_views_device(*head, views.data_ptr(), m, W, H, desired_channels, flags, fmt_arg, fill_arg, *tail,
+                                                    view_status.data_ptr(), _stream(stream, data.device))
+    check(rc, fn)
+    return out, info, status, view_status
+
+
+def _view_args(fn, views, fill, desired_channels, wide):
+    """ValueError unless views is a contiguous int32 tensor [m, 10] with 1 <= m <= 65535 and fill None, one value or one per channel,
+    each in 0..255 (0..65535 when wide: the call's source elements are uint16); returns fill as the C call takes it"""
+    import torch
+
+    if not isinstance(views, torch.Tensor) or views.dtype != torch.int32 or views.dim() != 2 or views.shape[1] != 10 or \
+            not views.is_contiguous() or not 1 <= views.shape[0] <= 65535:
+        what = f"dtype {views.dtype}, shape {tuple(views.shape)}" if isinstance(views, torch.Tensor) else type(views).__name__
+        raise ValueError(f"{fn}: views: {what}: a contiguous int32 [m, 10] tensor with 1 <= m <= 65535 is needed")
+    if fill is None:
+        return None
+    a = np.asarray(fill.detach().cpu().numpy() if hasattr(fill, "detach") else fill).reshape(-1)
+    if a.size == 1:
+        a = np.repeat(a, desired_channels)
+    top = 65535 if wide else 255
+    if a.size != desired_channels or not np.issubdtype(a.dtype, np.integer) or (a < 0).any() or (a > top).any():
+        raise ValueError(f"{fn}: fill {fill!r}: one integer or one per channel ({desired_channels}), each in 0..{top}")
+    return (C.c_uint32 * desired_channels)(*(int(v) for v in a))
+
+
+def _views_table(info, rh, rw, oy, ox, h, w):
+    """int32 [n, 10] rows (i, 0, 0, h, w, rh, rw, oy, ox, 0) from [n] int64 tensors"""
+    import torch
+
+    n = info.shape[0]
+    i = torch.arange(n, device=info.device, dtype=torch.int64)
+    z = torch.zeros_like(i)
+    return torch.stack([i, z, z, h, w, rh, rw, oy, ox, z], 1).to(torch.int32).contiguous()
+
+
+def resize_crop_views(info, resize, crop, max_size=None):
+    """View table [n, 10] (decode_packed_views_device) of torchvision v2's Resize(resize, max_size=max_size) followed by
+    CenterCrop(crop), for the files of info (get_info_batch_device's [n, 6]); use it with size = crop.  Each row is file i's whole
+    image resized to (rh, rw) and placed at (oy, ox), flags 0: torch ops on the device, no host synchronisation.
+      * resize: an int (the shorter side becomes resize, the longer int(resize * long / short) in float64; with max_size, when the
+        longer side would pass max_size, it becomes max_size and the shorter int(max_size * short / long)) or (h, w);
+      * crop: an int or (h, w).  Per axis the offset is -round((size - crop) / 2), half to even, when the crop fits and
+        +(crop - size) // 2 when it does not (torchvision pads with zeros: the fill).
+    Rows of files with w = h = 0 (a failed walk) hold anything: those views get the file's status first."""
+    import torch
+
+    ch, cw = (crop, crop) if isinstance(crop, int) else (int(crop[0]), int(crop[1]))
+    h = info[:, 2].to(torch.int64)
+    w = info[:, 1].to(torch.int64)
+    if isinstance(resize, int):
+        hf, wf = h.double(), w.double()
+        short, long_ = torch.minimum(hf, wf), torch.maximum(hf, wf)
+        new_short = torch.full_like(hf, float(resize))
+        new_long = torch.floor(resize * long_ / short.clamp(min=1))
+        if max_size is not None:
+            over = new_long > max_size
+            new_short = torch.where(over, torch.floor(max_size * new_short / new_long.clamp(min=1)), new_short)
+            new_long = torch.where(over, torch.full_like(new_long, float(max_size)), new_long)
+        rh = torch.where(hf <= wf, new_short, new_long).to(torch.int64)
+        rw = torch.where(hf <= wf, new_long, new_short).to(torch.int64)
+    else:
+        if max_size is not None:
+            raise ValueError("resize_crop_views: max_size applies to an int resize only (torchvision's rule)")
+        rh = torch.full_like(h, int(resize[0]))
+        rw = torch.full_like(w, int(resize[1]))
+
+    def offset(size, c):
+        fits = torch.round((size - c).double() / 2).to(torch.int64)     # torch.round: half to even, as Python's round
+        return torch.where(size >= c, -fits, torch.div(c - size, 2, rounding_mode="floor"))
+
+    return _views_table(info, rh, rw, offset(rh, ch), offset(rw, cw), h, w)
+
+
+def letterbox_views(info, size):
+    """View table [n, 10] (decode_packed_views_device) of the usual detection letterbox into a canvas size = (H, W): r = min(H / h,
+    W / w) in float64, the whole image resized to rw, rh = round(w * r), round(h * r) (half to even, at least 1) and placed at
+    round((canvas - resized) / 2 - 0.1) per axis, flags 0; pass the pad colour as fill.  The geometry is YOLO's; the resample is
+    this library's (torch's bilinear rule with antialias as the call sets it), not OpenCV's cv2.resize, so pixels differ from an
+    OpenCV pipeline.  Torch ops on the device, no host synchronisation; rows of files with w = h = 0 hold anything."""
+    import torch
+
+    H, W = (int(v) for v in size)
+    h = info[:, 2].to(torch.int64)
+    w = info[:, 1].to(torch.int64)
+    r = torch.minimum(H / h.double().clamp(min=1), W / w.double().clamp(min=1))
+    rh = torch.round(h.double() * r).clamp(min=1).to(torch.int64)
+    rw = torch.round(w.double() * r).clamp(min=1).to(torch.int64)
+    oy = torch.round((H - rh).double() / 2 - 0.1).to(torch.int64)
+    ox = torch.round((W - rw).double() / 2 - 0.1).to(torch.int64)
+    return _views_table(info, rh, rw, oy, ox, h, w)
 
 
 def decode_batch_host(file_ptrs, sizes, desired_channels: int, out, out_stride: int):

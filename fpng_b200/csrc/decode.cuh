@@ -189,6 +189,9 @@ void launch_png_decode(const PngParams& p, const TypedOut* typed, uint32_t flags
 // Files whose d_status is not 0 are skipped.  Output strides in bytes: element (f, y, x, c) at d_out + f*image + y*row + x*pixel
 // + c*chan, interleaved (pixel = desired * sizeof(T)) or planar (pixel = sizeof(T)).  A native call (src_dtype FPNGB_DTYPE_UINT16)
 // reads uint16 pixels (pitch w * desired * 2) instead, desired 1 .. 4, and stores the rules of decode_resize_kernels.cu.
+// Views call (fpngb_decode_packed_views_device, views != nullptr): output image v (at d_out + v*image, out_h x out_w) is view row v
+// instead of file v: its file's box resized to its own size, flipped and placed on the canvas, the stored fill elsewhere; the
+// kernel writes view_status[v].  boxes is then unused.
 struct ResizeParams {
     const uint8_t* px; const unsigned long long* px_offsets;   // the ragged decode's pixels and their placement
     const FileDesc* files; const int32_t* d_status;
@@ -197,8 +200,12 @@ struct ResizeParams {
     unsigned long long image, row, pixel, chan;
     uint32_t out_w, out_h, antialias;
     uint32_t nearest;                       // 0 bilinear, 1 FPNGB_RESIZE_NEAREST, 2 FPNGB_RESIZE_NEAREST_EXACT (decode_nearest_kernel)
+    const int32_t* views;                   // [m][10] view rows (include/fpng_b200.h), or nullptr
+    int32_t* view_status;                   // [m] with views
+    uint32_t n;                             // files: a view's file must be below it
+    uint32_t fill[4];                       // with views: per channel, the source value stored outside the placed image
 };
-void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s);
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, cudaStream_t s);
 // profiling (fpngb_decode_profile_read): the start (done false) and end (done true) of the resize kernel, reported in slot 8
 void decode_profile_mark_resize(cudaStream_t s, bool done);
 

@@ -241,15 +241,17 @@ static void ragged_workspace(uint32_t n, size_t base_bytes, uint32_t max_file_si
     z_cap = any_png ? sat_u64(z_bytes < z_max ? z_bytes : z_max) : 0ull;
 }
 
-// The resize step of fpngb_decode_packed_resized_device: its checked output and arguments.
+// The resize step of fpngb_decode_packed_resized_device and fpngb_decode_packed_views_device: its checked output and arguments.
+// views != nullptr (the views call): m output images from the view table, boxes unused.
 struct ResizeOut {
     const int32_t* boxes; uint32_t out_w, out_h, flags;
     uint8_t* d_out; Layout out; TypedOut t;
+    const int32_t* views; int32_t* view_status; uint32_t m; uint32_t fill[4];
 };
 
 // The ragged pipeline: walk, place, decode.  With rz (the resized call), the uint8 pixels and their offsets go to the decode
-// workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes, and the
-// resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
+// workspace instead of d_out / d_out_offsets (both unused), out_cap is the call's pixel_cap, the walk checks rz->boxes (none in a
+// views call: boxes belong to the views), and the resize kernel runs behind the decode, before the workspace is released.  any_png: the any-PNG walk and placement, and the
 // general files' gather, inflate and unfilter kernels behind the fpng decode (decode.cuh, PngDesc); png_flags: png_walk's flags
 // (FPNGB_PNG_ALL_FORMATS adds the ext files' unfilter kernel; FPNGB_PNG_NATIVE allows desired_chans 0..4 and the formats
 // decode_format takes for a native call, typed exactly when fmt is given; FPNGB_PNG_INDEX, with both, the raw samples of desired 1
@@ -299,7 +301,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
     WalkParams wp{};
     wp.base = (const uint8_t*)d_base; wp.offsets = (const unsigned long long*)d_offsets; wp.sizes = d_sizes; wp.n = n; wp.info = d_info;
     wp.files = (FileDesc*)p.files; wp.max_file_size = max_file_size; wp.w = max_w; wp.h = max_h; wp.chans = 0; wp.desired = desired_chans;
-    wp.base_bytes = base_bytes; wp.boxes = rz ? rz->boxes : nullptr; wp.index = index ? elem : 0u;
+    wp.base_bytes = base_bytes; wp.boxes = rz && !rz->views ? rz->boxes : nullptr; wp.index = index ? elem : 0u;
     if (any_png) launch_container_walk_any(wp, (PngDesc*)png, png_flags & FPNGB_PNG_ALL_FORMATS, s);
     else launch_container_walk(wp, s);
     PlaceParams pp{};
@@ -324,8 +326,9 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         rp.image = rz->out.image; rp.row = rz->out.row; rp.pixel = rz->out.pixel; rp.chan = rz->out.chan;
         rp.out_w = rz->out_w; rp.out_h = rz->out_h; rp.antialias = rz->flags & FPNGB_RESIZE_ANTIALIAS;
         rp.nearest = (rz->flags & FPNGB_RESIZE_NEAREST) ? 1u : (rz->flags & FPNGB_RESIZE_NEAREST_EXACT) ? 2u : 0u;
+        rp.views = rz->views; rp.view_status = rz->view_status; rp.n = n; memcpy(rp.fill, rz->fill, sizeof rp.fill);
         decode_profile_mark_resize(s, false);
-        launch_decode_resize(rp, rz->t, t.dtype, n, desired_chans, s);
+        launch_decode_resize(rp, rz->t, t.dtype, rz->views ? rz->m : n, desired_chans, s);
         decode_profile_mark_resize(s, true);
     }
     count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0) + (all_formats ? 1 : 0));
@@ -588,17 +591,24 @@ int fpngb_decode_packed_ragged_device_typed(const void* d_base, size_t base_byte
                                      d_out_offsets, d_info, true, fmt, d_status, stream);
 }
 
-int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
-                                       uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap, const int32_t* d_boxes,
-                                       uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags, const fpngb_pixel_format* fmt,
-                                       void* d_out, size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride,
-                                       size_t out_chan_stride, uint32_t* d_info, int32_t* d_status, void* stream)
+}  // extern "C"
+
+namespace fpngb {
+
+// The body of fpngb_decode_packed_resized_device (views nullptr, m = n) and fpngb_decode_packed_views_device (m views, boxes
+// unused): the call-level checks of both, then the ragged pipeline with the resize step.
+static int decode_resized_impl(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                               uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap, const int32_t* d_boxes,
+                               const int32_t* d_views, uint32_t m, uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags,
+                               const fpngb_pixel_format* fmt, const uint32_t* fill, void* d_out, size_t out_image_stride,
+                               size_t out_row_pitch, size_t out_pixel_stride, size_t out_chan_stride, uint32_t* d_info, int32_t* d_status,
+                               int32_t* d_view_status, void* stream)
 {
     if (!context().ready) return FPNGB_ERR_NOT_INITIALIZED;
     const bool native = (flags & FPNGB_RESIZE_NATIVE) != 0, index = (flags & FPNGB_RESIZE_INDEX) != 0;
     const uint32_t nearest = flags & (FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT);
     const uint32_t index_needs = FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE;
-    if (!d_out || n == 0 || n > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
+    if (!d_out || n == 0 || n > 65535 || m == 0 || m > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
         (native ? desired_chans < 1 || desired_chans > 4 : desired_chans != 3 && desired_chans != 4) ||
         (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE |
                              FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT | FPNGB_RESIZE_INDEX)) ||
@@ -608,9 +618,18 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
         return FPNGB_ERR_INVALID_ARG;
     ResizeOut rz{};
     rz.boxes = d_boxes; rz.out_w = out_w; rz.out_h = out_h; rz.flags = flags; rz.d_out = (uint8_t*)d_out;
+    rz.views = d_views; rz.view_status = d_view_status; rz.m = m;
+    if (d_views) {                  // the fill: a source value, so 16 bits where the call's source elements are uint16
+        if (!d_view_status) return FPNGB_ERR_INVALID_ARG;
+        const uint32_t fill_max = native && (!index || (fmt && fmt->dtype == FPNGB_DTYPE_UINT16)) ? 0xFFFFu : 0xFFu;
+        for (uint32_t c = 0; fill && c < desired_chans; c++) {
+            if (fill[c] > fill_max) return FPNGB_ERR_INVALID_ARG;
+            rz.fill[c] = fill[c];
+        }
+    }
     uint32_t elem;
     int rc = decode_format(fmt != nullptr, fmt, desired_chans, native, rz.t, elem); if (rc) return rc;
-    rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, n, out_h, out_w, desired_chans, elem, true,
+    rc = check_layout(d_out, out_image_stride, out_row_pitch, out_pixel_stride, out_chan_stride, m, out_h, out_w, desired_chans, elem, true,
                       rz.out);
     if (rc) return rc;
     // native: the ragged decode holds every file as uint16 values in the 16-bit domain (pixel_cap counts their bytes); index: as
@@ -622,6 +641,34 @@ int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, co
     return decode_packed_ragged_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, desired_chans, nullptr, pixel_cap,
                                      nullptr, d_info, mid != nullptr, mid, d_status, stream, &rz, (flags & FPNGB_RESIZE_ANY_PNG) != 0,
                                      png_flags);
+}
+
+}  // namespace fpngb
+
+extern "C" {
+
+int fpngb_decode_packed_resized_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                       uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap, const int32_t* d_boxes,
+                                       uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags, const fpngb_pixel_format* fmt,
+                                       void* d_out, size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride,
+                                       size_t out_chan_stride, uint32_t* d_info, int32_t* d_status, void* stream)
+{
+    return decode_resized_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, pixel_cap, d_boxes, nullptr, n, out_w,
+                               out_h, desired_chans, flags, fmt, nullptr, d_out, out_image_stride, out_row_pitch, out_pixel_stride,
+                               out_chan_stride, d_info, d_status, nullptr, stream);
+}
+
+int fpngb_decode_packed_views_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,
+                                     uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap, const int32_t* d_views,
+                                     uint32_t m, uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags,
+                                     const fpngb_pixel_format* fmt, const uint32_t* fill, void* d_out, size_t out_image_stride,
+                                     size_t out_row_pitch, size_t out_pixel_stride, size_t out_chan_stride, uint32_t* d_info,
+                                     int32_t* d_status, int32_t* d_view_status, void* stream)
+{
+    if (!d_views) return context().ready ? FPNGB_ERR_INVALID_ARG : FPNGB_ERR_NOT_INITIALIZED;
+    return decode_resized_impl(d_base, base_bytes, d_offsets, d_sizes, n, max_file_size, max_w, max_h, pixel_cap, nullptr, d_views, m, out_w,
+                               out_h, desired_chans, flags, fmt, fill, d_out, out_image_stride, out_row_pitch, out_pixel_stride,
+                               out_chan_stride, d_info, d_status, d_view_status, stream);
 }
 
 int fpngb_decode_packed_png_device_ex(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes, uint32_t n,

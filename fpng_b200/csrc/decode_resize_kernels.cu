@@ -7,6 +7,10 @@
 // output row vertically in registers, over the rows of the step its own taps cover.  Weights are computed on the fly from the
 // per-axis rule, so any tap count works, from 1 up to a whole 3840-pixel crop resized to one pixel; no weight table is kept.
 // All output addressing is 64-bit, and stores are the widest the address allows (store_elems).
+// Views (fpngb_decode_packed_views_device): CTA row blockIdx.y is one output image, a view of a file: its box resized to its own
+// rh x rw, flipped, and placed at an offset on the canvas, fill elsewhere (view_geom).  The flip maps an output index to the resized
+// index before any tap is computed, so each resized value is computed exactly as in the resized call; without a view table the
+// geometry is that call's (box, resize to the canvas, offset 0, no flips), so both calls run the same code.
 // Native calls (FPNGB_RESIZE_NATIVE): the ragged decode holds every file as uint16 values in the 16-bit domain (S = uint16_t), any
 // DST from 1 to 4; the resampled r is stored as cvt.rni.sat.u16(r), round_u8(r / 257) or T((r / 257) * scale + bias).
 //
@@ -98,20 +102,64 @@ __device__ __forceinline__ uint32_t resized_bits(float v, int c, const PixelAffi
     }
 }
 
+// The geometry of output image blockIdx.y.  With a view table: row blockIdx.y, and its status (include/fpng_b200.h, "views"),
+// written by the CTA with blockIdx.x == 0; without one: file blockIdx.y, its box or whole image resized to the canvas at offset 0.
+// The placed image covers canvas rows [y_in0, y_in1) and columns [x_in0, x_in1) (empty when it lies off the canvas).
+struct ViewGeom {
+    uint32_t f; int status;
+    int top, left, bh, bw;                  // the crop box
+    int rh, rw, oy, ox;                     // resized size and offset on the canvas
+    bool hflip, vflip;
+    int y_in0, y_in1, x_in0, x_in1;
+};
+
+__device__ __forceinline__ ViewGeom view_geom(const ResizeParams& p)
+{
+    ViewGeom g;
+    const uint32_t v = blockIdx.y;
+    g.top = 0; g.left = 0; g.rh = (int)p.out_h; g.rw = (int)p.out_w; g.oy = 0; g.ox = 0; g.hflip = g.vflip = false;
+    if (!p.views) {
+        g.f = v;
+        g.status = p.d_status[v];
+        if (p.boxes) { const int32_t* b = p.boxes + (size_t)v * 4; g.top = b[0]; g.left = b[1]; g.bh = b[2]; g.bw = b[3]; }
+        else { g.bh = (int)p.files[v].h; g.bw = (int)p.files[v].w; }
+    } else {
+        const int32_t* r = p.views + (size_t)v * 10;
+        const int file = r[0];
+        g.f = 0; g.top = r[1]; g.left = r[2]; g.bh = r[3]; g.bw = r[4]; g.rh = r[5]; g.rw = r[6]; g.oy = r[7]; g.ox = r[8];
+        const uint32_t flags = (uint32_t)r[9];
+        constexpr int kLim = 1 << 24;
+        if (file < 0 || (uint32_t)file >= p.n) g.status = FPNGB_DECODE_BAD_VIEW;
+        else if ((g.status = p.d_status[file]) != 0) {}
+        else if (g.bh < 1 || g.bw < 1 || g.top < 0 || g.left < 0 || (long long)g.top + g.bh > p.files[file].h ||
+                 (long long)g.left + g.bw > p.files[file].w)
+            g.status = FPNGB_DECODE_BAD_CROP;
+        else if (g.rh < 1 || g.rh > kLim || g.rw < 1 || g.rw > kLim || g.oy < -kLim || g.oy > kLim || g.ox < -kLim || g.ox > kLim ||
+                 (flags & ~(uint32_t)(FPNGB_VIEW_HFLIP | FPNGB_VIEW_VFLIP)))
+            g.status = FPNGB_DECODE_BAD_VIEW;
+        if (blockIdx.x == 0 && threadIdx.x == 0) p.view_status[v] = g.status;
+        if (g.status == 0) g.f = (uint32_t)file;
+        g.hflip = flags & FPNGB_VIEW_HFLIP; g.vflip = flags & FPNGB_VIEW_VFLIP;
+    }
+    g.y_in0 = max(g.oy, 0); g.y_in1 = min(g.oy + g.rh, (int)p.out_h);
+    g.x_in0 = max(g.ox, 0); g.x_in1 = min(g.ox + g.rw, (int)p.out_w);
+    return g;
+}
+
+// resized index of canvas index o (inside the placed image) along an axis placed at offset at, of resized length len
+__device__ __forceinline__ uint32_t resized_index(int o, int at, int len, bool flip) { return (uint32_t)(flip ? len - 1 - (o - at) : o - at); }
+
 template <int DST, bool PLANAR, typename T, typename S = uint8_t>
 __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams p, PixelAffine pa)
 {
     constexpr int ES = sizeof(T), SS = sizeof(S);
     __shared__ float hbuf[kRsStep][kRsCols][DST];
-    const uint32_t f = blockIdx.y;
-    if (p.d_status[f] != 0) return;                                             // the same for the whole CTA
-    const FileDesc& fd = p.files[f];
-    const uint32_t w = fd.w;
-    int top = 0, left = 0, bh = (int)fd.h, bw = (int)w;
-    if (p.boxes) { const int32_t* b = p.boxes + (size_t)f * 4; top = b[0]; left = b[1]; bh = b[2]; bw = b[3]; }
-    const uint8_t* src = p.px + p.px_offsets[f];
-    const size_t pitch = (size_t)w * DST * SS;
-    const float sx = __fdiv_rn((float)bw, (float)p.out_w), sy = __fdiv_rn((float)bh, (float)p.out_h);
+    const ViewGeom g = view_geom(p);
+    if (g.status != 0) return;                                                  // the same for the whole CTA
+    const int top = g.top, left = g.left, bh = g.bh, bw = g.bw;
+    const uint8_t* src = p.px + p.px_offsets[g.f];
+    const size_t pitch = (size_t)p.files[g.f].w * DST * SS;
+    const float sx = __fdiv_rn((float)bw, (float)g.rw), sy = __fdiv_rn((float)bh, (float)g.rh);
     const bool aax = p.antialias && sx >= 1.f, aay = p.antialias && sy >= 1.f;
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, slot = threadIdx.x >> 3, grp = threadIdx.x & 7u;
     const uint32_t col_tiles = (p.out_w + kRsCols - 1) / kRsCols;
@@ -119,12 +167,20 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
     for (unsigned long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
         const uint32_t x0 = (uint32_t)(tile % col_tiles) * kRsCols, y0 = (uint32_t)(tile / col_tiles) * kRsRows;
         const uint32_t ox = x0 + lane, oy = y0 + slot;
-        const Span hx = ox < p.out_w ? axis_span(bw, sx, aax, ox) : Span{0, 0, 0.f, 1.f, 0.f};
-        const Span vy = oy < p.out_h ? axis_span(bh, sy, aay, oy) : Span{0, 0, 0.f, 1.f, 0.f};
-        int r_lo, r_hi, unused_lo, unused_hi;
-        float c0, c1;
-        span_bounds(bh, sy, aay, y0, r_lo, unused_hi, c0);                                  // taps are monotone in the output index
-        span_bounds(bh, sy, aay, min(y0 + kRsRows, p.out_h) - 1, unused_lo, r_hi, c1);
+        const bool row_in = (int)oy >= g.y_in0 && (int)oy < g.y_in1;
+        const Span hx = (int)ox >= g.x_in0 && (int)ox < g.x_in1 ? axis_span(bw, sx, aax, resized_index((int)ox, g.ox, g.rw, g.hflip))
+                                                               : Span{0, 0, 0.f, 1.f, 0.f};
+        const Span vy = row_in ? axis_span(bh, sy, aay, resized_index((int)oy, g.oy, g.rh, g.vflip)) : Span{0, 0, 0.f, 1.f, 0.f};
+        // source rows: the taps of the tile's first and last in-image output rows (taps are monotone in the resized index, which
+        // runs backwards under VFLIP); none when no pixel of the tile lies in the placed image
+        int r_lo = 0, r_hi = 0, unused_lo, unused_hi;
+        const int ya = max((int)y0, g.y_in0), yb = min((int)y0 + (int)kRsRows, g.y_in1) - 1;
+        if (ya <= yb && max((int)x0, g.x_in0) < min((int)x0 + (int)kRsCols, g.x_in1)) {
+            const uint32_t ia = resized_index(g.vflip ? yb : ya, g.oy, g.rh, g.vflip), ib = resized_index(g.vflip ? ya : yb, g.oy, g.rh, g.vflip);
+            float c0, c1;
+            span_bounds(bh, sy, aay, ia, r_lo, unused_hi, c0);
+            span_bounds(bh, sy, aay, ib, unused_lo, r_hi, c1);
+        }
         float acc[4][DST];
 #pragma unroll
         for (int q = 0; q < 4; q++)
@@ -162,13 +218,16 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
         const uint32_t xg = x0 + 4 * grp;
         if (oy >= p.out_h || xg >= p.out_w) continue;
         const uint32_t npx = min(4u, p.out_w - xg);
-        uint8_t* o = p.d_out + (size_t)f * p.image + (size_t)oy * p.row + (size_t)xg * p.pixel;
+        bool in[4];                                                             // else the fill, a source value of the call
+#pragma unroll
+        for (int q = 0; q < 4; q++) in[q] = row_in && (int)(xg + q) >= g.x_in0 && (int)(xg + q) < g.x_in1;
+        uint8_t* o = p.d_out + (size_t)blockIdx.y * p.image + (size_t)oy * p.row + (size_t)xg * p.pixel;
         if (PLANAR) {                                                           // 4 * sizeof(T) contiguous bytes per plane
 #pragma unroll
             for (int c = 0; c < DST; c++) {
                 uint32_t e[4];
 #pragma unroll
-                for (int q = 0; q < 4; q++) e[q] = resized_bits<T, S>(__fmul_rn(acc[q][c], vy.norm), c, pa);
+                for (int q = 0; q < 4; q++) e[q] = resized_bits<T, S>(in[q] ? __fmul_rn(acc[q][c], vy.norm) : (float)p.fill[c], c, pa);
                 uint8_t* a = o + (size_t)c * p.chan;
                 if (npx == 4) store_elems<T>(a, e);
                 else for (uint32_t q = 0; q < npx; q++) store_elem(a + ES * q, e[q], ES);
@@ -176,7 +235,8 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
         } else {                                                                // 4 * DST * sizeof(T) contiguous bytes
             uint32_t e[4 * DST];
 #pragma unroll
-            for (int k = 0; k < 4 * DST; k++) e[k] = resized_bits<T, S>(__fmul_rn(acc[k / DST][k % DST], vy.norm), k % DST, pa);
+            for (int k = 0; k < 4 * DST; k++)
+                e[k] = resized_bits<T, S>(in[k / DST] ? __fmul_rn(acc[k / DST][k % DST], vy.norm) : (float)p.fill[k % DST], k % DST, pa);
             if (npx == 4) store_elems<T>(o, e);
             else {
 #pragma unroll
@@ -232,14 +292,13 @@ template <int DST, bool PLANAR, typename T, typename S>
 __global__ void __launch_bounds__(kRsThreads) decode_nearest_kernel(ResizeParams p, PixelAffine pa)
 {
     constexpr int ES = sizeof(T), SS = sizeof(S);
-    const uint32_t f = blockIdx.y;
-    if (p.d_status[f] != 0) return;                                             // the same for the whole CTA
-    const FileDesc& fd = p.files[f];
-    int top = 0, left = 0, bh = (int)fd.h, bw = (int)fd.w;
-    if (p.boxes) { const int32_t* b = p.boxes + (size_t)f * 4; top = b[0]; left = b[1]; bh = b[2]; bw = b[3]; }
-    const uint8_t* src = p.px + p.px_offsets[f] + ((size_t)top * fd.w + left) * DST * SS;
-    const size_t pitch = (size_t)fd.w * DST * SS;
-    const float sx = __fdiv_rn((float)bw, (float)p.out_w), sy = __fdiv_rn((float)bh, (float)p.out_h);
+    const ViewGeom vg = view_geom(p);
+    if (vg.status != 0) return;                                                  // the same for the whole CTA
+    const uint32_t fw = p.files[vg.f].w;
+    const int bh = vg.bh, bw = vg.bw;
+    const uint8_t* src = p.px + p.px_offsets[vg.f] + ((size_t)vg.top * fw + vg.left) * DST * SS;
+    const size_t pitch = (size_t)fw * DST * SS;
+    const float sx = __fdiv_rn((float)bw, (float)vg.rw), sy = __fdiv_rn((float)bh, (float)vg.rh);
     const bool exact = p.nearest == 2;
     // groups of 4 output pixels: gx per row; each thread steps through them by the grid's thread count, carried as (row, group)
     const uint32_t gx = (p.out_w + 3) / 4;
@@ -250,14 +309,20 @@ __global__ void __launch_bounds__(kRsThreads) decode_nearest_kernel(ResizeParams
     const uint32_t dy = (uint32_t)(step / gx), dq = (uint32_t)(step % gx);
     for (unsigned long long g = g0; g < groups; g += step) {
         const uint32_t xg = 4 * xq, npx = min(4u, p.out_w - xg);
-        const uint8_t* srow = src + (size_t)nearest_src(oy, sy, bh, exact) * pitch;
+        const bool row_in = (int)oy >= vg.y_in0 && (int)oy < vg.y_in1;
+        const uint8_t* srow = src + (row_in ? (size_t)nearest_src(resized_index((int)oy, vg.oy, vg.rh, vg.vflip), sy, bh, exact) * pitch : 0);
         uint32_t v[4][DST];
 #pragma unroll
         for (int q = 0; q < 4; q++) {
-            const int x = (uint32_t)q < npx ? nearest_src(xg + q, sx, bw, exact) : 0;
-            gather_px<DST, S>(srow + (size_t)x * DST * SS, v[q]);
+            if (row_in && (uint32_t)q < npx && (int)(xg + q) >= vg.x_in0 && (int)(xg + q) < vg.x_in1) {
+                const int x = nearest_src(resized_index((int)(xg + q), vg.ox, vg.rw, vg.hflip), sx, bw, exact);
+                gather_px<DST, S>(srow + (size_t)x * DST * SS, v[q]);
+            } else {                                                            // the fill, a source value of the call
+#pragma unroll
+                for (int c = 0; c < DST; c++) v[q][c] = p.fill[c];
+            }
         }
-        uint8_t* o = p.d_out + (size_t)f * p.image + (size_t)oy * p.row + (size_t)xg * p.pixel;
+        uint8_t* o = p.d_out + (size_t)blockIdx.y * p.image + (size_t)oy * p.row + (size_t)xg * p.pixel;
         if (PLANAR) {                                                           // 4 * sizeof(T) contiguous bytes per plane
 #pragma unroll
             for (int c = 0; c < DST; c++) {
@@ -284,30 +349,30 @@ __global__ void __launch_bounds__(kRsThreads) decode_nearest_kernel(ResizeParams
 }
 
 template <int DST, typename T, typename S>
-static void launch_nearest_dst(const ResizeParams& p, const PixelAffine& pa, uint32_t n, cudaStream_t s)
+static void launch_nearest_dst(const ResizeParams& p, const PixelAffine& pa, uint32_t m, cudaStream_t s)
 {
     const unsigned long long groups = (unsigned long long)((p.out_w + 3) / 4) * p.out_h, ctas = (groups + kRsThreads - 1) / kRsThreads;
-    const dim3 g((uint32_t)(ctas < 65535ull ? ctas : 65535ull), n);
+    const dim3 g((uint32_t)(ctas < 65535ull ? ctas : 65535ull), m);
     if constexpr (DST > 1) {                            // one channel: planar and interleaved address the same elements
         if (p.pixel == sizeof(T)) { decode_nearest_kernel<DST, true, T, S><<<g, kRsThreads, 0, s>>>(p, pa); return; }
     }
     decode_nearest_kernel<DST, false, T, S><<<g, kRsThreads, 0, s>>>(p, pa);
 }
 
-// the nearest resize: S uint16 for native calls and uint16 index calls (DST 1 .. 4), else uint8 (DST 3 / 4, or 1 for a uint8 index call)
-static void launch_decode_nearest(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s)
+// the nearest resize (m: output images, the grid's y): S uint16 for native calls and uint16 index calls (DST 1 .. 4), else uint8 (DST 3 / 4, or 1 for a uint8 index call)
+static void launch_decode_nearest(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, cudaStream_t s)
 {
     with_out_type(t.dtype, [&](auto v) {
         using T = decltype(v);
         if (src_dtype == FPNGB_DTYPE_UINT16) {
-            if (desired == 1) launch_nearest_dst<1, T, uint16_t>(p, t.aff, n, s);
-            else if (desired == 2) launch_nearest_dst<2, T, uint16_t>(p, t.aff, n, s);
-            else if (desired == 3) launch_nearest_dst<3, T, uint16_t>(p, t.aff, n, s);
-            else launch_nearest_dst<4, T, uint16_t>(p, t.aff, n, s);
+            if (desired == 1) launch_nearest_dst<1, T, uint16_t>(p, t.aff, m, s);
+            else if (desired == 2) launch_nearest_dst<2, T, uint16_t>(p, t.aff, m, s);
+            else if (desired == 3) launch_nearest_dst<3, T, uint16_t>(p, t.aff, m, s);
+            else launch_nearest_dst<4, T, uint16_t>(p, t.aff, m, s);
         } else if constexpr (!std::is_same<T, uint16_t>::value) {
-            if (desired == 1) { if constexpr (std::is_same<T, uint8_t>::value) launch_nearest_dst<1, T, uint8_t>(p, t.aff, n, s); }
-            else if (desired == 3) launch_nearest_dst<3, T, uint8_t>(p, t.aff, n, s);
-            else launch_nearest_dst<4, T, uint8_t>(p, t.aff, n, s);
+            if (desired == 1) { if constexpr (std::is_same<T, uint8_t>::value) launch_nearest_dst<1, T, uint8_t>(p, t.aff, m, s); }
+            else if (desired == 3) launch_nearest_dst<3, T, uint8_t>(p, t.aff, m, s);
+            else launch_nearest_dst<4, T, uint8_t>(p, t.aff, m, s);
         }
     });
 }
@@ -321,12 +386,13 @@ static void launch_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cud
     decode_resize_kernel<DST, false, T, S><<<g, kRsThreads, 0, s>>>(p, pa);
 }
 
-// src_dtype: the ragged decode's output, FPNGB_DTYPE_UINT16 for a native call (DST 1 .. 4), else 0 (uint8, DST 3 or 4)
-void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t n, uint32_t desired, cudaStream_t s)
+// src_dtype: the ragged decode's output, FPNGB_DTYPE_UINT16 for a native call (DST 1 .. 4), else 0 (uint8, DST 3 or 4); m: output
+// images (files, or views with p.views)
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, cudaStream_t s)
 {
-    if (p.nearest) { launch_decode_nearest(p, t, src_dtype, n, desired, s); return; }
+    if (p.nearest) { launch_decode_nearest(p, t, src_dtype, m, desired, s); return; }
     const unsigned long long tiles = (unsigned long long)((p.out_w + kRsCols - 1) / kRsCols) * ((p.out_h + kRsRows - 1) / kRsRows);
-    const dim3 g((uint32_t)(tiles < 65535ull ? tiles : 65535ull), n);
+    const dim3 g((uint32_t)(tiles < 65535ull ? tiles : 65535ull), m);
     with_out_type(t.dtype, [&](auto v) {
         using T = decltype(v);
         if (src_dtype == FPNGB_DTYPE_UINT16) {

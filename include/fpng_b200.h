@@ -665,6 +665,46 @@ enum { FPNGB_PNG_INDEX = 8 };
 enum { FPNGB_DECODE_NOT_INDEXED = 105 };   /* index decode: the file has no single sample the output type holds */
 enum { FPNGB_RESIZE_NEAREST = 32, FPNGB_RESIZE_NEAREST_EXACT = 64, FPNGB_RESIZE_INDEX = 128 };
 
+/* ---- views: any number of output images per call, each a crop of a file resized to its own size, flipped and placed ----------
+ * fpngb_decode_packed_views_device decodes the packed files as fpngb_decode_packed_resized_device does, then writes m output images
+ * ("views") of one canvas size out_h x out_w: element (v, y, x, c) at d_out + v*out_image_stride + y*out_row_pitch +
+ * x*out_pixel_stride + c*out_chan_stride, any layout of "Pixel layouts".  A view reads one file; a file may have any number of
+ * views, or none.  The view table d_views is a device int32 [m][10], row v = {file, top, left, height, width, resize_h, resize_w,
+ * offset_y, offset_x, flags}, flags a combination of FPNGB_VIEW_HFLIP and FPNGB_VIEW_VFLIP.  For view v of file f:
+ *   1. R = what fpngb_decode_packed_resized_device stores for file f with box {top, left, height, width}, out_h x out_w :=
+ *      resize_h x resize_w, and this call's flags, fmt, interpolation and native / index mode (every rule of that call applies);
+ *   2. R' = R with column j taken from resize_w - 1 - j (HFLIP) and row i from resize_h - 1 - i (VFLIP): flips act after the
+ *      resize, as an index map, so the taps and weights of each resized value are unchanged;
+ *   3. out[v, y, x, c] = R'[y - offset_y, x - offset_x, c] where that position lies inside R', else the fill: fill[c] taken as a
+ *      source value of the call and stored as the call stores one (uint8: as it is; float: T(fill * scale + bias); native: a
+ *      16-bit domain value under the native store rules of the interpolation; index: the raw sample, e.g. 255 for "ignore").
+ *   The result is bit-identical to the resized call at resize_h x resize_w, then the flip, then a paste into a filled canvas: the
+ *   accumulation order of each resized value depends neither on the tile nor on the placement.
+ * Fill: fill (host) holds desired_chans values, each in 0..255, or 0..65535 where the call's source elements are uint16 (native
+ *   calls, index calls into uint16); NULL is all zeros.
+ * View statuses in d_view_status [m], the first that applies: FPNGB_DECODE_BAD_VIEW when file is not in 0..n-1; the file's status
+ *   when it is not 0; FPNGB_DECODE_BAD_CROP for an empty box or one not inside the image (the walk's test of the resized call);
+ *   FPNGB_DECODE_BAD_VIEW for resize_h or resize_w outside 1..2^24, |offset_y| or |offset_x| above 2^24, or unknown flag bits;
+ *   else 0.  The output image of a view whose status is not 0 is left untouched.
+ * Files: every file is decoded, d_status [n] and d_info as in the ragged call; the walk checks no box (boxes belong to views), so
+ *   FPNGB_DECODE_BAD_CROP is never a file status here.  pixel_cap, the bounds and the verify switch as in the resized call.
+ * Call-level checks (a rejected call enqueues nothing and writes nothing): those of fpngb_decode_packed_resized_device, with the
+ *   layout checked for m images, plus FPNGB_ERR_INVALID_ARG for m == 0 or m > 65535, a NULL d_views or d_view_status, and a fill
+ *   value out of range.  n <= 65535 as there.
+ * Stream-ordered, no host synchronisation: the launches of the resized call with the same flags (12, 14 with verify on, for an
+ *   fpng-only call).  The resize or nearest kernel writes the view statuses itself and is profile slot 8. */
+enum { FPNGB_VIEW_HFLIP = 1, FPNGB_VIEW_VFLIP = 2 };
+enum { FPNGB_DECODE_BAD_VIEW = 106 };   /* views decode only: a view row names no file of the call, or a bad size, offset or flag */
+FPNGB_API int fpngb_decode_packed_views_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
+                                               uint32_t n, uint32_t max_file_size, uint32_t max_w, uint32_t max_h, size_t pixel_cap,
+                                               const int32_t* d_views /* m x 10, device */, uint32_t m,
+                                               uint32_t out_w, uint32_t out_h, uint32_t desired_chans, uint32_t flags,
+                                               const fpngb_pixel_format* fmt /* NULL = uint8 */,
+                                               const uint32_t* fill /* host, desired_chans values, or NULL */,
+                                               void* d_out, size_t out_image_stride, size_t out_row_pitch, size_t out_pixel_stride,
+                                               size_t out_chan_stride, uint32_t* d_info /* n*6 or NULL */, int32_t* d_status,
+                                               int32_t* d_view_status, void* stream);
+
 /* ---- typed encode input: float32 / float16 / bfloat16 pixels with a per-channel scale and bias, rounded to 8 bits ------------
  * The *_typed encode calls take the input as elements x of T (fmt->dtype: float32, float16 or bfloat16) and encode, for channel c,
  * the uint8 value
