@@ -22,5 +22,6 @@ from .api import (  # noqa: F401
     FPNGB_DECODE_UNSUPPORTED_PNG, FPNGB_RESIZE_ANY_PNG, get_png_info,
     FPNGB_PNG_ALL_FORMATS, FPNGB_RESIZE_ALL_PNG_FORMATS, FPNGB_PNG_NATIVE, FPNGB_DTYPE_UINT16, FPNGB_RESIZE_NATIVE,
     FPNGB_PNG_INDEX, FPNGB_DECODE_NOT_INDEXED, FPNGB_RESIZE_NEAREST, FPNGB_RESIZE_NEAREST_EXACT, FPNGB_RESIZE_INDEX,
+    FPNGB_RESIZE_BICUBIC,
     FPNGB_VIEW_HFLIP, FPNGB_VIEW_VFLIP, FPNGB_DECODE_BAD_VIEW, decode_packed_views_device, resize_crop_views, letterbox_views,
 )

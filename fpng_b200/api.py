@@ -919,18 +919,20 @@ FPNGB_RESIZE_NATIVE = 16
 FPNGB_RESIZE_NEAREST = 32            # interpolation="nearest": F.interpolate(mode="nearest")
 FPNGB_RESIZE_NEAREST_EXACT = 64      # interpolation="nearest-exact": F.interpolate(mode="nearest-exact")
 FPNGB_RESIZE_INDEX = 128             # indices=True in the resized call
+FPNGB_RESIZE_BICUBIC = 256           # interpolation="bicubic": F.interpolate(mode="bicubic")
 FPNGB_VIEW_HFLIP = 1                 # decode_packed_views_device: view row flag, flip after the resize (torch.flip(dims=[-1]))
 FPNGB_VIEW_VFLIP = 2                 # the same for rows
 FPNGB_DECODE_BAD_VIEW = 106          # decode_packed_views_device only: a view row names no file, or has a bad size, offset or flag
-_INTERPOLATION = {"bilinear": 0, "nearest": FPNGB_RESIZE_NEAREST, "nearest-exact": FPNGB_RESIZE_NEAREST_EXACT}
+_INTERPOLATION = {"bilinear": 0, "bicubic": FPNGB_RESIZE_BICUBIC, "nearest": FPNGB_RESIZE_NEAREST,
+                  "nearest-exact": FPNGB_RESIZE_NEAREST_EXACT}
 
 
-def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: int, boxes=None, antialias=True, out=None, dtype=None,
+def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: int, boxes=None, antialias=None, out=None, dtype=None,
                                  scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None,
                                  any_png=False, all_formats=False, native=False, interpolation="bilinear", indices=False):
     """Decode fpng files of ANY shapes packed in device memory (the layout of decode_packed_ragged_device) into one batch of a fixed
     size = (H, W): file i is cropped to boxes[i] and resized with F.interpolate's bilinear rule (align_corners=False, antialias as
-    given) on the GPU, then stored as decode_batch_device stores its pixels (uint8, rounded half to even and clamped, or dtype with
+    given, None meaning True) on the GPU, then stored as decode_batch_device stores its pixels (uint8, rounded half to even and clamped, or dtype with
     scale and bias).  Returns (out [n, H, W, desired_channels], info int32 [n, 6], status int32 [n]).
       * boxes: None (whole images) or an int32 CUDA tensor [n, 4] of (top, left, height, width), torchvision's resized_crop order;
       * out: any non-overlapping [n, H, W, C] view in one of the layouts of layout_strides, e.g. torch.empty(n, C, H, W,
@@ -952,7 +954,14 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     file).
     interpolation="nearest" / "nearest-exact" (FPNGB_RESIZE_NEAREST / _EXACT) resizes by nearest neighbour with F.interpolate's
     rule of that mode instead: each element is, bit for bit, the element decode_packed_ragged_device with the same arguments stores
-    at the source pixel, so at identity size the result is the ragged decode cropped to the box.  antialias applies to bilinear only.
+    at the source pixel, so at identity size the result is the ragged decode cropped to the box.  antialias applies to bilinear and
+    bicubic only.
+    interpolation="bicubic" (FPNGB_RESIZE_BICUBIC) resizes with F.interpolate's bicubic rule (align_corners=False; A = -0.75, the
+    border of the box replicated) or, with antialias=True, torch's antialiased bicubic, which applies at every scale, upscaling
+    included.  antialias must be given as True or False with bicubic (None raises ValueError): torch's F.interpolate defaults to
+    False and torchvision's resize to True, and unlike bilinear the two bicubic rules differ at every scale, so no default would
+    be right for both kinds of caller.  Bicubic overshoots: uint8 output is the rounded value clamped to 0..255 (torchvision v2's uint8 result on CUDA),
+    float output keeps values below 0 and above 255 (times scale, plus bias), as torch's float result does.
     indices=True (FPNGB_RESIZE_INDEX) takes decode_packed_ragged_device's indices rule and needs a nearest mode as well; pixel_cap
     then counts align_up(w*h*element_size, 16) bytes per file."""
     out, info, status, _ = _resized_call("decode_packed_resized_device", data, offsets, sizes, size, desired_channels, boxes, None, None,
@@ -961,7 +970,7 @@ def decode_packed_resized_device(data, offsets, sizes, size, desired_channels: i
     return out, info, status
 
 
-def decode_packed_views_device(data, offsets, sizes, views, size, desired_channels: int, fill=None, antialias=True, out=None, dtype=None,
+def decode_packed_views_device(data, offsets, sizes, views, size, desired_channels: int, fill=None, antialias=None, out=None, dtype=None,
                                scale=None, bias=None, max_file_size=None, max_w=None, max_h=None, pixel_cap=None, stream=None,
                                any_png=False, all_formats=False, native=False, interpolation="bilinear", indices=False):
     """Decode the packed files of decode_packed_resized_device once and write any number of output images from them: a "view" here
@@ -997,9 +1006,14 @@ def _resized_call(fn, data, offsets, sizes, size, desired_channels, boxes, views
 
     _all_formats_check(any_png, all_formats, fn, native)
     if interpolation not in _INTERPOLATION:
-        raise ValueError(f"{fn}: interpolation {interpolation!r}: 'bilinear', 'nearest' or 'nearest-exact'")
-    if indices and interpolation == "bilinear":
+        raise ValueError(f"{fn}: interpolation {interpolation!r}: 'bilinear', 'bicubic', 'nearest' or 'nearest-exact'")
+    if indices and interpolation in ("bilinear", "bicubic"):
         raise ValueError(f"{fn}: indices=True needs interpolation 'nearest' or 'nearest-exact'")
+    if antialias is None:
+        if interpolation == "bicubic":
+            raise ValueError(f"{fn}: interpolation 'bicubic' needs antialias=True (torchvision's resize) or antialias=False "
+                             "(F.interpolate's default); the two differ at every scale")
+        antialias = True
     if desired_channels not in ((1, 2, 3, 4) if native else (3, 4)):
         raise ValueError(f"{fn}: desired_channels {desired_channels}: " + ("1 .. 4" if native else "3 or 4"))
     H, W = (int(v) for v in size)
@@ -1036,7 +1050,7 @@ def _resized_call(fn, data, offsets, sizes, size, desired_channels, boxes, views
             pixel_cap = total
     info = torch.empty((n, 6), dtype=torch.int32, device=data.device)
     status = torch.empty((n,), dtype=torch.int32, device=data.device)
-    flags = ((FPNGB_RESIZE_ANTIALIAS if antialias and interpolation == "bilinear" else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
+    flags = ((FPNGB_RESIZE_ANTIALIAS if antialias and interpolation in ("bilinear", "bicubic") else 0) | (FPNGB_RESIZE_ANY_PNG if any_png else 0) |
              (FPNGB_RESIZE_ALL_PNG_FORMATS if all_formats else 0) | (FPNGB_RESIZE_NATIVE if native else 0) |
              _INTERPOLATION[interpolation] | (FPNGB_RESIZE_INDEX if indices else 0))
     head = (data.data_ptr(), data.numel(), offsets.data_ptr(), sizes.data_ptr(), n, min(int(max_file_size), 0xFFFFFFFF), int(max_w),

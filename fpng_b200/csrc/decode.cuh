@@ -205,7 +205,8 @@ struct ResizeParams {
     uint32_t n;                             // files: a view's file must be below it
     uint32_t fill[4];                       // with views: per channel, the source value stored outside the placed image
 };
-void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, cudaStream_t s);
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, bool cubic,
+                          cudaStream_t s);
 // profiling (fpngb_decode_profile_read): the start (done false) and end (done true) of the resize kernel, reported in slot 8
 void decode_profile_mark_resize(cudaStream_t s, bool done);
 

@@ -328,7 +328,7 @@ static int decode_packed_ragged_impl(const void* d_base, size_t base_bytes, cons
         rp.nearest = (rz->flags & FPNGB_RESIZE_NEAREST) ? 1u : (rz->flags & FPNGB_RESIZE_NEAREST_EXACT) ? 2u : 0u;
         rp.views = rz->views; rp.view_status = rz->view_status; rp.n = n; memcpy(rp.fill, rz->fill, sizeof rp.fill);
         decode_profile_mark_resize(s, false);
-        launch_decode_resize(rp, rz->t, t.dtype, rz->views ? rz->m : n, desired_chans, s);
+        launch_decode_resize(rp, rz->t, t.dtype, rz->views ? rz->m : n, desired_chans, (rz->flags & FPNGB_RESIZE_BICUBIC) != 0, s);
         decode_profile_mark_resize(s, true);
     }
     count_launch((verify ? 13 : 11) + (rz ? 1 : 0) + (any_png ? 3 : 0) + (all_formats ? 1 : 0));
@@ -611,9 +611,10 @@ static int decode_resized_impl(const void* d_base, size_t base_bytes, const uint
     if (!d_out || n == 0 || n > 65535 || m == 0 || m > 65535 || !out_w || !out_h || out_w > (1u << 24) || out_h > (1u << 24) ||
         (native ? desired_chans < 1 || desired_chans > 4 : desired_chans != 3 && desired_chans != 4) ||
         (flags & ~(uint32_t)(FPNGB_RESIZE_ANTIALIAS | FPNGB_RESIZE_ANY_PNG | FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE |
-                             FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT | FPNGB_RESIZE_INDEX)) ||
+                             FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT | FPNGB_RESIZE_INDEX | FPNGB_RESIZE_BICUBIC)) ||
         ((flags & (FPNGB_RESIZE_ALL_PNG_FORMATS | FPNGB_RESIZE_NATIVE)) && !(flags & FPNGB_RESIZE_ANY_PNG)) ||
         nearest == (FPNGB_RESIZE_NEAREST | FPNGB_RESIZE_NEAREST_EXACT) || (nearest && (flags & FPNGB_RESIZE_ANTIALIAS)) ||
+        ((flags & FPNGB_RESIZE_BICUBIC) && (nearest || index)) ||
         (index && ((flags & index_needs) != index_needs || !nearest || desired_chans != 1 || (fmt && fmt->dtype != FPNGB_DTYPE_UINT16))))
         return FPNGB_ERR_INVALID_ARG;
     ResizeOut rz{};

@@ -14,6 +14,11 @@
 // Native calls (FPNGB_RESIZE_NATIVE): the ragged decode holds every file as uint16 values in the 16-bit domain (S = uint16_t), any
 // DST from 1 to 4; the resampled r is stored as cvt.rni.sat.u16(r), round_u8(r / 257) or T((r / 257) * scale + bias).
 //
+// Bicubic (FPNGB_RESIZE_BICUBIC, the CUBIC instantiations): the same tiles and passes with torch's bicubic taps and weights.  The
+// antialiased filter keeps the span rule with support 2 * max(scale, 1); the plain filter has 4 taps at floorf(real) - 1 .. + 2
+// that may lie outside the crop: the staged rows and the column loads read the clamped index, so the border of the crop (not of
+// the file) is replicated, and the staged row range, taken from the unclamped taps, runs up to 2 rows past either end of the crop.
+//
 // decode_nearest_kernel takes decode_resize_kernel's place for FPNGB_RESIZE_NEAREST / FPNGB_RESIZE_NEAREST_EXACT.  It is a pure
 // gather: each thread owns 4 consecutive output pixels of one row (the store group of the bilinear kernel), computes their source
 // row and columns from the per-axis rule on the fly, and stores the source element converted to the ragged decode's element of the
@@ -58,6 +63,77 @@ __device__ __forceinline__ Span axis_span(int in, float scale, bool aa, uint32_t
     for (int j = lo; j < hi; j++) sum = __fadd_rn(sum, tap_weight(j, sp.center, sp.inv));
     sp.norm = sum != 0.f ? __fdiv_rn(1.f, sum) : 1.f;
     return sp;
+}
+
+// torch's cubic convolution kernel at distance d >= 0 (A = -0.75 plain, a = -0.5 antialiased), each operation separately rounded
+__device__ __forceinline__ float cubic_weight(float d, float a)
+{
+    if (d < 1.f) return __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(a, 2.f), d), __fadd_rn(a, 3.f)), d), d), 1.f);
+    if (d < 2.f) return __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(a, d), __fmul_rn(5.f, a)), d), __fmul_rn(8.f, a)), d),
+                                  __fmul_rn(4.f, a));
+    return 0.f;
+}
+
+// Bicubic taps of output index i (the CUBIC counterparts of span_bounds, tap_weight and axis_span).  Antialiased: the span rule
+// with support 2 * scale (2 below scale 1) and invscale 1 / scale (1 below scale 1), at every scale.  Plain: real = scale * (i +
+// 0.5) - 0.5, unclamped; lo = floorf(real) - 1, 4 taps; center holds t = real - floorf(real); the indices are clamped by the loads.
+__device__ __forceinline__ void cubic_bounds(int in, float scale, bool aa, uint32_t i, int& lo, int& hi, float& center)
+{
+    if (aa) {
+        const float support = scale >= 1.f ? __fmul_rn(2.f, scale) : 2.f;
+        center = __fmul_rn(scale, __fadd_rn((float)i, 0.5f));
+        lo = max((int)__fadd_rn(__fsub_rn(center, support), 0.5f), 0);
+        hi = min((int)__fadd_rn(__fadd_rn(center, support), 0.5f), in);
+    } else {
+        const float real = __fsub_rn(__fmul_rn(scale, __fadd_rn((float)i, 0.5f)), 0.5f), x0 = floorf(real);
+        center = __fsub_rn(real, x0);
+        lo = (int)x0 - 1; hi = lo + 4;
+    }
+}
+
+// weight of tap j: plain taps k = j - lo at distances t + 1, t, 1 - t, 2 - t (not normalised)
+__device__ __forceinline__ float cubic_tap(int j, const Span& sp, bool aa)
+{
+    if (aa) return cubic_weight(fabsf(__fmul_rn(__fadd_rn(__fsub_rn((float)j, sp.center), 0.5f), sp.inv)), -0.5f);
+    const int k = j - sp.lo;
+    const float t = sp.center;
+    const float d = k == 0 ? __fadd_rn(t, 1.f) : k == 1 ? t : k == 2 ? __fsub_rn(1.f, t) : __fsub_rn(2.f, t);
+    return cubic_weight(d, -0.75f);
+}
+
+__device__ __forceinline__ Span cubic_span(int in, float scale, bool aa, uint32_t i)
+{
+    int lo, hi;
+    Span sp;
+    cubic_bounds(in, scale, aa, i, lo, hi, sp.center);
+    sp.lo = lo; sp.size = hi - lo; sp.inv = aa && scale >= 1.f ? __fdiv_rn(1.f, scale) : 1.f; sp.norm = 1.f;
+    if (aa) {
+        float sum = 0.f;
+        for (int j = lo; j < hi; j++) sum = __fadd_rn(sum, cubic_tap(j, sp, true));
+        sp.norm = sum != 0.f ? __fdiv_rn(1.f, sum) : 1.f;
+    }
+    return sp;
+}
+
+template <bool CUBIC>
+__device__ __forceinline__ void filter_bounds(int in, float scale, bool aa, uint32_t i, int& lo, int& hi, float& center)
+{
+    if constexpr (CUBIC) cubic_bounds(in, scale, aa, i, lo, hi, center);
+    else span_bounds(in, scale, aa, i, lo, hi, center);
+}
+
+template <bool CUBIC>
+__device__ __forceinline__ Span filter_span(int in, float scale, bool aa, uint32_t i)
+{
+    if constexpr (CUBIC) return cubic_span(in, scale, aa, i);
+    else return axis_span(in, scale, aa, i);
+}
+
+template <bool CUBIC>
+__device__ __forceinline__ float filter_tap(int j, const Span& sp, bool aa)
+{
+    if constexpr (CUBIC) return cubic_tap(j, sp, aa);
+    else return tap_weight(j, sp.center, sp.inv);
 }
 
 template <int DST>
@@ -149,7 +225,7 @@ __device__ __forceinline__ ViewGeom view_geom(const ResizeParams& p)
 // resized index of canvas index o (inside the placed image) along an axis placed at offset at, of resized length len
 __device__ __forceinline__ uint32_t resized_index(int o, int at, int len, bool flip) { return (uint32_t)(flip ? len - 1 - (o - at) : o - at); }
 
-template <int DST, bool PLANAR, typename T, typename S = uint8_t>
+template <int DST, bool PLANAR, typename T, typename S = uint8_t, bool CUBIC = false>
 __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams p, PixelAffine pa)
 {
     constexpr int ES = sizeof(T), SS = sizeof(S);
@@ -160,7 +236,8 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
     const uint8_t* src = p.px + p.px_offsets[g.f];
     const size_t pitch = (size_t)p.files[g.f].w * DST * SS;
     const float sx = __fdiv_rn((float)bw, (float)g.rw), sy = __fdiv_rn((float)bh, (float)g.rh);
-    const bool aax = p.antialias && sx >= 1.f, aay = p.antialias && sy >= 1.f;
+    // bilinear: the antialiased span equals the plain one below scale 1; bicubic: the antialiased filter applies at every scale
+    const bool aax = p.antialias && (CUBIC || sx >= 1.f), aay = p.antialias && (CUBIC || sy >= 1.f);
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, slot = threadIdx.x >> 3, grp = threadIdx.x & 7u;
     const uint32_t col_tiles = (p.out_w + kRsCols - 1) / kRsCols;
     const unsigned long long tiles = (unsigned long long)col_tiles * ((p.out_h + kRsRows - 1) / kRsRows);
@@ -168,9 +245,9 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
         const uint32_t x0 = (uint32_t)(tile % col_tiles) * kRsCols, y0 = (uint32_t)(tile / col_tiles) * kRsRows;
         const uint32_t ox = x0 + lane, oy = y0 + slot;
         const bool row_in = (int)oy >= g.y_in0 && (int)oy < g.y_in1;
-        const Span hx = (int)ox >= g.x_in0 && (int)ox < g.x_in1 ? axis_span(bw, sx, aax, resized_index((int)ox, g.ox, g.rw, g.hflip))
+        const Span hx = (int)ox >= g.x_in0 && (int)ox < g.x_in1 ? filter_span<CUBIC>(bw, sx, aax, resized_index((int)ox, g.ox, g.rw, g.hflip))
                                                                : Span{0, 0, 0.f, 1.f, 0.f};
-        const Span vy = row_in ? axis_span(bh, sy, aay, resized_index((int)oy, g.oy, g.rh, g.vflip)) : Span{0, 0, 0.f, 1.f, 0.f};
+        const Span vy = row_in ? filter_span<CUBIC>(bh, sy, aay, resized_index((int)oy, g.oy, g.rh, g.vflip)) : Span{0, 0, 0.f, 1.f, 0.f};
         // source rows: the taps of the tile's first and last in-image output rows (taps are monotone in the resized index, which
         // runs backwards under VFLIP); none when no pixel of the tile lies in the placed image
         int r_lo = 0, r_hi = 0, unused_lo, unused_hi;
@@ -178,8 +255,8 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
         if (ya <= yb && max((int)x0, g.x_in0) < min((int)x0 + (int)kRsCols, g.x_in1)) {
             const uint32_t ia = resized_index(g.vflip ? yb : ya, g.oy, g.rh, g.vflip), ib = resized_index(g.vflip ? ya : yb, g.oy, g.rh, g.vflip);
             float c0, c1;
-            span_bounds(bh, sy, aay, ia, r_lo, unused_hi, c0);
-            span_bounds(bh, sy, aay, ib, unused_lo, r_hi, c1);
+            filter_bounds<CUBIC>(bh, sy, aay, ia, r_lo, unused_hi, c0);
+            filter_bounds<CUBIC>(bh, sy, aay, ib, unused_lo, r_hi, c1);
         }
         float acc[4][DST];
 #pragma unroll
@@ -192,14 +269,27 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
                 float h[DST];
 #pragma unroll
                 for (int c = 0; c < DST; c++) h[c] = 0.f;
-                const uint8_t* s = src + (size_t)(top + row) * pitch + (size_t)(left + hx.lo) * DST * SS;
-                for (int j = 0; j < hx.size; j++) {
-                    const float wt = tap_weight(hx.lo + j, hx.center, hx.inv);
-                    float v[DST];
-                    if constexpr (SS == 2) load_px16<DST>(s + (size_t)j * DST * SS, v);
-                    else load_px<DST>(s + (size_t)j * DST, v);
+                if constexpr (CUBIC) {                                          // plain taps past the crop read its edge
+                    const uint8_t* s = src + (size_t)(top + min(max(row, 0), bh - 1)) * pitch + (size_t)left * DST * SS;
+                    for (int j = hx.lo; j < hx.lo + hx.size; j++) {
+                        const float wt = cubic_tap(j, hx, aax);
+                        const size_t at = (size_t)min(max(j, 0), bw - 1) * DST * SS;
+                        float v[DST];
+                        if constexpr (SS == 2) load_px16<DST>(s + at, v);
+                        else load_px<DST>(s + at, v);
 #pragma unroll
-                    for (int c = 0; c < DST; c++) h[c] = fmaf(wt, v[c], h[c]);
+                        for (int c = 0; c < DST; c++) h[c] = fmaf(wt, v[c], h[c]);
+                    }
+                } else {
+                    const uint8_t* s = src + (size_t)(top + row) * pitch + (size_t)(left + hx.lo) * DST * SS;
+                    for (int j = 0; j < hx.size; j++) {
+                        const float wt = tap_weight(hx.lo + j, hx.center, hx.inv);
+                        float v[DST];
+                        if constexpr (SS == 2) load_px16<DST>(s + (size_t)j * DST * SS, v);
+                        else load_px<DST>(s + (size_t)j * DST, v);
+#pragma unroll
+                        for (int c = 0; c < DST; c++) h[c] = fmaf(wt, v[c], h[c]);
+                    }
                 }
 #pragma unroll
                 for (int c = 0; c < DST; c++) hbuf[warp][lane][c] = __fmul_rn(h[c], hx.norm);
@@ -207,7 +297,7 @@ __global__ void __launch_bounds__(kRsThreads) decode_resize_kernel(ResizeParams 
             __syncthreads();
             const int r_end = min(r0 + (int)kRsStep, vy.lo + vy.size);         // vertical pass: the rows of the step this row's taps cover
             for (int r = max(r0, vy.lo); r < r_end; r++) {
-                const float wt = tap_weight(r, vy.center, vy.inv);
+                const float wt = filter_tap<CUBIC>(r, vy, aay);
 #pragma unroll
                 for (int q = 0; q < 4; q++)
 #pragma unroll
@@ -377,18 +467,26 @@ static void launch_decode_nearest(const ResizeParams& p, const TypedOut& t, uint
     });
 }
 
-template <int DST, typename T, typename S>
-static void launch_dst(const ResizeParams& p, const PixelAffine& pa, dim3 g, cudaStream_t s)
+template <int DST, typename T, typename S, bool CUBIC>
+static void launch_filter(const ResizeParams& p, const PixelAffine& pa, dim3 g, cudaStream_t s)
 {
     if constexpr (DST > 1) {                            // one channel: planar and interleaved address the same elements
-        if (p.pixel == sizeof(T)) { decode_resize_kernel<DST, true, T, S><<<g, kRsThreads, 0, s>>>(p, pa); return; }
+        if (p.pixel == sizeof(T)) { decode_resize_kernel<DST, true, T, S, CUBIC><<<g, kRsThreads, 0, s>>>(p, pa); return; }
     }
-    decode_resize_kernel<DST, false, T, S><<<g, kRsThreads, 0, s>>>(p, pa);
+    decode_resize_kernel<DST, false, T, S, CUBIC><<<g, kRsThreads, 0, s>>>(p, pa);
+}
+
+template <int DST, typename T, typename S>
+static void launch_dst(const ResizeParams& p, const PixelAffine& pa, bool cubic, dim3 g, cudaStream_t s)
+{
+    if (cubic) launch_filter<DST, T, S, true>(p, pa, g, s);
+    else launch_filter<DST, T, S, false>(p, pa, g, s);
 }
 
 // src_dtype: the ragged decode's output, FPNGB_DTYPE_UINT16 for a native call (DST 1 .. 4), else 0 (uint8, DST 3 or 4); m: output
-// images (files, or views with p.views)
-void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, cudaStream_t s)
+// images (files, or views with p.views); cubic: FPNGB_RESIZE_BICUBIC (the bilinear kernel's other filter)
+void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src_dtype, uint32_t m, uint32_t desired, bool cubic,
+                          cudaStream_t s)
 {
     if (p.nearest) { launch_decode_nearest(p, t, src_dtype, m, desired, s); return; }
     const unsigned long long tiles = (unsigned long long)((p.out_w + kRsCols - 1) / kRsCols) * ((p.out_h + kRsRows - 1) / kRsRows);
@@ -396,13 +494,13 @@ void launch_decode_resize(const ResizeParams& p, const TypedOut& t, uint32_t src
     with_out_type(t.dtype, [&](auto v) {
         using T = decltype(v);
         if (src_dtype == FPNGB_DTYPE_UINT16) {
-            if (desired == 1) launch_dst<1, T, uint16_t>(p, t.aff, g, s);
-            else if (desired == 2) launch_dst<2, T, uint16_t>(p, t.aff, g, s);
-            else if (desired == 3) launch_dst<3, T, uint16_t>(p, t.aff, g, s);
-            else launch_dst<4, T, uint16_t>(p, t.aff, g, s);
+            if (desired == 1) launch_dst<1, T, uint16_t>(p, t.aff, cubic, g, s);
+            else if (desired == 2) launch_dst<2, T, uint16_t>(p, t.aff, cubic, g, s);
+            else if (desired == 3) launch_dst<3, T, uint16_t>(p, t.aff, cubic, g, s);
+            else launch_dst<4, T, uint16_t>(p, t.aff, cubic, g, s);
         } else if constexpr (!std::is_same<T, uint16_t>::value) {
-            if (desired == 3) launch_dst<3, T, uint8_t>(p, t.aff, g, s);
-            else launch_dst<4, T, uint8_t>(p, t.aff, g, s);
+            if (desired == 3) launch_dst<3, T, uint8_t>(p, t.aff, cubic, g, s);
+            else launch_dst<4, T, uint8_t>(p, t.aff, cubic, g, s);
         }
     });
 }

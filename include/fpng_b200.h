@@ -693,6 +693,32 @@ enum { FPNGB_RESIZE_NEAREST = 32, FPNGB_RESIZE_NEAREST_EXACT = 64, FPNGB_RESIZE_
  *   value out of range.  n <= 65535 as there.
  * Stream-ordered, no host synchronisation: the launches of the resized call with the same flags (12, 14 with verify on, for an
  *   fpng-only call).  The resize or nearest kernel writes the view statuses itself and is profile slot 8. */
+/* ---- bicubic resize in the resized and views decodes (opt-in: FPNGB_RESIZE_BICUBIC) ------------------------------------------
+ * With flags & FPNGB_RESIZE_BICUBIC, fpngb_decode_packed_resized_device and fpngb_decode_packed_views_device resample by torch's
+ * bicubic rule (F.interpolate(mode="bicubic", align_corners=False, antialias=...), torchvision's InterpolationMode.BICUBIC) in
+ * place of the bilinear one.  Per axis, crop length `in`, output length `out`, output index i, every operation a separately
+ * rounded fp32 one, scale = (float)in / (float)out as above:
+ *   With FPNGB_RESIZE_ANTIALIAS (torch's _upsample_bicubic2d_aa), at EVERY scale, upscaling included (unlike bilinear, where the
+ *   two rules coincide below scale 1 and aa needs scale >= 1):
+ *     support  = scale >= 1 ? 2 * scale : 2;   invscale = scale >= 1 ? 1 / scale : 1
+ *     center, xmin, xsize: the bilinear formulas above with this support
+ *     w_j      = cubic(-0.5)((j + xmin - center + 0.5f) * invscale), j < xsize; then w_j /= sum(w) if the sum != 0
+ *     cubic(a)(x) = ((a+2)|x| - (a+3)) x^2 + 1 for |x| < 1;  ((a|x| - 5a)|x| + 8a)|x| - 4a for 1 <= |x| < 2;  0 otherwise
+ *   Without it (torch's upsample_bicubic2d):
+ *     real = scale * (i + 0.5f) - 0.5f (not clamped at 0);  x0 = floorf(real);  t = real - x0
+ *     taps x0 - 1, x0, x0 + 1, x0 + 2, each clamped to [0, in - 1] (the border of the CROP is replicated: torch interpolates the
+ *     cropped tensor, so a tap left of `left` reads column `left`), weights, not normalised, with A = -0.75:
+ *       cc2(t + 1), cc1(t), cc1(1 - t), cc2(2 - t);   cc1(x) = ((A+2)x - (A+3))x^2 + 1,   cc2(x) = ((Ax - 5A)x + 8A)x - 4A
+ *   At identity size both give the weights (0, 1, 0, 0) exactly: the output is the source, bit for bit.
+ *   Bicubic overshoots (values below 0 and above 255 on the 0-255 scale); r is stored by the rules above: uint8 cvt.rni.sat.u8(r)
+ *   (torchvision v2's GPU uint8 path: float interpolate, clamp, round); float T(r * scale + bias) on the unclamped r; native calls
+ *   cvt.rni.sat.u16(r), round_u8(r / 257) or T((r / 257) * scale + bias).
+ * FPNGB_RESIZE_BICUBIC goes with FPNGB_RESIZE_ANTIALIAS, _ANY_PNG, _ALL_PNG_FORMATS, _NATIVE and views; with FPNGB_RESIZE_NEAREST,
+ *   _NEAREST_EXACT or _INDEX it gives FPNGB_ERR_INVALID_ARG (bicubic on class ids is refused, as bilinear is).  Statuses, the fill,
+ *   flips, placement, launches (12, 14 with verify on, for an fpng-only call), profile slot 8 and stream ordering are the bilinear
+ *   call's. */
+enum { FPNGB_RESIZE_BICUBIC = 256 };
+
 enum { FPNGB_VIEW_HFLIP = 1, FPNGB_VIEW_VFLIP = 2 };
 enum { FPNGB_DECODE_BAD_VIEW = 106 };   /* views decode only: a view row names no file of the call, or a bad size, offset or flag */
 FPNGB_API int fpngb_decode_packed_views_device(const void* d_base, size_t base_bytes, const uint64_t* d_offsets, const uint32_t* d_sizes,
