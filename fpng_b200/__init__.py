@@ -16,6 +16,7 @@ from .api import (  # noqa: F401
     FPNGB_DECODE_OUT_OF_SPACE, decode_packed_ragged_device, ragged_views,
     encode_ragged_device, ragged_slot_offsets, compact_packed_device, encode_png_device, png_slot_offsets,
     encode_labels_device, label_slot_offsets, max_label_encoded_size,
+    FPNGB_ENCODE_REDUCE, reduced_slot_offsets, max_reduced_encoded_size,
     FPNGB_DECODE_ADLER_MISMATCH, set_decode_verify, decode_verify,
     normalize_scale_bias, denormalize_scale_bias, typed_layout,
     FPNGB_DECODE_BAD_CROP, FPNGB_RESIZE_ANTIALIAS, decode_packed_resized_device,

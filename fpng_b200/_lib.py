@@ -124,6 +124,8 @@ def lib() -> C.CDLL:
                                              C.c_void_p, C.c_void_p, C.c_void_p]
     L.fpngb_encode_png_ragged_device.restype = C.c_int
     L.fpngb_encode_png_ragged_device.argtypes = L.fpngb_encode_ragged_device.argtypes
+    L.fpngb_max_reduced_encoded_size.restype = C.c_size_t
+    L.fpngb_max_reduced_encoded_size.argtypes = [C.c_uint32] * 4
     L.fpngb_max_label_encoded_size.restype = C.c_size_t
     L.fpngb_max_label_encoded_size.argtypes = [C.c_uint32] * 3 + [C.POINTER(LabelPalette)]
     L.fpngb_encode_label_ragged_device.restype = C.c_int

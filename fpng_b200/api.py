@@ -16,6 +16,7 @@ from ._lib import FpngB200Error, LabelPalette, PixelFormat, check, lib
 
 FPNG_ENCODE_SLOWER = 1          # src/fpng.h:38
 FPNG_FORCE_UNCOMPRESSED = 2     # src/fpng.h:41
+FPNGB_ENCODE_REDUCE = 256       # include/fpng_b200.h: each image in the smallest PNG format that holds it exactly
 (FPNG_DECODE_SUCCESS, FPNG_DECODE_NOT_FPNG, FPNG_DECODE_INVALID_ARG, FPNG_DECODE_FAILED_NOT_PNG,
  FPNG_DECODE_FAILED_HEADER_CRC32, FPNG_DECODE_FAILED_INVALID_DIMENSIONS, FPNG_DECODE_FAILED_DIMENSIONS_TOO_LARGE,
  FPNG_DECODE_FAILED_CHUNK_PARSING, FPNG_DECODE_FAILED_INVALID_IDAT, FPNG_DECODE_FILE_OPEN_FAILED,
@@ -251,10 +252,11 @@ def ragged_slot_offsets(shapes):
     return png_slot_offsets([(h, w, c, 8) for (h, w, c) in shapes])
 
 
-def _encode_images(images, depths, fmt, flags, out, stream, png, what):
+def _encode_images(images, depths, fmt, flags, out, stream, png, what, bound=None):
     """Encodes images, a list of [h, w, c] CUDA tensors of which image i is written at depths[i] bits per sample, with one call
     of fpngb_encode_png_ragged_device (png, dims {w, h, c, depth}) or fpngb_encode_ragged_device (dims {w, h, c}), or of its
-    _typed twin when fmt is given.  out defaults to the slot total.  Returns (out, offsets, sizes)."""
+    _typed twin when fmt is given.  out defaults to the slot total, a slot being bound(w, h, c, depth) (default: max_encoded_size
+    of the pixel bytes) rounded up to 16.  Returns (out, offsets, sizes)."""
     import torch
 
     # the per-image work here is the host cost of the call: attribute reads only; the layout rules are checked by the C call
@@ -275,7 +277,7 @@ def _encode_images(images, depths, fmt, flags, out, stream, png, what):
         for key in keys:
             if key not in slot:
                 w, h, c, d = key
-                slot[key] = (max_encoded_size(w, h, c * d // 8) + 15) // 16 * 16
+                slot[key] = ((bound(w, h, c, d) if bound else max_encoded_size(w, h, c * d // 8)) + 15) // 16 * 16
         total = sum(slot[key] for key in keys)
         out = torch.empty((max(total, 16),), dtype=torch.uint8, device=device)[:total]
     _check_arg(out, "out", device, torch.uint8)
@@ -328,7 +330,24 @@ def png_slot_offsets(shapes):
     return ofs
 
 
-def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None, depth=None):
+def max_reduced_encoded_size(w: int, h: int, chans: int, depth: int) -> int:
+    """fpngb_max_reduced_encoded_size: the slot bound of encode_png_device(reduce=True) for a w x h image of chans channels at
+    depth bits: every format the reduction can pick fits, a 256-entry palette with a full tRNS included."""
+    if chans not in (1, 2, 3, 4) or depth not in (8, 16):
+        raise ValueError(f"max_reduced_encoded_size: chans 1..4 and depth 8 or 16 are needed, got {chans}, {depth}")
+    return int(lib().fpngb_max_reduced_encoded_size(w, h, chans, depth))
+
+
+def reduced_slot_offsets(shapes):
+    """The slot offsets of encode_png_device(reduce=True) for images of the given (h, w, chans, depth) shapes: the exclusive
+    prefix of max_reduced_encoded_size rounded up to 16 bytes, with the total as the last of the n + 1 entries."""
+    ofs = np.zeros(len(shapes) + 1, dtype=np.int64)
+    for i, (h, w, c, depth) in enumerate(shapes):
+        ofs[i + 1] = ofs[i] + (max_reduced_encoded_size(int(w), int(h), int(c), int(depth)) + 15) // 16 * 16
+    return ofs
+
+
+def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None, depth=None, reduce=False):
     """Encode device images of 1 to 4 channels to PNG in one call (fpngb_encode_png_ragged_device, or its _typed twin for float
     images).
 
@@ -349,7 +368,14 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None,
     dtypes, a mixed float list and the argument combinations above raise ValueError.
     Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]) as encode_ragged_device does, offsets being
     png_slot_offsets of the (h, w, c, depth) shapes -- the (data, offsets, sizes) that decode_packed_ragged_device(any_png=True,
-    all_formats=True) reads.  Kernels are enqueued on the current torch stream (or `stream`), with no host synchronisation."""
+    all_formats=True) reads.  Kernels are enqueued on the current torch stream (or `stream`), with no host synchronisation.
+
+    reduce=True (uint8 / uint16 images only; float images raise ValueError) writes each image in the smallest PNG format that
+    holds its pixels exactly, decided on the GPU (include/fpng_b200.h, FPNGB_ENCODE_REDUCE): 1/2/4/8-bit gray, a 1/2/4/8-bit
+    palette for at most 256 colours, gray+alpha, RGB or RGBA, at 8 bits when every sample of a uint16 image is a multiple of 257.
+    A colour-coded mask becomes a palette file, an RGB binary mask a 1-bit file, an opaque RGBA render an fpng RGB file.  The
+    slots are then reduced_slot_offsets of the shapes.  get_info_batch_device / get_png_info report the format written.  The call
+    waits once on the host, for the analysis of the images, before it enqueues the encode."""
     import torch
 
     n = len(images)
@@ -358,6 +384,8 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None,
     for dt in dtypes:
         if dt not in floats and dt not in (torch.uint8, torch.uint16):
             raise ValueError(f"encode_png_device: torch.uint8, uint16, float32, float16 or bfloat16 images are needed, got {dt}")
+    if reduce and dtypes & floats:
+        raise ValueError("encode_png_device: reduce=True takes uint8 / uint16 images, not float ones")
     fmt = None
     if dtypes & floats:
         if len(dtypes) > 1:
@@ -371,6 +399,9 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None,
     elif depth is not None or scale is not None or bias is not None:
         raise ValueError("encode_png_device: depth, scale and bias apply to float images only; uint8 / uint16 are taken as they are")
     depths = depths if fmt is not None else [8 * t.element_size() for t in images]
+    if reduce:
+        return _encode_images(images, depths, None, flags | FPNGB_ENCODE_REDUCE, out, stream, True, "encode_png_device",
+                              bound=lambda w, h, c, d: max_reduced_encoded_size(w, h, c, d))
     return _encode_images(images, depths, fmt, flags, out, stream, True, "encode_png_device")
 
 

@@ -151,9 +151,12 @@ Context& context() { return g_ctx; }
 
 // Optional per-kernel timing with CUDA events on the launching stream (bench.py's roofline numbers).
 // kProfConvert: the conversion pre-pass (convert_pixels_kernel), which runs before the first slot and has its own start event.
+// kProfReduce: the colour-type analysis of FPNGB_ENCODE_REDUCE (analysis and palette finalise), before the conversion, own start event.
 enum ProfSlot { kProfHist = 0, kProfHuff, kProfScan, kProfOffsets, kProfFused, kProfFinish, kProfPack, kProfAdler, kProfCrc, kProfConvert,
-                kProfSlots };
-struct ProfSet { cudaEvent_t ev[kProfSlots + 1]; cudaEvent_t crc_start, conv_start; bool used[kProfSlots]; bool crc_side; uint64_t call; };
+                kProfReduce, kProfSlots };
+struct ProfSet {
+    cudaEvent_t ev[kProfSlots + 1]; cudaEvent_t crc_start, conv_start, red_start; bool used[kProfSlots]; bool crc_side; uint64_t call;
+};
 static uint64_t g_prof_call = 0;                // encode calls seen while profiling (a chunked call owns several ProfSets)
 static bool g_profile = false;
 static std::vector<ProfSet*> g_prof_sets;      // one per encode call since the last read
@@ -167,7 +170,8 @@ static ProfSet* prof_alloc()
     else {
         ps = new ProfSet();
         for (int i = 0; i <= kProfSlots; i++) if (cudaEventCreate(&ps->ev[i]) != cudaSuccess) { delete ps; return nullptr; }
-        if (cudaEventCreate(&ps->crc_start) != cudaSuccess || cudaEventCreate(&ps->conv_start) != cudaSuccess) { delete ps; return nullptr; }
+        if (cudaEventCreate(&ps->crc_start) != cudaSuccess || cudaEventCreate(&ps->conv_start) != cudaSuccess ||
+            cudaEventCreate(&ps->red_start) != cudaSuccess) { delete ps; return nullptr; }
     }
     ps->crc_side = false;
     for (int i = 0; i < kProfSlots; i++) ps->used[i] = false;
@@ -854,14 +858,21 @@ int fpngb_encode_batch_device(const void* d_pixels, size_t image_stride, uint32_
                                              d_sizes, stream);
 }
 
+static size_t reduced_bound(uint32_t w, uint32_t h, uint32_t chans, uint32_t depth);
+static int reduce_images_locked(Context& c, std::vector<RaggedImage>& im, const std::vector<Layout>& src, std::vector<uint32_t>& depth,
+                                cudaStream_t s, std::vector<std::vector<uint8_t>>& hdrs, std::vector<ReduceConvDesc>& conv,
+                                std::vector<uint32_t>& conv_img, uint64_t& conv_bytes);
+
 // Body of the ragged encode calls: fpngb_encode_png_ragged_device and fpngb_encode_ragged_device (typed false, fmt unused) and their
 // _typed twins (fmt required), with dims n x {w, h, chans, depth}.  Images of depth 8 with 3 or 4 channels take fpng's route, the
 // others encode_png_locked.  A typed call first converts every image in one launch into tight rows of its output depth in c.conv;
 // from there on it is the untyped call on those rows.  The conversion and both routes sit inside one workspace bracket
 // (ws_acquire ... the last ws_release), so a call on another stream cannot overwrite c.conv before this call's kernels have read it.
+// reduce (FPNGB_ENCODE_REDUCE, untyped only): reduce_images_locked first picks each image's format, waiting once on the host, and
+// rewrites the images whose format changed as reduced rows in c.conv; the routes then take every image in its reduced format.
 static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides, bool typed,
                               const fpngb_pixel_format* fmt, uint32_t flags, void* d_out, size_t out_cap, uint64_t* d_out_offsets,
-                              uint32_t* d_sizes, void* stream)
+                              uint32_t* d_sizes, void* stream, bool reduce = false)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
     if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
@@ -884,6 +895,8 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         if (fpng ? !valid_dims(w, h, chans)
                  : (w < 1 || h < 1 || w > (1u << 24) || h > (1u << 24) || max_encoded_size(w, h, bpp) > 0x7FFFFFFFull))
             return FPNGB_ERR_INVALID_ARG;                                 // one IDAT chunk must hold the stored file
+        const uint64_t bound = reduce ? reduced_bound(w, h, chans, dep) : max_encoded_size(w, h, bpp);
+        if (reduce && bound > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
         const uint64_t row = strides ? strides[3 * i] : (uint64_t)w * chans * es, pixel = strides ? strides[3 * i + 1] : chans * es;
         const uint64_t chan = (strides && chans > 1) ? strides[3 * i + 2] : es;   // a single channel's stride addresses nothing
         Layout& L = src[i];
@@ -893,7 +906,7 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         im[i] = RaggedImage{(const uint8_t*)(uintptr_t)pixels[i], L.row, L.planar ? L.chan : 0, w, h, chans, total};
         depth[i] = dep;
         (fpng ? fpng_ids : png_ids).push_back(i);
-        total += align_up(max_encoded_size(w, h, bpp), 16);
+        total += align_up(bound, 16);
     }
     if (out_cap < total) return FPNGB_ERR_BUFFER_TOO_SMALL;
     if ((uintptr_t)d_out % 16) return FPNGB_ERR_ALIGNMENT;
@@ -902,6 +915,24 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
     FPNGB_CUDA_OK(cudaSetDevice(c.device));
     cudaStream_t s = (cudaStream_t)stream;
     uint8_t* out = (uint8_t*)d_out;
+
+    // reduce: the images in their reduced formats; the headers of the PNG route's images; the conversions into c.conv
+    std::vector<std::vector<uint8_t>> hdrs;
+    std::vector<ReduceConvDesc> rconv;
+    std::vector<uint32_t> rconv_img;                                     // the image of rconv[j]
+    uint64_t rconv_bytes = 0;
+    size_t png_hdr_bytes = png_ids.size() * kPngEncHeaderSize;
+    if (reduce) {
+        flags &= ~(uint32_t)FPNGB_ENCODE_REDUCE;
+        const int rc = reduce_images_locked(c, im, src, depth, s, hdrs, rconv, rconv_img, rconv_bytes);
+        if (rc) { c.ws_release(s); return rc; }
+        fpng_ids.clear(); png_ids.clear(); png_hdr_bytes = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            const bool fpng = depth[i] == 8 && im[i].chans >= 3;
+            (fpng ? fpng_ids : png_ids).push_back(i);
+            if (!fpng) png_hdr_bytes += hdrs[i].size();
+        }
+    }
 
     // typed: the conversion buffer holds image i's tight rows (w * chans samples of depth / 8 bytes) at a 16-byte aligned offset
     // at[i], then the descriptor table at desc_at
@@ -918,10 +949,10 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
     // (typed) the conversion descriptors
     const size_t ofs_bytes = align_up((size_t)(n + 1) * 8, 16);
     const size_t fpng_table = align_up(align_up(fpng_ids.size() * sizeof(ImageDesc), 16) + fpng_ids.size() * 5 * 4, 16);
-    const size_t conv_stage = align_up(ofs_bytes + fpng_table + png_table_bytes(png_ids.size(), png_ids.size() * kPngEncHeaderSize), 16);
+    const size_t conv_stage = align_up(ofs_bytes + fpng_table + png_table_bytes(png_ids.size(), png_hdr_bytes), 16);
     StageSlot* sl = nullptr;
-    int rc = c.stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : 0), &sl);
-    if (rc) return rc;
+    int rc = c.stage_slot(conv_stage + (typed ? (size_t)n * sizeof(ConvDesc) : rconv.size() * sizeof(ReduceConvDesc)), &sl);
+    if (rc) { if (reduce) c.ws_release(s); return rc; }
     uint8_t* stage = (uint8_t*)sl->buf.p;
     uint64_t* h_ofs = (uint64_t*)stage;
     for (uint32_t i = 0; i < n; i++) h_ofs[i] = im[i].slot;
@@ -946,13 +977,33 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         convert_enqueue(hd, n, (const ConvDesc*)(cb + desc_at), f, cb, s, !png_ids.empty());
     }
     // a route that fails after the conversion still closes the bracket, so that later calls wait for the conversion
-    auto fail = [&](int code) { prof_drop_conv(); if (typed) c.ws_release(s); cudaEventRecord(sl->ev, s); return code; };
+    auto fail = [&](int code) { prof_drop_conv(); if (typed || reduce) c.ws_release(s); cudaEventRecord(sl->ev, s); return code; };
+    if (!rconv.empty()) {                  // the reduced rows: one launch over the images whose format changed (profile slot 9)
+        const uint64_t rdesc_at = align_up(rconv_bytes, 256);
+        rc = c.conv.reserve(rdesc_at + rconv.size() * sizeof(ReduceConvDesc));
+        if (rc) return fail(rc);
+        uint8_t* cb = (uint8_t*)c.conv.p;
+        unsigned long long ctas = 0;
+        for (size_t j = 0; j < rconv.size(); j++) {
+            im[rconv_img[j]].pixels = cb + rconv[j].dst;
+            rconv[j].cta_start = ctas; ctas += reduce_convert_ctas(rconv[j].words, rconv[j].h);
+        }
+        if (ctas > 0x7FFFFFFFull) return fail(FPNGB_ERR_INVALID_ARG);
+        memcpy(stage + conv_stage, rconv.data(), rconv.size() * sizeof(ReduceConvDesc));
+        FPNGB_CUDA_OK(cudaMemcpyAsync(cb + rdesc_at, stage + conv_stage, rconv.size() * sizeof(ReduceConvDesc), cudaMemcpyHostToDevice, s));
+        ProfSet* ps = g_prof_conv;
+        if (ps) cudaEventRecord(ps->conv_start, s);
+        launch_reduce_convert(ReduceConvParams{(const ReduceConvDesc*)(cb + rdesc_at), (uint32_t)rconv.size(), cb}, ctas, s);
+        count_launch(1);
+        if (ps) prof_mark(ps, kProfConvert, s);
+    }
     if (!fpng_ids.empty()) {
         rc = encode_ragged_locked(c, im, fpng_ids, flags, out, d_sizes, s, stage + ofs_bytes);
         if (rc) return fail(rc);
     }
     if (!png_ids.empty()) {
-        rc = encode_png_locked(c, im, depth, png_ids, flags, out, d_sizes, s, stage + ofs_bytes + fpng_table, fpng_ids.empty());
+        rc = encode_png_locked(c, im, depth, png_ids, flags, out, d_sizes, s, stage + ofs_bytes + fpng_table, fpng_ids.empty(),
+                               reduce ? &hdrs : nullptr);
         if (rc) return fail(rc);
     }
     prof_drop_conv();
@@ -1024,6 +1075,135 @@ static std::vector<uint8_t> make_label_header(uint32_t w, uint32_t h, uint32_t d
 size_t fpngb_max_label_encoded_size(uint32_t w, uint32_t h, uint32_t depth, const fpngb_label_palette* pal)
 {
     return label_bound(w, h, depth, pal);
+}
+
+// ---- colour-type reduction (FPNGB_ENCODE_REDUCE) ---------------------------------------------------------------------------
+// The largest file of any format the reduction can pick: the unreduced bound, or a depth-8 palette file with 256 entries and a
+// full tRNS.  Every other candidate has at most the input's bytes per pixel (max_encoded_size grows with the row bytes).
+static size_t reduced_bound(uint32_t w, uint32_t h, uint32_t chans, uint32_t depth)
+{
+    static const uint8_t clear[4 * 256] = {};                             // alpha 0 throughout: tRNS of 256 entries
+    const fpngb_label_palette full{clear, 256, 4};
+    return std::max(max_encoded_size(w, h, chans * depth / 8), label_bound(w, h, 8, &full));
+}
+
+size_t fpngb_max_reduced_encoded_size(uint32_t w, uint32_t h, uint32_t chans, uint32_t depth)
+{
+    if (chans < 1 || chans > 4 || (depth != 8 && depth != 16)) return 0;
+    return reduced_bound(w, h, chans, depth);
+}
+
+// The formats of the rule in include/fpng_b200.h, in its tie order
+enum RedFormat { kFmtGray = 0, kFmtPalette, kFmtGA, kFmtRGB, kFmtRGBA };
+struct RedChoice { int fmt; uint32_t bits; uint32_t depth; };      // bits per pixel; sample depth (gray: d, or 16)
+
+static uint32_t pil_palette_depth(uint32_t K) { return K <= 2 ? 1 : K <= 4 ? 2 : K <= 16 ? 4 : 8; }
+
+// The format of an image of chans channels at depth bits from its analysis flags and colour count K
+static RedChoice reduce_choice(uint32_t chans, uint32_t depth, uint32_t flags, uint32_t K)
+{
+    const bool rep8 = depth == 8 || !(flags & kRedNotRep8);
+    const bool opaque = (chans & 1u) || !(flags & kRedNotOpaque);
+    const bool gray = chans <= 2 || !(flags & kRedNotGray);
+    const uint32_t D = rep8 ? 8 : 16;
+    RedChoice best{-1, 0, 0};
+    auto offer = [&](int fmt, uint32_t bits, uint32_t dep) { if (best.fmt < 0 || bits < best.bits) best = RedChoice{fmt, bits, dep}; };
+    if (gray && opaque) {
+        const uint32_t d = !rep8 ? 16 : !(flags & kRedNotL1) ? 1 : !(flags & kRedNotL2) ? 2 : !(flags & kRedNotL4) ? 4 : 8;
+        offer(kFmtGray, d, d);
+    }
+    if (rep8 && !(flags & kRedOverflow)) offer(kFmtPalette, pil_palette_depth(K), pil_palette_depth(K));
+    if (gray) offer(kFmtGA, 2 * D, D);
+    if (opaque) offer(kFmtRGB, 3 * D, D);
+    offer(kFmtRGBA, 4 * D, D);
+    return best;
+}
+
+// FPNGB_ENCODE_REDUCE's analysis and decision, inside the call's workspace bracket (it opens it: ws_acquire on s).  Enqueues the
+// analysis and finalise kernels (profile slot 10) over every image, reads back each image's ReduceResult and waits for it: the one
+// host synchronisation of the call.  Then, per image whose format changed, rewrites im[i] / depth[i] as the rows the routes encode
+// (tight rows or packed gray8 rows of a label file, words * 4 bytes apart, at byte conv_bytes of c.conv, filled by conv[j] for image
+// conv_img[j] once the caller has placed them) and sets hdrs[i], the container header of every image bound for the PNG route.
+static int reduce_images_locked(Context& c, std::vector<RaggedImage>& im, const std::vector<Layout>& src, std::vector<uint32_t>& depth,
+                                cudaStream_t s, std::vector<std::vector<uint8_t>>& hdrs, std::vector<ReduceConvDesc>& conv,
+                                std::vector<uint32_t>& conv_img, uint64_t& conv_bytes)
+{
+    const uint32_t n = (uint32_t)im.size();
+    // c.red: ReduceState[n] | ReduceTable[n] (cleared) | ReduceResult[n] | ReduceDesc[n]
+    const size_t o_tab = align_up((size_t)n * sizeof(ReduceState), 256), o_res = align_up(o_tab + (size_t)n * sizeof(ReduceTable), 256);
+    const size_t o_desc = align_up(o_res + (size_t)n * sizeof(ReduceResult), 256), bytes = o_desc + (size_t)n * sizeof(ReduceDesc);
+    std::vector<ReduceDesc> rd(n);
+    unsigned long long ctas = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const RaggedImage& r = im[i];
+        rd[i] = ReduceDesc{r.pixels, r.row, src[i].pixel, src[i].chan, ctas, r.w, r.h, r.chans, depth[i] / 8};
+        ctas += reduce_analyze_ctas(r.w, r.h);
+    }
+    if (ctas > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
+    int rc = c.ws_acquire(s);
+    if (rc) return rc;
+    rc = c.red.reserve(bytes);
+    if (rc) return rc;
+    StageSlot* sl = nullptr;                                              // the descriptors up, then the results down
+    rc = c.stage_slot(std::max((size_t)n * sizeof(ReduceDesc), (size_t)n * sizeof(ReduceResult)), &sl);
+    if (rc) return rc;
+    uint8_t* b = (uint8_t*)c.red.p;
+    memcpy(sl->buf.p, rd.data(), (size_t)n * sizeof(ReduceDesc));
+    FPNGB_CUDA_OK(cudaMemcpyAsync(b + o_desc, sl->buf.p, (size_t)n * sizeof(ReduceDesc), cudaMemcpyHostToDevice, s));
+    FPNGB_CUDA_OK(cudaMemsetAsync(b, 0, o_res, s));
+    ReduceParams p{(const ReduceDesc*)(b + o_desc), n, (ReduceState*)b, (ReduceTable*)(b + o_tab), (ReduceResult*)(b + o_res)};
+    prof_drop_conv();
+    ProfSet* ps = g_profile ? prof_alloc() : nullptr;                      // slots 10 and 9 of the encode that follows
+    if (ps) cudaEventRecord(ps->red_start, s);
+    launch_reduce_analyze(p, ctas, s);
+    count_launch(2);
+    if (ps) { prof_mark(ps, kProfReduce, s); g_prof_conv = ps; }
+    FPNGB_CUDA_OK(cudaGetLastError());
+    FPNGB_CUDA_OK(cudaMemcpyAsync(sl->buf.p, b + o_res, (size_t)n * sizeof(ReduceResult), cudaMemcpyDeviceToHost, s));
+    FPNGB_CUDA_OK(cudaEventRecord(sl->ev, s));
+    FPNGB_CUDA_OK(cudaEventSynchronize(sl->ev));
+    const ReduceResult* res = (const ReduceResult*)sl->buf.p;
+
+    hdrs.assign(n, std::vector<uint8_t>());
+    conv.clear(); conv_img.clear(); conv_bytes = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        RaggedImage& r = im[i];
+        const RedChoice ch = reduce_choice(r.chans, depth[i], res[i].flags, res[i].count);
+        ReduceConvDesc d{};
+        d.src = r.pixels; d.row = r.row; d.pixel = src[i].pixel; d.chan = src[i].chan;
+        d.tab = p.tab + i; d.st = p.st + i; d.w = r.w; d.h = r.h; d.chans = r.chans; d.elem = depth[i] / 8;
+        uint32_t out_w = r.w, out_chans = 1, out_depth = 8;
+        if (ch.fmt == kFmtPalette || (ch.fmt == kFmtGray && ch.depth < 8)) {   // a label file: packed rows as a gray8 image
+            d.mode = ch.fmt == kFmtPalette ? 0 : 1; d.bits = ch.depth; d.step = 255u / ((1u << ch.depth) - 1u);
+            d.words = (uint32_t)(((uint64_t)r.w * ch.depth + 31) / 32);
+            out_w = label_packed_width(r.w, ch.depth);
+            std::vector<uint8_t> colors;
+            fpngb_label_palette pal{nullptr, 0, 4};
+            if (ch.fmt == kFmtPalette) {
+                for (uint32_t e = 0; e < res[i].count; e++)
+                    for (int k = 0; k < 4; k++) colors.push_back((uint8_t)(res[i].pal[e] >> (24 - 8 * k)));
+                pal = fpngb_label_palette{colors.data(), res[i].count, 4};
+            }
+            hdrs[i] = make_label_header(r.w, r.h, ch.depth, ch.fmt == kFmtPalette ? &pal : nullptr);
+        } else {
+            out_chans = ch.fmt == kFmtGray ? 1 : ch.fmt == kFmtGA ? 2 : ch.fmt == kFmtRGB ? 3 : 4;
+            out_depth = ch.depth;
+            d.mode = 2; d.bits = out_chans; d.out_bytes = out_depth / 8;
+            d.words = (uint32_t)(((uint64_t)r.w * out_chans * d.out_bytes + 3) / 4);
+            if (out_depth != 8 || out_chans < 3) {
+                hdrs[i].resize(kPngEncHeaderSize);
+                make_png_enc_header(hdrs[i].data(), r.w, r.h, out_chans, out_depth);
+            }
+            if (out_chans == r.chans && out_depth == depth[i]) continue;      // read in place, as without the flag
+        }
+        conv.push_back(d);
+        conv.back().dst = conv_bytes;
+        conv_img.push_back(i);
+        conv_bytes += align_up((uint64_t)d.words * 4 * r.h, 16);
+        r = RaggedImage{nullptr, (uint64_t)d.words * 4, 0, out_w, r.h, out_chans, r.slot};
+        depth[i] = out_depth;
+    }
+    return FPNGB_OK;
 }
 
 // The label-map encode: call-level checks; the slots; then, in one workspace bracket, the pre-pass (label_pack_kernel) into tight
@@ -1116,8 +1296,9 @@ int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uin
                                    void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
-    return encode_images_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
+    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED | FPNGB_ENCODE_REDUCE)) return FPNGB_ERR_INVALID_ARG;
+    return encode_images_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream,
+                              (flags & FPNGB_ENCODE_REDUCE) != 0);
 }
 
 int fpngb_encode_png_ragged_device_typed(uint32_t n, const uint64_t* pixels, const uint32_t* dims, const uint64_t* strides,
@@ -1263,8 +1444,9 @@ int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
 }
 
 // Per-kernel device times (ms) averaged over the encode calls since the last read; slots in ProfSlot order:
-// hist, huffman, scan, offsets, fused, finish, pack, adler, crc, conversion pre-pass (slot 9: the *_typed calls, and the uint8 copy of a
-// strided batch bound for the single-pass encoder).  A caller asking for 9 slots gets the first nine.  Returns the number
+// hist, huffman, scan, offsets, fused, finish, pack, adler, crc, conversion pre-pass (slot 9: the *_typed calls, the uint8 copy of a
+// strided batch bound for the single-pass encoder, the label and reduce pre-passes), colour-type analysis (slot 10:
+// FPNGB_ENCODE_REDUCE).  A caller asking for 9 slots gets the first nine.  Returns the number
 // of calls averaged.
 FPNGB_API int fpngb_profile_enable(int on)
 {
@@ -1286,8 +1468,8 @@ FPNGB_API int fpngb_profile_read(float* ms, int nslots)
             cudaEventSynchronize(ps->ev[i + 1]);
             // the CRC of a chunk may run on the side stream, overlapped with the next chunk: its own start event brackets it
             // and the conversion pre-pass, which runs before slot 0 opens
-            const bool own_start = (i == kProfCrc && ps->crc_side) || i == kProfConvert;
-            cudaEvent_t from = i == kProfConvert ? ps->conv_start : own_start ? ps->crc_start : ps->ev[last];
+            const bool own_start = (i == kProfCrc && ps->crc_side) || i == kProfConvert || i == kProfReduce;
+            cudaEvent_t from = i == kProfConvert ? ps->conv_start : i == kProfReduce ? ps->red_start : own_start ? ps->crc_start : ps->ev[last];
             if (cudaEventElapsedTime(&t, from, ps->ev[i + 1]) == cudaSuccess) sum[i] += t;
             if (!own_start) last = i + 1;
         }

@@ -238,6 +238,54 @@ struct LabelPackParams {
 uint32_t label_pack_ctas(uint32_t words, uint32_t h);
 void launch_label_pack(const LabelPackParams& p, unsigned long long total_ctas, cudaStream_t s);
 
+// Colour-type reduction (reduce_kernels.cu, FPNGB_ENCODE_REDUCE).  Image i's w x h x chans samples of elem bytes (1: uint8, 2: uint16)
+// are at src + y*row + x*pixel + c*chan.  The analysis ORs the negative evidence below into ReduceState::flags and collects the
+// image's distinct 8-bit RGBA colours (key R << 24 | G << 16 | B << 8 | A; a gray sample g is (g, g, g), a missing alpha 255) in a
+// 512-slot open-addressing set.  Slot value 0 means empty, so the colour 0x00000000 is not stored there but kept as kRedHasZero.
+enum : uint32_t {
+    kRedNotRep8 = 1u,                             // a 16-bit sample is not a multiple of 257
+    kRedNotOpaque = 2u,                           // an alpha below its maximum
+    kRedNotGray = 4u,                             // a pixel with R, G, B not all equal
+    kRedNotL1 = 8u, kRedNotL2 = 16u, kRedNotL4 = 32u,   // an 8-bit gray value off the 1-, 2-, 4-bit lattice (255, 85, 17)
+    kRedOverflow = 64u,                           // at least 257 distinct colours
+    kRedHasZero = 128u                            // the colour 0x00000000 occurs
+};
+constexpr uint32_t kReduceSlots = 512;
+struct ReduceState { uint32_t flags, count, zero_index, pad_; };     // count: distinct colours (kRedHasZero's included)
+struct ReduceTable { uint32_t key[kReduceSlots]; uint8_t index[kReduceSlots]; };   // palette index of key[s] (finalise)
+// the read-back of one image: flags and count of its ReduceState, the palette in order (keys as above), K = count entries
+struct ReduceResult { uint32_t flags, count, pad_[2]; uint32_t pal[256]; };
+struct ReduceDesc {
+    const uint8_t* src;
+    unsigned long long row, pixel, chan;          // byte strides
+    unsigned long long cta_start;                 // first CTA of the image in the analysis launch
+    uint32_t w, h, chans, elem;
+};
+struct ReduceParams {
+    const ReduceDesc* desc; uint32_t count;
+    ReduceState* st; ReduceTable* tab; ReduceResult* res;
+};
+uint32_t reduce_analyze_ctas(uint32_t w, uint32_t h);
+// the analysis over every image of the call (total_ctas CTAs), then the palette finalise (one CTA per image): two launches
+void launch_reduce_analyze(const ReduceParams& p, unsigned long long total_ctas, cudaStream_t s);
+
+// The conversion pre-pass of the images whose format changed: rows of `words` 32-bit words at dst.  mode 0: palette indices (looked up
+// in tab) packed MSB-first at `bits` bits; mode 1: gray levels g / step packed the same way; mode 2: tight samples of `bits` output
+// channels (source channel j, or chans - 1 for the alpha of a gray+alpha output) at out_bytes bytes (1: the 8-bit value, 2: the
+// native uint16).
+struct ReduceConvDesc {
+    const uint8_t* src;
+    unsigned long long row, pixel, chan;
+    unsigned long long dst;                       // byte offset of the rows in ReduceConvParams::dst
+    unsigned long long cta_start;
+    const ReduceTable* tab; const ReduceState* st;
+    uint32_t w, h, chans, elem;
+    uint32_t mode, bits, out_bytes, step, words, pad_;
+};
+struct ReduceConvParams { const ReduceConvDesc* desc; uint32_t count; uint8_t* dst; };
+uint32_t reduce_convert_ctas(uint32_t words, uint32_t h);
+void launch_reduce_convert(const ReduceConvParams& p, unsigned long long total_ctas, cudaStream_t s);
+
 bool walk16_eligible(const void* base, size_t image_stride, uint32_t row_pitch, uint32_t w, uint32_t chans);
 void launch_scan16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);
 void launch_hist16(const ScanParams& p, uint32_t n, uint32_t chans, cudaStream_t s);

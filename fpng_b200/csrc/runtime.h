@@ -37,6 +37,7 @@ struct Context {
     CodeBook h_static_books[2];
     Buffer ws;                                    // kernel workspace (row tables, image state, histograms, books)
     Buffer conv;                                  // uint8 images the *_typed encode calls convert their input into (used under ws_acquire)
+    Buffer red;                                   // FPNGB_ENCODE_REDUCE: per-image analysis state, colour sets and results (under ws_acquire)
     Buffer dev_in, dev_out;                       // staging for the *_host entry points
     Buffer pin_small;                             // pinned scratch for sizes / status words
     std::mutex mu;                                // the *_host entry points and the workspace are serialised

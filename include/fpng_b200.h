@@ -185,6 +185,43 @@ FPNGB_API int fpngb_encode_label_ragged_device(uint32_t n, const uint64_t* pixel
                                                const fpngb_label_palette* palettes, uint32_t flags, void* d_out, size_t out_cap,
                                                uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream);
 
+/* ---- colour-type reduction (opt-in: FPNGB_ENCODE_REDUCE on fpngb_encode_png_ragged_device) ----------------------------------
+ * With flags & FPNGB_ENCODE_REDUCE every image is written in the smallest PNG format that holds its pixels exactly ("lossless
+ * reductions" in PNG optimisers).  For an image of c channels at depth D (8 or 16), over the whole image:
+ *   8-bit representable  D = 8, or every sample is a multiple of 257; the samples are then read as v / 257;
+ *   opaque               c is 1 or 3, or every alpha is at its maximum;
+ *   gray-valued          c is 1 or 2, or R = G = B at every pixel;
+ *   lattice depth d      (gray-valued, opaque, 8-bit representable) the least d in {1, 2, 4, 8} such that every gray value is a
+ *                        multiple of 255 / (2^d - 1), the values the sub-byte expansion s * 255 / (2^d - 1) of a decoder produces;
+ *   K                    the number of distinct 8-bit (R, G, B, A), gray as (g, g, g), a missing alpha as 255 (needed up to 256).
+ * The formats that hold the image: gray at depth d, or gray16 (opaque, gray-valued, not 8-bit representable); palette at PIL's
+ * depth p(K) (1 for K <= 2, 2 for K <= 4, 4 for K <= 16, else 8; needs 8-bit representable and K <= 256); gray+alpha at D'
+ * (gray-valued); RGB at D' (opaque); RGBA at D', where D' is 8 for an 8-bit representable image and 16 otherwise.  The call
+ * writes the one with the fewest bits per pixel (d, p(K), 2D', 3D', 4D'), ties in the order gray, palette, gray+alpha, RGB,
+ * RGBA.  No trial compression.  A palette lists first the entries whose alpha is below 255, ascending by their big-endian
+ * RGBA value, then the opaque entries ascending by RGB, so that tRNS is as short as it can be.
+ * The file of an image is byte for byte the file an existing call writes for the reduced input with the same flags:
+ *   palette         fpngb_encode_label_ragged_device(index map, the palette as RGBA, depth p(K));
+ *   gray, d < 8     fpngb_encode_label_ragged_device(gray / (255 / (2^d - 1)), gray, depth d);
+ *   the others      fpngb_encode_png_ragged_device(reduced image): gray8, GA8, gray16, GA16, RGB16 and RGBA16 PNGs, and fpng
+ *                   files for RGB8 and RGBA8.
+ * FPNGB_ENCODE_SLOWER and FPNGB_FORCE_UNCOMPRESSED keep their meaning.  The fpngb_*_typed calls reject the flag
+ * (FPNGB_ERR_INVALID_ARG).  Slot i is sized by fpngb_max_reduced_encoded_size(w_i, h_i, chans_i, depth_i); an image whose bound
+ * exceeds 2^31 - 1 is rejected.  The format written is in the file: fpngb_get_info_batch_device reads it back.
+ * One host synchronisation: the container header and the row kernels of an image depend on its pixels, so the call enqueues
+ * the analysis, reads back each image's flags and palette (1040 bytes per image) and waits for them, with the library's lock
+ * held.  Everything after that is enqueued as without the flag; a call without the flag stays stream-ordered and unchanged.
+ * Workspace: 3.6 KiB per image (a 512-slot colour set with palette indices, 16 bytes of state, the 1040-byte result and the
+ * descriptor), 230 MiB at 65535 images; the reduced rows of the images whose format changed go to the conversion buffer.
+ * Launches: two more than the call on the reduced images -- the analysis (one pass over every image; a CTA stops once nothing
+ * it could still read would change the format) and the palette finalise (one CTA per image), both in fpngb_profile_read slot
+ * 10 -- plus one conversion pre-pass (slot 9) when any image's format changed. */
+enum { FPNGB_ENCODE_REDUCE = 256 };
+/* the slot bound of FPNGB_ENCODE_REDUCE: the larger of fpngb_max_encoded_size(w, h, chans * depth / 8) and the label bound at
+ * depth 8 with a 256-entry palette and a full tRNS (which dominates for small images); every candidate format fits.  0 for chans
+ * outside 1..4 or depth other than 8 and 16. */
+FPNGB_API size_t fpngb_max_reduced_encoded_size(uint32_t w, uint32_t h, uint32_t chans, uint32_t depth);
+
 /* Batch of n equally sized images in HOST memory (ideally pinned: see fpngb_host_alloc) -> n files in host memory,
  * out + i*out_stride, sizes[i].  Internally pipelines H2D copy / kernels / D2H copy over chunks of the batch. */
 FPNGB_API int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
