@@ -184,13 +184,39 @@ def combos():
 
 
 # ---- a reader for files other writers produced (PIL, OpenCV): samples, palette and tRNS as the model takes them ------------------
+def _unfilter_run(f: np.ndarray, ft: np.ndarray, prev: np.ndarray, bpp: int) -> np.ndarray:
+    """rows of a run of None / Sub / Up rows at once: None and Sub rows stand alone, an Up row adds the row above, so each row
+    is the last stand-alone row at or above it (or prev) plus the Up rows' bytes since"""
+    n, rb = f.shape
+    own = f.copy()
+    sub = ft == 1
+    if sub.any():
+        own[sub] = np.cumsum(f[sub].reshape(int(sub.sum()), rb // bpp, bpp), 1).reshape(-1, rb)
+    up = ft == 2
+    c = np.cumsum(np.where(up[:, None], f, 0), 0)
+    anchor = np.maximum.accumulate(np.where(up, -1, np.arange(n)))
+    a = np.maximum(anchor, 0)
+    start = np.where(anchor[:, None] >= 0, own[a] - c[a], prev[None, :])
+    return (start + c) & 255
+
+
 def _unfilter(raw: np.ndarray, rb: int, ph: int, bpp: int) -> np.ndarray:
-    buf = raw.reshape(ph, rb + 1).astype(np.int32)
-    out = np.zeros((ph, rb), np.int32)
-    prev = np.zeros(rb, np.int32)
-    for y in range(ph):
-        ft, f = int(buf[y, 0]), buf[y, 1:]
-        assert ft <= 4
+    buf = raw.reshape(ph, rb + 1).astype(np.int64)
+    out = np.zeros((ph, rb), np.int64)
+    prev = np.zeros(rb, np.int64)
+    fts = buf[:, 0]
+    assert (fts <= 4).all()
+    y = 0
+    while y < ph:
+        if fts[y] <= 2:                                                # the run of None / Sub / Up rows from y
+            e = y
+            while e < ph and fts[e] <= 2:
+                e += 1
+            out[y:e] = _unfilter_run(buf[y:e, 1:], fts[y:e], prev, bpp)
+            prev = out[e - 1]
+            y = e
+            continue
+        ft, f = int(fts[y]), buf[y, 1:]
         if ft in (0, 2):
             cur = (f + (prev if ft == 2 else 0)) & 255
         elif ft == 1:
@@ -203,6 +229,7 @@ def _unfilter(raw: np.ndarray, rb: int, ph: int, bpp: int) -> np.ndarray:
                 cur[x] = (f[x] + ((a + prev[x]) // 2 if ft == 3 else int(paeth(np.int32(a), np.int32(prev[x]), np.int32(c))))) & 255
         out[y] = cur
         prev = cur
+        y += 1
     return out.astype(np.uint8)
 
 
