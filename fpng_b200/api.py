@@ -347,7 +347,14 @@ def reduced_slot_offsets(shapes):
     return ofs
 
 
-def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None, depth=None, reduce=False):
+def _lz77_flags(lz77, name):
+    """FPNGB_LZ77_CHAIN(lz77): the flag bits of a chain depth 0 (off) to 256, ValueError otherwise"""
+    if isinstance(lz77, bool) or not isinstance(lz77, (int, np.integer)) or not 0 <= int(lz77) <= 256:
+        raise ValueError(f"{name}: lz77 is a chain depth from 0 (off) to 256, got {lz77!r}")
+    return int(lz77) << 16
+
+
+def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None, bias=None, depth=None, reduce=False, lz77=0):
     """Encode device images of 1 to 4 channels to PNG in one call (fpngb_encode_png_ragged_device, or its _typed twin for float
     images).
 
@@ -375,9 +382,16 @@ def encode_png_device(images, flags: int = 0, out=None, stream=None, scale=None,
     palette for at most 256 colours, gray+alpha, RGB or RGBA, at 8 bits when every sample of a uint16 image is a multiple of 257.
     A colour-coded mask becomes a palette file, an RGB binary mask a 1-bit file, an opaque RGBA render an fpng RGB file.  The
     slots are then reduced_slot_offsets of the shapes.  get_info_batch_device / get_png_info report the format written.  The call
-    waits once on the host, for the analysis of the images, before it enqueues the encode."""
+    waits once on the host, for the analysis of the images, before it enqueues the encode.
+
+    lz77=K (1 to 256; include/fpng_b200.h, FPNGB_LZ77_CHAIN) writes every image, 8-bit RGB and RGBA included, as a PNG whose
+    stream holds LZ77 matches at any distance up to 32 KiB and across rows, found by a hash-chain search of depth K; no fpng
+    file is written.  Whether that is smaller than the default files depends on the content (DESIGN §4.6 "LZ77").  Slots and
+    offsets are unchanged.  It combines with reduce and FPNG_FORCE_UNCOMPRESSED, not with FPNG_ENCODE_SLOWER.  The files decode
+    through the any-PNG inflate, one warp per file."""
     import torch
 
+    flags |= _lz77_flags(lz77, "encode_png_device")
     n = len(images)
     dtypes = {t.dtype for t in images}
     floats = {torch.float32, torch.float16, torch.bfloat16}
@@ -456,7 +470,7 @@ def label_slot_offsets(shapes, palettes=None):
     return ofs
 
 
-def encode_labels_device(images, palette=None, depth=None, flags: int = 0, out=None, stream=None):
+def encode_labels_device(images, palette=None, depth=None, flags: int = 0, out=None, stream=None, lz77=0):
     """Encode label maps (class ids, masks) on the GPU to palette or gray PNGs in one call (fpngb_encode_label_ragged_device).
 
     images: list of CUDA tensors [h, w] or [h, w, 1], torch.uint8 or torch.int64 ids (the output of logits.argmax(1)[i] goes in
@@ -469,9 +483,11 @@ def encode_labels_device(images, palette=None, depth=None, flags: int = 0, out=N
     unaffected.  Returns (out uint8 [total], offsets int64 [n + 1], sizes int32 [n]) as encode_png_device does, offsets being
     label_slot_offsets -- the (data, offsets, sizes) decode_packed_ragged_device(any_png=True, all_formats=True) reads, with
     indices=True giving the ids back.  Kernels are enqueued on the current torch stream (or `stream`), with no host
-    synchronisation.  Other dtypes, shapes and argument values raise ValueError."""
+    synchronisation.  Other dtypes, shapes and argument values raise ValueError.  lz77=K (1 to 256): the LZ77 mode of
+    encode_png_device."""
     import torch
 
+    lz_flags = _lz77_flags(lz77, "encode_labels_device")
     n = len(images)
     if n == 0:
         raise ValueError("encode_labels_device: at least one image is needed")
@@ -522,7 +538,7 @@ def encode_labels_device(images, palette=None, depth=None, flags: int = 0, out=N
     dims = np.array(dims, dtype=np.uint32).reshape(n, 4)
     strides = np.array(strides, dtype=np.uint64).reshape(n, 2)
     rc = lib().fpngb_encode_label_ragged_device(n, ptrs.ctypes.data_as(C.c_void_p), dims.ctypes.data_as(C.c_void_p),
-                                                strides.ctypes.data_as(C.c_void_p), C.cast(structs, C.c_void_p), flags,
+                                                strides.ctypes.data_as(C.c_void_p), C.cast(structs, C.c_void_p), flags | lz_flags,
                                                 out.data_ptr(), out.numel(), offsets.data_ptr(), sizes.data_ptr(),
                                                 _stream(stream, device))
     check(rc, "encode_labels_device")

@@ -152,8 +152,9 @@ Context& context() { return g_ctx; }
 // Optional per-kernel timing with CUDA events on the launching stream (bench.py's roofline numbers).
 // kProfConvert: the conversion pre-pass (convert_pixels_kernel), which runs before the first slot and has its own start event.
 // kProfReduce: the colour-type analysis of FPNGB_ENCODE_REDUCE (analysis and palette finalise), before the conversion, own start event.
+// kProfMatch: the LZ77 match kernel, between the filter pass (kProfHist) and the Huffman build (kProfHuff), which then starts at its end.
 enum ProfSlot { kProfHist = 0, kProfHuff, kProfScan, kProfOffsets, kProfFused, kProfFinish, kProfPack, kProfAdler, kProfCrc, kProfConvert,
-                kProfReduce, kProfSlots };
+                kProfReduce, kProfMatch, kProfSlots };
 struct ProfSet {
     cudaEvent_t ev[kProfSlots + 1]; cudaEvent_t crc_start, conv_start, red_start; bool used[kProfSlots]; bool crc_side; uint64_t call;
 };
@@ -607,9 +608,10 @@ static void make_png_enc_header(uint8_t* hdr, uint32_t w, uint32_t h, uint32_t c
     memcpy(hdr + 37, "IDAT", 4);
 }
 
-// the (bytes per pixel, depth) classes of the PNG row kernels: gray8, GA8, gray16, GA16, RGB16, RGBA16
-constexpr int kPngClasses = 6;
-static const uint32_t kPngClassBpp[kPngClasses] = {1, 2, 2, 4, 6, 8}, kPngClassDepth[kPngClasses] = {8, 8, 16, 16, 16, 16};
+// the (bytes per pixel, depth) classes of the PNG row kernels: gray8, GA8, gray16, GA16, RGB16, RGBA16, and in LZ77 mode only
+// RGB8 and RGBA8
+constexpr int kPngClasses = 8;
+static const uint32_t kPngClassBpp[kPngClasses] = {1, 2, 2, 4, 6, 8, 3, 4}, kPngClassDepth[kPngClasses] = {8, 8, 16, 16, 16, 16, 8, 8};
 static int png_class(uint32_t bpp, uint32_t depth)
 {
     for (int k = 0; k < kPngClasses; k++) if (kPngClassBpp[k] == bpp && kPngClassDepth[k] == depth) return k;
@@ -617,11 +619,24 @@ static int png_class(uint32_t bpp, uint32_t depth)
 }
 
 // bytes of the descriptor table, work lists and container headers (hdr_bytes in all) encode_png_locked stages for m images
-static size_t png_table_bytes(size_t m, size_t hdr_bytes) { return align_up(m * sizeof(ImageDesc), 16) + m * 4 * 4 + hdr_bytes; }
+static size_t png_table_bytes(size_t m, size_t hdr_bytes) { return align_up(m * sizeof(ImageDesc), 16) + m * 5 * 4 + hdr_bytes; }
+
+// LZ77 mode (FPNGB_LZ77_CHAIN): the chain depth K of the flags, 0 when the mode is off
+static uint32_t lz77_chain(uint32_t flags) { return (flags >> 16) & 0x1FFu; }
+// the chain bits hold at most 256, and the mode writes no fpng file, so FPNGB_ENCODE_SLOWER has no meaning in it
+static bool lz77_flags_ok(uint32_t flags)
+{
+    const uint32_t k = lz77_chain(flags);
+    return k <= 256 && !(k && (flags & FPNGB_ENCODE_SLOWER));
+}
+constexpr uint32_t kLz77FlagBits = 0x1FFu << 16;
 
 // Enqueues the PNG pipeline for images im[k] (k in `ids`, depth[k] bits per sample) into their slots.  Caller holds ctx.mu.
 // Launches: per non-empty (bytes per pixel, depth) class a filter/histogram, a row-size and a pack kernel, then four per-image
 // kernels: Huffman build, offsets, Adler-32, stream CRC.  own_call: no fpng pipeline ran in this call (a new profile call).
+// With a chain depth in flags (LZ77 mode): per class a filter pass into S and a stored-row pass, and per call the match kernel
+// and two segment kernels (bits, pack) in place of the row-size and pack kernels; the workspace adds S, its tokens (2 bytes per
+// byte of S) and 16 bytes per segment.
 // hdrs: the container header of image k is (*hdrs)[k] (a label map's, with PLTE / tRNS), or the 41-byte make_png_enc_header
 // one when hdrs is null; d_bad: the label pre-pass's per-image flags (size 0 for a flagged image), or null.
 static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, const std::vector<uint32_t>& depth, const std::vector<uint32_t>& ids,
@@ -630,7 +645,9 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
 {
     const uint32_t m = (uint32_t)ids.size();
     const uint32_t rpc = png_rows_per_cta();
+    const uint32_t chain = lz77_chain(flags);
     size_t rows = 0;
+    uint64_t s_bytes = 0, segs = 0;                                           // LZ77 mode: S and its segments
     std::vector<int> cls(m);
     uint32_t cls_count[kPngClasses] = {0};
     for (uint32_t j = 0; j < m; j++) {
@@ -638,7 +655,12 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
         rows += r.h;
         cls[j] = png_class(r.chans * depth[ids[j]] / 8, depth[ids[j]]);
         cls_count[cls[j]]++;
+        if (chain) {
+            const uint64_t N = ((uint64_t)r.w * (r.chans * depth[ids[j]] / 8) + 1) * r.h;
+            s_bytes += align_up(N, 16); segs += (N + kLzSegment - 1) / kLzSegment;
+        }
     }
+    if (segs > 0x7FFFFFFFull) return FPNGB_ERR_INVALID_ARG;
     size_t hdr_bytes = 0;
     for (uint32_t k : ids) hdr_bytes += hdrs ? (*hdrs)[k].size() : kPngEncHeaderSize;
     const size_t table = png_table_bytes(m, hdr_bytes);
@@ -651,6 +673,12 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
     const size_t o_hist = o; o = align_up(o + (size_t)m * 288 * 4, 256);
     const size_t o_books = o; o = align_up(o + (size_t)m * sizeof(CodeBook), 256);
     const size_t o_table = o; o = align_up(o + table, 256);
+    const size_t o_s = o; o = align_up(o + s_bytes, 256);
+    const size_t o_tok = o; o = align_up(o + 2 * s_bytes, 256);
+    const size_t o_segu = o; o = align_up(o + segs * 4, 256);
+    const size_t o_segb = o; o = align_up(o + segs * 4, 256);
+    const size_t o_sego = o; o = align_up(o + segs * 8, 256);
+    const size_t o_dhist = o; o = align_up(o + (chain ? (size_t)m * 32 * 4 : 0), 256);
     int rc = c.ws.reserve(o);
     if (rc) return rc;
     rc = c.ws_acquire(s);
@@ -661,14 +689,16 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
     p.row_filter = b + o_filt; p.st = (ImageState*)(b + o_st); p.hist = (uint32_t*)(b + o_hist);
     CodeBook* books = (CodeBook*)(b + o_books);
     const ImageDesc* d_desc = (const ImageDesc*)(b + o_table);
-    const size_t lists_at = align_up((size_t)m * sizeof(ImageDesc), 16), hdr_at = lists_at + (size_t)m * 4 * 4;
+    const size_t lists_at = align_up((size_t)m * sizeof(ImageDesc), 16), hdr_at = lists_at + (size_t)m * 5 * 4;
     p.out = d_out; p.sizes = d_sizes; p.flags = flags; p.desc = d_desc; p.headers = (const uint8_t*)d_desc + hdr_at; p.bad = d_bad;
 
     // the table in staging: ImageDesc[m] | row-kernel img[] and CTA prefix[] per class, in class order | crc img[], crc prefix[] |
-    // the container headers
+    // LZ77 segment prefix[] | the container headers
     ImageDesc* desc = (ImageDesc*)stage;
     uint32_t* lists = (uint32_t*)(stage + lists_at);
     uint32_t* l_img = lists; uint32_t* l_cta = lists + m; uint32_t* l_crc_img = lists + 2 * m; uint32_t* l_crc = lists + 3 * m;
+    uint32_t* l_seg = lists + 4 * m;
+    uint64_t s_fill = 0, seg_fill = 0;
     uint8_t* headers = stage + hdr_at;
     uint32_t hdr_fill = 0;
     uint32_t cls_first[kPngClasses], fill[kPngClasses];
@@ -693,6 +723,10 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
         }
         hdr_fill += d.hdr_len;
         row_base += r.h;
+        const uint64_t N = ((uint64_t)r.w * bpp + 1) * r.h;
+        d.lz_ofs = s_fill; d.seg_base = seg_fill; d.nseg = (uint32_t)((N + kLzSegment - 1) / kLzSegment);
+        l_seg[j] = (uint32_t)seg_fill;
+        if (chain) { s_fill += align_up(N, 16); seg_fill += d.nseg; }
         const int k = cls[j];
         const uint32_t q = fill[k]++;
         l_img[q] = j; l_cta[q] = (uint32_t)cls_ctas[k]; cls_ctas[k] += (r.h + rpc - 1) / rpc;
@@ -716,17 +750,48 @@ static int encode_png_locked(Context& c, const std::vector<RaggedImage>& im, con
     };
 
     FPNGB_CUDA_OK(cudaMemsetAsync(p.hist, 0, (size_t)m * 288 * 4, s));
-    rows_pass(0);
-    prof_mark(ps, kProfHist, s);
-    HuffParams hp{p.hist, books, 0u, 0u, d_desc};
-    launch_huffman_build_png(hp, m, s);
-    prof_mark(ps, kProfHuff, s);
-    rows_pass(1);
-    prof_mark(ps, kProfScan, s);
-    launch_png_offsets(p, m, s);
-    prof_mark(ps, kProfOffsets, s);
-    rows_pass(2);
-    prof_mark(ps, kProfPack, s);
+    if (chain) {
+        PngLzParams q{p};
+        q.lz_s = b + o_s; q.lz_tok = (uint16_t*)(b + o_tok); q.seg_units = (uint32_t*)(b + o_segu); q.seg_bits = (uint32_t*)(b + o_segb);
+        q.seg_ofs = (unsigned long long*)(b + o_sego); q.dhist = (uint32_t*)(b + o_dhist); q.chain = chain;
+        auto lz_rows_pass = [&](int mode) {
+            for (int k = 0; k < kPngClasses; k++) {
+                if (!cls_count[k]) continue;
+                q.ragged = RaggedWork{d_desc, d_lists + cls_first[k], d_lists + m + cls_first[k], cls_count[k]};
+                launch_png_lz_rows(q, (uint32_t)cls_ctas[k], kPngClassBpp[k], kPngClassDepth[k], mode, s);
+                launches++;
+            }
+        };
+        FPNGB_CUDA_OK(cudaMemsetAsync(q.dhist, 0, (size_t)m * 32 * 4, s));
+        lz_rows_pass(0);
+        prof_mark(ps, kProfHist, s);
+        q.ragged = RaggedWork{d_desc, d_lists + 2 * (size_t)m, d_lists + 4 * (size_t)m, m};    // one CTA per segment
+        launch_lz_match(q, (uint32_t)segs, s);
+        prof_mark(ps, kProfMatch, s);
+        HuffParams hp{p.hist, books, 0u, 0u, d_desc, q.dhist};
+        launch_huffman_build_lz(hp, m, s);
+        prof_mark(ps, kProfHuff, s);
+        launch_lz_segments(q, (uint32_t)segs, false, s);
+        prof_mark(ps, kProfScan, s);
+        launch_png_lz_offsets(q, m, s);
+        prof_mark(ps, kProfOffsets, s);
+        launch_lz_segments(q, (uint32_t)segs, true, s);
+        lz_rows_pass(1);
+        prof_mark(ps, kProfPack, s);
+        launches += 3;
+    } else {
+        rows_pass(0);
+        prof_mark(ps, kProfHist, s);
+        HuffParams hp{p.hist, books, 0u, 0u, d_desc};
+        launch_huffman_build_png(hp, m, s);
+        prof_mark(ps, kProfHuff, s);
+        rows_pass(1);
+        prof_mark(ps, kProfScan, s);
+        launch_png_offsets(p, m, s);
+        prof_mark(ps, kProfOffsets, s);
+        rows_pass(2);
+        prof_mark(ps, kProfPack, s);
+    }
     AdlerParams ap{p.row_adler, p.st, d_out, 0, 0, 0, 0, d_desc};
     launch_adler_finalize_png(ap, m, s);
     prof_mark(ps, kProfAdler, s);
@@ -891,7 +956,7 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         const uint32_t w = dims[4 * i], h = dims[4 * i + 1], chans = dims[4 * i + 2], dep = dims[4 * i + 3];
         if (!pixels[i] || (dep != 8 && dep != 16) || chans < 1 || chans > 4) return FPNGB_ERR_INVALID_ARG;
         const uint32_t es = typed ? f.elem : dep / 8, bpp = chans * dep / 8;   // input element and output pixel bytes
-        const bool fpng = dep == 8 && chans >= 3;                        // fpng's files, as fpngb_encode_ragged_device writes them
+        const bool fpng = dep == 8 && chans >= 3 && !lz77_chain(flags);  // fpng's files, as fpngb_encode_ragged_device writes them
         if (fpng ? !valid_dims(w, h, chans)
                  : (w < 1 || h < 1 || w > (1u << 24) || h > (1u << 24) || max_encoded_size(w, h, bpp) > 0x7FFFFFFFull))
             return FPNGB_ERR_INVALID_ARG;                                 // one IDAT chunk must hold the stored file
@@ -928,7 +993,7 @@ static int encode_images_impl(uint32_t n, const uint64_t* pixels, const uint32_t
         if (rc) { c.ws_release(s); return rc; }
         fpng_ids.clear(); png_ids.clear(); png_hdr_bytes = 0;
         for (uint32_t i = 0; i < n; i++) {
-            const bool fpng = depth[i] == 8 && im[i].chans >= 3;
+            const bool fpng = depth[i] == 8 && im[i].chans >= 3 && !lz77_chain(flags);
             (fpng ? fpng_ids : png_ids).push_back(i);
             if (!fpng) png_hdr_bytes += hdrs[i].size();
         }
@@ -1190,10 +1255,8 @@ static int reduce_images_locked(Context& c, std::vector<RaggedImage>& im, const 
             out_depth = ch.depth;
             d.mode = 2; d.bits = out_chans; d.out_bytes = out_depth / 8;
             d.words = (uint32_t)(((uint64_t)r.w * out_chans * d.out_bytes + 3) / 4);
-            if (out_depth != 8 || out_chans < 3) {
-                hdrs[i].resize(kPngEncHeaderSize);
-                make_png_enc_header(hdrs[i].data(), r.w, r.h, out_chans, out_depth);
-            }
+            hdrs[i].resize(kPngEncHeaderSize);                                // also read for RGB8 / RGBA8 in LZ77 mode
+            make_png_enc_header(hdrs[i].data(), r.w, r.h, out_chans, out_depth);
             if (out_chans == r.chans && out_depth == depth[i]) continue;      // read in place, as without the flag
         }
         conv.push_back(d);
@@ -1213,7 +1276,7 @@ int fpngb_encode_label_ragged_device(uint32_t n, const uint64_t* pixels, const u
                                      uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (flags & ~(uint32_t)FPNGB_FORCE_UNCOMPRESSED) return FPNGB_ERR_INVALID_ARG;
+    if ((flags & ~(uint32_t)(FPNGB_FORCE_UNCOMPRESSED | kLz77FlagBits)) || !lz77_flags_ok(flags)) return FPNGB_ERR_INVALID_ARG;
     if (n == 0 || n > 65535 || !pixels || !dims || !d_out || !d_out_offsets || !d_sizes) return FPNGB_ERR_INVALID_ARG;
     std::vector<RaggedImage> im(n);
     std::vector<uint32_t> depth(n), ids(n);
@@ -1296,7 +1359,8 @@ int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels, const uin
                                    void* d_out, size_t out_cap, uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED | FPNGB_ENCODE_REDUCE)) return FPNGB_ERR_INVALID_ARG;
+    if ((flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED | FPNGB_ENCODE_REDUCE | kLz77FlagBits)) || !lz77_flags_ok(flags))
+        return FPNGB_ERR_INVALID_ARG;
     return encode_images_impl(n, pixels, dims, strides, false, nullptr, flags, d_out, out_cap, d_out_offsets, d_sizes, stream,
                               (flags & FPNGB_ENCODE_REDUCE) != 0);
 }
@@ -1306,7 +1370,8 @@ int fpngb_encode_png_ragged_device_typed(uint32_t n, const uint64_t* pixels, con
                                          uint64_t* d_out_offsets, uint32_t* d_sizes, void* stream)
 {
     if (!g_ctx.ready) return FPNGB_ERR_NOT_INITIALIZED;
-    if (flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED)) return FPNGB_ERR_INVALID_ARG;
+    if ((flags & ~(uint32_t)(FPNGB_ENCODE_SLOWER | FPNGB_FORCE_UNCOMPRESSED | kLz77FlagBits)) || !lz77_flags_ok(flags))
+        return FPNGB_ERR_INVALID_ARG;
     return encode_images_impl(n, pixels, dims, strides, true, fmt, flags, d_out, out_cap, d_out_offsets, d_sizes, stream);
 }
 
@@ -1446,7 +1511,7 @@ int fpngb_encode_batch_host(const void* pixels, size_t image_stride, uint32_t n,
 // Per-kernel device times (ms) averaged over the encode calls since the last read; slots in ProfSlot order:
 // hist, huffman, scan, offsets, fused, finish, pack, adler, crc, conversion pre-pass (slot 9: the *_typed calls, the uint8 copy of a
 // strided batch bound for the single-pass encoder, the label and reduce pre-passes), colour-type analysis (slot 10:
-// FPNGB_ENCODE_REDUCE).  A caller asking for 9 slots gets the first nine.  Returns the number
+// FPNGB_ENCODE_REDUCE), LZ77 match kernel (slot 11: FPNGB_LZ77_CHAIN).  A caller asking for 9 slots gets the first nine.  Returns the number
 // of calls averaged.
 FPNGB_API int fpngb_profile_enable(int on)
 {
@@ -1468,8 +1533,10 @@ FPNGB_API int fpngb_profile_read(float* ms, int nslots)
             cudaEventSynchronize(ps->ev[i + 1]);
             // the CRC of a chunk may run on the side stream, overlapped with the next chunk: its own start event brackets it
             // and the conversion pre-pass, which runs before slot 0 opens
-            const bool own_start = (i == kProfCrc && ps->crc_side) || i == kProfConvert || i == kProfReduce;
-            cudaEvent_t from = i == kProfConvert ? ps->conv_start : i == kProfReduce ? ps->red_start : own_start ? ps->crc_start : ps->ev[last];
+            const bool own_start = (i == kProfCrc && ps->crc_side) || i == kProfConvert || i == kProfReduce || i == kProfMatch;
+            cudaEvent_t from = i == kProfConvert ? ps->conv_start : i == kProfReduce ? ps->red_start : i == kProfMatch ? ps->ev[kProfHist + 1]
+                             : own_start ? ps->crc_start : ps->ev[last];
+            if (i == kProfHuff && ps->used[kProfMatch]) from = ps->ev[kProfMatch + 1];
             if (cudaEventElapsedTime(&t, from, ps->ev[i + 1]) == cudaSuccess) sum[i] += t;
             if (!own_start) last = i + 1;
         }

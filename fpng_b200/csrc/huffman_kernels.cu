@@ -115,12 +115,17 @@ struct DevBitWriter {
 // PNG: the books of fpngb_encode_png_ragged_device, where p.desc's chans is B, the bytes per pixel.  The distance table is
 //   {d(B): 1 bit, d(B) + 1: 1 bit} with d(B) + 2 codes (d(B) the distance code of distance B; for B = 3, 4 fpng's table), and
 //   match[j] holds length symbol 257 + j as code | size << 16 (j < 29) instead of fpng's matches in pixels
-template <bool RAGGED = false, bool PNG = false>
+// LZ (with PNG): the LZ77 books.  The distance code is built from p.dhist by the same construction, or, with fewer than two
+//   distance symbols used, is {s: 1 bit, s ^ 1: 1 bit} for the used symbol s (0 if none); HDIST is its last symbol of nonzero
+//   length + 1; match[32 + j] holds distance symbol j as code | size << 16 (j < 30)
+template <bool RAGGED = false, bool PNG = false, bool LZ = false>
 __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
 {
     __shared__ HuffScratch s;
     __shared__ uint8_t s_size0[288];
     __shared__ uint16_t s_code0[288];
+    __shared__ uint8_t s_dsize[LZ ? 30 : 1];
+    __shared__ uint16_t s_dcode[LZ ? 30 : 1];
     const uint32_t img = blockIdx.x, lane = threadIdx.x;
     const uint32_t* hist = p.hist + (size_t)img * 288;
     CodeBook* cb = p.books + img;
@@ -155,13 +160,48 @@ __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
     for (uint32_t i = lane; i < 288; i += 32) { s_size0[i] = s.size[i]; s_code0[i] = s.code[i]; }
     __syncwarp();
 
+    // --- LZ77 distance table (limit 12), from 16-bit scaled counts
+    if constexpr (LZ) {
+        if (lane == 0) {
+            const uint32_t* dh = p.dhist + (size_t)img * 32;
+            uint32_t tot = 0, n = 0;
+            for (uint32_t i = 0; i < 30; i++) tot += dh[i];
+            for (uint32_t i = 0; i < 30; i++) if (dh[i]) {
+                const uint32_t v = (uint32_t)(((unsigned long long)dh[i] * 65535ull) / tot);
+                s.ukey[n] = (uint16_t)(v < 1 ? 1 : v); s.usym[n] = (uint16_t)i; n++;
+            }
+            s.n_used = n;
+        }
+        __syncwarp();
+        const uint32_t n = s.n_used;
+        rank_sort(s, n, lane);
+        if (lane == 0) {
+            if (n >= 2) {
+                lengths_and_codes(s, (int)n, 30, 12);
+                for (int i = 0; i < 30; i++) { s_dsize[i] = s.size[i]; s_dcode[i] = s.code[i]; }
+            } else {
+                const uint32_t u = n ? s.usym[0] : 0u;
+                for (int i = 0; i < 30; i++) { s_dsize[i] = 0; s_dcode[i] = 0; }
+                s_dsize[u] = s_dsize[u ^ 1u] = 1;
+                s_dcode[u | 1u] = 1;                        // canonical: the lower symbol gets 0
+            }
+        }
+        __syncwarp();
+    }
+
     // --- header (lane 0): the distance table is always {chans-1: 1 bit, chans: 1 bit} (fpng.cpp:1096-1098)
     if (lane == 0) {
         const int dsym = PNG ? (chans <= 4 ? (int)chans - 1 : (chans <= 6 ? 4 : 5)) : (int)chans - 1;
         int nlit = 286, ndist = dsym + 2;
         while (nlit > 257 && !s_size0[nlit - 1]) nlit--;
         for (int i = 0; i < nlit; i++) s.seq[i] = s_size0[i];
-        for (int i = 0; i < ndist; i++) s.seq[nlit + i] = (i == dsym || i == dsym + 1) ? 1 : 0;
+        if constexpr (LZ) {
+            ndist = 30;
+            while (!s_dsize[ndist - 1]) ndist--;
+            for (int i = 0; i < ndist; i++) s.seq[nlit + i] = s_dsize[i];
+        } else {
+            for (int i = 0; i < ndist; i++) s.seq[nlit + i] = (i == dsym || i == dsym + 1) ? 1 : 0;
+        }
         const int totalc = nlit + ndist;
         uint16_t cnt2[19];
         for (int i = 0; i < 19; i++) cnt2[i] = 0;
@@ -226,7 +266,9 @@ __global__ void __launch_bounds__(32) huffman_build_kernel(HuffParams p)
     for (uint32_t i = lane; i < 288; i += 32) cb->sym_size[i] = s_size0[i];
     if constexpr (PNG) {
         for (uint32_t j = lane; j < 88; j += 32) {
-            cb->match[j] = j < 29 ? s_code0[257 + j] | ((uint32_t)s_size0[257 + j] << 16) : 0u;
+            uint32_t v = j < 29 ? s_code0[257 + j] | ((uint32_t)s_size0[257 + j] << 16) : 0u;
+            if (LZ && j >= 32 && j < 62) v = s_dcode[j - 32] | ((uint32_t)s_dsize[j - 32] << 16);
+            cb->match[j] = v;
             cb->match_bits[j] = 0;
         }
         return;
@@ -258,6 +300,11 @@ void launch_huffman_build_ragged(const HuffParams& p, uint32_t n, cudaStream_t s
 void launch_huffman_build_png(const HuffParams& p, uint32_t n, cudaStream_t s)
 {
     huffman_build_kernel<true, true><<<n, 32, 0, s>>>(p);
+}
+
+void launch_huffman_build_lz(const HuffParams& p, uint32_t n, cudaStream_t s)
+{
+    huffman_build_kernel<true, true, true><<<n, 32, 0, s>>>(p);
 }
 
 }  // namespace fpngb

@@ -23,6 +23,9 @@ struct ImageDesc {
     uint8_t pad_[2];
     uint32_t hdr_len;                             // PNG call: container header bytes L (41, or 41 + PLTE / tRNS for a label map),
     uint32_t hdr_at;                              // staged at PngEncParams::headers + hdr_at; the zlib stream starts at file byte L
+    unsigned long long lz_ofs;                    // LZ77 PNG call: byte offset of the image's filtered stream S in PngEncParams::lz_s
+    unsigned long long seg_base;                  // LZ77 PNG call: the image's first segment in the seg_* tables
+    uint32_t nseg, pad2_;                         // LZ77 PNG call: segments of S (ceil(N / kLzSegment))
 };
 
 // The images one ragged launch covers: CTA b works on image img[j] for the j with cta_start[j] <= b < cta_start[j + 1] (every
@@ -124,6 +127,7 @@ struct HuffParams {
     uint32_t chans;
     uint32_t training;                            // 1: table training (fpng.cpp:909-988): symbol 256 keeps its own count in the scaling
     const ImageDesc* desc;                        // ragged kernel: the channel count of image blockIdx.x
+    const uint32_t* dhist;                        // LZ77 PNG books: [n*32] distance-symbol histogram
 };
 
 // fpngb_encode_png_ragged_device and fpngb_encode_label_ragged_device (png_encode_kernels.cu): the images are ImageDesc entries
@@ -143,11 +147,33 @@ struct PngEncParams {
     const uint32_t* bad;                          // [call images] nonzero: a label map with an out-of-range id, size 0 (nullptr: none)
     RaggedWork ragged;                            // the images and CTA map of a row-kernel launch
 };
+// LZ77 mode (FPNGB_LZ77_CHAIN): S, its tokens (one 16-bit unit per byte of S at most, at the same index) and per-segment records.
+// (A separate type, so that the other PNG kernels' parameter block stays as it is.)
+struct PngLzParams : PngEncParams {
+    uint8_t* lz_s;                                // the images' filtered streams (ImageDesc::lz_ofs)
+    uint16_t* lz_tok;                             // literal v < 256 | 256 + match length | 0x8000 + distance - 1
+    uint32_t* seg_units;                          // [segments] token units of each segment
+    uint32_t* seg_bits;                           // [segments] code bits of each segment
+    unsigned long long* seg_ofs;                  // [segments] file bit offset of each segment
+    uint32_t* dhist;                              // [m * 32] distance-symbol histogram
+    uint32_t chain;                               // K: candidates walked per position
+};
+constexpr uint32_t kLzSegment = 16384;            // bytes of S parsed independently (include/fpng_b200.h, "LZ77")
+constexpr uint32_t kLzWindow = 32768;             // largest match distance
 uint32_t png_rows_per_cta();
 // mode 0: filter choice + histogram, 1: row bits, 2: pack; one launch over the images of one (bpp, depth) class
 void launch_png_rows(const PngEncParams& p, uint32_t ctas, uint32_t bpp, uint32_t depth, int mode, cudaStream_t s);
 void launch_png_offsets(const PngEncParams& p, uint32_t n, cudaStream_t s);
 void launch_huffman_build_png(const HuffParams& p, uint32_t n, cudaStream_t s);
+// LZ77 mode: mode 0 filter choice writing S and the row Adler partials, 1 the raw rows of the images that fell back to stored
+// blocks; classes also RGB8 (bpp 3) and RGBA8 (bpp 4, depth 8)
+void launch_png_lz_rows(const PngLzParams& p, uint32_t ctas, uint32_t bpp, uint32_t depth, int mode, cudaStream_t s);
+void launch_png_lz_offsets(const PngLzParams& p, uint32_t n, cudaStream_t s);
+void launch_huffman_build_lz(const HuffParams& p, uint32_t n, cudaStream_t s);
+// lz77_kernels.cu: one CTA per segment over p.ragged (cta_start: the images' seg_base); match search and greedy parse, then the
+// code bits of each segment, then the pack
+void launch_lz_match(const PngLzParams& p, uint32_t segs, cudaStream_t s);
+void launch_lz_segments(const PngLzParams& p, uint32_t segs, bool pack, cudaStream_t s);
 void launch_adler_finalize_png(const AdlerParams& p, uint32_t n, cudaStream_t s);
 
 // opt in to > 48 KiB of dynamic shared memory (per kernel instantiation, once per process)

@@ -15,6 +15,10 @@
 // pixels that differ from their left neighbour, carried across steps; every token is written by the lane of the pixel it ends on
 // (a full match of floor(258 / B) pixels), or by the pixel that ends the run (the run's remainder), so no lane looks ahead.
 // The pack kernel re-tokenises the rows instead of reading stored tokens (DESIGN §4.6).
+//
+// LZ77 mode (FPNGB_LZ77_CHAIN) uses two more modes of the row kernel, also for RGB8 and RGBA8: kPngFilt chooses the filter as
+// kPngHist does and writes the filtered row, filter byte first, into the image's stream S with the row's Adler partials;
+// kPngRaw writes the raw rows of the images that fell back to stored blocks.  lz77_kernels.cu tokenises and packs S.
 #include "row_walk.cuh"
 #include "kernels.cuh"
 
@@ -22,7 +26,7 @@ namespace fpngb {
 
 constexpr int kPngRows = 8;                       // warps (scanlines) per CTA
 constexpr int kPngStageWords = 136;               // >= (31 + 32 * 116 + 12) / 32 + 1: one step's codes, 116 bits per lane at most
-enum { kPngHist = 0, kPngBits = 1, kPngPack = 2 };
+enum { kPngHist = 0, kPngBits = 1, kPngPack = 2, kPngFilt = 3, kPngRaw = 4 };
 
 uint32_t png_rows_per_cta() { return kPngRows; }
 
@@ -151,8 +155,8 @@ __device__ __forceinline__ void pixel_tokens(Sink& k, bool eq, uint32_t x, uint3
     }
 }
 
-template <int B, int ES, int MODE>
-__global__ void __launch_bounds__(32 * kPngRows) png_row_kernel(PngEncParams p)
+template <int B, int ES, int MODE, class P = PngEncParams>
+__global__ void __launch_bounds__(32 * kPngRows) png_row_kernel(P p)
 {
     __shared__ uint32_t s_hist[MODE == kPngHist ? 288 : 1];
     __shared__ uint32_t s_lit[MODE == kPngHist ? 1 : 256];        // code | size << 16
@@ -165,10 +169,11 @@ __global__ void __launch_bounds__(32 * kPngRows) png_row_kernel(PngEncParams p)
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint32_t y = local * kPngRows + warp, w = d.w, h = d.h;
     const CodeBook* book = d.book;
-    const bool stored = MODE == kPngPack && p.st[img].stored;
+    const bool stored = (MODE == kPngPack || MODE == kPngRaw) && p.st[img].stored;
+    if (MODE == kPngRaw && !stored) return;
     if (MODE == kPngHist) {
         for (uint32_t i = threadIdx.x; i < 288; i += blockDim.x) s_hist[i] = 0u;
-    } else if (!stored) {
+    } else if (!stored && MODE != kPngFilt) {
         for (uint32_t i = threadIdx.x; i < 256; i += blockDim.x) s_lit[i] = book->lit[i];
         if (threadIdx.x < 29) s_len[threadIdx.x] = book->match[threadIdx.x];
         if (MODE == kPngPack) for (uint32_t i = lane; i < kPngStageWords; i += 32) s_stage[warp][i] = 0u;
@@ -194,7 +199,7 @@ __global__ void __launch_bounds__(32 * kPngRows) png_row_kernel(PngEncParams p)
         }
 
         uint32_t ft;
-        if (MODE == kPngHist) {                                                 // the filter with the smallest cost, ties to the lower id
+        if (MODE == kPngHist || MODE == kPngFilt) {                                                 // the filter with the smallest cost, ties to the lower id
             uint32_t cost[5] = {0u, 0u, 0u, 0u, 0u};
             uint2 ca = make_uint2(0u, 0u), cc = ca;
             for (uint32_t x0 = 0; x0 < w; x0 += 32) {
@@ -214,6 +219,37 @@ __global__ void __launch_bounds__(32 * kPngRows) png_row_kernel(PngEncParams p)
             if (lane == 0) p.row_filter[r] = (uint8_t)ft;
         } else {
             ft = p.row_filter[r];
+        }
+
+        if constexpr (MODE == kPngFilt) {                                       // S row: filter byte, filtered bytes; Adler partials
+            uint8_t* srow = p.lz_s + d.lz_ofs + (unsigned long long)y * (bpl + 1u);
+            unsigned long long s1 = 0, si = 0;
+            uint2 ca = make_uint2(0u, 0u), cc = ca;
+            for (uint32_t x0 = 0; x0 < w; x0 += 32) {
+                const uint32_t x = x0 + lane;
+                const bool valid = x < w;
+                const uint2 cx = valid ? load_png_px<B, ES>(row, x, ps, cs) : make_uint2(0u, 0u);
+                const uint2 bx = (valid && y) ? load_png_px<B, ES>(up, x, ps, cs) : make_uint2(0u, 0u);
+                uint2 a = shfl_up2(cx), c = shfl_up2(bx);
+                if (lane == 0) { a = ca; c = cc; }
+                ca = shfl_last2(cx); cc = shfl_last2(bx);
+                if (valid) {
+                    const uint2 fx = filter_png_px<B>(ft, cx, a, bx, c);
+#pragma unroll
+                    for (int j = 0; j < B; j++) {
+                        const uint32_t v = byte_of(fx, j);
+                        srow[1u + x * B + j] = (uint8_t)v;
+                        s1 += v; si += (1ull + (unsigned long long)x * B + j) * v;
+                    }
+                }
+            }
+            s1 = warp_sum_u64(s1); si = warp_sum_u64(si);
+            if (lane == 0) {
+                srow[0] = (uint8_t)ft;
+                const unsigned long long S1 = s1 + ft, n = (unsigned long long)bpl + 1ull;
+                p.row_adler[r] = make_uint2((uint32_t)(S1 % kAdlerMod), (uint32_t)((n * S1 - si) % kAdlerMod));
+            }
+            return;
         }
 
         HistSink hs{s_hist};
@@ -310,26 +346,32 @@ __device__ __forceinline__ void store_be32_png(uint8_t* q, uint32_t v)
 // compressed zlib stream would be longer), the L-byte container header (L = hdr_len) with the IDAT length at L - 8, the zlib and
 // block headers, the stored block headers or the end-of-block code, the IEND chunk and the file size (0 for a label map with an
 // out-of-range id: the file is written in its slot all the same, and read by nothing).  Zeroes the words neighbouring rows share.
-__global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncParams p)
+// LZ (P = PngLzParams): the units are the image's segments of S (seg_bits / seg_ofs) instead of its rows.
+template <class P>
+__device__ __forceinline__ void png_offsets_body(const P& p)
 {
+    constexpr bool LZ = std::is_same<P, PngLzParams>::value;
     __shared__ unsigned long long s_warp[kOffsetsThreads / 32];
     const uint32_t img = blockIdx.x, tid = threadIdx.x;
     const ImageDesc& d = p.desc[img];
     const CodeBook* book = d.book;
     const uint32_t h = d.h, hdr_bits = book->hdr_bits, L = d.hdr_len;
     const unsigned long long base = 8ull * L + hdr_bits;
-    const uint32_t* row_bits = p.row_bits + d.row_base;
-    unsigned long long* row_ofs = p.row_ofs + d.row_base;
+    const uint32_t* row_bits;
+    unsigned long long* row_ofs;
+    uint32_t units;
+    if constexpr (LZ) { row_bits = p.seg_bits + d.seg_base; row_ofs = p.seg_ofs + d.seg_base; units = d.nseg; }
+    else { row_bits = p.row_bits + d.row_base; row_ofs = p.row_ofs + d.row_base; units = h; }
     uint8_t* file = p.out + d.out_ofs;
     uint32_t* file_words = reinterpret_cast<uint32_t*>(file);
     ImageState* st = p.st + img;
 
     unsigned long long running = 0;
-    for (uint32_t y0 = 0; y0 < h; y0 += blockDim.x) {
+    for (uint32_t y0 = 0; y0 < units; y0 += blockDim.x) {
         const uint32_t y = y0 + tid;
         unsigned long long tot;
-        const unsigned long long ex = block_excl_scan_u64(y < h ? row_bits[y] : 0ull, s_warp, tot);
-        if (y < h) row_ofs[y] = base + running + ex;
+        const unsigned long long ex = block_excl_scan_u64(y < units ? row_bits[y] : 0ull, s_warp, tot);
+        if (y < units) row_ofs[y] = base + running + ex;
         running += tot;
     }
     const unsigned long long raw = ((unsigned long long)d.w * d.chans + 1ull) * h, nblk = (raw + 65534ull) / 65535ull;
@@ -340,7 +382,7 @@ __global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncPara
 
     __syncthreads();
     if (compressed) {
-        for (uint32_t y = 1 + tid; y < h; y += blockDim.x) file_words[row_ofs[y] >> 5] = 0u;
+        for (uint32_t y = 1 + tid; y < units; y += blockDim.x) file_words[row_ofs[y] >> 5] = 0u;
         const unsigned long long e = base + running;
         if (tid == 0) { file_words[e >> 5] = 0u; file_words[(e >> 5) + 1] = 0u; }
     }
@@ -386,6 +428,9 @@ __global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncPara
     }
 }
 
+__global__ void __launch_bounds__(kOffsetsThreads) png_offsets_kernel(PngEncParams p) { png_offsets_body(p); }
+__global__ void __launch_bounds__(kOffsetsThreads) png_lz_offsets_kernel(PngLzParams p) { png_offsets_body(p); }
+
 template <int B, int ES>
 static void launch_rows_t(const PngEncParams& p, uint32_t ctas, int mode, cudaStream_t s)
 {
@@ -408,6 +453,30 @@ void launch_png_rows(const PngEncParams& p, uint32_t ctas, uint32_t bpp, uint32_
 void launch_png_offsets(const PngEncParams& p, uint32_t n, cudaStream_t s)
 {
     png_offsets_kernel<<<n, kOffsetsThreads, 0, s>>>(p);
+}
+
+template <int B, int ES>
+static void launch_lz_rows_t(const PngLzParams& p, uint32_t ctas, int mode, cudaStream_t s)
+{
+    if (mode == 0) png_row_kernel<B, ES, kPngFilt, PngLzParams><<<ctas, 32 * kPngRows, 0, s>>>(p);
+    else png_row_kernel<B, ES, kPngRaw><<<ctas, 32 * kPngRows, 0, s>>>(p);
+}
+
+void launch_png_lz_rows(const PngLzParams& p, uint32_t ctas, uint32_t bpp, uint32_t depth, int mode, cudaStream_t s)
+{
+    switch (bpp) {
+    case 1: launch_lz_rows_t<1, 1>(p, ctas, mode, s); break;
+    case 2: if (depth == 8) launch_lz_rows_t<2, 1>(p, ctas, mode, s); else launch_lz_rows_t<2, 2>(p, ctas, mode, s); break;
+    case 3: launch_lz_rows_t<3, 1>(p, ctas, mode, s); break;
+    case 4: if (depth == 8) launch_lz_rows_t<4, 1>(p, ctas, mode, s); else launch_lz_rows_t<4, 2>(p, ctas, mode, s); break;
+    case 6: launch_lz_rows_t<6, 2>(p, ctas, mode, s); break;
+    default: launch_lz_rows_t<8, 2>(p, ctas, mode, s); break;
+    }
+}
+
+void launch_png_lz_offsets(const PngLzParams& p, uint32_t n, cudaStream_t s)
+{
+    png_lz_offsets_kernel<<<n, kOffsetsThreads, 0, s>>>(p);
 }
 
 }  // namespace fpngb

@@ -170,7 +170,8 @@ FPNGB_API int fpngb_encode_png_ragged_device(uint32_t n, const uint64_t* pixels,
  *   written and every other image of the call is as without it.  The decoders take a size of 0 as FPNGB_DECODE_INVALID_ARG.
  *   Output slots: the exclusive prefix of align_up(fpngb_max_label_encoded_size(w_i, h_i, d_i, palette_i), 16) in d_out_offsets
  *   (n + 1 entries, the last the total); d_sizes[i] the file size.  No byte of d_out past the total is written.
- *   Call-level checks, before anything is enqueued: FPNGB_ERR_INVALID_ARG for flags other than 0 / FPNGB_FORCE_UNCOMPRESSED,
+ *   Call-level checks, before anything is enqueued: FPNGB_ERR_INVALID_ARG for flags other than FPNGB_FORCE_UNCOMPRESSED and
+ *   FPNGB_LZ77_CHAIN(k),
  *   n outside 1..65535, a NULL pointer, w or h outside 1..2^24, a bad depth, elem, palette size or chans, a palette at depth 16,
  *   an unsupported layout or a slot bound above 2^31 - 1; FPNGB_ERR_BUFFER_TOO_SMALL when out_cap is below the total;
  *   FPNGB_ERR_ALIGNMENT unless d_out % 16 == 0 and each image's address and strides are multiples of elem.  A rejected call
@@ -221,6 +222,36 @@ enum { FPNGB_ENCODE_REDUCE = 256 };
  * depth 8 with a 256-entry palette and a full tRNS (which dominates for small images); every candidate format fits.  0 for chans
  * outside 1..4 or depth other than 8 and 16. */
 FPNGB_API size_t fpngb_max_reduced_encoded_size(uint32_t w, uint32_t h, uint32_t chans, uint32_t depth);
+
+/* ---- LZ77 mode (opt-in: FPNGB_LZ77_CHAIN(k) on fpngb_encode_png_ragged_device, its _typed twin and
+ * fpngb_encode_label_ragged_device) ---------------------------------------------------------------------------------------------
+ * With a chain depth k in 1..256 in the flags, every image of the call, 8-bit RGB and RGBA included (no fpng file is written), is
+ * a PNG whose zlib stream holds LZ77 matches at any distance up to 32768, across rows.  The rule (DESIGN.md §4.6 "LZ77"):
+ *   S        the filtered stream: per row the filter byte of the row filter rule above, then the filtered row (a label map's or a
+ *            reduced image's packed rows as those paths make them).  N = h * (1 + row bytes).
+ *   hash     H(p) = ((S[p] << 16 | S[p+1] << 8 | S[p+2]) * 0x9E3779B1 mod 2^32) >> 17, 15 bits.
+ *   segments S is cut into segments of 16384 bytes (the last may be shorter), each parsed on its own: no match ends past its
+ *            segment's end; sources may lie anywhere earlier in S.
+ *   search   at p with p + 3 <= segment end: the earlier positions q with H(q) = H(p), newest first, at most k of them (hash
+ *            collisions count), stopping at the first q with p - q > 32768.  A candidate's length is the number of i <
+ *            min(258, segment end - p) with S[q+i] = S[p+i] (sources may overlap p).  The longest wins, ties to the nearest;
+ *            the walk stops once a candidate reaches the maximum.
+ *   parse    greedy: a best length >= 3 emits the match (L, p - q) and advances by L, else the literal S[p] and 1.
+ *   code     one dynamic block, BFINAL set, zlib header 78 01.  Literal/length: the 286-symbol histogram with end-of-block counted
+ *            once, fpng's 2-pass construction (16-bit scaling, Moffat-Katajainen, limit 12).  Distance: the 30-symbol histogram by
+ *            the same construction; with fewer than two distance symbols used, the used symbol s (0 if none) and s ^ 1 get 1-bit
+ *            codes.  HDIST is the last distance symbol of nonzero length + 1.  Code-length code as for the other PNG files.
+ *   stored   as without the mode: stored blocks (filter 0) when the compressed stream is longer, or with FPNGB_FORCE_UNCOMPRESSED.
+ * Containers, slot bounds and offsets are unchanged (the stored fallback bounds every file; RGB8 and RGBA8 use
+ * fpngb_max_encoded_size(w, h, 3 | 4)).  It combines with FPNGB_ENCODE_REDUCE and FPNGB_FORCE_UNCOMPRESSED; FPNGB_ENCODE_SLOWER
+ * with a chain depth, and a depth above 256, are FPNGB_ERR_INVALID_ARG, checked before anything is enqueued.
+ * These files decode through the any-PNG inflate (one warp per file), not fpng's parallel decoder: a single large file decodes
+ * more slowly than an fpng file.
+ * Launches: per non-empty class a filter pass writing S and a stored-row pass; the match kernel (one CTA per segment:
+ * fpngb_profile_read slot 11), the Huffman build, a segment-bits kernel, the offsets, a segment-pack kernel, Adler-32 and CRC.
+ * Workspace: about 3 bytes per byte of S (S, one 16-bit token unit per byte at most) plus 16 bytes per segment; a call whose
+ * workspace cannot be allocated fails with the CUDA error code, as other calls do. */
+#define FPNGB_LZ77_CHAIN(k) ((uint32_t)(k) << 16)
 
 /* Batch of n equally sized images in HOST memory (ideally pinned: see fpngb_host_alloc) -> n files in host memory,
  * out + i*out_stride, sizes[i].  Internally pipelines H2D copy / kernels / D2H copy over chunks of the batch. */
